@@ -1,8 +1,9 @@
-"""bench.py — tokens/sec of one ProGen training step (BASELINE.json configs[1]) on N B200s of one node.
+"""bench.py — tokens/sec of one ProGen training step (BASELINE.json configs[1]) on N H100s of one node.
 
     python bench.py --gpus 1 --steps 10 --warmup 3
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P bench.py --gpus N ...
     python bench.py --impl reference ...      # the CPU arm: the oracle port timed on the host cores
+    python bench.py --dump-outputs DIR ...    # also write the last timed step's outputs as DIR/<name>.npy
 
 A "step" is one pass of the hot path over one synthetic batch: forward + loss + backward + (DDP gradient all-reduce) +
 clip/AdamW/apply_every, i.e. one iteration of the reference's inner loop (train.py:186-190).  Prints ONE JSON line.
@@ -64,7 +65,50 @@ def measured_peaks():
         j = json.load(open(p))
         return dict(burst=j['bf16_tflops'], sustained=j.get('bf16_tflops_sustained', j['bf16_tflops']), hbm=j['hbm_gbs'],
                     source='measured (MEASURED_PEAKS.json)')
-    return dict(burst=1590.0, sustained=1400.0, hbm=6650.0, source='fallback (B200_PROFILING.md)')
+    return dict(burst=989.0, sustained=989.0, hbm=3350.0, source='NVIDIA H100 SXM data sheet (dense BF16, 700 W), not measured')
+
+
+def gpu_info(index):
+    """name, power limit and max SM clock of the card the numbers are measured on (read-only nvidia-smi query)"""
+    try:
+        out = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader,nounits',
+                              '-i', str(index)], capture_output=True, text=True, timeout=30).stdout.strip().split(',')
+        return dict(name=out[0].strip(), power_limit_w=float(out[1]), sm_max_mhz=float(out[2]))
+    except Exception:
+        return dict(name=torch.cuda.get_device_name(index), power_limit_w=None, sm_max_mhz=None)
+
+
+DUMP_BYTES_MAX = 64 << 20
+
+
+def dump_outputs(out_dir, arrays):
+    """arrays: name -> numpy array (float32 / float64), written as out_dir/<name>.npy; at most 64 MB in all"""
+    os.makedirs(out_dir, exist_ok=True)
+    total = sum(a.nbytes for a in arrays.values())
+    assert total <= DUMP_BYTES_MAX, total
+    for name, a in arrays.items():
+        assert a.dtype in (np.float32, np.float64), (name, a.dtype)
+        np.save(os.path.join(out_dir, name + '.npy'), a)
+
+
+def sample_index(n, k, seed):
+    """a fixed, seeded, sorted sample of min(n, k) indices of [0, n)"""
+    if n <= k:
+        return np.arange(n)
+    return np.sort(np.random.default_rng(seed).choice(n, size=k, replace=False))
+
+
+def training_outputs(eng):
+    """What one training step hands its caller: the loss, the logits, the gradient and the updated parameters.  Logit
+    rows and parameter / gradient elements are fixed seeded samples (the full arrays exceed the dump budget)."""
+    rows = torch.as_tensor(sample_index(eng.logits.shape[0], 4096, 1), device=eng.logits.device)
+    idx = torch.as_tensor(sample_index(eng.n_params_padded, 1 << 20, 2), device=eng.params.device)
+    return dict(loss=eng.loss.detach().float().cpu().numpy(),
+                logits_rows=rows.cpu().numpy().astype(np.float64),
+                logits_sample=eng.logits.index_select(0, rows).float().cpu().numpy(),
+                param_index=idx.cpu().numpy().astype(np.float64),
+                grads_sample=eng.grads.index_select(0, idx).float().cpu().numpy(),
+                params_sample=eng.params.index_select(0, idx).float().cpu().numpy())
 
 
 class ClockSampler:
@@ -236,6 +280,8 @@ def run_decode_bench(args, cfgd):
         gen_tokens += gen
     barrier()
     wall_s = time.perf_counter() - t0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, dict(ids=np.asarray(ids.cpu() if torch.is_tensor(ids) else ids).astype(np.float64)))
     clocks = sampler.stop() if sampler else None
     launches = L.load().progen_launch_count() - c0
     t = torch.tensor([dev_s, wall_s], device='cuda')
@@ -256,13 +302,8 @@ def run_decode_bench(args, cfgd):
         achieved = (wb + rest) / per_tok_s / 1e9
         per_step_b = secb / (genb / Bb)
         achieved_b = (wb + Bb * rest) / per_step_b / 1e9
-        try:
-            dk = json.load(open(os.path.join(ROOT, 'profiles', 'r02_decode_kernel.json')))
-            traffic, traffic_b = dk['single']['dram_bytes_per_token'], dk['batched']['dram_bytes_per_step']
-        except Exception:
-            traffic = traffic_b = None
+        traffic = traffic_b = None
         roofline = dict(bound='hbm', achieved=achieved, peak=peaks['hbm'], unit='GB/s', frac=achieved / peaks['hbm'], traffic=traffic,
-                        traffic_unit='DRAM bytes per token (ncu --set full of one 8-position launch, profiles/r02_ncu_decode_persistent.txt)',
                         kernel='decode_persistent_kernel<1, bf16> (one cooperative kernel for the whole generation)',
                         algorithmic_bytes_per_token=wb + rest, us_per_token=per_tok_s * 1e6, peak_source=peaks['source'],
                         batched=dict(batch=Bb, tokens_per_sec=genb / secb, us_per_step=per_step_b * 1e6, achieved=achieved_b, traffic=traffic_b,
@@ -271,11 +312,11 @@ def run_decode_bench(args, cfgd):
                     ms_per_step=dev_s / args.steps * 1e3, higher_is_better=True, scaling='weak', vs_baseline=None,
                     dtype='f32' if args.fp32 else 'bf16', data='synthetic',
                     config=dict(workload=cfgd['name'], global_batch=world, seq_len=n, parallelism=f'replicas x{world}',
-                                l2='103 MB of bf16 weights + K/V do not stay in the 126 MB L2 between positions: ncu measures 125 MB of DRAM reads per token, the algorithmic 122 MB',
+                                l2='%.0f MB of weights + K/V per position do not stay in the 50 MB L2 between positions' % ((wb + rest) / 1e6),
                                 step='one generation of %d tokens' % (gen_tokens // args.steps)),
                     e2e=dict(value=tps_e2e, unit='tokens/s', h2d_bytes_per_step=int(n * 4 + 4), d2h_bytes_per_step=int(n * 4),
                              ms_per_step=wall_s / args.steps * 1e3),
-                    gpu_launches=int(launches), clocks=clocks, roofline=roofline)
+                    gpu_launches=int(launches), clocks=clocks, gpu=gpu_info(local_rank), roofline=roofline)
         if not args.no_cpu_baseline and world == 1:
             v, timed = cpu_decode_tokens_per_sec(kw, prime)
             line['cpu_baseline'] = dict(value=v, unit='tokens/s', cores=cpu_threads(), kind='port',
@@ -352,10 +393,10 @@ def time_step_kernels(eng, kw, iters=20):
     if eng.attn_tc:
         fa = attn_fwd_flops_per_token(kw) * T
         ms = _time_launch(lambda: eng.attn_fwd(s0['qkv'], s0['att'], s0['lse']), iters)
-        out.append(dict(key='attn_fwd', kernel='sliding-window attention forward (tcgen05, P and O in TMEM)', per_step=nl, ms=ms,
+        out.append(dict(key='attn_fwd', kernel='sliding-window attention forward (%s)' % ('wgmma, TMA-fed K/V' if eng.attn_wgmma else 'mma.sync'), per_step=nl, ms=ms,
                         flops=fa, shape=[eng.B, eng.h, eng.n, eng.w]))
         ms = _time_launch(lambda: eng.attn_bwd(s0['qkv'], s0['att'], eng.datt, s0['lse'], eng.dqkv), iters)
-        out.append(dict(key='attn_bwd', kernel='sliding-window attention backward (dQ kernel + dK/dV kernel, tcgen05)', per_step=nl,
+        out.append(dict(key='attn_bwd', kernel='sliding-window attention backward (dQ kernel + dK/dV kernel, %s)' % ('wgmma' if eng.attn_wgmma else 'mma.sync'), per_step=nl,
                         ms=ms, flops=2.0 * fa, shape=[eng.B, eng.h, eng.n, eng.w]))
     i = next((j for j, k in enumerate(eng.kinds) if k == 'glu'), None)
     if i is not None:
@@ -363,34 +404,21 @@ def time_step_kernels(eng, kw, iters=20):
         f = P + f'ff{i}/~/'
         n_glu = sum(1 for k in eng.kinds if k == 'glu')
         ms = _time_launch(lambda: eng.wgrad_gemm(s['y2'], d, eng.du, 2 * hid, eng.G(f + 'linear', 'w')), iters)
-        out.append(dict(key='wgrad_ffin', kernel='gemm_tc2_kernel<MN-major A, MN-major B, EPI_ACCUM, fp32> (CTA-pair tcgen05, FF proj_in '
-                                                 'weight gradient, split-K + TMA reduce-add)', per_step=n_glu, ms=ms,
+        out.append(dict(key='wgrad_ffin', kernel='gemm_tc_kernel<MN-major A, MN-major B, EPI_ACCUM, fp32> (wgmma, FF proj_in '
+                                                 'weight gradient, split-K %d)' % eng.wgrad_split(d, 2 * hid), per_step=n_glu, ms=ms,
                         flops=2.0 * T * d * 2 * hid, shape=[d, 2 * hid, T]))
         ms = _time_launch(lambda: eng.fwd_gemm(s['y2'], d, eng.W(f + 'linear', 'w'), 2 * hid, s['hact'], epi=L.EPI_GLU, ldo=hid,
                                                out2=s['u'], ldo2=2 * hid, bias=eng.Pf(f + 'linear', 'b')), iters)
-        out.append(dict(key='ffin_glu', kernel='gemm_tc2_kernel<K-major A, MN-major B, EPI_GLU, bf16> (CTA-pair tcgen05, FF proj_in fwd)',
+        out.append(dict(key='ffin_glu', kernel='gemm_tc_kernel<K-major A, MN-major B, EPI_GLU, bf16> (wgmma, FF proj_in fwd)',
                         per_step=n_glu, ms=ms, flops=2.0 * T * d * 2 * hid, shape=[T, 2 * hid, d]))
         ms = _time_launch(lambda: eng.dgrad_gemm(eng.dres_lp, d, eng.W(f + 'linear_1', 'w'), hid, eng.du, epi=L.EPI_GLU_BWD,
                                                  ldo=2 * hid, aux=s['u'], ldaux=2 * hid), iters)
-        out.append(dict(key='ffout_dgrad_glu_bwd', kernel='gemm_tc2_kernel<K-major, K-major, EPI_GLU_BWD, bf16> (FF proj_out dgrad + GLU backward)',
+        out.append(dict(key='ffout_dgrad_glu_bwd', kernel='gemm_tc_kernel<K-major, K-major, EPI_GLU_BWD, bf16> (wgmma, FF proj_out dgrad + GLU backward)',
                         per_step=n_glu, ms=ms, flops=2.0 * T * d * hid, shape=[T, hid, d]))
     for o in out:
         o['tflops'] = o['flops'] / o['ms'] / 1e9
         o['step_ms'] = o['ms'] * o['per_step']
     return out
-
-
-def dominant_kernel_traffic(config, batch, key):
-    """dram__bytes_read.sum + dram__bytes_write.sum of ONE launch of kernel `key`, from the committed `ncu --set full`
-    captures (profiles/r02_dominant_kernel.json, else round 1's file); null for any other shape."""
-    for name in ('r02_dominant_kernel.json', 'r01_dominant_kernel.json'):
-        try:
-            j = json.load(open(os.path.join(ROOT, 'profiles', name)))
-            if j.get('config') == config and j.get('batch') == batch and key in j['kernels']:
-                return j['kernels'][key]['dram_bytes_per_launch']
-        except Exception:
-            pass
-    return None
 
 
 def main():
@@ -403,6 +431,8 @@ def main():
     ap.add_argument('--batch', type=int, default=None, help='per-GPU batch override')
     ap.add_argument('--fp32', action='store_true', help='fp32 engine (parity path) instead of bf16')
     ap.add_argument('--no-cpu-baseline', action='store_true')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help="write the last timed step's outputs as DIR/<name>.npy (float32/float64, <= 64 MB, seeded samples)")
     args = ap.parse_args()
     args.warmup = max(3, args.warmup) if args.impl == 'b200' else args.warmup
     cfgd = CONFIGS[args.config]
@@ -471,7 +501,7 @@ def main():
     sampler = ClockSampler(local_rank) if rank == 0 else None
     launches0 = L.load().progen_launch_count()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    prof_range = os.environ.get('PROGEN_PROFILE_RANGE') == '1'    # ncu --profile-from-start off: only the timed steps
+    prof_range = os.environ.get('PROGEN_PROFILE_RANGE') == '1'    # cudaProfilerStart/Stop around the timed steps only
     if prof_range:
         torch.cuda.profiler.start()
     e0.record()
@@ -483,6 +513,8 @@ def main():
     if prof_range:
         torch.cuda.profiler.stop()
     launches = L.load().progen_launch_count() - launches0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, training_outputs(eng))
     if graph_nodes:
         launches = graph_nodes * args.steps            # replayed graph: the host-side counter only sees the capture
     ms = torch.tensor([e0.elapsed_time(e1)], device='cuda')
@@ -575,13 +607,13 @@ def main():
             step_ms = ms_total / args.steps
             dom = max(kernels, key=lambda k: k['step_ms'])
             roofline = dict(bound='tensor', achieved=dom['tflops'], peak=peaks['burst'], unit='TFLOP/s',
-                            frac=dom['tflops'] / peaks['burst'], traffic=dominant_kernel_traffic(args.config, B, dom['key']),
+                            frac=dom['tflops'] / peaks['burst'], traffic=None,
                             kernel=dom['kernel'], shape=dom['shape'], ms=dom['ms'], launches_per_step=dom['per_step'],
                             share_of_step=dom['step_ms'] / step_ms,
                             peak_source=peaks['source'] + ', burst figure (kernel timed alone)', whole_step=whole_step,
                             others=[dict(key=k['key'], kernel=k['kernel'], shape=k['shape'], ms=k['ms'], launches_per_step=k['per_step'],
                                          share_of_step=k['step_ms'] / step_ms, achieved=k['tflops'], frac=k['tflops'] / peaks['burst'],
-                                         traffic=dominant_kernel_traffic(args.config, B, k['key']))
+                                         traffic=None)
                                     for k in kernels if k is not dom])
         else:
             roofline = dict(bound='tensor', traffic=None, **whole_step)
@@ -589,7 +621,7 @@ def main():
                     ms_per_step=ms_total / args.steps, higher_is_better=True, scaling='weak', vs_baseline=None,
                     dtype='f32' if args.fp32 else 'bf16', data='synthetic',
                     config=dict(workload=cfgd['name'], global_batch=B * world, seq_len=n, parallelism=f'dp{world}',
-                                l2='activations (~%.1f GB/step) far exceed the 126 MB L2; no explicit flush' % (eng_bytes(eng) / 1e9),
+                                l2='activations (~%.1f GB/step) far exceed the 50 MB L2; no explicit flush' % (eng_bytes(eng) / 1e9),
                                 optimizer='clip_by_global_norm(0.5)+adamw(2e-4,wd=1e-3,mask)+apply_every(4), every step',
                                 launch='CUDA graph of the whole step (%d kernels%s), replayed' % (graph_nodes, ' + the NCCL all-reduce' if world > 1 else '') if graph_nodes
                                        else 'eager launches'),
@@ -599,7 +631,7 @@ def main():
                              blocking_read=dict(ms_per_step=ms_e2e_blocking / args.steps,
                                                 value=tokens_per_step * args.steps / (ms_e2e_blocking / 1e3),
                                                 reader='loss.item() after every step (the reference train.py style)')),
-                    gpu_launches=int(launches), clocks=clocks, roofline=roofline, final_loss=final_loss,
+                    gpu_launches=int(launches), clocks=clocks, gpu=gpu_info(local_rank), roofline=roofline, final_loss=final_loss,
                     per_rank_ms_per_step=per_rank_ms)
         if comm:
             line['comm'] = comm

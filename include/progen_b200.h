@@ -1,4 +1,4 @@
-/* libprogen_b200.so — C ABI of the B200-native ProGen hot path.
+/* libprogen_b200.so — C ABI of the CUDA-native ProGen hot path (NVIDIA H100, sm_90a).
  *
  * Drop-in boundary (SURVEY.md §8(b)): the reference exposes `ProGen(**kwargs) -> .init / .apply`
  * (lucidrains/progen progen_transformer/progen.py:235-243) and everything below that call is executed by XLA.
@@ -11,7 +11,7 @@
  *    descriptors keyed by (pointer, shape).
  *  - tokens are rows: activations are row-major [T = B * seq_len, features]; `ld*` are element strides.
  *  - dtype codes: PROGEN_F32 = 0, PROGEN_BF16 = 1.  The residual stream and all parameter gradients are fp32.
- *  - sm_100a only (`progen_device_check`); there is no CPU or other-architecture fallback.
+ *  - sm_90a only (`progen_device_check`); there is no CPU or other-architecture fallback.
  */
 #ifndef PROGEN_B200_H
 #define PROGEN_B200_H
@@ -25,7 +25,7 @@ extern "C" {
 #define PROGEN_BF16 1
 
 #define PROGEN_BACKEND_SIMT 0     /* fp32-exact CUDA-core GEMM (mixed_precision=False path, progen.py:235) */
-#define PROGEN_BACKEND_TCGEN05 1  /* TMA + tcgen05.mma + TMEM GEMM, bf16 operands / fp32 accumulate */
+#define PROGEN_BACKEND_TC 1       /* TMA + wgmma GEMM, bf16 operands / fp32 accumulate */
 
 /* GEMM epilogues (fused with the matmul the reference line performs) */
 #define PROGEN_EPI_STORE 0     /* out = acc (+bias)                      progen.py:219-222 (logits), 185 (SGU proj)   */
@@ -109,19 +109,18 @@ int progen_local_attn_bwd_simt(const void* qkv, const void* out, const void* dou
                                float* delta, int dtype, int B, int seq_len, int window, int heads, int dim_head,
                                void* stream);
 
-/* tensor-core version (bf16, dim_head 64, window % 64 == 0): flash-style, scores stay on chip; same buffers as above */
+/* tensor-core version (bf16, dim_head 64, window % 64 == 0; mma.sync): flash-style, scores stay on chip; same buffers
+ * as above.  The backward applies the rotary backward to dq|dk|dv in its epilogue. */
 int progen_local_attn_fwd(const void* qkv, void* out, float* lse, int B, int seq_len, int window, int heads, int dim_head,
                           void* stream);
 int progen_local_attn_bwd(const void* qkv, const void* out, const void* dout, const float* lse, void* dqkv, float* delta,
                           const float* rot_sin, const float* rot_cos, int B, int seq_len, int window, int heads, int dim_head,
                           void* stream);
 
-/* tcgen05 forward (TMA-staged K/V, QK^T and PV as tcgen05.mma with S/O in TMEM, softmax by row-owning threads);
- * window % 128 == 0.  Same buffers as progen_local_attn_fwd. */
+/* Hopper version (bf16, dim_head 64, window % 128 == 0): the same algorithm with TMA-fed K/V (or Q/dO) tiles and wgmma;
+ * same buffers as progen_local_attn_fwd / _bwd. */
 int progen_local_attn_fwd_tc(const void* qkv, void* out, float* lse, int B, int seq_len, int window, int heads, int dim_head,
                              void* stream);
-
-/* tcgen05 backward (dQ kernel + dK/dV kernel, no atomics; delta produced by the dQ kernel); window % 128 == 0 */
 int progen_local_attn_bwd_tc(const void* qkv, const void* out, const void* dout, const float* lse, void* dqkv, float* delta,
                              const float* rot_sin, const float* rot_cos, int B, int seq_len, int window, int heads, int dim_head,
                              void* stream);

@@ -1,4 +1,4 @@
-"""progen_b200 — B200-native ProGen training + sampling engine (drop-in for lucidrains/progen's `ProGen`)."""
+"""progen_b200 — H100-native (sm_90a) ProGen training + sampling engine (drop-in for lucidrains/progen's `ProGen`)."""
 
 
 def __getattr__(name):

@@ -47,7 +47,7 @@ def file_save_checkpoint(path, package, keep_last_n=None):
 
 def get_checkpoint_fns(path):
     if str(path).startswith('gs://'):
-        raise NotImplementedError('GCS checkpoints are out of scope of the B200 engine (no network in this environment)')
+        raise NotImplementedError('GCS checkpoints are out of scope of this engine (local files only)')
     obj = Path(path)
     obj.mkdir(exist_ok=True, parents=True)
     return tuple(partial(fn, obj) for fn in (file_reset_checkpoint, file_get_last_checkpoint, file_save_checkpoint))

@@ -15,20 +15,20 @@ void progen_set_error(const char* fmt, ...) {
 
 extern "C" {
 
-const char* progen_version(void) { return "progen_b200 0.1.0 (sm_100a; tcgen05/TMA GEMM, CUDA " CUDA_VERSION_STR ")"; }
+const char* progen_version(void) { return "progen_b200 0.1.0 (sm_90a; wgmma/TMA GEMM, CUDA " CUDA_VERSION_STR ")"; }
 
 const char* progen_last_error(void) { return g_err; }
 
 long long progen_launch_count(void) { return (long long)__atomic_load_n(&g_progen_launches, __ATOMIC_RELAXED); }
 
-// north_star: no CPU fallback, sm_100 only.  Returns 0 iff the current device can run every kernel in this library.
+// No CPU fallback, sm_90 only.  Returns 0 iff the current device can run every kernel in this library.
 int progen_device_check(void) {
   int dev = 0;
   PG_CUDA(cudaGetDevice(&dev));
   cudaDeviceProp prop;
   PG_CUDA(cudaGetDeviceProperties(&prop, dev));
-  if (prop.major != 10) {
-    progen_set_error("device %d (%s) is sm_%d%d; libprogen_b200 is built for sm_100a only", dev, prop.name, prop.major,
+  if (prop.major != 9) {
+    progen_set_error("device %d (%s) is sm_%d%d; libprogen_b200 is built for sm_90a only", dev, prop.name, prop.major,
                      prop.minor);
     return PROGEN_ERR_DEVICE;
   }
@@ -55,7 +55,7 @@ int progen_gemm(const progen_gemm_t* d, void* stream) {
   if (g.epi_kind == EPI_GLU || g.epi_kind == EPI_GELU) PG_CHECK_ARG(g.epi.out2 != nullptr && g.epi.bias != nullptr);
   if (g.epi_kind == EPI_GLU_BWD || g.epi_kind == EPI_GELU_BWD) PG_CHECK_ARG(g.epi.aux != nullptr);
   if (g.epi_kind == EPI_ROTARY) PG_CHECK_ARG(g.epi.rot_sin && g.epi.rot_cos && d->seq_len > 0 && d->dim_head > 0 && d->dim_head % 2 == 0);
-  if (d->backend == PROGEN_BACKEND_TCGEN05) return gemm_tc_launch(g, (cudaStream_t)stream);
+  if (d->backend == PROGEN_BACKEND_TC) return gemm_tc_launch(g, (cudaStream_t)stream);
   if (d->backend == PROGEN_BACKEND_SIMT) return gemm_simt_launch(g, (cudaStream_t)stream);
   progen_set_error("progen_gemm: unknown backend %d", d->backend);
   return PROGEN_ERR_ARG;

@@ -9,8 +9,8 @@
 // Backward is two kernels without atomics: dQ (same tiling as forward) and dK/dV (one CTA per key tile, streaming the
 // query tiles that can see it); both recompute P from the saved log-sum-exp.
 //
-// TODO(next round): move QK^T / PV to tcgen05 with S/P in TMEM (north_star); this mma.sync version is the correct,
-// fused, already-compute-bound stepping stone (attention is ~11% of the model FLOPs at d=512, w=256).
+// The mixed-precision engine runs this version for windows that are multiples of 64 but not of 128; attn_wgmma.cu
+// (wgmma, TMA-fed tiles) covers the others.
 #include <stdlib.h>
 #include "common.cuh"
 #include "../../include/progen_b200.h"
@@ -506,7 +506,7 @@ template <typename K> int set_smem(K kern, int bytes) {
 struct TileChoice { int fwd, dq, dkv; };
 TileChoice tile_choice(int window) {
   static TileChoice env = [] {
-    TileChoice t{64, 64, 64};      // measured on B200 at B=64, n=1024, w=256, h=8: 64-row tiles win (occupancy)
+    TileChoice t{64, 64, 64};      // 64-row tiles by default: more CTAs per SM
     if (const char* e = getenv("PROGEN_ATTN_TILES")) sscanf(e, "%d,%d,%d", &t.fwd, &t.dq, &t.dkv);
     return t;
   }();

@@ -1,14 +1,14 @@
 #!/usr/bin/env bash
-# Build libprogen_b200.so in-tree for sm_100a (cross-compiles without a GPU).  Usage: build.sh [-j N]
+# Build libprogen_b200.so in-tree for sm_90a (H100) (cross-compiles without a GPU).  Usage: build.sh [-j N]
 set -euo pipefail
 HERE="$(cd "$(dirname "${BASH_SOURCE[0]}")" && pwd)"
 OUT="$HERE/../libprogen_b200.so"
 OBJ="$HERE/build"
 mkdir -p "$OBJ"
 NVCC="${NVCC:-/usr/local/cuda/bin/nvcc}"
-FLAGS=(-gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC,-O3
+FLAGS=(-gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC,-O3
        --expt-relaxed-constexpr -DCUDA_VERSION_STR="\"12.9\"" -I"$HERE" -I"$HERE/../../include")
-SRCS=(api gemm_tc gemm_tc2 gemm_simt elementwise ln_stream attn_simt attn_mma attn_tc attn_tc_pair attn_fwd_ts attn_tc_bwd attn_bwd_ts optim decode decode_persist)
+SRCS=(api gemm_tc gemm_simt elementwise ln_stream attn_simt attn_mma attn_wgmma optim decode decode_persist)
 pids=()
 for s in "${SRCS[@]}"; do
   [ -f "$HERE/$s.cu" ] || continue

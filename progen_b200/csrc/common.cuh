@@ -1,4 +1,4 @@
-// Shared helpers for libprogen_b200.so (sm_100a only).
+// Shared helpers for libprogen_b200.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -52,7 +52,7 @@ static inline int pg_num_sms() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;
   }
   return n;
 }

@@ -1,7 +1,7 @@
 // KV-cached autoregressive decode as ONE persistent kernel (BASELINE config 5; reference utils.py:106-135, sample.py:66-71).
 //
-// Round 1 replayed a CUDA graph of ~150 tiny kernels per token: 1.0 ms / token for 103 MB of bf16 weights = 1.6 % of the
-// HBM roofline, pure launch latency.  Here one cooperative kernel (one CTA per SM) generates every position of the
+// The per-step path (decode.cu) replays a CUDA graph of ~150 tiny kernels per token and is bound by launch latency.  Here
+// one cooperative kernel (one CTA per SM) generates every position of the
 // launch: the phases of a layer (LN + shift + QKV + rotary + cache | windowed attention | out-proj + residual | LN + shift +
 // FF-in + GLU/GELU | [gMLP: gate LN + causal spatial mix | SGU proj] | FF-out + residual) are separated by a grid barrier
 // (one atomic + one acquire poll per CTA), and the token loop, the sampler (top-k filter that keeps k-1 and zeroes the
@@ -32,9 +32,9 @@ using namespace tc;
 constexpr int WSEGS = 32;               // (row pair, 256-column segment) weight units of one CTA per wave
 constexpr int MAXEV = 160;              // profile events per sampled CTA (grid barriers of one step)
 constexpr int MAXSPLIT = 8;             // SGU: most splits of the history range
-// threads per CTA by batch tile.  A single sequence is a latency chain: 8 warps are enough.  For B > 8 both 256 threads (255
-// registers) and 512 (128 registers, some spills) were measured: 31.6 k tokens/s at B = 64 either way — the phases are bound by
-// L2 traffic of the activation staging and by memory latency, not by issue slots — so the default is the spill-free one.
+// threads per CTA by batch tile.  A single sequence is a latency chain: 8 warps are enough.  For B > 8 the phases are bound by
+// L2 traffic of the activation staging and by memory latency, not by issue slots, so the default is 256 threads (no
+// spills) rather than 512.
 #ifndef PROGEN_DECODE_BATCH_THREADS
 #define PROGEN_DECODE_BATCH_THREADS 256
 #endif
@@ -1564,7 +1564,7 @@ static __device__ __forceinline__ void run(const progen_decode_run_t& r) {
         } else {
           // more sequences than the batch tile: sub-batches of BT sequences run through the phase one after the other with
           // the same weights (per warp, 32 sequences cost 4 LayerNorm rows and 8 k-steps; a 64-wide tile costs twice that
-          // in series — measured: 32 sequences 0.73 ms per step, a 64-wide tile 1.31 ms)
+          // in series, and half the shared memory of a 64-wide tile)
           for (int b0 = 0; b0 < B; b0 += BT) {
             if (b0 > 0) __syncthreads();                       // every warp is done reading the previous pass's staged rows
             Phase ps = ph;

@@ -1,4 +1,4 @@
-// GEMM epilogues shared by the tcgen05 GEMM (gemm_tc.cu) and the fp32 SIMT GEMM (gemm_simt.cu).
+// GEMM epilogues shared by the wgmma GEMM (gemm_tc.cu) and the fp32 SIMT GEMM (gemm_simt.cu).
 // A thread hands over NV consecutive accumulator columns of one output row; the epilogue fuses what the
 // reference does right after the matmul (bias, rotary, residual add, GELU / GLU, their backward forms).
 #pragma once
@@ -30,12 +30,8 @@ struct EpiArgs {
 };
 
 // ---------------------------------------------------------------------------------------------------------
-// How an epilogue thread moves its row slice to / from global memory.
-//   DirectIO      : per-thread vector accesses (CUDA-core GEMM: 8 consecutive columns per thread)
-//   WarpStagedIO  : the tcgen05 epilogue owns one ROW per lane (TMEM lane == row), so direct stores would touch 32
-//                   different 128-byte lines per instruction (LSU wavefront bound).  Instead the warp transposes 64-byte
-//                   row slices through a private shared-memory buffer so each instruction moves 8 rows x 64 contiguous
-//                   bytes; same for the loads of residual / saved pre-activations.
+// How an epilogue thread moves its row slice to / from global memory: per-thread vector accesses (both GEMMs hand
+// every thread 8 consecutive columns of one row).
 struct DirectIO {
   template <int N, typename T> __device__ __forceinline__ void store(T* p, long long, const float (&v)[N], bool valid) const {
     if (valid) store_vec<N>(p, v);
@@ -49,117 +45,6 @@ struct DirectIO {
   }
 };
 
-constexpr int STAGE_WARP_BYTES = 32 * 64;                // 32 rows x (at most) 64 B per epilogue warp, 128 B aligned
-
-// Byte offset of 16-byte piece q of row r in a warp's staging buffer whose rows hold PPR pieces (dense, no padding).
-// The piece index is XOR-swizzled with the 128-byte line the row sits in, so that BOTH access patterns are
-// bank-conflict free: lane = row (8 consecutive rows, one piece) and lane = (row, piece) in row-major order.
-template <int PPR> __device__ __forceinline__ int stage_off(int r, int q) {
-  return r * (PPR * 16) + ((q ^ ((r * PPR / 8) & (PPR - 1))) << 4);
-}
-
-struct WarpStagedIO {
-  uint8_t* buf;          // this warp's staging buffer (generic pointer into shared memory)
-  int lane;
-  unsigned valid_mask;   // bit r: row r of this warp's 32-row block is inside the matrix
-
-  template <typename T> static __device__ __forceinline__ uint4 pack16(const float* v) {
-    uint4 t;
-    if constexpr (sizeof(T) == 2) {
-      t.x = pack_bf16x2(v[0], v[1]); t.y = pack_bf16x2(v[2], v[3]); t.z = pack_bf16x2(v[4], v[5]); t.w = pack_bf16x2(v[6], v[7]);
-    } else {
-      t.x = __float_as_uint(v[0]); t.y = __float_as_uint(v[1]); t.z = __float_as_uint(v[2]); t.w = __float_as_uint(v[3]);
-    }
-    return t;
-  }
-  // by value: a reference to shared memory makes the compiler read the four words with separate 4-byte LDS
-  template <typename T> static __device__ __forceinline__ void unpack16(const uint4 t, float* v) {
-    if constexpr (sizeof(T) == 2) {
-      const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&t);
-#pragma unroll
-      for (int j = 0; j < 4; ++j) { const float2 f = __bfloat1622float2(h[j]); v[2 * j] = f.x; v[2 * j + 1] = f.y; }
-    } else {
-      v[0] = __uint_as_float(t.x); v[1] = __uint_as_float(t.y); v[2] = __uint_as_float(t.z); v[3] = __uint_as_float(t.w);
-    }
-  }
-
-  // p: this lane's (row, col) element; rows of the warp are consecutive, `ld` elements apart
-  template <int N, typename T> __device__ __forceinline__ void store(T* p, long long ld, const float (&v)[N], bool) const {
-    constexpr int BYTES = N * (int)sizeof(T);
-    constexpr int SW = BYTES < 64 ? BYTES : 64;          // slice width in bytes per pass
-    constexpr int PPR = SW / 16;                         // 16-byte pieces per row slice
-    constexpr int EPP = 16 / (int)sizeof(T);             // elements per piece
-    uint8_t* base = reinterpret_cast<uint8_t*>(p - (long long)lane * ld);
-#pragma unroll
-    for (int s = 0; s < BYTES / SW; ++s) {
-#pragma unroll
-      for (int q = 0; q < PPR; ++q)
-        *reinterpret_cast<uint4*>(buf + stage_off<PPR>(lane, q)) = pack16<T>(&v[s * (SW / (int)sizeof(T)) + q * EPP]);
-      __syncwarp();
-#pragma unroll
-      for (int it = 0; it < PPR; ++it) {
-        const int idx = it * 32 + lane;
-        const int r = idx / PPR, q = idx % PPR;
-        if ((valid_mask >> r) & 1u) {
-          const uint4 t = *reinterpret_cast<const uint4*>(buf + stage_off<PPR>(r, q));
-          *reinterpret_cast<uint4*>(base + (long long)r * ld * (int)sizeof(T) + s * SW + q * 16) = t;
-        }
-      }
-      __syncwarp();
-    }
-  }
-  // load = load_issue (coalesced global loads into raw registers; `p` is only used for address arithmetic, `mask` says
-  // which of the warp's 32 rows exist) + load_finish (transpose through the staging buffer).  (Issuing the next chunk's
-  // loads between the two halves was measured and is slower: the bytes in flight stay capped by registers.  The CTA-pair
-  // kernel gemm_tc2.cu stages this operand with TMA instead.)
-  template <int N, typename T>
-  __device__ __forceinline__ void load_issue(const T* p, long long ld, uint4 (&t)[N * (int)sizeof(T) / 16], unsigned mask) const {
-    constexpr int BYTES = N * (int)sizeof(T);
-    constexpr int SW = BYTES < 64 ? BYTES : 64;
-    constexpr int PPR = SW / 16;
-    constexpr int PASSES = BYTES / SW;
-    const uint8_t* base = reinterpret_cast<const uint8_t*>(p - (long long)lane * ld);
-#pragma unroll
-    for (int s = 0; s < PASSES; ++s) {
-#pragma unroll
-      for (int it = 0; it < PPR; ++it) {
-        const int idx = it * 32 + lane;
-        const int r = idx / PPR, q = idx % PPR;
-        t[s * PPR + it] = make_uint4(0u, 0u, 0u, 0u);
-        if ((mask >> r) & 1u)
-          t[s * PPR + it] = *reinterpret_cast<const uint4*>(base + (long long)r * ld * (int)sizeof(T) + s * SW + q * 16);
-      }
-    }
-  }
-  template <int N, typename T> __device__ __forceinline__ void load(const T* p, long long ld, float (&v)[N], bool) const {
-    uint4 t[N * (int)sizeof(T) / 16];
-    load_issue<N, T>(p, ld, t, valid_mask);
-    load_finish<N, T>(t, v);
-  }
-  template <int N, typename T>
-  __device__ __forceinline__ void load_finish(const uint4 (&t)[N * (int)sizeof(T) / 16], float (&v)[N]) const {
-    constexpr int BYTES = N * (int)sizeof(T);
-    constexpr int SW = BYTES < 64 ? BYTES : 64;
-    constexpr int PPR = SW / 16;
-    constexpr int EPP = 16 / (int)sizeof(T);
-    constexpr int PASSES = BYTES / SW;
-#pragma unroll
-    for (int s = 0; s < PASSES; ++s) {
-#pragma unroll
-      for (int it = 0; it < PPR; ++it) {
-        const int idx = it * 32 + lane;
-        const int r = idx / PPR, q = idx % PPR;
-        *reinterpret_cast<uint4*>(buf + stage_off<PPR>(r, q)) = t[s * PPR + it];
-      }
-      __syncwarp();
-#pragma unroll
-      for (int q = 0; q < PPR; ++q)
-        unpack16<T>(*reinterpret_cast<const uint4*>(buf + stage_off<PPR>(lane, q)), &v[s * (SW / (int)sizeof(T)) + q * EPP]);
-      __syncwarp();
-    }
-  }
-};
-
 // v[i] += bias[col + i]: the same NV floats for every lane (broadcast), fetched with 16-byte loads
 template <int NV> __device__ __forceinline__ void add_bias(const float* __restrict__ bias, int col, float (&v)[NV]) {
 #pragma unroll
@@ -169,7 +54,7 @@ template <int NV> __device__ __forceinline__ void add_bias(const float* __restri
   }
 }
 
-// Every lane of the calling warp must enter (staged IO is warp-cooperative); `valid` says whether this lane's row exists.
+// `valid` says whether this thread's row exists.
 template <int KIND, typename TO, int NV, typename IO>
 __device__ __forceinline__ void epi_apply(const EpiArgs& e, const IO& io, long long row, int col, float (&v)[NV], bool valid) {
   constexpr bool FAST = sizeof(TO) == 2;      // bf16 outputs: hardware tanh is below the output rounding
@@ -286,6 +171,3 @@ __device__ __forceinline__ void epi_apply(const EpiArgs& e, const IO& io, long l
     }
   }
 }
-
-// kinds whose epilogue reads a second [rows x cols] operand from global memory (residual stream / saved pre-activations)
-template <int KIND> constexpr bool epi_has_aux = KIND == EPI_RESIDUAL || KIND == EPI_GLU_BWD || KIND == EPI_GELU_BWD;

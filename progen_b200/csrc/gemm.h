@@ -1,5 +1,5 @@
 // Internal GEMM interface: D[M,N] (+)= A[M,K] * B[N,K]^T with a fused epilogue.  Two backends:
-//   gemm_tc.cu   — bf16 operands, TMA -> 128B-swizzled smem -> tcgen05.mma -> TMEM -> epilogue (sm_100a)
+//   gemm_tc.cu   — bf16 operands, TMA -> 128B-swizzled smem -> wgmma -> registers -> epilogue (sm_90a)
 //   gemm_simt.cu — fp32 (or bf16) operands on CUDA cores, exact fp32 accumulation (the fp32 parity path)
 #pragma once
 #include "epilogues.cuh"
@@ -23,7 +23,4 @@ struct GemmArgs {
 };
 
 int gemm_tc_launch(const GemmArgs& g, cudaStream_t stream);
-// CTA-pair (cta_group::2, 256x256 tiles) variant for the un-batched activation GEMMs; gemm_tc_launch routes to it
-bool gemm_tc2_eligible(const GemmArgs& g);
-int gemm_tc2_launch(const GemmArgs& g, cudaStream_t stream);
 int gemm_simt_launch(const GemmArgs& g, cudaStream_t stream);

@@ -1,156 +1,38 @@
-// tcgen05 GEMM for sm_100a: D[M,N] (+)= A[M,K] * B[N,K]^T, bf16 operands, fp32 accumulation in TMEM.
+// wgmma GEMM for sm_90a: D[M,N] (+)= A[M,K] * B[N,K]^T, bf16 operands, fp32 accumulation in registers.
 //
-//   warp 0      : TMA producer   (cp.async.bulk.tensor.2d, 128B swizzle, mbarrier complete_tx)
-//   warp 1      : MMA issuer     (one thread: tcgen05.mma.cta_group::1.kind::f16, 128 x BN x 16 per instruction)
-//   warp 2      : TMEM allocator (2 accumulator stages of BN fp32 columns)
-//   warps 4..7  : epilogue       (tcgen05.ld 32x32b -> registers -> fused epilogue -> global)
+//   warpgroup 0    : TMA producer (one thread: cp.async.bulk.tensor.2d, 128B swizzle, mbarrier complete_tx)
+//   warpgroups 1, 2: consumers, 64 rows of the 128 x 128 tile each (wgmma.mma_async m64n128k16, both operands read
+//                    from shared memory), then the fused epilogue
 //
-// Persistent: one CTA per SM loops over output tiles; the two TMEM accumulator stages let the epilogue of
-// tile i overlap the mainloop of tile i+1.  Operands may be K-major or MN-major (wgrad reads the activations
-// and the output gradient with the token dimension as K, i.e. MN-major) — both go through the same 128B-swizzled
-// shared-memory layout, only the UMMA descriptors differ.
+// One CTA per output tile; the shared-memory ring holds STAGES k-blocks so the TMA loads run ahead of the MMAs.  Operands
+// may be K-major or MN-major (wgrad reads the activations and the output gradient with the token dimension as K, i.e.
+// MN-major): TMA writes both into the same 128B-swizzled layout and only the wgmma descriptors and transpose bits differ.
+// After the last k-block the accumulators go through shared memory (the drained ring) so that every epilogue thread
+// owns 8 consecutive columns of one row: the global loads / stores of the epilogue are 16-byte vectors, coalesced
+// along the row.
 #include <cuda.h>
 #include <mutex>
 #include <unordered_map>
 #include "gemm.h"
+#include "tc_ptx.cuh"
 
 namespace {
 
+using namespace tc;
+
 constexpr int BM = 128;
+constexpr int BN = 128;
 constexpr int BK = 64;                 // 64 bf16 = 128 bytes = one swizzle row
-constexpr int UMMA_K = 16;
-constexpr int SMEM_LIMIT = 227 * 1024;
-
-// Epilogue shape per kind.  The math-heavy epilogues (GLU / GELU forward and backward: tanh, two outputs, saved
-// pre-activations) are bound by instruction issue and latency of the epilogue warps, not by the tensor pipe: they get 16
-// epilogue warps (4 per TMEM lane quarter) working on 16-column chunks (small register footprint: 640 threads must fit
-// 64K registers).  The light epilogues keep 8 warps and 32-column chunks.
-template <int KIND> struct EpiCfg {
-  // Measured on B200 (config-2 FF proj_in + GLU): 16 warps / 16-column chunks / 3 smem stages = 0.348 ms vs 0.334 ms for
-  // 8 warps / 32 columns / 4 stages — these GEMMs are bound by L2 traffic (operand re-reads + two outputs), not by the
-  // epilogue's issue rate, so every kind uses the 8-warp shape; the 16-warp shape stays selectable here.
-  static constexpr bool HEAVY = false && (KIND == EPI_GLU || KIND == EPI_GLU_BWD || KIND == EPI_GELU || KIND == EPI_GELU_BWD);
-  static constexpr int EW = HEAVY ? 16 : 8;             // epilogue warps
-  static constexpr int CW = HEAVY ? 16 : 32;            // accumulator columns per tcgen05.ld
-  static constexpr int THREADS = 128 + 32 * EW;         // 4 control warps + epilogue warps
-};
-
-template <int BN, int KIND> struct TileCfg {
-  static constexpr int A_BYTES = BM * BK * 2;           // 16 KiB
-  static constexpr int B_BYTES = BN * BK * 2;           // 16 / 32 KiB
-  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int BAR_BYTES = 256;
-  static constexpr int FIXED = 1024 /*align slack*/ + BAR_BYTES + EpiCfg<KIND>::EW * STAGE_WARP_BYTES;
-  static constexpr int STAGES_FIT = (SMEM_LIMIT - FIXED) / STAGE_BYTES;
-  static constexpr int STAGES = STAGES_FIT > 6 ? 6 : STAGES_FIT;        // 4 (BN=256, 8 warps) / 3 (BN=256, 16 warps) / 6 (BN=128)
-  static constexpr int TMEM_COLS = 2 * BN;              // 256 / 512
-  static constexpr int SMEM_TOTAL = STAGES * STAGE_BYTES + FIXED;
-};
-
-// ------------------------------------------------------------------------------------------------ PTX
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t ok = 0;
-  uint32_t spins = 0;
-  do {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(bar), "r"(parity)
-        : "memory");
-    if (!ok && ++spins > (1u << 26)) __trap();   // a protocol bug must fail loudly instead of hanging the GPU
-  } while (!ok);
-}
-__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tcgen05_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tcgen05_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tcgen05_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-__device__ __forceinline__ void umma_bf16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum)
-      : "memory");
-}
-
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-  uint32_t r[32];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-template <int CW> __device__ __forceinline__ void tmem_ld(uint32_t taddr, float (&v)[CW]) {
-  if constexpr (CW == 32) tmem_ld32(taddr, v); else tmem_ld16(taddr, v);
-}
-
-// ---------------------------------------------------------------------------------- UMMA descriptors
-// Shared-memory matrix descriptor (cute/arch/mma_sm100_desc.hpp SmemDescriptor): start>>4 [0,14), LBO>>4 [16,30),
-// SBO>>4 [32,46), version=1 [46,48), layout_type [61,64) with SWIZZLE_128B = 2.
-//   K-major  tile (rows x 64 bf16, 128 B per row): 8-row groups 1024 B apart -> SBO = 1024; LBO unused (1).
-//   MN-major tile (64-element MN chunks of [64 k-rows x 128 B], chunks 8192 B apart): LBO = 8192 (next MN chunk),
-//            SBO = 1024 (next 8 k-rows).
-template <bool MN_MAJOR>
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-  d |= (uint64_t)(MN_MAJOR ? (8192 >> 4) : 1) << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-// advancing one UMMA_K (16 elements) inside a stage: K-major +32 B; MN-major +16 k-rows * 128 B = 2048 B
-template <bool MN_MAJOR> __device__ __forceinline__ uint32_t desc_k_step() { return MN_MAJOR ? (2048 >> 4) : (32 >> 4); }
-
-// Instruction descriptor (InstrDescriptor): c_format F32 (1) [4,6), a/b_format BF16 (1) [7,10)/[10,13),
-// a_major [15], b_major [16], N>>3 [17,23), M>>4 [24,29).
-template <int BN, bool A_MN, bool B_MN> __device__ __forceinline__ uint32_t make_idesc() {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((A_MN ? 1u : 0u) << 15) | ((B_MN ? 1u : 0u) << 16) |
-         ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-}
+constexpr int WG_K = 16;               // K of one wgmma
+constexpr int THREADS = 384;           // producer warpgroup + two consumer warpgroups
+constexpr int A_BYTES = BM * BK * 2;   // 16 KiB
+constexpr int B_BYTES = BN * BK * 2;   // 16 KiB
+constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
+constexpr int STAGES = 6;
+constexpr int CS_LD = BN + 4;          // fp32 row stride of the accumulator tile staged for the epilogue
+constexpr int SMEM_TOTAL = 1024 /*align slack*/ + STAGES * STAGE_BYTES + 2 * STAGES * 8;
+static_assert(BM * CS_LD * 4 <= STAGES * STAGE_BYTES, "the epilogue tile reuses the operand ring");
+static_assert(SMEM_TOTAL <= 227 * 1024, "H100: 227 KiB of shared memory per block");
 
 struct GemmDev {
   int M, N, K;
@@ -162,19 +44,17 @@ struct GemmDev {
 };
 
 struct TileInfo {
-  int z, ks, m0, n0, kb_begin, kb_end;
+  int z, m0, n0, kb_begin, kb_end;
 };
 
-template <int BN>
-__device__ __forceinline__ bool decode_tile(const GemmDev& g, int t, TileInfo& ti) {
+__device__ __forceinline__ void decode_tile(const GemmDev& g, int t, TileInfo& ti) {
   const int m_tiles = (g.M + BM - 1) / BM;
   const int n_tiles = (g.N + BN - 1) / BN;
   const int per_z = g.split_k * m_tiles * n_tiles;
-  if (t >= per_z * g.batch) return false;
   ti.z = t / per_z;
   int r = t - ti.z * per_z;
-  ti.ks = r / (m_tiles * n_tiles);
-  r -= ti.ks * (m_tiles * n_tiles);
+  const int ks = r / (m_tiles * n_tiles);
+  r -= ks * (m_tiles * n_tiles);
   ti.m0 = (r / n_tiles) * BM;
   ti.n0 = (r % n_tiles) * BN;
   const int kb_total = (g.K + BK - 1) / BK;
@@ -183,202 +63,130 @@ __device__ __forceinline__ bool decode_tile(const GemmDev& g, int t, TileInfo& t
   if (g.causal == 2) b = min(kb_total, ti.m0 / BK);
   if (g.split_k > 1) {
     const int per = (kb_total + g.split_k - 1) / g.split_k;
-    b = ti.ks * per;
+    b = min(kb_total, ks * per);
     e = min(kb_total, b + per);
   }
   ti.kb_begin = b;
   ti.kb_end = e;
-  return true;
 }
 
-template <int BN, bool A_MN, bool B_MN, int KIND, typename TO>
-__global__ void __launch_bounds__(EpiCfg<KIND>::THREADS, 1)
+template <bool A_MN, bool B_MN, int KIND, typename TO>
+__global__ void __launch_bounds__(THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b, const GemmDev g) {
-  using Cfg = TileCfg<BN, KIND>;
-  constexpr int STAGES = Cfg::STAGES;
-  constexpr int EW = EpiCfg<KIND>::EW, CW = EpiCfg<KIND>::CW;
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;      // SWIZZLE_128B needs 1024 B alignment
-  const uint32_t bar_base = smem_base + STAGES * Cfg::STAGE_BYTES;
-  // barrier layout (8 B each): full[STAGES], empty[STAGES], tmem_full[2], tmem_empty[2], then the TMEM base slot
+  const uint32_t raw_u32 = smem_u32(smem_raw);
+  const uint32_t smem_base = (raw_u32 + 1023u) & ~1023u;      // SWIZZLE_128B needs 1024 B alignment
+  const uint32_t bar_base = smem_base + STAGES * STAGE_BYTES;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-  auto tfull_bar = [&](int s) { return bar_base + 8u * (2 * STAGES + s); };
-  auto tempty_bar = [&](int s) { return bar_base + 8u * (2 * STAGES + 2 + s); };
-  const uint32_t tmem_slot = bar_base + 8u * (2 * STAGES + 4);
-  volatile uint32_t* tmem_slot_ptr =
-      reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7;
+  TileInfo ti;
+  decode_tile(g, blockIdx.x, ti);
 
-  if (warp == 0 && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tma_a) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tma_b) : "memory");
-  }
-  if (warp == 1 && lane == 0) {
+  if (threadIdx.x == 0) {
+    prefetch_tensormap(&tma_a);
+    prefetch_tensormap(&tma_b);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
+      mbar_init(empty_bar(s), 2);                 // one arrival per consumer warpgroup
     }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(tfull_bar(s), 1);
-      mbar_init(tempty_bar(s), EW);              // one arrival per epilogue warp
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    fence_barrier_init();
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "n"(Cfg::TMEM_COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
 
-  if (warp == 0) {
+  if (wg == 0) {
     // ===================================================================== TMA producer
-    if (lane == 0) {
+    if (threadIdx.x == 0) {
+      const int a_row0 = ti.z * g.a_batch_rows;
+      const int b_row0 = ti.z * g.b_batch_rows;
       int stage = 0;
       uint32_t phase = 0;
-      TileInfo ti;
-      for (int t = blockIdx.x; decode_tile<BN>(g, t, ti); t += gridDim.x) {
-        const int a_row0 = ti.z * g.a_batch_rows;
-        const int b_row0 = ti.z * g.b_batch_rows;
-        for (int kb = ti.kb_begin; kb < ti.kb_end; ++kb) {
-          mbar_wait(empty_bar(stage), phase ^ 1);
-          const uint32_t sa = smem_base + stage * Cfg::STAGE_BYTES;
-          const uint32_t sb = sa + Cfg::A_BYTES;
-          mbar_expect_tx(full_bar(stage), Cfg::STAGE_BYTES);
-          const int k0 = kb * BK;
-          if constexpr (!A_MN) {
-            tma_load_2d(sa, &tma_a, full_bar(stage), k0, a_row0 + ti.m0);                 // box {64 k, 128 m}
-          } else {
+      for (int kb = ti.kb_begin; kb < ti.kb_end; ++kb) {
+        mbar_wait(empty_bar(stage), phase ^ 1);
+        const uint32_t sa = smem_base + stage * STAGE_BYTES;
+        const uint32_t sb = sa + A_BYTES;
+        mbar_expect_tx(full_bar(stage), STAGE_BYTES);
+        const int k0 = kb * BK;
+        if constexpr (!A_MN) {
+          tma_load_2d(sa, &tma_a, full_bar(stage), k0, a_row0 + ti.m0);                   // box {64 k, 128 m}
+        } else {
 #pragma unroll
-            for (int i = 0; i < BM / 64; ++i)                                              // boxes {64 m, 64 k}
-              tma_load_2d(sa + i * 8192, &tma_a, full_bar(stage), ti.m0 + 64 * i, a_row0 + k0);
-          }
-          if constexpr (!B_MN) {
-            tma_load_2d(sb, &tma_b, full_bar(stage), k0, b_row0 + ti.n0);                 // box {64 k, BN n}
-          } else {
-#pragma unroll
-            for (int i = 0; i < BN / 64; ++i)                                              // boxes {64 n, 64 k}
-              tma_load_2d(sb + i * 8192, &tma_b, full_bar(stage), ti.n0 + 64 * i, b_row0 + k0);
-          }
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+          for (int i = 0; i < BM / 64; ++i)                                                // boxes {64 m, 64 k}
+            tma_load_2d(sa + i * 8192, &tma_a, full_bar(stage), ti.m0 + 64 * i, a_row0 + k0);
         }
+        if constexpr (!B_MN) {
+          tma_load_2d(sb, &tma_b, full_bar(stage), k0, b_row0 + ti.n0);                   // box {64 k, 128 n}
+        } else {
+#pragma unroll
+          for (int i = 0; i < BN / 64; ++i)                                                // boxes {64 n, 64 k}
+            tma_load_2d(sb + i * 8192, &tma_b, full_bar(stage), ti.n0 + 64 * i, b_row0 + k0);
+        }
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    // ===================================================================== MMA issuer
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc<BN, A_MN, B_MN>();
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      TileInfo ti;
-      for (int t = blockIdx.x; decode_tile<BN>(g, t, ti); t += gridDim.x) {
-        mbar_wait(tempty_bar(acc), acc_phase ^ 1);      // epilogue has drained this accumulator stage
-        tcgen05_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        for (int kb = ti.kb_begin; kb < ti.kb_end; ++kb) {
-          mbar_wait(full_bar(stage), phase);
-          tcgen05_fence_after();
-          const uint32_t sa = smem_base + stage * Cfg::STAGE_BYTES;
-          const uint64_t adesc = make_smem_desc<A_MN>(sa);
-          const uint64_t bdesc = make_smem_desc<B_MN>(sa + Cfg::A_BYTES);
-#pragma unroll
-          for (int k = 0; k < BK / UMMA_K; ++k) {
-            umma_bf16(d_tmem, adesc + (uint64_t)(k * desc_k_step<A_MN>()), bdesc + (uint64_t)(k * desc_k_step<B_MN>()),
-                      idesc, (kb > ti.kb_begin || k > 0) ? 1u : 0u);
-          }
-          tcgen05_commit(empty_bar(stage));             // smem slot is free once these MMAs retire
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        tcgen05_commit(tfull_bar(acc));                 // accumulator complete -> epilogue
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-    }
-  } else if (warp >= 4) {
-    // ===================================================================== epilogue (warps 4..7 <-> TMEM lanes 0..127)
-    const int q = warp & 3;                    // TMEM lane quarter this warp may touch
-    constexpr int GROUPS = EW / 4;              // warps per TMEM lane quarter
-    constexpr int CHUNKS_PER_GROUP = BN / GROUPS / CW;
-    const int cgroup = (warp - 4) >> 2;        // which slice of the tile columns this warp drains
-    const int r_in_tile = q * 32 + lane;
-    WarpStagedIO io;
-    io.buf = smem_raw + (bar_base - smem_u32(smem_raw)) + Cfg::BAR_BYTES + (warp - 4) * STAGE_WARP_BYTES;
-    io.lane = lane;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    TileInfo ti;
-    for (int t = blockIdx.x; decode_tile<BN>(g, t, ti); t += gridDim.x) {
-      mbar_wait(tfull_bar(acc), acc_phase);
-      tcgen05_fence_after();
-      const int m = ti.m0 + r_in_tile;
-      const long long row = (g.batch_reduce ? 0 : (long long)ti.z * g.d_batch_rows) + m;
-      const uint32_t taddr = tmem_base + acc * BN + ((uint32_t)(q * 32) << 16);
-      const bool has_k = ti.kb_end > ti.kb_begin;
-      const bool valid = m < g.M;
-      io.valid_mask = __ballot_sync(0xffffffffu, valid);
-      // EPI_ROTARY, dim_head 64: the 32 (sin, cos) pairs of this row's position serve every head of the tile; fetch them
-      // once per tile (two coalesced staged loads) instead of once per 32-column chunk
-      float rs[KIND == EPI_ROTARY ? 32 : 1], rc[KIND == EPI_ROTARY ? 32 : 1];
-      bool rot_cached = false;
-      if constexpr (KIND == EPI_ROTARY) {
-        if (g.epi.dim_head == 64) {
-          const long long pos = row % g.epi.seq_len;
-          io.template load<32>(g.epi.rot_sin + pos * 32, 32, rs, true);
-          io.template load<32>(g.epi.rot_cos + pos * 32, 32, rc, true);
-          rot_cached = true;
-        }
-      }
-#pragma unroll 1
-      for (int c = cgroup * CHUNKS_PER_GROUP; c < (cgroup + 1) * CHUNKS_PER_GROUP; ++c) {
-        const int col = ti.n0 + c * CW;
-        if (col >= g.N) break;                          // warp-uniform
-        float v[CW];
-        tmem_ld<CW>(taddr + c * CW, v);                 // .sync.aligned: executed by the whole warp
-        if (!has_k) {
-#pragma unroll
-          for (int i = 0; i < CW; ++i) v[i] = 0.f;
-        }
-        if constexpr (KIND == EPI_ROTARY && CW == 32) {
-          if (rot_cached) {
-            float o[32];
-            if ((col & 32) == 0) {                      // first / second half of the head: pairs 0..15 / 16..31
-#pragma unroll
-              for (int i = 0; i < 32; i += 2) {
-                o[i] = v[i] * rc[i >> 1] - v[i + 1] * rs[i >> 1];
-                o[i + 1] = v[i + 1] * rc[i >> 1] + v[i] * rs[i >> 1];
-              }
-            } else {
-#pragma unroll
-              for (int i = 0; i < 32; i += 2) {
-                o[i] = v[i] * rc[16 + (i >> 1)] - v[i + 1] * rs[16 + (i >> 1)];
-                o[i + 1] = v[i + 1] * rc[16 + (i >> 1)] + v[i] * rs[16 + (i >> 1)];
-              }
-            }
-            io.template store<32>(reinterpret_cast<TO*>(g.epi.out) + row * g.epi.ldo + col, g.epi.ldo, o, valid);
-            continue;
-          }
-        }
-        epi_apply<KIND, TO, CW>(g.epi, io, row, col, v, valid);
-      }
-      tcgen05_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty_bar(acc));
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-    }
+    return;
   }
 
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tcgen05_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(Cfg::TMEM_COLS) : "memory");
+  // ======================================================================= consumers: rows 64 c .. 64 c + 63 of the tile
+  const int c = wg - 1;
+  const int t = threadIdx.x - 128;              // 0..255 over both consumer warpgroups
+  float acc[64];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+  {
+    int stage = 0, prev = -1;
+    uint32_t phase = 0;
+    for (int kb = ti.kb_begin; kb < ti.kb_end; ++kb) {
+      mbar_wait(full_bar(stage), phase);
+      const uint32_t sa = smem_base + stage * STAGE_BYTES;
+      // both majors: this warpgroup's 64 rows of A start 8 KiB in (K-major: 64 rows x 128 B; MN-major: the second box)
+      const uint64_t adesc = make_smem_desc<A_MN>(sa + c * 8192);
+      const uint64_t bdesc = make_smem_desc<B_MN>(sa + A_BYTES);
+      constexpr uint32_t a_step = A_MN ? (2048 >> 4) : (32 >> 4), b_step = B_MN ? (2048 >> 4) : (32 >> 4);
+      fence_regs(acc);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < BK / WG_K; ++k)
+        wgmma_m64n128k16_bf16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, adesc + (uint64_t)(k * a_step), bdesc + (uint64_t)(k * b_step));
+      wgmma_commit();
+      fence_regs(acc);
+      wgmma_wait<1>();                          // the previous k-block's MMAs are done: its stage can be refilled
+      if (prev >= 0 && (t & 127) == 0) mbar_arrive(empty_bar(prev));
+      prev = stage;
+      if (++stage == STAGES) { stage = 0; phase ^= 1; }
+    }
+    wgmma_wait<0>();
+    fence_regs(acc);
+  }
+
+  // ---- stage the fp32 tile in shared memory (every MMA of both warpgroups has read its operands: the ring is free)
+  asm volatile("bar.sync 1, 256;" ::: "memory");
+  float* cs = reinterpret_cast<float*>(smem_raw + (smem_base - raw_u32));
+  {
+    const int w = (t & 127) >> 5, lane = t & 31;
+    const int r0 = 64 * c + 16 * w + (lane >> 2);
+    const int c0 = 2 * (lane & 3);
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      *reinterpret_cast<float2*>(cs + r0 * CS_LD + 8 * j + c0) = make_float2(acc[4 * j], acc[4 * j + 1]);
+      *reinterpret_cast<float2*>(cs + (r0 + 8) * CS_LD + 8 * j + c0) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+    }
+  }
+  asm volatile("bar.sync 1, 256;" ::: "memory");
+
+  // ---- epilogue: 8 consecutive columns of one row per thread, 16 threads per row
+#pragma unroll 1
+  for (int idx = t; idx < BM * (BN / 8); idx += 256) {
+    const int r = idx / (BN / 8), cc = (idx % (BN / 8)) * 8;
+    const int m = ti.m0 + r, col = ti.n0 + cc;
+    if (m >= g.M || col >= g.N) continue;
+    float v[8];
+    const float4 x0 = *reinterpret_cast<const float4*>(cs + r * CS_LD + cc);
+    const float4 x1 = *reinterpret_cast<const float4*>(cs + r * CS_LD + cc + 4);
+    v[0] = x0.x; v[1] = x0.y; v[2] = x0.z; v[3] = x0.w; v[4] = x1.x; v[5] = x1.y; v[6] = x1.z; v[7] = x1.w;
+    const long long row = (g.batch_reduce ? 0 : (long long)ti.z * g.d_batch_rows) + m;
+    epi_apply<KIND, TO, 8>(g.epi, DirectIO{}, row, col, v, true);
   }
 }
 
@@ -450,54 +258,39 @@ int get_tensor_map(const void* ptr, uint64_t inner, uint64_t outer, uint64_t row
   return PROGEN_OK;
 }
 
-template <int BN, bool A_MN, bool B_MN, int KIND, typename TO>
+
+template <bool A_MN, bool B_MN, int KIND, typename TO>
 int launch_inst(const CUtensorMap& ta, const CUtensorMap& tb, const GemmDev& gd, int tiles, cudaStream_t stream) {
-  using Cfg = TileCfg<BN, KIND>;
-  auto kern = gemm_tc_kernel<BN, A_MN, B_MN, KIND, TO>;
+  auto kern = gemm_tc_kernel<A_MN, B_MN, KIND, TO>;
   static bool attr_set = false;
   if (!attr_set) {
-    PG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_TOTAL));
+    PG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL));
     attr_set = true;
   }
-  const int grid = tiles < pg_num_sms() ? tiles : pg_num_sms();
-  kern<<<grid, EpiCfg<KIND>::THREADS, Cfg::SMEM_TOTAL, stream>>>(ta, tb, gd);
+  kern<<<tiles, THREADS, SMEM_TOTAL, stream>>>(ta, tb, gd);
   PG_LAUNCH_CHECK();
   return PROGEN_OK;
 }
 
-template <bool A_MN, bool B_MN, int KIND, typename TO>
-int launch_bn(int bn, const CUtensorMap& ta, const CUtensorMap& tb, const GemmDev& gd, int tiles, cudaStream_t s) {
-  if (bn == 256) return launch_inst<256, A_MN, B_MN, KIND, TO>(ta, tb, gd, tiles, s);
-  return launch_inst<128, A_MN, B_MN, KIND, TO>(ta, tb, gd, tiles, s);
-}
-
 }  // namespace
 
-// shared with the other tensor-core kernels (attn_tc.cu)
+// shared with the wgmma attention kernels (attn_wgmma.cu)
 int pg_tensor_map_2d_bf16(const void* ptr, uint64_t inner, uint64_t outer, uint64_t row_stride_elems, uint32_t box_inner,
                           uint32_t box_outer, CUtensorMap* out) {
   return get_tensor_map(ptr, inner, outer, row_stride_elems, box_inner, box_outer, out);
 }
-// epilogue boxes (gemm_tc2.cu): bf16 or fp32 elements, swizzle span = bytes of one box row
-int pg_tensor_map_2d(const void* ptr, uint32_t elem_bytes, uint64_t inner, uint64_t outer, uint64_t row_stride_elems,
-                     uint32_t box_inner, uint32_t box_outer, uint32_t swizzle_bytes, CUtensorMap* out) {
-  return get_tensor_map(ptr, inner, outer, row_stride_elems, box_inner, box_outer, out, elem_bytes, swizzle_bytes);
-}
 
 int gemm_tc_launch(const GemmArgs& a, cudaStream_t stream) {
   PG_CHECK_ARG(a.in_dtype == PG_BF16);
-  if (gemm_tc2_eligible(a)) return gemm_tc2_launch(a, stream);        // CTA-pair kernel: less L2 operand traffic per FLOP
   PG_CHECK_ARG(a.M > 0 && a.N > 0 && a.K > 0 && a.batch >= 1 && a.split_k >= 1);
   PG_CHECK_ARG(a.N % 32 == 0);
   PG_CHECK_ARG(a.K % BK == 0);                       // TMA would zero-fill a K tail, but batched operands must not bleed
   PG_CHECK_ARG(a.lda % 8 == 0 && a.ldb % 8 == 0);    // 16-byte global strides for TMA
   PG_CHECK_ARG((reinterpret_cast<uintptr_t>(a.A) & 15) == 0 && (reinterpret_cast<uintptr_t>(a.B) & 15) == 0);
   PG_CHECK_ARG(!(a.split_k > 1 && a.causal));
-  if (a.epi_kind == EPI_ROTARY) PG_CHECK_ARG(a.epi.seq_len % 32 == 0);   // staged sin/cos loads: a warp's rows stay in one sequence
+  if (a.epi_kind == EPI_ROTARY) PG_CHECK_ARG(a.epi.seq_len % 32 == 0);
   PG_CHECK_ARG(!(a.split_k > 1 || a.batch_reduce) || (a.epi_kind == EPI_ACCUM && a.epi.atomic));
-  if (a.batch > 1 && a.a_batch_rows > 0 && !a.a_mn_major) PG_CHECK_ARG(a.M % BM == 0 || a.batch_reduce || true);
 
-  const int bn = (a.N >= 256 && a.N % 256 == 0) ? 256 : 128;
   // stored 2D extents of each operand
   const uint64_t a_rows = (a.batch > 1 && a.a_batch_rows > 0) ? (uint64_t)a.a_batch_rows * a.batch
                                                               : (uint64_t)(a.a_mn_major ? a.K : a.M);
@@ -508,7 +301,7 @@ int gemm_tc_launch(const GemmArgs& a, cudaStream_t stream) {
   if (!a.a_mn_major) rc = get_tensor_map(a.A, a.K, a_rows, a.lda, BK, BM, &ta);
   else               rc = get_tensor_map(a.A, a.M, a_rows, a.lda, 64, BK, &ta);
   if (rc) return rc;
-  if (!a.b_mn_major) rc = get_tensor_map(a.B, a.K, b_rows, a.ldb, BK, bn, &tb);
+  if (!a.b_mn_major) rc = get_tensor_map(a.B, a.K, b_rows, a.ldb, BK, BN, &tb);
   else               rc = get_tensor_map(a.B, a.N, b_rows, a.ldb, 64, BK, &tb);
   if (rc) return rc;
 
@@ -518,11 +311,12 @@ int gemm_tc_launch(const GemmArgs& a, cudaStream_t stream) {
   gd.a_batch_rows = (int)a.a_batch_rows; gd.b_batch_rows = (int)a.b_batch_rows; gd.d_batch_rows = a.d_batch_rows;
   gd.causal = a.causal; gd.split_k = a.split_k;
   gd.epi = a.epi;
-  const int tiles = a.batch * a.split_k * ((a.M + BM - 1) / BM) * ((a.N + bn - 1) / bn);
+  const long long tiles = (long long)a.batch * a.split_k * ((a.M + BM - 1) / BM) * ((a.N + BN - 1) / BN);
+  PG_CHECK_ARG(tiles < (1ll << 31));
 
   const int am = a.a_mn_major ? 1 : 0, bm = a.b_mn_major ? 1 : 0;
   const bool obf = a.out_dtype == PG_BF16;
-#define TC_CASE(AM, BMJ, KIND, TO) return launch_bn<AM, BMJ, KIND, TO>(bn, ta, tb, gd, tiles, stream)
+#define TC_CASE(AM, BMJ, KIND, TO) return launch_inst<AM, BMJ, KIND, TO>(ta, tb, gd, (int)tiles, stream)
   switch (a.epi_kind) {
     case EPI_STORE:
       if (!am && bm) { if (obf) TC_CASE(false, true, EPI_STORE, bf16); else TC_CASE(false, true, EPI_STORE, float); }

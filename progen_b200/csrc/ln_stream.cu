@@ -1,14 +1,13 @@
 // LayerNorm(scale-only)+token-shift BACKWARD as a bulk-copy (TMA 1D) streaming kernel.
 //
 // The row-per-warp kernel in elementwise.cu keeps every in-flight byte in registers: at 128 registers/thread only
-// 16 warps/SM are resident and ncu shows 77 % long-scoreboard stalls with DRAM at 37 % of peak.  Here the in-flight
+// 16 warps/SM are resident and the loads stall on memory latency.  Here the in-flight
 // bytes live in shared memory instead: one producer warp streams 8-row chunks (x, dy [+1 row for the un-shift], the
 // residual gradient, mean/rstd) into a ring of up to 5 stages with cp.async.bulk + mbarrier complete_tx (one request per
-// ARRAY when rows are contiguous: the TMA unit costs ~100 cycles per request); two groups of eight consumer warps (one
+// ARRAY when rows are contiguous: every bulk request has a fixed cost in the copy unit); two groups of eight consumer warps (one
 // row each, alternating chunks) compute dx from shared memory, update the residual gradient IN PLACE in the stage and
 // write the low-precision copy straight to global memory; the producer warp then bulk-stores the residual gradient back
-// and recycles the stage.  ~160 KB of loads are in flight per SM, independent of register pressure.
-// [65536 x 512]: 172 us (row-per-warp) -> 104 us = 5.1 TB/s of algorithmic bytes.
+// and recycles the stage.  The bytes in flight per SM no longer depend on register pressure.
 //
 // Same math as ln_shift_bwd_kernel (reference progen.py:22,74-77 backward):
 //   dyn(t,c) = c < d/2 ? dy(t+1,c) [0 at the last position of a sequence] : dy(t,c);   g = dyn*scale

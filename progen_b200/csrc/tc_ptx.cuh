@@ -1,4 +1,4 @@
-// tcgen05 / TMA / mbarrier PTX wrappers shared by the tensor-core kernels (sm_100a).
+// mbarrier / TMA / wgmma PTX wrappers shared by the tensor-core GEMM and the bulk-copy kernels (sm_90a).
 #pragma once
 #include <cuda.h>
 #include "common.cuh"
@@ -39,279 +39,78 @@ __device__ __forceinline__ void prefetch_tensormap(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
 
-template <int COLS> __device__ __forceinline__ void tmem_alloc(uint32_t slot_smem_addr) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(slot_smem_addr), "n"(COLS) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int COLS> __device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(COLS) : "memory");
-}
-__device__ __forceinline__ void tcgen05_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tcgen05_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tcgen05_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem desc] * B[smem desc], bf16 operands, fp32 accumulate
-__device__ __forceinline__ void umma_bf16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum) : "memory");
-}
-
-// 32 lanes x 32 consecutive fp32 columns of this warp's TMEM lane quarter
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-  uint32_t r[32];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-// Split form of tmem_ld32: issue now, wait later (the registers must not be read in between; the wait names them as
-// read-write operands so the compiler cannot move a use above it).  Lets an epilogue prefetch its next chunk.
-__device__ __forceinline__ void tmem_ld32_issue(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld32_wait(uint32_t (&r)[32]) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]), "+r"(r[8]), "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15]), "+r"(r[16]), "+r"(r[17]), "+r"(r[18]), "+r"(r[19]), "+r"(r[20]), "+r"(r[21]), "+r"(r[22]), "+r"(r[23]), "+r"(r[24]), "+r"(r[25]), "+r"(r[26]), "+r"(r[27]), "+r"(r[28]), "+r"(r[29]), "+r"(r[30]), "+r"(r[31]) :: "memory");
-}
-
-// 32 lanes x 64 consecutive fp32 columns in ONE tcgen05.ld (half as many issue + wait round trips as two x32 loads)
-__device__ __forceinline__ void tmem_ld64(uint32_t taddr, float (&v)[64]) {
-  uint32_t r[64];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x64.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, [%64];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31]), "=r"(r[32]), "=r"(r[33]), "=r"(r[34]), "=r"(r[35]), "=r"(r[36]), "=r"(r[37]), "=r"(r[38]), "=r"(r[39]), "=r"(r[40]), "=r"(r[41]), "=r"(r[42]), "=r"(r[43]), "=r"(r[44]), "=r"(r[45]), "=r"(r[46]), "=r"(r[47]), "=r"(r[48]), "=r"(r[49]), "=r"(r[50]), "=r"(r[51]), "=r"(r[52]), "=r"(r[53]), "=r"(r[54]), "=r"(r[55]), "=r"(r[56]), "=r"(r[57]), "=r"(r[58]), "=r"(r[59]), "=r"(r[60]), "=r"(r[61]), "=r"(r[62]), "=r"(r[63])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 64; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-// two 32-column loads (different TMEM addresses) issued back to back, ONE wait
-__device__ __forceinline__ void tmem_ld32x2(uint32_t taddr_a, uint32_t taddr_b, float (&a)[32], float (&b)[32]) {
-  uint32_t ra[32], rb[32];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%64];\n\t"
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, [%65];\n\t"
-      "tcgen05.wait::ld.sync.aligned;"
-      : "=r"(ra[0]), "=r"(ra[1]), "=r"(ra[2]), "=r"(ra[3]), "=r"(ra[4]), "=r"(ra[5]), "=r"(ra[6]), "=r"(ra[7]), "=r"(ra[8]), "=r"(ra[9]), "=r"(ra[10]), "=r"(ra[11]), "=r"(ra[12]), "=r"(ra[13]), "=r"(ra[14]), "=r"(ra[15]), "=r"(ra[16]), "=r"(ra[17]), "=r"(ra[18]), "=r"(ra[19]), "=r"(ra[20]), "=r"(ra[21]), "=r"(ra[22]), "=r"(ra[23]), "=r"(ra[24]), "=r"(ra[25]), "=r"(ra[26]), "=r"(ra[27]), "=r"(ra[28]), "=r"(ra[29]), "=r"(ra[30]), "=r"(ra[31]), "=r"(rb[0]), "=r"(rb[1]), "=r"(rb[2]), "=r"(rb[3]), "=r"(rb[4]), "=r"(rb[5]), "=r"(rb[6]), "=r"(rb[7]), "=r"(rb[8]), "=r"(rb[9]), "=r"(rb[10]), "=r"(rb[11]), "=r"(rb[12]), "=r"(rb[13]), "=r"(rb[14]), "=r"(rb[15]), "=r"(rb[16]), "=r"(rb[17]), "=r"(rb[18]), "=r"(rb[19]), "=r"(rb[20]), "=r"(rb[21]), "=r"(rb[22]), "=r"(rb[23]), "=r"(rb[24]), "=r"(rb[25]), "=r"(rb[26]), "=r"(rb[27]), "=r"(rb[28]), "=r"(rb[29]), "=r"(rb[30]), "=r"(rb[31])
-      : "r"(taddr_a), "r"(taddr_b) : "memory");
-#pragma unroll
-  for (int i = 0; i < 32; ++i) { a[i] = __uint_as_float(ra[i]); b[i] = __uint_as_float(rb[i]); }
-}
-
-// Shared-memory matrix descriptor, 128B swizzle (cute/arch/mma_sm100_desc.hpp): start>>4 [0,14), LBO>>4 [16,30),
-// SBO>>4 [32,46), version 1 [46,48), layout SWIZZLE_128B = 2 [61,64).
-//   K-major : rows of 64 bf16 (128 B), 8-row groups 1024 B apart (SBO); one UMMA_K step = +32 B
-//   MN-major: [k rows x 128 B] chunks of 64 MN elements, `lbo_bytes` apart; 8-k-row groups 1024 B apart; UMMA_K step = +2048 B
+// Shared-memory matrix descriptor of wgmma, 128B swizzle (PTX ISA "Matrix Descriptor Format"): start>>4 [0,14),
+// LBO>>4 [16,30), SBO>>4 [32,46), layout SWIZZLE_128B = 1 [62,64).
+//   K-major : rows of 64 bf16 (128 B), 8-row groups 1024 B apart (SBO); LBO unused; one K step of 16 = +32 B
+//   MN-major: [k rows x 128 B] chunks of 64 MN elements, `lbo_bytes` apart; 8-k-row groups 1024 B apart; K step = +2048 B
 template <bool MN_MAJOR>
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, uint32_t lbo_bytes = 8192) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
   d |= (uint64_t)(MN_MAJOR ? (lbo_bytes >> 4) : 1) << 16;
   d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
 }
-// instruction descriptor: fp32 accumulate, bf16 x bf16, M x N, operand majors
-__device__ __forceinline__ constexpr uint32_t make_idesc(int M, int N, bool a_mn, bool b_mn) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((a_mn ? 1u : 0u) << 15) | ((b_mn ? 1u : 0u) << 16) |
-         ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs
+template <int R> __device__ __forceinline__ void fence_regs(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// TMA store of one box (shared -> global, rows/columns outside the tensor are clipped); bulk-group completion
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t src, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
-               ::"l"(map), "r"(src), "r"(c0), "r"(c1) : "memory");
-}
-// TMA reduction: global[box] += shared[box] (element type and the fp32 add come from the tensor map; done in the L2)
-__device__ __forceinline__ void tma_reduce_add_2d(const CUtensorMap* map, uint32_t src, int c0, int c1) {
-  asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3}], [%1];"
-               ::"l"(map), "r"(src), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-// wait until at most N of this thread's bulk groups still have to READ their shared-memory source
-template <int N> __device__ __forceinline__ void bulk_wait_group_read() {
-  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
-}
-template <int N> __device__ __forceinline__ void bulk_wait_group() {
-  asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
-}
-
-// ------------------------------------------------------------------------------------------------ round-2 additions
-// D[tmem] (+)= A[tmem] * B[smem desc]: the A operand (M = 128 lanes x K, bf16 pairs packed along K in 32-bit columns:
-// element (m, k) = lane m, column k/2, half k&1) is read from tensor memory — what a thread wrote with tcgen05.st for its
-// own row.  cute: SM100_MMA_F16BF16_TS (mma_sm100_umma.hpp); A from TMEM is always K-major.
-__device__ __forceinline__ void umma_bf16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
+// D[64 x 128] += A[64 x 16] * B[16 x 128] for one warpgroup, bf16 operands from shared memory, fp32 accumulators in
+// registers.  Thread t of the warpgroup holds rows 16 (t / 32) + (t % 32) / 4 (+ 8) and column pairs 8 j + 2 (t % 4):
+// d[4 j + 0, 1] = (row, col + 0, 1), d[4 j + 2, 3] = (row + 8, col + 0, 1).  TA / TB: operand stored MN-major.
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n128k16_bf16(float (&d)[64], uint64_t adesc, uint64_t bdesc) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(accum) : "memory");
+      "{\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+      "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, "
+      "%47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, 1, 1, 1, %66, %67;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+        "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+        "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),
+        "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+        "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),
+        "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),
+        "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "n"(TA), "n"(TB));
 }
-// shared memory -> tensor memory, 128 lanes x 256 bits (8 columns): the SAME matrix a K-major SS MMA reads as its 128 x 16
-// bf16 A operand of one K step (same descriptor, same +2 per K step), landing where a TS MMA expects its A operand.
-// Asynchronous, ordered with the tcgen05.mma / tcgen05.commit of the issuing thread.  cute: SM100_UTCCP_128dp256bit_1cta.
-__device__ __forceinline__ void tmem_cp_128x256b(uint32_t taddr, uint64_t sdesc) {
-  asm volatile("tcgen05.cp.cta_group::1.128x256b [%0], %1;" ::"r"(taddr), "l"(sdesc) : "memory");
-}
-// registers -> tensor memory: thread (lane L of the warp's lane quarter) writes N consecutive 32-bit columns of its lane
-template <int N> __device__ __forceinline__ void tmem_st(uint32_t taddr, const uint32_t (&r)[N]);
-template <> __device__ __forceinline__ void tmem_st<8>(uint32_t taddr, const uint32_t (&r)[8]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};"
-               ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]) : "memory");
-}
-template <> __device__ __forceinline__ void tmem_st<16>(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-               ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]) : "memory");
-}
-template <> __device__ __forceinline__ void tmem_st<32>(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-               ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31]) : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
-// packed fp32x2 arithmetic (sm_100: FFMA2 / FADD2 / FMUL2 — one issue slot for two results)
-__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
-  float2 d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(reinterpret_cast<uint64_t&>(d))
-      : "l"(reinterpret_cast<uint64_t&>(a)), "l"(reinterpret_cast<uint64_t&>(b)), "l"(reinterpret_cast<uint64_t&>(c)));
-  return d;
+// D[64 x 64] += A[64 x 16] * B[16 x 64], same register layout as above (d[4 j + e], j < 8); A from shared memory
+template <int TB>
+__device__ __forceinline__ void wgmma_m64n64k16_ss(float (&d)[32], uint64_t adesc, uint64_t bdesc) {
+  asm volatile(
+      "{\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "%32, %33, 1, 1, 1, 0, %34;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(adesc), "l"(bdesc), "n"(TB));
 }
-__device__ __forceinline__ float2 fadd2(float2 a, float2 b) {
-  float2 d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(reinterpret_cast<uint64_t&>(d))
-      : "l"(reinterpret_cast<uint64_t&>(a)), "l"(reinterpret_cast<uint64_t&>(b)));
-  return d;
+// same with A from registers: a[0..3] of warp w hold rows 16 w + (lane / 4) (+ 8) and k columns 2 (lane % 4) (+ 8), i.e.
+// the accumulator pairs d[8 kk .. 8 kk + 7] of a previous m64n64 result packed to bf16 give the A operand of k-step kk
+template <int TB>
+__device__ __forceinline__ void wgmma_m64n64k16_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t bdesc) {
+  asm volatile(
+      "{\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "{%32, %33, %34, %35}, %36, 1, 1, 1, %37;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "n"(TB));
 }
-__device__ __forceinline__ float2 fmul2(float2 a, float2 b) {
-  float2 d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(reinterpret_cast<uint64_t&>(d))
-      : "l"(reinterpret_cast<uint64_t&>(a)), "l"(reinterpret_cast<uint64_t&>(b)));
-  return d;
-}
-__device__ __forceinline__ float fmax3(float a, float b, float c) {
-  float d;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));
-  return d;
-}
-__device__ __forceinline__ float ex2f(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-// 2^x on the FMA / ALU pipes (no MUFU): floor by a round-down add of 1.5 * 2^23, cubic minimax of 2^f on [0, 1), the
-// integer part added straight into the exponent field.  |rel err| < 1.1e-4 (the result is rounded to bf16 anyway);
-// x must be <= 127; x < -126 is clamped (result 2^-126 ~ 0).
-__device__ __forceinline__ float ex2_poly(float x) {
-  x = fmaxf(x, -126.f);
-  float r;
-  asm("add.rm.ftz.f32 %0, %1, %2;" : "=f"(r) : "f"(x), "f"(12582912.f));
-  const float f = x - (r - 12582912.f);
-  float p = fmaf(0.07711908966302872f, f, 0.22756439447402954f);
-  p = fmaf(p, f, 0.6951461434364319f);
-  p = fmaf(p, f, 1.0f);
-  return __uint_as_float(__float_as_uint(p) + (__float_as_uint(r) << 23));
-}
-// One lane of a CONVERGED warp (the lowest active one: lane 0 when all 32 are there).  The MMA / TMA roles run their loops
-// with the whole warp and predicate only the tcgen05 / bulk-copy instructions on this: descriptors and addresses are then
-// warp-uniform values and ptxas keeps them in uniform registers.  Inside `if (lane == 0) { loop }` every operand is
-// treated as per-thread and each UTCHMMA is wrapped in an ELECT / R2UR.BROADCAST / BRA.U.ANY waterfall — measured 117
-// cycles per MMA instruction regardless of its shape (scripts/ubench/attn_ubench.cu), against 35-115 when uniform.
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred = 0;
-  asm volatile("{\n\t.reg .pred P1;\n\telect.sync _|P1, 0xffffffff;\n\tselp.u32 %0, 1, 0, P1;\n\t}" : "=r"(pred));
-  return pred != 0;
-}
-template <int REGS> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(REGS)); }
-template <int REGS> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(REGS)); }
 
 }  // namespace tc
 
-// host: cached 2-D bf16 tensor map with 128B swizzle (defined in gemm_tc.cu)
+// host: cached 2-D bf16 tensor map with 128B swizzle, zero fill out of bounds (defined in gemm_tc.cu)
 int pg_tensor_map_2d_bf16(const void* ptr, uint64_t inner, uint64_t outer, uint64_t row_stride_elems, uint32_t box_inner,
                           uint32_t box_outer, CUtensorMap* out);
-// host: same cache, bf16 (2) or fp32 (4) elements, swizzle span 32 / 64 / 128 bytes
-int pg_tensor_map_2d(const void* ptr, uint32_t elem_bytes, uint64_t inner, uint64_t outer, uint64_t row_stride_elems,
-                     uint32_t box_inner, uint32_t box_outer, uint32_t swizzle_bytes, CUtensorMap* out);
-
-// ------------------------------------------------------------------------------------------------ CTA-pair (cta_group::2)
-namespace tc2 {
-
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// shared::cluster address of the same smem offset in CTA `rank` of the cluster
-__device__ __forceinline__ uint32_t mapa(uint32_t smem_addr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_addr), "r"(rank));
-  return r;
-}
-// Relaxed: the arrival only says "my tcgen05.ld reads of this accumulator stage are complete" (ordered by the preceding
-// tcgen05.fence::before_thread_sync); no global/shared writes are published through it.  The .release form compiles
-// to MEMBAR.ALL.GPU + ERRBAR, i.e. every epilogue warp drains its outstanding global stores once per tile (13 % of the
-// stall samples of the FF proj_in kernel before this change).
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.relaxed.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// TMA load issued by either CTA of the pair; the bytes are accounted on the barrier at `bar_cluster_addr` (the leader's)
-__device__ __forceinline__ void tma_load_2d_pair(uint32_t dst, const CUtensorMap* map, uint32_t bar_cluster_addr, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(dst), "l"(map), "r"(bar_cluster_addr), "r"(c0), "r"(c1) : "memory");
-}
-// Multicast form: the box lands at the same shared-memory offset of every CTA in `cta_mask`, and (cta_group::2) its bytes
-// are accounted on the barrier at `bar_own_addr`'s offset in the LEADER (even) CTA of each destination's pair — the
-// operand is the issuing CTA's own barrier address with the peer bit cleared, as cute's SM100_TMA_2SM_LOAD_MULTICAST does.
-__device__ __forceinline__ void tma_load_2d_pair_mc(uint32_t dst, const CUtensorMap* map, uint32_t bar_own_addr, uint16_t cta_mask,
-                                                    int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
-      " [%0], [%1, {%4, %5}], [%2], %3;"
-      ::"r"(dst), "l"(map), "r"(bar_own_addr & 0xFEFFFFFFu), "h"(cta_mask), "r"(c0), "r"(c1) : "memory");
-}
-template <int COLS> __device__ __forceinline__ void tmem_alloc_pair(uint32_t slot_smem_addr) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(slot_smem_addr), "n"(COLS) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-template <int COLS> __device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(COLS) : "memory");
-}
-// commit all prior MMAs of the pair to the barrier at this smem offset in BOTH CTAs
-__device__ __forceinline__ void tcgen05_commit_pair(uint32_t bar, uint16_t cta_mask = 3) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(bar), "h"(cta_mask) : "memory");
-}
-// D[tmem, 256 rows over the CTA pair] (+)= A * B, issued by the leader CTA only
-__device__ __forceinline__ void umma_bf16_pair(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum) : "memory");
-}
-
-}  // namespace tc2

@@ -97,11 +97,8 @@ class Engine:
         # tensor-core attention kernels: bf16, dim_head 64, 64-aligned windows (checked below — no silent CUDA-core fallback);
         # the fp32 engine (mixed_precision=False) runs the exact CUDA-core kernels
         self.attn_tc = self.mp
-        import os
-        self.attn_fwd_kind = os.environ.get('PROGEN_ATTN_FWD', 'tcgen05')
-        self.attn_bwd_kind = os.environ.get('PROGEN_ATTN_BWD', 'tcgen05')
-        if cfg['window_size'] % 128 != 0:
-            self.attn_fwd_kind = self.attn_bwd_kind = 'mma'
+        # wgmma kernels (attn_wgmma.cu) for windows that are multiples of 128, the mma.sync kernels (attn_mma.cu) otherwise
+        self.attn_wgmma = self.mp and cfg['window_size'] % 128 == 0
         d, n, w = cfg['dim'], cfg['seq_len'], cfg['window_size']
         self.d, self.n, self.w, self.V = d, n, w, cfg['num_tokens']
         self.h, self.dh = cfg['heads'], cfg['dim_head']
@@ -124,7 +121,7 @@ class Engine:
         if self.mp:
             bad = [k for k, v in dict(dim=d, inner=self.I, seq_len=n, num_tokens=self.V).items() if v % 64]
             if bad:
-                raise L.ProgenError(f'mixed_precision (tcgen05 path) needs {bad} to be multiples of 64')
+                raise L.ProgenError(f'mixed_precision (tensor-core path) needs {bad} to be multiples of 64')
         self.specs, self.n_params_padded, self.n_decay = build_param_specs(cfg)
         self.by_key = {(s.module, s.name): s for s in self.specs}
         self.num_params = sum(s.size for s in self.specs)
@@ -146,6 +143,7 @@ class Engine:
         self.loaded_token = None
         self.on_layer_grads = None        # optional callback(layer_index) fired when a layer's weight gradients are final
         self.lib = L.load()
+        self.num_sms = torch.cuda.get_device_properties(self.dev).multi_processor_count
 
     def layer_grad_range(self, i):
         """[start, stop) of layer i's ndim>1 parameters inside the flat buffers (contiguous by construction)."""
@@ -275,13 +273,16 @@ class Engine:
 
     def wgrad_gemm(self, x, K_in, dy, N_out, dw):
         """dw[K_in,N_out] += x[T,K_in]^T @ dy[T,N_out]  (both operands MN-major, the token dimension is K)"""
-        split = 1
-        if self.backend == L.BACKEND_TC:
-            bn = 256 if (N_out % 256 == 0) else 128
-            tiles = ((K_in + 127) // 128) * ((N_out + bn - 1) // bn)
-            split = max(1, min(self.T // 64, 148 // tiles))
+        split = self.wgrad_split(K_in, N_out) if self.backend == L.BACKEND_TC else 1
         self._mm(M=K_in, N=N_out, K=self.T, A=x, lda=K_in, a_mn=True, B=dy, ldb=N_out, b_mn=True, out=dw, ldo=N_out,
                  epi=L.EPI_ACCUM, out_dtype=L.F32, split_k=split, atomic=split > 1)
+
+    def wgrad_split(self, K_in, N_out):
+        """K split of a weight-gradient GEMM (one CTA per 128 x 128 output tile and K slice): the split in 1..8 whose CTAs
+        fill the largest fraction of their waves over the SMs, the smallest such split on ties"""
+        tiles = ((K_in + 127) // 128) * ((N_out + 127) // 128)
+        fill = lambda s: tiles * s / (-(-tiles * s // self.num_sms) * self.num_sms)
+        return max(range(1, min(8, max(1, self.T // 64)) + 1), key=lambda s: (round(fill(s), 6), -s))
 
     def colsum(self, t, N, out, ld=None):
         L.check(self.lib.progen_colsum(t.data_ptr(), N if ld is None else ld, L.dt(t), out.data_ptr(), self.T, N, L.stream()), 'colsum')
@@ -348,14 +349,8 @@ class Engine:
 
     def attn_fwd(self, qkv, out, lse):
         if self.attn_tc:
-            # two tensor-core forwards: `tcgen05` (default: TMA + tcgen05.mma + TMEM, attn_fwd_ts.cu / attn_tc_pair.cu /
-            # attn_tc.cu by window size; needs window % 128 == 0) and `mma` (mma.sync flash kernel, any window % 64 == 0).
-            # PROGEN_ATTN_FWD selects.
-            if self.attn_fwd_kind == 'tcgen05':
-                L.check(self.lib.progen_local_attn_fwd_tc(qkv.data_ptr(), out.data_ptr(), lse.data_ptr(), self.B, self.n, self.w,
-                                                          self.h, self.dh, L.stream()), 'local_attn_fwd_tc')
-                return
-            L.check(self.lib.progen_local_attn_fwd(qkv.data_ptr(), out.data_ptr(), lse.data_ptr(), self.B, self.n, self.w, self.h,
+            fn = self.lib.progen_local_attn_fwd_tc if self.attn_wgmma else self.lib.progen_local_attn_fwd
+            L.check(fn(qkv.data_ptr(), out.data_ptr(), lse.data_ptr(), self.B, self.n, self.w, self.h,
                                                    self.dh, L.stream()), 'local_attn_fwd')
             return
         L.check(self.lib.progen_local_attn_fwd_simt(qkv.data_ptr(), out.data_ptr(), lse.data_ptr(), self.act_dt, self.B, self.n,
@@ -363,7 +358,7 @@ class Engine:
 
     def attn_bwd(self, qkv, out, dout, lse, dqkv):
         if self.attn_tc:
-            fn = self.lib.progen_local_attn_bwd_tc if self.attn_bwd_kind == 'tcgen05' else self.lib.progen_local_attn_bwd
+            fn = self.lib.progen_local_attn_bwd_tc if self.attn_wgmma else self.lib.progen_local_attn_bwd
             L.check(fn(qkv.data_ptr(), out.data_ptr(), dout.data_ptr(), lse.data_ptr(), dqkv.data_ptr(),
                                                    self.delta.data_ptr(), self.rot_sin.data_ptr(), self.rot_cos.data_ptr(), self.B,
                                                    self.n, self.w, self.h, self.dh, L.stream()), 'local_attn_bwd')

@@ -1,7 +1,7 @@
 """ctypes binding of libprogen_b200.so (the C ABI in include/progen_b200.h).
 
 PyTorch is used for device memory and streams only; every kernel on the hot path lives in the shared library.
-There is no fallback: if the library is missing, or the device is not sm_100, calls raise.
+There is no fallback: if the library is missing, or the device is not sm_90 (H100), calls raise.
 """
 import ctypes as C
 import os
@@ -56,8 +56,8 @@ PROTOTYPES = {
     'progen_local_attn_fwd_simt': [_P, _P, _P, _I, _I, _I, _I, _I, _I, _P],
     'progen_local_attn_bwd_simt': [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P],
     'progen_local_attn_fwd': [_P, _P, _P, _I, _I, _I, _I, _I, _P],
-    'progen_local_attn_fwd_tc': [_P, _P, _P, _I, _I, _I, _I, _I, _P],
     'progen_local_attn_bwd': [_P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P],
+    'progen_local_attn_fwd_tc': [_P, _P, _P, _I, _I, _I, _I, _I, _P],
     'progen_local_attn_bwd_tc': [_P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P],
     'progen_sgu_gate_fwd': [_P, _LL, _P, _LL, _P, _P, _LL, _I, _LL, _I, _I, _P],
     'progen_sgu_gate_bwd': [_P, _LL, _P, _LL, _P, _LL, _P, _P, _LL, _P, _LL, _P, _I, _LL, _I, _I, _P],
@@ -102,7 +102,7 @@ def check(rc, what=''):
 
 def require_device():
     if not torch.cuda.is_available():
-        raise ProgenError('no CUDA device: progen_b200 has no CPU fallback (sm_100a only)')
+        raise ProgenError('no CUDA device: progen_b200 has no CPU fallback (sm_90a only)')
     check(load().progen_device_check(), 'progen_device_check')
 
 

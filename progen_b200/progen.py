@@ -3,7 +3,7 @@
 Same constructor keywords (including the accepted-and-ignored `attn_dim`, `clamp_gate`), and an object with
 `.init(rng, seq) -> params` and `.apply(params, rng, seq) -> logits`, where `params` is the haiku-shaped nested dict
 `{module_path: {name: array}}` of the reference (SURVEY §8(b)), so reference checkpoints and oracle parameters
-interchange.  Everything below `.apply` runs as sm_100a kernels behind the C ABI (include/progen_b200.h).
+interchange.  Everything below `.apply` runs as sm_90a kernels behind the C ABI (include/progen_b200.h).
 
 Beyond the reference surface: `.apply` also accepts a batch (B, n); `.loss_and_grad(params, data)` is the fused
 equivalent of `value_and_grad(get_loss_fn(model))` (utils.py:61-93); `.trainer(...)` owns device-resident training

@@ -32,9 +32,8 @@ class Trainer:
         self._auto_graph, self._eager_key, self._eager_run = bool(cuda_graph), None, 0
         self._bucket, self._bucket_layers = None, max(1, int(os.environ.get('PROGEN_DDP_BUCKET_LAYERS', '3')))
         # Gradient exchange (world > 1).  Default: ONE SUM all-reduce of the whole flat buffer after the backward pass, on
-        # the compute stream, inside the captured CUDA graph.  Round 1 overlapped per-layer buckets with the backward pass:
-        # the NCCL kernels then hold SMs that the persistent one-CTA-per-SM kernels count on, and every such kernel ends
-        # late by the wait (2.2 ms per step at 8 GPUs for 0.5 ms of transfer).  PROGEN_DDP_OVERLAP=1 restores that mode
+        # the compute stream, inside the captured CUDA graph.  Overlapping per-layer buckets with the backward pass lets the
+        # NCCL kernels take SMs from the backward kernels and needs eager launches.  PROGEN_DDP_OVERLAP=1 selects that mode
         # (eager launches only) for models whose gradient is large enough to make the transfer itself matter.
         self.overlap = os.environ.get('PROGEN_DDP_OVERLAP', '0') == '1'
         self.skip_allreduce = False                       # bench.py: "step without the exchange" for comm_exposed_ms

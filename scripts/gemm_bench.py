@@ -1,4 +1,5 @@
-"""Micro-benchmark of the tcgen05 GEMM on the shapes of BASELINE config 2 (d=512, T=65536).  CUDA-event timed."""
+"""Micro-benchmark of the wgmma GEMM (gemm_tc.cu) against cuBLAS (torch.matmul) on the shapes of BASELINE config 2
+(d=512, T=65536).  CUDA-event timed; one JSON line per shape."""
 import json, sys, os, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from progen_b200 import lib as L

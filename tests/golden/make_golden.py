@@ -1,8 +1,7 @@
-"""Generate tests/golden/*.npz by EXECUTING THE REFERENCE'S OWN SOURCE (/root/reference/progen_transformer/
-{progen,utils}.py, unmodified) under the numpy stand-ins in oracle/ref_shim/ (jax/haiku are not installable).
-
-Run in the dev container only (the GPU box has no /root/reference):
-    python tests/golden/make_golden.py
+"""Generate tests/golden/*.npz by EXECUTING THE REFERENCE'S OWN SOURCE (a checkout of lucidrains/progen:
+progen_transformer/{progen,utils}.py, unmodified) under the numpy stand-ins in oracle/ref_shim/ (jax/haiku need not be
+installed).  The tests only read the stored .npz files; regenerating them needs the reference checkout:
+    python tests/golden/make_golden.py /path/to/progen
 
 For each case the parameters come from the oracle's seeded initialiser (`init_params` + `randomize_params`,
 numpy default_rng => reproducible), are fed to the reference `model.apply`, and the reference's logits, loss
@@ -53,7 +52,7 @@ def main():
 
     # ---- reference source under the shim
     sys.path.insert(0, os.path.join(ROOT, 'oracle', 'ref_shim'))
-    sys.path.insert(0, '/root/reference')
+    sys.path.insert(0, os.path.abspath(sys.argv[1]))
     import haiku as hk
     from progen_transformer.progen import ProGen
     from progen_transformer import utils as RU

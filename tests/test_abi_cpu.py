@@ -33,7 +33,7 @@ def test_library_exports_every_declared_symbol(lib):
 
 
 def test_version_and_error_text(lib):
-    assert 'sm_100a' in lib.version()
+    assert 'sm_90a' in lib.version()
     assert lib.load().progen_last_error() is not None
 
 

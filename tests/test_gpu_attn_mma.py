@@ -64,8 +64,8 @@ def test_local_attn_mma_fwd_bwd(cfg):
 
 @pytest.mark.parametrize('cfg', [(2, 256, 128, 2), (1, 512, 256, 3), (1, 1024, 256, 8), (3, 128, 128, 1), (2, 1024, 512, 2),
                                  (5, 512, 256, 8)])
-def test_local_attn_tcgen05_fwd(cfg):
-    """tcgen05 / TMEM forward kernel (attn_tc.cu) vs the float64 reference and the mma.sync kernel's log-sum-exp."""
+def test_local_attn_wgmma_fwd(cfg):
+    """wgmma / TMA forward kernel (attn_wgmma.cu) vs the float64 reference and the mma.sync kernel's output and log-sum-exp."""
     from progen_b200 import lib as L
     L.require_device()
     B, n, w, h = cfg
@@ -92,8 +92,8 @@ def test_local_attn_tcgen05_fwd(cfg):
 @pytest.mark.parametrize('cfg', [(2, 256, 128, 2), (1, 512, 256, 3), (1, 1024, 256, 8), (3, 128, 128, 1), (2, 1024, 512, 2),
                                  (5, 512, 256, 8)])
 @pytest.mark.parametrize('fused_rotary', [False, True])
-def test_local_attn_tcgen05_bwd(cfg, fused_rotary):
-    """tcgen05 backward kernels (attn_tc_bwd.cu) vs torch float64 autograd of the reference attention on the same bf16 q|k|v."""
+def test_local_attn_wgmma_bwd(cfg, fused_rotary):
+    """wgmma backward kernels (attn_wgmma.cu, dQ + dK/dV) vs torch float64 autograd of the reference attention on the same bf16 q|k|v."""
     from progen_b200 import lib as L
     from gemm_cases import rotary_tables
     L.require_device()

@@ -1,4 +1,4 @@
-"""tcgen05 / TMA GEMM (gemm_tc.cu): every operand-major combination and epilogue the engine uses, against a torch
+"""wgmma / TMA GEMM (gemm_tc.cu): every operand-major combination and epilogue the engine uses, against a torch
 float64 reference computed from the same bf16 operands (so the only differences are fp32 accumulation order and the
 final rounding of bf16 outputs)."""
 import pytest
@@ -33,7 +33,7 @@ def test_tc_gemm(a_mn, b_mn, epi, shape):
 
 
 def test_tc_gemm_many_tiles_and_long_k():
-    """More tiles than SMs (persistent loop, both TMEM stages, every smem stage phase) and a long K loop."""
+    """More tiles than SMs and a long K loop (the shared-memory ring wraps many times)."""
     from progen_b200 import lib as L
     from gemm_cases import run_case
     err, scale = run_case(L.BACKEND_TC, torch.bfloat16, 4096, 1536, 512, False, True, L.EPI_STORE, seed=3)
@@ -74,7 +74,7 @@ def test_tc_batched_causal_and_reduce():
 
 
 def test_tc_gemm_rotary_dim_head_64_cached_tables():
-    """dim_head 64 takes the per-tile cached sin/cos path of the epilogue; several sequences per tile column block."""
+    """dim_head 64 rotary epilogue: several heads per tile, several sequences per tile's rows, and a row tail."""
     from progen_b200 import lib as L
     from gemm_cases import run_case
     err, scale = run_case(L.BACKEND_TC, torch.bfloat16, 512, 384, 128, False, True, L.EPI_ROTARY, seed=11, seq_len=128, dim_head=64)
@@ -83,14 +83,26 @@ def test_tc_gemm_rotary_dim_head_64_cached_tables():
     assert err <= BF16_OUT_TOL * max(1.0, scale), (err, scale)
 
 
-# (b_mn, epi) combinations of the CTA-pair kernel (gemm_tc2.cu): TMA-staged epilogue slots
+@pytest.mark.parametrize('b_mn', [False, True])
+@pytest.mark.parametrize('N', [160, 224])
+def test_tc_gemm_column_tail(N, b_mn):
+    """N not a multiple of the 128-column tile: the last tile's TMA boxes are partly (K-major B) or wholly (MN-major B)
+    outside the matrix and the epilogue skips the columns past N."""
+    from progen_b200 import lib as L
+    from gemm_cases import run_case
+    for epi in (L.EPI_STORE, L.EPI_ACCUM) if not b_mn else (L.EPI_STORE,):
+        err, scale = run_case(L.BACKEND_TC, torch.bfloat16, 384, N, 128, False, b_mn, epi, seed=30 + N)
+        assert err <= _tol(epi) * max(1.0, scale), (N, b_mn, epi, err, scale)
+
+
+# (b_mn, epi) combinations of the activation GEMMs (K-major A)
 PAIR_COMBOS = [(True, 0), (False, 0), (True, 1), (True, 2), (True, 3), (True, 4), (False, 5), (False, 6)]
 
 
 @pytest.mark.parametrize('b_mn,epi', PAIR_COMBOS)
 def test_tc2_pair_kernel_many_tiles_row_tail(b_mn, epi):
-    """162 tiles over 74 CTA pairs (every epilogue slot and smem stage wraps several times), a row tail that leaves the
-    second CTA of the last pair partly and the TMA boxes partly outside the matrix, two column tiles."""
+    """648 tiles (several waves over the SMs), a row tail that leaves the last row tile and its TMA boxes partly outside
+    the matrix, four column tiles."""
     from progen_b200 import lib as L
     from gemm_cases import run_case
     M, N, K = 256 * 80 + 136, 512, 192
@@ -100,7 +112,7 @@ def test_tc2_pair_kernel_many_tiles_row_tail(b_mn, epi):
 
 
 def test_tc2_pair_kernel_fp32_store_and_residual_aux():
-    """fp32 STORE output (128-byte rows in the slot) and the RESIDUAL epilogue reading its input from a second buffer."""
+    """fp32 STORE output and the RESIDUAL epilogue reading its input from a second buffer."""
     from progen_b200 import lib as L
     from gemm_cases import run_case
     dev = 'cuda'

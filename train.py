@@ -1,5 +1,5 @@
 """train.py — drop-in for the reference CLI (lucidrains/progen train.py:36-57: same flags and defaults), running the
-B200 engine.  Additions: --synthetic (uniform-random tokens, the BASELINE workload), --num_steps, --text_file (one
+H100 engine.  Additions: --synthetic (uniform-random tokens, the BASELINE workload), --num_steps, --text_file (one
 sequence per line, instead of TFRecords whose reader needs tensorflow).  Launch with torchrun for --data_parallel.
 
 The loop is the reference's (train.py:184-222): for each effective batch, grad_accum_every micro-steps of
