@@ -1,16 +1,20 @@
 // wgmma GEMM for sm_90a: D[M,N] (+)= A[M,K] * B[N,K]^T, bf16 operands, fp32 accumulation in registers.
 //
-//   warpgroup 0    : TMA producer (one thread: cp.async.bulk.tensor.2d, 128B swizzle, mbarrier complete_tx)
-//   warpgroups 1, 2: consumers, 64 rows of the 128 x 128 tile each (wgmma.mma_async m64n128k16, both operands read
-//                    from shared memory), then the fused epilogue
+// Persistent and warp-specialized: min(tiles, SMs) CTAs, CTA b takes the 128 x 128 output tiles b, b + grid, b + 2 grid, ...
+//   warpgroup 0    : TMA producer (one thread: cp.async.bulk.tensor.2d, 128B swizzle, mbarrier complete_tx); it walks
+//                    the CTA's tiles with one ring position, so the next tile's k-blocks load during the epilogues
+//   warpgroups 1, 2: ping-pong consumers: each owns whole tiles (alternate tiles of the CTA's list), two
+//                    wgmma.mma_async m64n128k16 per k-step (both operands from shared memory), then the fused epilogue.
+//                    A named-barrier handshake lets one warpgroup issue MMAs at a time, so one warpgroup's mainloop
+//                    runs while the other is in its epilogue.
 //
-// One CTA per output tile; the shared-memory ring holds STAGES k-blocks so the TMA loads run ahead of the MMAs.  Operands
-// may be K-major or MN-major (wgrad reads the activations and the output gradient with the token dimension as K, i.e.
-// MN-major): TMA writes both into the same 128B-swizzled layout and only the wgmma descriptors and transpose bits differ.
-// After the last k-block the accumulators go through shared memory (the drained ring) so that every epilogue thread
-// owns 8 consecutive columns of one row: the global loads / stores of the epilogue are 16-byte vectors, coalesced
-// along the row.
+// Operands may be K-major or MN-major (wgrad reads the activations and the output gradient with the token dimension as
+// K, i.e. MN-major): TMA writes both into the same 128B-swizzled layout and only the wgmma descriptors and transpose bits
+// differ.  After the last k-block the accumulators go through a per-warpgroup shared-memory buffer, 64 rows at a time,
+// so that every epilogue thread owns 8 consecutive columns of one row: the global loads / stores of the epilogue are
+// 16-byte vectors, coalesced along the row.
 #include <cuda.h>
+#include <algorithm>
 #include <mutex>
 #include <unordered_map>
 #include "gemm.h"
@@ -28,11 +32,21 @@ constexpr int THREADS = 384;           // producer warpgroup + two consumer warp
 constexpr int A_BYTES = BM * BK * 2;   // 16 KiB
 constexpr int B_BYTES = BN * BK * 2;   // 16 KiB
 constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-constexpr int STAGES = 6;
-constexpr int CS_LD = BN + 4;          // fp32 row stride of the accumulator tile staged for the epilogue
-constexpr int SMEM_TOTAL = 1024 /*align slack*/ + STAGES * STAGE_BYTES + 2 * STAGES * 8;
-static_assert(BM * CS_LD * 4 <= STAGES * STAGE_BYTES, "the epilogue tile reuses the operand ring");
+constexpr int STAGES = 4;                // a fifth stage fits only with epilogue passes of 64 x 64; measured slower on the step
+constexpr int EPI_ROWS = 64;           // the epilogue stages and applies the tile in two passes of 64 rows
+constexpr int CS_LD = BN + 4;          // fp32 row stride of the staged accumulator rows
+constexpr int CS_BYTES = EPI_ROWS * CS_LD * 4;
+constexpr int SMEM_TOTAL = 1024 /*align slack*/ + STAGES * STAGE_BYTES + 2 * CS_BYTES + 2 * STAGES * 8;
 static_assert(SMEM_TOTAL <= 227 * 1024, "H100: 227 KiB of shared memory per block");
+// named barriers (0 is __syncthreads): MMA turn of consumer c = 1 + c, epilogue buffer of consumer c = 3 + c
+constexpr int BAR_TURN = 1, BAR_EPI = 3;
+constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;     // setmaxnreg: 128 x 40 + 256 x 232 <= 64 K registers
+static_assert(128 * PRODUCER_REGS + 256 * CONSUMER_REGS <= 65536, "register file");
+
+__device__ __forceinline__ void named_bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+__device__ __forceinline__ void named_bar_arrive(int id, int n) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+template <int R> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 
 struct GemmDev {
   int M, N, K;
@@ -72,121 +86,147 @@ __device__ __forceinline__ void decode_tile(const GemmDev& g, int t, TileInfo& t
 
 template <bool A_MN, bool B_MN, int KIND, typename TO>
 __global__ void __launch_bounds__(THREADS, 1)
-gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b, const GemmDev g) {
+gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b, const GemmDev g,
+               const int tiles) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_u32 = smem_u32(smem_raw);
   const uint32_t smem_base = (raw_u32 + 1023u) & ~1023u;      // SWIZZLE_128B needs 1024 B alignment
-  const uint32_t bar_base = smem_base + STAGES * STAGE_BYTES;
+  const uint32_t cs_base = smem_base + STAGES * STAGE_BYTES;
+  const uint32_t bar_base = cs_base + 2 * CS_BYTES;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
 
   const int wg = threadIdx.x >> 7;
-  TileInfo ti;
-  decode_tile(g, blockIdx.x, ti);
-
   if (threadIdx.x == 0) {
     prefetch_tensormap(&tma_a);
     prefetch_tensormap(&tma_b);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 2);                 // one arrival per consumer warpgroup
+      mbar_init(empty_bar(s), 1);                 // released by the one consumer warpgroup that read the stage
     }
     fence_barrier_init();
   }
   __syncthreads();
 
+  // The ring position runs on across tiles: the producer and both consumers see the same sequence of k-blocks (the
+  // CTA's tiles in order), each consumer reading only its own tiles' k-blocks and stepping over the other's.
+  int stage = 0;
+  uint32_t phase = 0;
+  auto advance = [&](int n) {
+    stage += n;
+    phase ^= (uint32_t)(stage / STAGES) & 1u;
+    stage %= STAGES;
+  };
+
   if (wg == 0) {
     // ===================================================================== TMA producer
+    setmaxnreg_dec<PRODUCER_REGS>();
     if (threadIdx.x == 0) {
-      const int a_row0 = ti.z * g.a_batch_rows;
-      const int b_row0 = ti.z * g.b_batch_rows;
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int kb = ti.kb_begin; kb < ti.kb_end; ++kb) {
-        mbar_wait(empty_bar(stage), phase ^ 1);
-        const uint32_t sa = smem_base + stage * STAGE_BYTES;
-        const uint32_t sb = sa + A_BYTES;
-        mbar_expect_tx(full_bar(stage), STAGE_BYTES);
-        const int k0 = kb * BK;
-        if constexpr (!A_MN) {
-          tma_load_2d(sa, &tma_a, full_bar(stage), k0, a_row0 + ti.m0);                   // box {64 k, 128 m}
-        } else {
+      for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
+        TileInfo ti;
+        decode_tile(g, t, ti);
+        const int a_row0 = ti.z * g.a_batch_rows;
+        const int b_row0 = ti.z * g.b_batch_rows;
+        for (int kb = ti.kb_begin; kb < ti.kb_end; ++kb) {
+          mbar_wait(empty_bar(stage), phase ^ 1);
+          const uint32_t sa = smem_base + stage * STAGE_BYTES;
+          const uint32_t sb = sa + A_BYTES;
+          mbar_expect_tx(full_bar(stage), STAGE_BYTES);
+          const int k0 = kb * BK;
+          if constexpr (!A_MN) {
+            tma_load_2d(sa, &tma_a, full_bar(stage), k0, a_row0 + ti.m0);                   // box {64 k, 128 m}
+          } else {
 #pragma unroll
-          for (int i = 0; i < BM / 64; ++i)                                                // boxes {64 m, 64 k}
-            tma_load_2d(sa + i * 8192, &tma_a, full_bar(stage), ti.m0 + 64 * i, a_row0 + k0);
-        }
-        if constexpr (!B_MN) {
-          tma_load_2d(sb, &tma_b, full_bar(stage), k0, b_row0 + ti.n0);                   // box {64 k, 128 n}
-        } else {
+            for (int i = 0; i < BM / 64; ++i)                                                // boxes {64 m, 64 k}
+              tma_load_2d(sa + i * 8192, &tma_a, full_bar(stage), ti.m0 + 64 * i, a_row0 + k0);
+          }
+          if constexpr (!B_MN) {
+            tma_load_2d(sb, &tma_b, full_bar(stage), k0, b_row0 + ti.n0);                   // box {64 k, 128 n}
+          } else {
 #pragma unroll
-          for (int i = 0; i < BN / 64; ++i)                                                // boxes {64 n, 64 k}
-            tma_load_2d(sb + i * 8192, &tma_b, full_bar(stage), ti.n0 + 64 * i, b_row0 + k0);
+            for (int i = 0; i < BN / 64; ++i)                                                // boxes {64 n, 64 k}
+              tma_load_2d(sb + i * 8192, &tma_b, full_bar(stage), ti.n0 + 64 * i, b_row0 + k0);
+          }
+          advance(1);
         }
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
     }
     return;
   }
 
-  // ======================================================================= consumers: rows 64 c .. 64 c + 63 of the tile
+  // ======================================================================= consumer c: tiles at even / odd positions
+  setmaxnreg_inc<CONSUMER_REGS>();
   const int c = wg - 1;
-  const int t = threadIdx.x - 128;              // 0..255 over both consumer warpgroups
-  float acc[64];
+  const int tid = threadIdx.x & 127;
+  float* cs = reinterpret_cast<float*>(smem_raw + (cs_base - raw_u32)) + c * (CS_BYTES / 4);
+  for (int p = 0, t = blockIdx.x; t < tiles; ++p, t += gridDim.x) {
+    TileInfo ti;
+    decode_tile(g, t, ti);
+    if ((p & 1) != c) {
+      advance(ti.kb_end - ti.kb_begin);
+      continue;
+    }
+    // acc[h]: rows 64 h .. 64 h + 63 of the tile
+    float acc[2][64];
 #pragma unroll
-  for (int i = 0; i < 64; ++i) acc[i] = 0.f;
-  {
-    int stage = 0, prev = -1;
-    uint32_t phase = 0;
+    for (int i = 0; i < 64; ++i) acc[0][i] = acc[1][i] = 0.f;
+    if (p > 0) named_bar_sync(BAR_TURN + c, 256);          // the other consumer has issued the MMAs of tile p - 1
+    int prev = -1;
     for (int kb = ti.kb_begin; kb < ti.kb_end; ++kb) {
       mbar_wait(full_bar(stage), phase);
       const uint32_t sa = smem_base + stage * STAGE_BYTES;
-      // both majors: this warpgroup's 64 rows of A start 8 KiB in (K-major: 64 rows x 128 B; MN-major: the second box)
-      const uint64_t adesc = make_smem_desc<A_MN>(sa + c * 8192);
+      // both majors: rows 64 .. 127 of A start 8 KiB in (K-major: 64 rows x 128 B; MN-major: the second box)
+      const uint64_t adesc0 = make_smem_desc<A_MN>(sa), adesc1 = make_smem_desc<A_MN>(sa + 8192);
       const uint64_t bdesc = make_smem_desc<B_MN>(sa + A_BYTES);
       constexpr uint32_t a_step = A_MN ? (2048 >> 4) : (32 >> 4), b_step = B_MN ? (2048 >> 4) : (32 >> 4);
-      fence_regs(acc);
+      fence_regs(acc[0]);
+      fence_regs(acc[1]);
       wgmma_fence();
 #pragma unroll
-      for (int k = 0; k < BK / WG_K; ++k)
-        wgmma_m64n128k16_bf16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, adesc + (uint64_t)(k * a_step), bdesc + (uint64_t)(k * b_step));
+      for (int k = 0; k < BK / WG_K; ++k) {
+        wgmma_m64n128k16_bf16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc[0], adesc0 + (uint64_t)(k * a_step), bdesc + (uint64_t)(k * b_step));
+        wgmma_m64n128k16_bf16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc[1], adesc1 + (uint64_t)(k * a_step), bdesc + (uint64_t)(k * b_step));
+      }
       wgmma_commit();
-      fence_regs(acc);
+      fence_regs(acc[0]);
+      fence_regs(acc[1]);
       wgmma_wait<1>();                          // the previous k-block's MMAs are done: its stage can be refilled
-      if (prev >= 0 && (t & 127) == 0) mbar_arrive(empty_bar(prev));
+      if (prev >= 0 && tid == 0) mbar_arrive(empty_bar(prev));
       prev = stage;
-      if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      advance(1);
     }
+    if (t + (int)gridDim.x < tiles) named_bar_arrive(BAR_TURN + (c ^ 1), 256);   // tile p + 1 may issue its MMAs
     wgmma_wait<0>();
-    fence_regs(acc);
-  }
+    fence_regs(acc[0]);
+    fence_regs(acc[1]);
+    if (prev >= 0 && tid == 0) mbar_arrive(empty_bar(prev));
 
-  // ---- stage the fp32 tile in shared memory (every MMA of both warpgroups has read its operands: the ring is free)
-  asm volatile("bar.sync 1, 256;" ::: "memory");
-  float* cs = reinterpret_cast<float*>(smem_raw + (smem_base - raw_u32));
-  {
-    const int w = (t & 127) >> 5, lane = t & 31;
-    const int r0 = 64 * c + 16 * w + (lane >> 2);
-    const int c0 = 2 * (lane & 3);
+    // ---- epilogue, 64 rows per pass: stage the fp32 rows in this warpgroup's buffer, then 8 consecutive columns of
+    // one row per thread, 16 threads per row
+    const int w = tid >> 5, lane = tid & 31;
+    const int r0 = 16 * w + (lane >> 2), c0 = 2 * (lane & 3);
 #pragma unroll
-    for (int j = 0; j < BN / 8; ++j) {
-      *reinterpret_cast<float2*>(cs + r0 * CS_LD + 8 * j + c0) = make_float2(acc[4 * j], acc[4 * j + 1]);
-      *reinterpret_cast<float2*>(cs + (r0 + 8) * CS_LD + 8 * j + c0) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
-    }
-  }
-  asm volatile("bar.sync 1, 256;" ::: "memory");
-
-  // ---- epilogue: 8 consecutive columns of one row per thread, 16 threads per row
+    for (int h = 0; h < 2; ++h) {
+      named_bar_sync(BAR_EPI + c, 128);         // every thread has read the rows staged before
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        *reinterpret_cast<float2*>(cs + r0 * CS_LD + 8 * j + c0) = make_float2(acc[h][4 * j], acc[h][4 * j + 1]);
+        *reinterpret_cast<float2*>(cs + (r0 + 8) * CS_LD + 8 * j + c0) = make_float2(acc[h][4 * j + 2], acc[h][4 * j + 3]);
+      }
+      named_bar_sync(BAR_EPI + c, 128);
 #pragma unroll 1
-  for (int idx = t; idx < BM * (BN / 8); idx += 256) {
-    const int r = idx / (BN / 8), cc = (idx % (BN / 8)) * 8;
-    const int m = ti.m0 + r, col = ti.n0 + cc;
-    if (m >= g.M || col >= g.N) continue;
-    float v[8];
-    const float4 x0 = *reinterpret_cast<const float4*>(cs + r * CS_LD + cc);
-    const float4 x1 = *reinterpret_cast<const float4*>(cs + r * CS_LD + cc + 4);
-    v[0] = x0.x; v[1] = x0.y; v[2] = x0.z; v[3] = x0.w; v[4] = x1.x; v[5] = x1.y; v[6] = x1.z; v[7] = x1.w;
-    const long long row = (g.batch_reduce ? 0 : (long long)ti.z * g.d_batch_rows) + m;
-    epi_apply<KIND, TO, 8>(g.epi, DirectIO{}, row, col, v, true);
+      for (int idx = tid; idx < EPI_ROWS * (BN / 8); idx += 128) {
+        const int r = idx / (BN / 8), cc = (idx % (BN / 8)) * 8;
+        const int m = ti.m0 + EPI_ROWS * h + r, col = ti.n0 + cc;
+        if (m >= g.M || col >= g.N) continue;
+        float v[8];
+        const float4 x0 = *reinterpret_cast<const float4*>(cs + r * CS_LD + cc);
+        const float4 x1 = *reinterpret_cast<const float4*>(cs + r * CS_LD + cc + 4);
+        v[0] = x0.x; v[1] = x0.y; v[2] = x0.z; v[3] = x0.w; v[4] = x1.x; v[5] = x1.y; v[6] = x1.z; v[7] = x1.w;
+        const long long row = (g.batch_reduce ? 0 : (long long)ti.z * g.d_batch_rows) + m;
+        epi_apply<KIND, TO, 8>(g.epi, DirectIO{}, row, col, v, true);
+      }
+    }
   }
 }
 
@@ -267,7 +307,7 @@ int launch_inst(const CUtensorMap& ta, const CUtensorMap& tb, const GemmDev& gd,
     PG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL));
     attr_set = true;
   }
-  kern<<<tiles, THREADS, SMEM_TOTAL, stream>>>(ta, tb, gd);
+  kern<<<std::min(tiles, pg_num_sms()), THREADS, SMEM_TOTAL, stream>>>(ta, tb, gd, tiles);
   PG_LAUNCH_CHECK();
   return PROGEN_OK;
 }
