@@ -31,8 +31,8 @@ extern "C" {
 #define PROGEN_EPI_STORE 0     /* out = acc (+bias)                      progen.py:219-222 (logits), 185 (SGU proj)   */
 #define PROGEN_EPI_ROTARY 1    /* out = rotary(acc)                      progen.py:83-87 (to_qkv, rotary on q,k,v)    */
 #define PROGEN_EPI_RESIDUAL 2  /* out(f32) = (aux|out)(f32) + acc + bias   progen.py:103+230, 148+231                    */
-#define PROGEN_EPI_GLU 3       /* out2 = pre-act, out = val*gelu(gate)   progen.py:137-141                             */
-#define PROGEN_EPI_GELU 4      /* out2 = pre-act, out = gelu(pre)        progen.py:137,143                             */
+#define PROGEN_EPI_GLU 3       /* out = val*gelu(gate), out2 = pre-act   progen.py:137-141; out2 NULL: not stored     */
+#define PROGEN_EPI_GELU 4      /* out = gelu(pre), out2 = pre-act        progen.py:137,143;  out2 NULL: not stored     */
 #define PROGEN_EPI_GLU_BWD 5   /* out = d(pre-act) from acc = d(GLU out) (backward of 3)                               */
 #define PROGEN_EPI_GELU_BWD 6  /* out = acc * gelu'(pre-act)             (backward of 4)                               */
 #define PROGEN_EPI_ACCUM 7     /* out(f32) += acc  (weight gradients; optional tril mask for SGU spatial_weights)     */
@@ -96,6 +96,17 @@ int progen_colsum(const void* in, long long ld, int dtype, float* out, long long
  * *loss must be zeroed by the caller; inv_batch = 1/global_batch (DDP: a sum over ranks yields the global mean). */
 int progen_ce_fwd_bwd(const void* logits, int dtype, const int* labels, float* weights, float* loss, void* dlogits,
                       int dlogits_dtype, int B, int n, int V, float inv_batch, void* stream);
+
+/* scoring (inference): logp[t] = mask_t * log_softmax(logits[t])[label_t] with the loss mask of utils.py:54-56 (Q8: non-pad
+ * labels plus the first pad; labels clamped to [0, V) like progen_ce_fwd_bwd); seq_ll[b] = sum_t logp[b, t] and
+ * seq_count[b] = sum_t mask_t, reduced in a fixed order (bitwise independent of B).  logp: [B*n]; seq_ll, seq_count: [B].
+ * -seq_ll / seq_count is the per-sequence cross_entropy of utils.py:45-59. */
+int progen_token_logprob(const void* logits, int dtype, const int* labels, float* logp, float* seq_ll, float* seq_count,
+                         int B, int n, int V, void* stream);
+/* out[b, :] = sum_t mask_t x[b, t, :] / sum_t mask_t (fp32, fixed order) over rows of x [B*n, d] (stride ldx), with the
+ * same mask as above: for a sequence of L residues, input positions 0..L (BOS and every residue). */
+int progen_masked_mean_pool(const void* x, long long ldx, int dtype, const int* labels, float* out, int B, int n, int d,
+                            void* stream);
 
 /* backward of apply_rotary_pos_emb (progen.py:36-41) on the [T, ncols] q|k|v gradient, in place */
 int progen_rotary_bwd(void* dqkv, long long ld, int dtype, const float* sin_t, const float* cos_t, long long T, int ncols,

@@ -52,7 +52,7 @@ int progen_gemm(const progen_gemm_t* d, void* stream) {
   g.epi.atomic = d->atomic; g.epi.tril = d->tril; g.epi.tril_rows = d->tril_rows > 0 ? d->tril_rows : 1;
   PG_CHECK_ARG(g.epi_kind >= 0 && g.epi_kind < EPI_NUM_KINDS);
   PG_CHECK_ARG(g.epi.out != nullptr);
-  if (g.epi_kind == EPI_GLU || g.epi_kind == EPI_GELU) PG_CHECK_ARG(g.epi.out2 != nullptr && g.epi.bias != nullptr);
+  if (g.epi_kind == EPI_GLU || g.epi_kind == EPI_GELU) PG_CHECK_ARG(g.epi.bias != nullptr);   // out2 may be null (inference)
   if (g.epi_kind == EPI_GLU_BWD || g.epi_kind == EPI_GELU_BWD) PG_CHECK_ARG(g.epi.aux != nullptr);
   if (g.epi_kind == EPI_ROTARY) PG_CHECK_ARG(g.epi.rot_sin && g.epi.rot_cos && d->seq_len > 0 && d->dim_head > 0 && d->dim_head % 2 == 0);
   if (d->backend == PROGEN_BACKEND_TC) return gemm_tc_launch(g, (cudaStream_t)stream);

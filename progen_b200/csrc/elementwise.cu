@@ -324,6 +324,31 @@ __global__ void ce_weights_kernel(const int* __restrict__ labels, float* __restr
   for (int i = threadIdx.x; i < n; i += blockDim.x) w[(long long)b * n + i] = (lb[i] != 0 || i == s_first) ? wv : 0.f;
 }
 
+// Row max and sum of exp(x - max) of one V-wide logits row, computed by one warp in a fixed order (every lane gets both);
+// log-sum-exp = mx + logf(se).  Shared by the training loss and the inference log-likelihood, so both see the same bits.
+template <typename TL>
+__device__ __forceinline__ void warp_row_max_sumexp(const TL* __restrict__ lr, int V, int lane, float& mx, float& se) {
+  mx = -INFINITY;
+  for (int c = lane * 4; c < V; c += 128) {
+    float v[4];
+    load4<TL>(lr + c, v);
+    mx = fmaxf(mx, fmaxf(fmaxf(v[0], v[1]), fmaxf(v[2], v[3])));
+  }
+  mx = warp_max(mx);
+  se = 0.f;
+  for (int c = lane * 4; c < V; c += 128) {
+    float v[4];
+    load4<TL>(lr + c, v);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) se += expf(v[i] - mx);
+  }
+  se = warp_sum(se);
+}
+
+// out-of-range labels are clamped like the token ids in embed_fwd / embed_bwd (jnp indexing clamps); byte 0xFF + 1 = 256
+// with V = 256 is reachable from real data (data.py tokenizer) and must not read past the logits row
+__device__ __forceinline__ int clamp_label(int lab, int V) { return min(max(lab, 0), V - 1); }
+
 // Kernel 2: one warp per token over V logits: loss += w * (lse - logit[label]); dlogits = w * (softmax - onehot).
 template <typename TL, typename TD>
 __global__ void ce_fwd_bwd_kernel(const TL* __restrict__ logits, const int* __restrict__ labels,
@@ -333,24 +358,9 @@ __global__ void ce_fwd_bwd_kernel(const TL* __restrict__ logits, const int* __re
   float block_loss = 0.f;
   for (long long t = blockIdx.x * (long long)ROWS_PER_BLOCK + warp; t < T; t += (long long)gridDim.x * ROWS_PER_BLOCK) {
     const TL* lr = logits + t * V;
-    float mx = -INFINITY;
-    for (int c = lane * 4; c < V; c += 128) {
-      float v[4];
-      load4<TL>(lr + c, v);
-      mx = fmaxf(mx, fmaxf(fmaxf(v[0], v[1]), fmaxf(v[2], v[3])));
-    }
-    mx = warp_max(mx);
-    float se = 0.f;
-    for (int c = lane * 4; c < V; c += 128) {
-      float v[4];
-      load4<TL>(lr + c, v);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) se += expf(v[i] - mx);
-    }
-    se = warp_sum(se);
-    // out-of-range labels are clamped like the token ids in embed_fwd / embed_bwd (jnp indexing clamps); byte 0xFF + 1 = 256
-    // with V = 256 is reachable from real data (data.py tokenizer) and must not read past the logits row
-    const int lab = min(max(labels[t], 0), V - 1);
+    float mx, se;
+    warp_row_max_sumexp<TL>(lr, V, lane, mx, se);
+    const int lab = clamp_label(labels[t], V);
     const float wt = w[t];
     const float lse = mx + logf(se);
     if (lane == 0) block_loss += wt * (lse - to_f32(lr[lab]));
@@ -372,6 +382,106 @@ __global__ void ce_fwd_bwd_kernel(const TL* __restrict__ logits, const int* __re
     float s = 0.f;
     for (int i = 0; i < ROWS_PER_BLOCK; ++i) s += red[i];
     atomicAdd(loss, s);
+  }
+}
+
+// ------------------------------------------------------------------------------------------ scoring (inference)
+// Per-token log-likelihood under the same mask as the loss (utils.py:45-59):  logp[t] = mask_t * log_softmax(logits[t])[label_t].
+// Pass 1, one warp per token: the unmasked log-probability of the label.
+template <typename TL>
+__global__ void token_logprob_kernel(const TL* __restrict__ logits, const int* __restrict__ labels, float* __restrict__ logp,
+                                     long long T, int V) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (long long t = blockIdx.x * (long long)ROWS_PER_BLOCK + warp; t < T; t += (long long)gridDim.x * ROWS_PER_BLOCK) {
+    const TL* lr = logits + t * V;
+    float mx, se;
+    warp_row_max_sumexp<TL>(lr, V, lane, mx, se);
+    const int lab = clamp_label(labels[t], V);
+    if (lane == 0) logp[t] = to_f32(lr[lab]) - (mx + logf(se));
+  }
+}
+
+// The loss mask of one sequence (quirk Q8): non-pad labels plus the first pad.  Block-wide; returns the position of the
+// first pad (n if none) and the number of masked-in positions.  Integer atomics only: the result does not depend on timing.
+__device__ __forceinline__ void seq_loss_mask(const int* __restrict__ lb, int n, int& first, int& count) {
+  __shared__ int s_first, s_count;
+  if (threadIdx.x == 0) { s_first = n; s_count = 0; }
+  __syncthreads();
+  int f = n, cnt = 0;
+  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+    if (lb[i] == 0) f = min(f, i); else cnt++;
+  }
+  atomicMin(&s_first, f);
+  atomicAdd(&s_count, cnt);
+  __syncthreads();
+  first = s_first;
+  count = s_count + (s_first < n ? 1 : 0);
+}
+
+// Fixed-order sum over a 256-thread block (lane shuffles, then the 8 warp partials in order); valid in thread 0.
+__device__ __forceinline__ float block_sum_fixed(float v) {
+  __shared__ float red[ROWS_PER_BLOCK];
+  v = warp_sum(v);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (lane == 0) red[warp] = v;
+  __syncthreads();
+  float s = 0.f;
+  if (threadIdx.x == 0)
+    for (int i = 0; i < ROWS_PER_BLOCK; ++i) s += red[i];
+  return s;
+}
+
+// Pass 2, one 256-thread block per sequence: apply the mask in place and reduce it in a fixed order (no float atomics), so
+// a sequence's sums are the same bits whatever batch it is scored in.
+__global__ void seq_logprob_sum_kernel(const int* __restrict__ labels, float* __restrict__ logp, float* __restrict__ seq_ll,
+                                       float* __restrict__ seq_count, int n) {
+  const int b = blockIdx.x;
+  const int* lb = labels + (long long)b * n;
+  float* lp = logp + (long long)b * n;
+  int first, count;
+  seq_loss_mask(lb, n, first, count);
+  float acc = 0.f;
+  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+    const float v = (lb[i] != 0 || i == first) ? lp[i] : 0.f;
+    lp[i] = v;
+    acc += v;
+  }
+  const float s = block_sum_fixed(acc);
+  if (threadIdx.x == 0) {
+    seq_ll[b] = s;
+    seq_count[b] = (float)count;
+  }
+}
+
+// out[b, :] = sum_t mask_t x[b, t, :] / sum_t mask_t.  Grid (ceil(d / 128), B), 256 threads: lane owns 4 columns, warp w sums
+// rows t = w, w + 8, ... in order, then the 8 warp partials are added in order: fixed order, fp32 accumulation.
+template <typename TX>
+__global__ void masked_mean_pool_kernel(const TX* __restrict__ x, long long ldx, const int* __restrict__ labels,
+                                        float* __restrict__ out, int n, int d) {
+  __shared__ float part[ROWS_PER_BLOCK][128];
+  const int b = blockIdx.y;
+  const int* lb = labels + (long long)b * n;
+  int first, count;
+  seq_loss_mask(lb, n, first, count);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int c = blockIdx.x * 128 + lane * 4;
+  float acc[4] = {0.f, 0.f, 0.f, 0.f};
+  if (c < d) {
+    for (int t = warp; t < n; t += ROWS_PER_BLOCK) {
+      if (lb[t] == 0 && t != first) continue;
+      float v[4];
+      load4<TX>(x + ((long long)b * n + t) * ldx + c, v);
+#pragma unroll
+      for (int i = 0; i < 4; ++i) acc[i] += v[i];
+    }
+  }
+#pragma unroll
+  for (int i = 0; i < 4; ++i) part[warp][lane * 4 + i] = acc[i];
+  __syncthreads();
+  if (threadIdx.x < 128 && blockIdx.x * 128 + (int)threadIdx.x < d) {
+    float s = 0.f;
+    for (int w = 0; w < ROWS_PER_BLOCK; ++w) s += part[w][threadIdx.x];
+    out[(long long)b * d + blockIdx.x * 128 + threadIdx.x] = s / (float)count;
   }
 }
 
@@ -600,6 +710,33 @@ int progen_ce_fwd_bwd(const void* logits, int dtype, const int* labels, float* w
   else if (dtype == PG_BF16 && dlogits_dtype == PG_BF16) CE_CASE(bf16, bf16);
   else { progen_set_error("ce_fwd_bwd: unsupported dtypes %d / %d", dtype, dlogits_dtype); return PROGEN_ERR_UNSUPPORTED; }
 #undef CE_CASE
+  PG_LAUNCH_CHECK();
+  return PROGEN_OK;
+}
+
+int progen_token_logprob(const void* logits, int dtype, const int* labels, float* logp, float* seq_ll, float* seq_count,
+                         int B, int n, int V, void* stream) {
+  PG_CHECK_ARG(B > 0 && n > 0 && V % 4 == 0 && logits && labels && logp && seq_ll && seq_count);
+  cudaStream_t s = (cudaStream_t)stream;
+  const long long T = (long long)B * n;
+  const int grid = row_grid(T);
+  if (dtype == PG_F32) token_logprob_kernel<float><<<grid, 256, 0, s>>>((const float*)logits, labels, logp, T, V);
+  else if (dtype == PG_BF16) token_logprob_kernel<bf16><<<grid, 256, 0, s>>>((const bf16*)logits, labels, logp, T, V);
+  else { progen_set_error("token_logprob: unsupported dtype %d", dtype); return PROGEN_ERR_UNSUPPORTED; }
+  PG_LAUNCH_CHECK();
+  seq_logprob_sum_kernel<<<B, 256, 0, s>>>(labels, logp, seq_ll, seq_count, n);
+  PG_LAUNCH_CHECK();
+  return PROGEN_OK;
+}
+
+int progen_masked_mean_pool(const void* x, long long ldx, int dtype, const int* labels, float* out, int B, int n, int d,
+                            void* stream) {
+  PG_CHECK_ARG(B > 0 && n > 0 && d > 0 && d % 4 == 0 && ldx >= d && ldx % 4 == 0 && x && labels && out);
+  cudaStream_t s = (cudaStream_t)stream;
+  dim3 grid((d + 127) / 128, B);
+  if (dtype == PG_F32) masked_mean_pool_kernel<float><<<grid, 256, 0, s>>>((const float*)x, ldx, labels, out, n, d);
+  else if (dtype == PG_BF16) masked_mean_pool_kernel<bf16><<<grid, 256, 0, s>>>((const bf16*)x, ldx, labels, out, n, d);
+  else { progen_set_error("masked_mean_pool: unsupported dtype %d", dtype); return PROGEN_ERR_UNSUPPORTED; }
   PG_LAUNCH_CHECK();
   return PROGEN_OK;
 }

@@ -8,8 +8,8 @@ enum EpiKind : int {
   EPI_STORE = 0,      // out = acc (+ bias[col])
   EPI_ROTARY = 1,     // out = rotary(acc)            qkv projection, progen.py:83-87 (rotary on q, k AND v)
   EPI_RESIDUAL = 2,   // out(f32) += acc + bias       to_out / proj_out + residual, progen.py:103,148,230-231
-  EPI_GLU = 3,        // out2 = pre-activation (interleaved value,gate), out = value * gelu(gate)   progen.py:139-141
-  EPI_GELU = 4,       // out2 = pre-activation, out = gelu(pre)                                     progen.py:143
+  EPI_GLU = 3,        // out = value * gelu(gate); out2 (nullable) = pre-activation (interleaved value,gate)   progen.py:139-141
+  EPI_GELU = 4,       // out = gelu(pre); out2 (nullable) = pre-activation                                     progen.py:143
   EPI_GLU_BWD = 5,    // acc = d(out of GLU); aux = saved pre-activation; out = d(pre) interleaved
   EPI_GELU_BWD = 6,   // acc = d(gelu out); aux = saved pre-activation; out = acc * gelu'(pre)
   EPI_ACCUM = 7,      // out(f32) += acc  (atomic when several CTAs own the same tile; optional tril mask)
@@ -18,7 +18,7 @@ enum EpiKind : int {
 
 struct EpiArgs {
   void* out; long long ldo;
-  void* out2; long long ldo2;
+  void* out2; long long ldo2;       // EPI_GLU / EPI_GELU: pre-activation for the backward pass; nullptr = not stored
   const float* bias;                 // [N] (already interleaved for GLU) or nullptr
   const void* aux; long long ldaux;  // saved pre-activations for the *_BWD kinds
   const float* rot_sin;              // [seq_len, dim_head/2]
@@ -107,7 +107,8 @@ __device__ __forceinline__ void epi_apply(const EpiArgs& e, const IO& io, long l
     io.template store<NV>(p, e.ldo, r, valid);
   } else if constexpr (KIND == EPI_GLU) {
     add_bias<NV>(e.bias, col, v);
-    io.template store<NV>(reinterpret_cast<TO*>(e.out2) + row * e.ldo2 + col, e.ldo2, v, valid);
+    // uniform branch: inference (no backward) passes out2 = nullptr and skips the pre-activation store
+    if (e.out2) io.template store<NV>(reinterpret_cast<TO*>(e.out2) + row * e.ldo2 + col, e.ldo2, v, valid);
     TO* po = reinterpret_cast<TO*>(e.out) + row * e.ldo + (col >> 1);
     if constexpr (NV >= 16) {
       float o[NV / 2];
@@ -122,7 +123,7 @@ __device__ __forceinline__ void epi_apply(const EpiArgs& e, const IO& io, long l
     }
   } else if constexpr (KIND == EPI_GELU) {
     add_bias<NV>(e.bias, col, v);
-    io.template store<NV>(reinterpret_cast<TO*>(e.out2) + row * e.ldo2 + col, e.ldo2, v, valid);
+    if (e.out2) io.template store<NV>(reinterpret_cast<TO*>(e.out2) + row * e.ldo2 + col, e.ldo2, v, valid);
     float o[NV];
 #pragma unroll
     for (int i = 0; i < NV; ++i) o[i] = gelu_fwd<FAST>(v[i]);

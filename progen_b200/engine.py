@@ -5,7 +5,8 @@ batched over sequences (the reference's `vmap`, utils.py:67).  PyTorch provides 
 
 Data layout in HBM (tokens are rows, T = B * seq_len):
   * residual stream: fp32 [T, d], one buffer per LayerNorm input (the residual epilogue of each GEMM writes the next
-    one, so nothing is copied and every LN backward still has its input);
+    one, so nothing is copied and every LN backward still has its input); the inference set (`Engine.score`) keeps one
+    buffer and updates it in place;
   * activations: act dtype (bf16 with mixed_precision, fp32 without), row-major [T, features];
   * q|k|v: one [T, 3*heads*dim_head] buffer, rotated in the QKV GEMM epilogue;
   * parameters, gradients, Adam moments: FLAT fp32 buffers in "engine layout" (ndim > 1 leaves first, then the
@@ -84,6 +85,28 @@ def _deinterleave(a):
     return np.concatenate((a[..., 0::2], a[..., 1::2]), axis=-1)
 
 
+class Acts:
+    """One activation set: the buffers one forward pass runs on (B sequences, T = B * seq_len token rows).
+    `X` lists the residual stream at every LayerNorm input and `lay` one scratch dict per layer.  The training set keeps
+    all of them (the backward pass reads them); the inference set (`inplace`) repeats one residual buffer, updated in
+    place, and one layer's scratch, and stores no GLU / GELU pre-activation (`u` is None)."""
+
+    def __init__(self, B, T, tok, labels, X, lay, meanf, rstdf, yf, logits, inplace=False, rows=None, res=None):
+        self.B, self.T, self.tok, self.labels, self.X, self.lay = B, T, tok, labels, X, lay
+        self.meanf, self.rstdf, self.yf, self.logits = meanf, rstdf, yf, logits
+        self.inplace = inplace
+        self.rows = rows        # inference: [B, n+1] int32 staging of the input rows (one H2D copy per chunk)
+        self.res = res          # inference: flat fp32 per-chunk results (see Engine.score)
+
+    def view(self, B, n):
+        """the first B sequences of this set (same memory): a ragged last chunk runs on the cached buffers"""
+        T = B * n
+        cut = lambda t: None if t is None else t[:T]
+        return Acts(B, T, cut(self.tok), cut(self.labels), [cut(x) for x in self.X],
+                    [{k: cut(v) for k, v in s.items()} for s in self.lay], cut(self.meanf), cut(self.rstdf), cut(self.yf),
+                    cut(self.logits), self.inplace, None if self.rows is None else self.rows[:B], self.res)
+
+
 class Engine:
     def __init__(self, cfg, mixed_precision=False, device=None):
         L.require_device()
@@ -139,6 +162,8 @@ class Engine:
         self.rot_sin = torch.tensor(np.sin(ang), **f32).contiguous()
         self.rot_cos = torch.tensor(np.cos(ang), **f32).contiguous()
         self.B = 0
+        self.acts = None          # training activation set (ensure_batch)
+        self.infer = None         # inference activation set (inference_acts), cached by row count
         self.loss = torch.zeros(1, device=self.dev)       # exists before the first batch: a rank without rows still reports 0
         self.loaded_token = None
         self.on_layer_grads = None        # optional callback(layer_index) fired when a layer's weight gradients are final
@@ -256,14 +281,45 @@ class Engine:
         half = hid // 2
         if 'sgu' in self.kinds:
             self.dpj, self.dsg, self.dgp, self.dgn = A(T, half), A(T, half), A(T, half), A(T, half)
+        self.acts = Acts(B, T, self.tok, self.labels, self.X, self.lay, self.meanf, self.rstdf, self.yf, self.logits)
+
+    def inference_acts(self, B):
+        """Activation set of a forward pass that keeps no training state, for up to B sequences: one fp32 residual buffer
+        [T, d] updated in place, one layer's scratch shared by every layer (no pre-activation store), the final LN output,
+        the fp32 logits and the scoring outputs.  Allocated on first use and kept for later calls of the same or smaller
+        row count, apart from the training set: `ensure_batch`, `alloc_epoch` and captured training graphs are untouched."""
+        if self.infer is not None and self.infer.B >= B:
+            return self.infer if self.infer.B == B else self.infer.view(B, self.n)
+        self.infer = None                                       # release the smaller set before allocating the larger one
+        n, d, I, hid, V = self.n, self.d, self.I, self.hid, self.V
+        T = B * n
+        dev, act = self.dev, self.act
+        A = lambda *shape: torch.empty(*shape, device=dev, dtype=act)
+        F = lambda *shape: torch.empty(*shape, device=dev, dtype=torch.float32)
+        x = F(T, d)
+        y, mean, rstd = A(T, d), F(T), F(T)
+        s = dict(mean1=mean, rstd1=rstd, y1=y, qkv=A(T, 3 * I), att=A(T, I), lse=F(T, self.h), mean2=mean, rstd2=rstd, y2=y,
+                 u=None, hact=A(T, hid))
+        if 'sgu' in self.kinds:
+            half = hid // 2
+            gn, gp = A(T, half), A(T, half)
+            # the gate output overwrites the normalised gate (dead once the spatial GEMM has read it) and the projection
+            # overwrites the spatial GEMM output (dead once the gate has read it)
+            s.update(mean3=F(T), rstd3=F(T), gn=gn, gp=gp, sg=gn, pj=gp)
+        nl = len(self.kinds)
+        self.infer = Acts(B, T, torch.empty(T, device=dev, dtype=torch.int32), torch.empty(T, device=dev, dtype=torch.int32),
+                          [x] * (2 * nl + 1), [s] * nl, F(T), F(T), A(T, d), F(T, V), inplace=True,
+                          rows=torch.empty(B, n + 1, device=dev, dtype=torch.int32), res=F(B * (2 + n + d)))
+        return self.infer
 
     # ------------------------------------------------------------------------------------------ GEMM helpers
     def _mm(self, **kw):
         L.gemm(backend=self.backend, in_dtype=self.act_dt, **kw)
 
-    def fwd_gemm(self, x, K, w, N, out, epi=L.EPI_STORE, out_dtype=None, **kw):
-        """out[T,N] = x[T,K] @ w[K,N]  (w stored (in, out) like hk.Linear: MN-major B operand)"""
-        self._mm(M=self.T, N=N, K=K, A=x, lda=K, B=w, ldb=N, b_mn=True, out=out, ldo=kw.pop('ldo', N), epi=epi,
+    def fwd_gemm(self, x, K, w, N, out, epi=L.EPI_STORE, out_dtype=None, acts=None, **kw):
+        """out[T,N] = x[T,K] @ w[K,N]  (w stored (in, out) like hk.Linear: MN-major B operand); T from `acts` (default:
+        the training set)"""
+        self._mm(M=(acts or self.acts).T, N=N, K=K, A=x, lda=K, B=w, ldb=N, b_mn=True, out=out, ldo=kw.pop('ldo', N), epi=epi,
                  out_dtype=self.act_dt if out_dtype is None else out_dtype, **kw)
 
     def dgrad_gemm(self, dy, N_out, w, K_in, out, epi=L.EPI_STORE, **kw):
@@ -287,9 +343,9 @@ class Engine:
     def colsum(self, t, N, out, ld=None):
         L.check(self.lib.progen_colsum(t.data_ptr(), N if ld is None else ld, L.dt(t), out.data_ptr(), self.T, N, L.stream()), 'colsum')
 
-    def ln_fwd(self, x, ldx, scale, y, ldy, mean, rstd, dcols, shift):
+    def ln_fwd(self, x, ldx, scale, y, ldy, mean, rstd, dcols, shift, acts=None):
         L.check(self.lib.progen_ln_shift_fwd(x.data_ptr(), ldx, L.dt(x), scale.data_ptr(), y.data_ptr(), ldy, L.dt(y),
-                                             mean.data_ptr(), rstd.data_ptr(), self.T, dcols, self.n, int(shift), L.stream()), 'ln_fwd')
+                                             mean.data_ptr(), rstd.data_ptr(), (acts or self.acts).T, dcols, self.n, int(shift), L.stream()), 'ln_fwd')
 
     # ------------------------------------------------------------------------------------------ forward
     def forward(self, ids):
@@ -300,60 +356,67 @@ class Engine:
         self._forward_device()
         return self.logits
 
-    def _forward_device(self):
+    def _forward_device(self, acts=None):
+        """forward pass on activation set `acts` (default: the training set, which keeps what the backward pass reads)"""
+        acts = self.acts if acts is None else acts
         lib, st = self.lib, L.stream()
-        cfg, d, I, hid, T, n = self.cfg, self.d, self.I, self.hid, self.T, self.n
+        cfg, d, I, hid, T, n = self.cfg, self.d, self.I, self.hid, acts.T, self.n
         shift = cfg['shift_tokens']
-        L.check(lib.progen_embed_fwd(self.tok.data_ptr(), self.Pf(P + 'embed', 'embeddings').data_ptr(), self.X[0].data_ptr(),
+        L.check(lib.progen_embed_fwd(acts.tok.data_ptr(), self.Pf(P + 'embed', 'embeddings').data_ptr(), acts.X[0].data_ptr(),
                                      T, d, self.V, st), 'embed_fwd')
         for i, kind in enumerate(self.kinds):
-            s = self.lay[i]
+            s = acts.lay[i]
             a, f = P + f'attn{i}/~/', P + f'ff{i}/~/'
-            x0, x1, x2 = self.X[2 * i], self.X[2 * i + 1], self.X[2 * i + 2]
+            # in place (inference): x0 = x1 = x2 is one buffer, and the residual epilogue without aux reads its output
+            x0, x1, x2 = acts.X[2 * i], acts.X[2 * i + 1], acts.X[2 * i + 2]
             # ---- LocalAttention (progen.py:73-103)
-            self.ln_fwd(x0, d, self.Pf(a + 'layer_norm', 'scale'), s['y1'], d, s['mean1'], s['rstd1'], d, shift)
+            self.ln_fwd(x0, d, self.Pf(a + 'layer_norm', 'scale'), s['y1'], d, s['mean1'], s['rstd1'], d, shift, acts=acts)
             self.fwd_gemm(s['y1'], d, self.W(a + 'linear', 'w'), 3 * I, s['qkv'], epi=L.EPI_ROTARY, rot_sin=self.rot_sin,
-                          rot_cos=self.rot_cos, seq_len=n, dim_head=self.dh)
-            self.attn_fwd(s['qkv'], s['att'], s['lse'])
+                          rot_cos=self.rot_cos, seq_len=n, dim_head=self.dh, acts=acts)
+            self.attn_fwd(s['qkv'], s['att'], s['lse'], acts=acts)
             self.fwd_gemm(s['att'], I, self.W(a + 'linear_1', 'w'), d, x1, epi=L.EPI_RESIDUAL, bias=self.Pf(a + 'linear_1', 'b'),
-                          aux=x0, ldaux=d)
-            # ---- FeedForward (progen.py:131-149)
-            self.ln_fwd(x1, d, self.Pf(f + 'layer_norm', 'scale'), s['y2'], d, s['mean2'], s['rstd2'], d, shift)
+                          aux=None if acts.inplace else x0, ldaux=d, acts=acts)
+            # ---- FeedForward (progen.py:131-149); s['u'] is None in the inference set: no pre-activation store
+            self.ln_fwd(x1, d, self.Pf(f + 'layer_norm', 'scale'), s['y2'], d, s['mean2'], s['rstd2'], d, shift, acts=acts)
             if kind == 'glu':
                 self.fwd_gemm(s['y2'], d, self.W(f + 'linear', 'w'), 2 * hid, s['hact'], epi=L.EPI_GLU, ldo=hid, out2=s['u'],
-                              ldo2=2 * hid, bias=self.Pf(f + 'linear', 'b'))
+                              ldo2=2 * hid, bias=self.Pf(f + 'linear', 'b'), acts=acts)
                 last, last_k = s['hact'], hid
             else:
                 self.fwd_gemm(s['y2'], d, self.W(f + 'linear', 'w'), hid, s['hact'], epi=L.EPI_GELU, out2=s['u'], ldo2=hid,
-                              bias=self.Pf(f + 'linear', 'b'))
+                              bias=self.Pf(f + 'linear', 'b'), acts=acts)
                 last, last_k = s['hact'], hid
             if kind == 'sgu':
                 half = hid // 2
                 g = f + 'sgu'
                 gate = s['hact'][:, half:]
-                self.ln_fwd(gate, hid, self.Pf(g + '/~/layer_norm', 'scale'), s['gn'], half, s['mean3'], s['rstd3'], half, False)
+                self.ln_fwd(gate, hid, self.Pf(g + '/~/layer_norm', 'scale'), s['gn'], half, s['mean3'], s['rstd3'], half, False,
+                            acts=acts)
                 # gate_b = tril(W) @ gn_b for every sequence b; masked K tiles are skipped (causal=1)
                 self._mm(M=n, N=half, K=n, A=self.wm[i], lda=n, B=s['gn'], ldb=half, b_mn=True, out=s['gp'], ldo=half,
-                         out_dtype=self.act_dt, batch=self.B, b_batch_rows=n, d_batch_rows=n, causal=1)
+                         out_dtype=self.act_dt, batch=acts.B, b_batch_rows=n, d_batch_rows=n, causal=1)
                 L.check(lib.progen_sgu_gate_fwd(s['hact'].data_ptr(), hid, s['gp'].data_ptr(), half,
                                                 self.Pf(g, 'spatial_biases').data_ptr(), s['sg'].data_ptr(), half, self.act_dt,
                                                 T, half, n, st), 'sgu_gate_fwd')
-                self.fwd_gemm(s['sg'], half, self.W(g + '/~/linear', 'w'), half, s['pj'], bias=self.Pf(g + '/~/linear', 'b'))
+                self.fwd_gemm(s['sg'], half, self.W(g + '/~/linear', 'w'), half, s['pj'], bias=self.Pf(g + '/~/linear', 'b'),
+                              acts=acts)
                 last, last_k = s['pj'], half
             self.fwd_gemm(last, last_k, self.W(f + 'linear_1', 'w'), d, x2, epi=L.EPI_RESIDUAL, bias=self.Pf(f + 'linear_1', 'b'),
-                          aux=x1, ldaux=d)
+                          aux=None if acts.inplace else x1, ldaux=d, acts=acts)
         # ---- to_logits (progen.py:219-222)
-        xl = self.X[-1]
-        self.ln_fwd(xl, d, self.Pf(P + 'layer_norm', 'scale'), self.yf, d, self.meanf, self.rstdf, d, False)
-        self.fwd_gemm(self.yf, d, self.W(P + 'linear', 'w'), self.V, self.logits, bias=self.Pf(P + 'linear', 'b'), out_dtype=L.F32)
+        xl = acts.X[-1]
+        self.ln_fwd(xl, d, self.Pf(P + 'layer_norm', 'scale'), acts.yf, d, acts.meanf, acts.rstdf, d, False, acts=acts)
+        self.fwd_gemm(acts.yf, d, self.W(P + 'linear', 'w'), self.V, acts.logits, bias=self.Pf(P + 'linear', 'b'), out_dtype=L.F32,
+                      acts=acts)
 
-    def attn_fwd(self, qkv, out, lse):
+    def attn_fwd(self, qkv, out, lse, acts=None):
+        B = (acts or self.acts).B
         if self.attn_tc:
             fn = self.lib.progen_local_attn_fwd_tc if self.attn_wgmma else self.lib.progen_local_attn_fwd
-            L.check(fn(qkv.data_ptr(), out.data_ptr(), lse.data_ptr(), self.B, self.n, self.w, self.h,
+            L.check(fn(qkv.data_ptr(), out.data_ptr(), lse.data_ptr(), B, self.n, self.w, self.h,
                                                    self.dh, L.stream()), 'local_attn_fwd')
             return
-        L.check(self.lib.progen_local_attn_fwd_simt(qkv.data_ptr(), out.data_ptr(), lse.data_ptr(), self.act_dt, self.B, self.n,
+        L.check(self.lib.progen_local_attn_fwd_simt(qkv.data_ptr(), out.data_ptr(), lse.data_ptr(), self.act_dt, B, self.n,
                                                     self.w, self.h, self.dh, L.stream()), 'local_attn_fwd')
 
     def attn_bwd(self, qkv, out, dout, lse, dqkv):
@@ -366,6 +429,55 @@ class Engine:
         L.check(self.lib.progen_local_attn_bwd_simt(qkv.data_ptr(), out.data_ptr(), dout.data_ptr(), lse.data_ptr(), dqkv.data_ptr(),
                                                     self.delta.data_ptr(), self.act_dt, self.B, self.n, self.w, self.h, self.dh,
                                                     L.stream()), 'local_attn_bwd')
+
+    # ------------------------------------------------------------------------------------------ scoring (inference)
+    def score(self, data, batch_size=64, tokens=False, embeddings=False):
+        """data: (N, n+1) integer rows (ids = data[:, :-1], labels = data[:, 1:], as in loss_and_grad) -> dict of numpy
+        arrays: log_likelihood [N] (sum of the label log-probabilities under the loss mask), num_tokens [N] (mask size);
+        token_logp [N, n] with `tokens`; embedding [N, d] (masked mean of the final LayerNorm output) with `embeddings`.
+        Runs the forward on the inference activation set, `batch_size` rows at a time: one H2D copy of the rows, the
+        forward, progen_token_logprob (+ progen_masked_mean_pool) and one D2H copy of the results per chunk."""
+        rows = torch.as_tensor(np.asarray(data).astype(np.int32)) if not isinstance(data, torch.Tensor) else data
+        rows = rows.to(device='cpu', dtype=torch.int32)
+        if rows.dim() != 2 or rows.shape[1] != self.n + 1:
+            raise L.ProgenError(f'score: rows must be (B, seq_len + 1 = {self.n + 1}), got {tuple(rows.shape)}')   # Q12
+        if batch_size < 1:
+            raise L.ProgenError(f'score: batch_size must be >= 1, got {batch_size}')
+        N, n, d = rows.shape[0], self.n, self.d
+        out = dict(log_likelihood=np.zeros(N, np.float32), num_tokens=np.zeros(N, np.int64))
+        if tokens:
+            out['token_logp'] = np.zeros((N, n), np.float32)
+        if embeddings:
+            out['embedding'] = np.zeros((N, d), np.float32)
+        if N == 0:
+            return out
+        full = self.inference_acts(min(batch_size, N))
+        lib, st = self.lib, L.stream()
+        for r0 in range(0, N, batch_size):
+            chunk = rows[r0:r0 + batch_size]
+            B = chunk.shape[0]
+            acts = full if B == full.B else full.view(B, n)
+            T = acts.T
+            acts.rows.copy_(chunk)
+            acts.tok.view(B, n).copy_(acts.rows[:, :-1])
+            acts.labels.view(B, n).copy_(acts.rows[:, 1:])
+            self._forward_device(acts)
+            # results, packed for one D2H copy: seq_ll [B] | seq_count [B] | logp [T] | embedding [B, d]
+            ll, cnt, lp, emb = full.res[:B], full.res[B:2 * B], full.res[2 * B:2 * B + T], full.res[2 * B + T:2 * B + T + B * d]
+            L.check(lib.progen_token_logprob(acts.logits.data_ptr(), L.F32, acts.labels.data_ptr(), lp.data_ptr(), ll.data_ptr(),
+                                             cnt.data_ptr(), B, n, self.V, st), 'token_logprob')
+            if embeddings:
+                L.check(lib.progen_masked_mean_pool(acts.yf.data_ptr(), d, self.act_dt, acts.labels.data_ptr(), emb.data_ptr(),
+                                                    B, n, d, st), 'masked_mean_pool')
+            used = 2 * B + (T + B * d if embeddings else T if tokens else 0)
+            host = full.res[:used].cpu().numpy()
+            out['log_likelihood'][r0:r0 + B] = host[:B]
+            out['num_tokens'][r0:r0 + B] = host[B:2 * B].astype(np.int64)
+            if tokens:
+                out['token_logp'][r0:r0 + B] = host[2 * B:2 * B + T].reshape(B, n)
+            if embeddings:
+                out['embedding'][r0:r0 + B] = host[2 * B + T:].reshape(B, d)
+        return out
 
     # ------------------------------------------------------------------------------------------ loss + backward
     def loss_and_grad(self, data, global_batch=None, zero_grads=True):

@@ -52,6 +52,8 @@ PROTOTYPES = {
     'progen_ln_shift_bwd': [_P, _LL, _I, _P, _LL, _I, _P, _P, _P, _P, _P, _LL, _P, _P, _LL, _I, _I, _I, _I, _P],
     'progen_colsum': [_P, _LL, _I, _P, _LL, _I, _P],
     'progen_ce_fwd_bwd': [_P, _I, _P, _P, _P, _P, _I, _I, _I, _I, _F, _P],
+    'progen_token_logprob': [_P, _I, _P, _P, _P, _P, _I, _I, _I, _P],
+    'progen_masked_mean_pool': [_P, _LL, _I, _P, _P, _I, _I, _I, _P],
     'progen_rotary_bwd': [_P, _LL, _I, _P, _P, _LL, _I, _I, _I, _P],
     'progen_local_attn_fwd_simt': [_P, _P, _P, _I, _I, _I, _I, _I, _I, _P],
     'progen_local_attn_bwd_simt': [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P],

@@ -7,7 +7,9 @@ interchange.  Everything below `.apply` runs as sm_90a kernels behind the C ABI 
 
 Beyond the reference surface: `.apply` also accepts a batch (B, n); `.loss_and_grad(params, data)` is the fused
 equivalent of `value_and_grad(get_loss_fn(model))` (utils.py:61-93); `.trainer(...)` owns device-resident training
-state (parameters, Adam moments, apply_every accumulator) for the train.py loop.
+state (parameters, Adam moments, apply_every accumulator) for the train.py loop; `.score(params, data)` is an
+inference-only forward returning per-sequence log-likelihoods (and optionally per-token log-probabilities and pooled
+embeddings).
 """
 import numpy as np
 import torch
@@ -102,6 +104,33 @@ class ProGen:
         self._ensure_loaded(params)
         loss = self.engine.loss_and_grad(data)
         return float(loss.item()), self.engine.export_grads()
+
+    def score(self, params, data, *, batch_size=64, return_tokens=False, return_embeddings=False):
+        """Log-likelihood of sequences under the model, without keeping any training state.
+        data: (B, n+1) integer rows, the contract of `loss_and_grad` and `data.collate`: ids = data[:, :-1] are fed to the
+        model, labels = data[:, 1:] are scored.  A label counts when it is not pad, plus the first pad (the end of the
+        sequence, quirk Q8: utils.py:54-56), so for a sequence of L residues the positions 0..L count.  Labels outside
+        [0, num_tokens) are clamped, as in the training loss.
+
+        Returns a dict of numpy arrays:
+          log_likelihood [B] float32: sum over the counted positions of log softmax(logits)[label];
+          num_tokens [B] int64: number of counted positions;
+          token_logp [B, n] float32 and token_mask [B, n] bool (with return_tokens): per-position log-probability (0 where
+            not counted) and the mask;
+          embedding [B, d] float32 (with return_embeddings): mean over the counted positions of the final-LayerNorm output,
+            the input of the logits head.
+        Per row, -log_likelihood / num_tokens is exactly the reference's `cross_entropy` (utils.py:45-59), the quantity
+        whose batch mean is the training loss.  `batch_size` rows run per forward pass; results do not depend on it."""
+        rows = torch.as_tensor(np.asarray(data).astype(np.int64) if not isinstance(data, torch.Tensor) else data)
+        if rows.dim() != 2 or rows.shape[-1] != self.config['seq_len'] + 1:
+            raise L.ProgenError(f"score: rows must be (B, seq_len + 1 = {self.config['seq_len'] + 1}), got {tuple(rows.shape)}")  # Q12
+        self._ensure_loaded(params)
+        out = self.engine.score(rows, batch_size=batch_size, tokens=return_tokens, embeddings=return_embeddings)
+        if return_tokens:
+            labels = rows[:, 1:].cpu().numpy()
+            pad = labels == 0
+            out['token_mask'] = ~pad | ((np.cumsum(pad, axis=-1) == 1) & pad)
+        return out
 
     def trainer(self, params, **optim_kwargs):
         from .trainer import Trainer
