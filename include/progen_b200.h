@@ -120,16 +120,9 @@ int progen_local_attn_bwd_simt(const void* qkv, const void* out, const void* dou
                                float* delta, int dtype, int B, int seq_len, int window, int heads, int dim_head,
                                void* stream);
 
-/* tensor-core version (bf16, dim_head 64, window % 64 == 0; mma.sync): flash-style, scores stay on chip; same buffers
- * as above.  The backward applies the rotary backward to dq|dk|dv in its epilogue. */
-int progen_local_attn_fwd(const void* qkv, void* out, float* lse, int B, int seq_len, int window, int heads, int dim_head,
-                          void* stream);
-int progen_local_attn_bwd(const void* qkv, const void* out, const void* dout, const float* lse, void* dqkv, float* delta,
-                          const float* rot_sin, const float* rot_cos, int B, int seq_len, int window, int heads, int dim_head,
-                          void* stream);
-
-/* Hopper version (bf16, dim_head 64, window % 128 == 0): the same algorithm with TMA-fed K/V (or Q/dO) tiles and wgmma;
- * same buffers as progen_local_attn_fwd / _bwd. */
+/* tensor-core version (bf16, dim_head 64, window % 64 == 0): flash-style with TMA-fed K/V (or Q/dO) tiles and wgmma,
+ * scores stay on chip; same buffers as above.  With rot_sin/rot_cos set, the backward applies the rotary backward to
+ * dq|dk|dv in its epilogue. */
 int progen_local_attn_fwd_tc(const void* qkv, void* out, float* lse, int B, int seq_len, int window, int heads, int dim_head,
                              void* stream);
 int progen_local_attn_bwd_tc(const void* qkv, const void* out, const void* dout, const float* lse, void* dqkv, float* delta,

@@ -1,6 +1,6 @@
 // Sliding-window causal attention with one look-back window (reference progen.py:88-102), CUDA-core version.
 // Exact fp32 arithmetic: this is the `mixed_precision=False` path and the on-device cross-check for the
-// tensor-core kernel (attn_mma.cu).  q, k, v are already rotated (qkv GEMM epilogue) and live in one [T, 3*I]
+// tensor-core kernels (attn_wgmma.cu).  q, k, v are already rotated (qkv GEMM epilogue) and live in one [T, 3*I]
 // buffer (q | k | v, each head-major), the output is [T, I].
 //
 // Query at position pos = win*w + i sees: the w keys of the previous window (for win == 0 these are w ZERO keys that

@@ -1,6 +1,5 @@
 // Sliding-window causal attention (reference progen.py:88-102) on Hopper warpgroup MMAs, bf16 in / fp32 accumulate,
-// dim_head 64.  Same algorithm and buffer contract as attn_mma.cu, which stays the path for windows that are not a
-// multiple of 128.
+// dim_head 64, any window that is a multiple of 64.  Same buffer contract as the exact-fp32 attn_simt.cu.
 //
 // One warpgroup (128 threads) per CTA owns a 64-row tile (queries in the forward and dQ kernels, keys in the dK/dV
 // kernel).  The streamed 64-row operand tiles arrive by TMA (128-byte swizzle) in a two-stage ring completed on mbarriers;
@@ -429,7 +428,7 @@ template <typename K> int prepare(K kern) {
 }
 
 int check_dims(const void* qkv, int B, int seq_len, int window, int heads, int dim_head) {
-  PG_CHECK_ARG(qkv != nullptr && B > 0 && heads > 0 && dim_head == DH && window % 128 == 0 && seq_len % window == 0);
+  PG_CHECK_ARG(qkv != nullptr && B > 0 && heads > 0 && dim_head == DH && window % TILE == 0 && seq_len % window == 0);
   PG_CHECK_ARG((long long)B * seq_len < (1ll << 31));
   return PROGEN_OK;
 }
@@ -438,7 +437,8 @@ int check_dims(const void* qkv, int B, int seq_len, int window, int heads, int d
 
 extern "C" {
 
-// bf16, dim_head == 64, window % 128 == 0.  qkv [T, 3*heads*64] (rotated), out [T, heads*64], lse [T, heads].
+// bf16, dim_head == 64, window % 64 == 0 (every tile lies inside one window).  qkv [T, 3*heads*64] (rotated),
+// out [T, heads*64], lse [T, heads].
 int progen_local_attn_fwd_tc(const void* qkv, void* out, float* lse, int B, int seq_len, int window, int heads, int dim_head,
                              void* stream) {
   int rc = check_dims(qkv, B, seq_len, window, heads, dim_head);

@@ -117,11 +117,10 @@ class Engine:
         self.act_dt = L.BF16 if self.mp else L.F32
         self.backend = L.BACKEND_TC if self.mp else L.BACKEND_SIMT
         self.kinds = layer_kinds(cfg['depth'], cfg['global_mlp_depth'], cfg['ff_glu'])
-        # tensor-core attention kernels: bf16, dim_head 64, 64-aligned windows (checked below — no silent CUDA-core fallback);
-        # the fp32 engine (mixed_precision=False) runs the exact CUDA-core kernels
-        self.attn_tc = self.mp
-        # wgmma kernels (attn_wgmma.cu) for windows that are multiples of 128, the mma.sync kernels (attn_mma.cu) otherwise
-        self.attn_wgmma = self.mp and cfg['window_size'] % 128 == 0
+        # tensor-core (wgmma) attention kernels: bf16, dim_head 64, 64-aligned windows (checked below — no silent CUDA-core
+        # fallback); the fp32 engine (mixed_precision=False) runs the exact CUDA-core kernels.  Two names for one flag
+        # because bench.py reads both.
+        self.attn_tc = self.attn_wgmma = self.mp
         d, n, w = cfg['dim'], cfg['seq_len'], cfg['window_size']
         self.d, self.n, self.w, self.V = d, n, w, cfg['num_tokens']
         self.h, self.dh = cfg['heads'], cfg['dim_head']
@@ -412,19 +411,17 @@ class Engine:
     def attn_fwd(self, qkv, out, lse, acts=None):
         B = (acts or self.acts).B
         if self.attn_tc:
-            fn = self.lib.progen_local_attn_fwd_tc if self.attn_wgmma else self.lib.progen_local_attn_fwd
-            L.check(fn(qkv.data_ptr(), out.data_ptr(), lse.data_ptr(), B, self.n, self.w, self.h,
-                                                   self.dh, L.stream()), 'local_attn_fwd')
+            L.check(self.lib.progen_local_attn_fwd_tc(qkv.data_ptr(), out.data_ptr(), lse.data_ptr(), B, self.n, self.w, self.h,
+                                                      self.dh, L.stream()), 'local_attn_fwd')
             return
         L.check(self.lib.progen_local_attn_fwd_simt(qkv.data_ptr(), out.data_ptr(), lse.data_ptr(), self.act_dt, B, self.n,
                                                     self.w, self.h, self.dh, L.stream()), 'local_attn_fwd')
 
     def attn_bwd(self, qkv, out, dout, lse, dqkv):
         if self.attn_tc:
-            fn = self.lib.progen_local_attn_bwd_tc if self.attn_wgmma else self.lib.progen_local_attn_bwd
-            L.check(fn(qkv.data_ptr(), out.data_ptr(), dout.data_ptr(), lse.data_ptr(), dqkv.data_ptr(),
-                                                   self.delta.data_ptr(), self.rot_sin.data_ptr(), self.rot_cos.data_ptr(), self.B,
-                                                   self.n, self.w, self.h, self.dh, L.stream()), 'local_attn_bwd')
+            L.check(self.lib.progen_local_attn_bwd_tc(qkv.data_ptr(), out.data_ptr(), dout.data_ptr(), lse.data_ptr(), dqkv.data_ptr(),
+                                                      self.delta.data_ptr(), self.rot_sin.data_ptr(), self.rot_cos.data_ptr(),
+                                                      self.B, self.n, self.w, self.h, self.dh, L.stream()), 'local_attn_bwd')
             return     # rotary backward is fused into the kernel's epilogue
         L.check(self.lib.progen_local_attn_bwd_simt(qkv.data_ptr(), out.data_ptr(), dout.data_ptr(), lse.data_ptr(), dqkv.data_ptr(),
                                                     self.delta.data_ptr(), self.act_dt, self.B, self.n, self.w, self.h, self.dh,

@@ -57,8 +57,6 @@ PROTOTYPES = {
     'progen_rotary_bwd': [_P, _LL, _I, _P, _P, _LL, _I, _I, _I, _P],
     'progen_local_attn_fwd_simt': [_P, _P, _P, _I, _I, _I, _I, _I, _I, _P],
     'progen_local_attn_bwd_simt': [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P],
-    'progen_local_attn_fwd': [_P, _P, _P, _I, _I, _I, _I, _I, _P],
-    'progen_local_attn_bwd': [_P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P],
     'progen_local_attn_fwd_tc': [_P, _P, _P, _I, _I, _I, _I, _I, _P],
     'progen_local_attn_bwd_tc': [_P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P],
     'progen_sgu_gate_fwd': [_P, _LL, _P, _LL, _P, _P, _LL, _I, _LL, _I, _I, _P],

@@ -14,7 +14,7 @@ timeout 900 compute-sanitizer --tool "$tool" --error-exitcode 9 --print-limit 20
 echo "decode: exit $? : $(grep -E 'ERROR SUMMARY|passed|failed' "$out/sanitize_${tool}_decode.log" | tail -n 2 | tr '\n' ' ')"
 # kernels the tiny model configs do not reach: many-tile / tail GEMMs (all epilogues), wgmma attention, streaming LN backward
 timeout 1200 compute-sanitizer --tool "$tool" --error-exitcode 9 --print-limit 20 \
-  python -m pytest tests/test_gpu_gemm_tc.py tests/test_gpu_attn_mma.py tests/test_gpu_elementwise.py -x -q -m gpu \
-  -k "many_tiles or column_tail or wgmma or stream_path" -p no:cacheprovider > "$out/sanitize_${tool}_kernels.log" 2>&1
+  python -m pytest tests/test_gpu_gemm_tc.py tests/test_gpu_attn_tc.py tests/test_gpu_elementwise.py -x -q -m gpu \
+  -k "many_tiles or column_tail or attn_tc or stream_path" -p no:cacheprovider > "$out/sanitize_${tool}_kernels.log" 2>&1
 echo "kernels: exit $? : $(grep -E 'ERROR SUMMARY|passed|failed' "$out/sanitize_${tool}_kernels.log" | tail -n 2 | tr '\n' ' ')"
 echo "logs in $out"
