@@ -1,0 +1,77 @@
+"""generate.py — sample many sequences per prompt from the newest checkpoint with the standard sampler.
+
+    python generate.py --checkpoint_path ./ckpts --prompt "[Tax=Mammalia] #" [--prompt ... | --prompts_file f.txt]
+        --num_samples 100 --temperature 1.0 [--top_k K] [--top_p 0.95] --seed 0 --batch_size 64 [--max_length L]
+        [--mixed_precision] --output samples.fasta
+
+Runs ProGen.generate: each prompt is laid out like training data (BOS, prompt), every sequence stops at its own EOS,
+temperature / top-k / nucleus (top-p) filtering happen in the persistent decode kernel.  Unlike sample.py (the reference
+drop-in, one sequence, top_k=25 with the reference's quirks), the result of a row depends only on the seed and the row.
+The FASTA has one record per row (row = prompt index * num_samples + sample index):
+    >{row} prompt={i} sample={j} log_likelihood={sum of log p of the generated tokens, EOS included} length={...} eos={0|1}
+    <generated residues, without the EOS; characters outside printable ASCII are written as '?'>"""
+import time
+
+import click
+import numpy as np
+
+from progen_b200 import ProGen
+from progen_b200.checkpoint import get_checkpoint_fns
+from progen_b200.data import decode_tokens
+
+
+def fasta_safe(residues):
+    """one character per token: anything outside printable ASCII (line breaks included) and a leading '>' become '?', so
+    every record stays two lines"""
+    s = ''.join(ch if ' ' <= ch <= '~' else '?' for ch in residues)
+    return '?' + s[1:] if s.startswith('>') else s
+
+
+@click.command()
+@click.option('--checkpoint_path', default='./ckpts')
+@click.option('--prompt', 'prompts', multiple=True, help='prompt text (repeatable)')
+@click.option('--prompts_file', default=None, help='text file, one prompt per line')
+@click.option('--num_samples', default=1, help='samples per prompt')
+@click.option('--temperature', default=1.0, help='softmax temperature; 0 = greedy')
+@click.option('--top_k', default=None, type=int, help='keep the k largest logits (ties kept)')
+@click.option('--top_p', default=None, type=float, help='nucleus: smallest set of tokens whose probability reaches top_p')
+@click.option('--seed', default=0)
+@click.option('--batch_size', default=64, help='sequences per kernel launch (<= 64)')
+@click.option('--max_length', default=None, type=int, help='BOS + prompt + generated tokens (default: seq_len)')
+@click.option('--mixed_precision', default=False, is_flag=True, help='bf16 weights in the decode kernel')
+@click.option('--output', default='samples.fasta')
+def main(checkpoint_path, prompts, prompts_file, num_samples, temperature, top_k, top_p, seed, batch_size, max_length,
+         mixed_precision, output):
+    _, get_last_checkpoint, _ = get_checkpoint_fns(checkpoint_path)
+    last_checkpoint = get_last_checkpoint()
+    if last_checkpoint is None:
+        exit(f'no checkpoints found at {checkpoint_path}')
+    params = last_checkpoint['params']
+    model_kwargs = last_checkpoint['model_config']
+    model = ProGen(**{**model_kwargs, 'mixed_precision': mixed_precision})
+    prompts = list(prompts)
+    if prompts_file is not None:
+        with open(prompts_file) as f:
+            prompts += [l.rstrip('\n') for l in f if l.strip()]
+    if not prompts:
+        prompts = ['']
+    print(f'sequence length: {model_kwargs["seq_len"]}')
+    t0 = time.perf_counter()
+    res = model.generate(params, prompts, num_samples=num_samples, temperature=temperature, top_k=top_k, top_p=top_p,
+                         max_length=max_length, seed=seed, batch_size=batch_size)
+    secs = time.perf_counter() - t0
+    N = len(res['length'])
+    with open(output, 'w') as f:
+        for row in range(N):
+            s, ln, fin = int(res['start'][row]), int(res['length'][row]), bool(res['finished'][row])
+            body = fasta_safe(decode_tokens(res['tokens'][row, s:s + ln - int(fin)]))
+            f.write(f'>{row} prompt={row // num_samples} sample={row % num_samples} '
+                    f'log_likelihood={res["log_likelihood"][row]:.6f} length={ln} eos={int(fin)}\n{body}\n')
+    gen = int(res['length'].sum())
+    print(f'{N} sequences, {gen} generated tokens, {int(res["finished"].sum())} ended with EOS')
+    print(f'{N / secs:.2f} sequences/s, {gen / secs:.0f} generated tokens/s (wall clock, including setup)')
+    print(f'wrote {output}')
+
+
+if __name__ == '__main__':
+    main()

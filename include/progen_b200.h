@@ -217,7 +217,7 @@ typedef struct progen_decode_run_t {
   const float* rot_sin;        /* [n, dim_head/2] */
   const float* rot_cos;
   const progen_decode_layer_t* layers;   /* device */
-  int32_t* seq;                /* [B, n] token ids; sampled ids are ADDED in place */
+  int32_t* seq;                /* [B, n] token ids; sampled ids are ADDED in place (sampler 0) or written (sampler 1) */
   const int32_t* start;        /* [B] first sampled position of each sequence */
   const float* noise;          /* [B, n, V] gumbel noise, or NULL for the greedy limit */
   float* logits_all;           /* [B, n, V] every step's logits (may be NULL) */
@@ -233,6 +233,24 @@ typedef struct progen_decode_run_t {
   uint32_t* grid_bar;          /* grid barrier counter */
   long long* prof;             /* optional [2][160][2] clock64 at entry / exit of every grid barrier of the launch's last
                                   step, for CTA 0 and the last CTA, then [160][8] marks inside CTA 0's phases (NULL: off) */
+  /* Sampler selector.  0: the reference sampler above (quirks Q5-Q7, `noise`, seq[b][p+1] += id).  1: the standard sampler:
+   * keep the logits >= the top_k-th largest (ties kept; top_k 0 = off), q = softmax(l / temperature) over them, keep the
+   * smallest prefix of the q-descending order (ties: lower id first) whose mass reaches top_p, draw the first maximal
+   * l / temperature + Gumbel over the kept ids (temperature 0: first maximal raw logit), seq[b][p+1] = id.  The Gumbel noise
+   * is Philox4x32-10 generated in the kernel: key (seed lo, seed hi), counter (c >> 2, p + 1, sample_id lo, sample_id hi),
+   * word c & 3 = x, u = (2 (x >> 9) + 1) 2^-24, g = -log(-log u).  Drawing id 0 (EOS) sets end[b] = p + 1 and counts the
+   * sequence in n_ended; it draws nothing after that (a row with no id to draw, all logits NaN, draws EOS).  When every sequence has ended the launch stops after that position's
+   * sampler phase. */
+  int32_t sampler;
+  float temperature;           /* sampler 1: >= 0, finite; 0 = greedy */
+  float top_p;                 /* sampler 1: (0, 1]; 1 = off */
+  int32_t _pad1;
+  uint64_t seed;               /* sampler 1: Philox key */
+  const int64_t* sample_id;    /* [B] sampler 1: each sequence's Philox stream */
+  float* token_logp;           /* [B, n] or NULL: log_softmax(logits[p])[seq[p+1]] at [b, p+1] for every drawn p+1 */
+  int32_t* end;                /* [B] sampler 1: position of the sampled EOS, n if none (initialised to n by the caller) */
+  int32_t* n_ended;            /* sampler 1: sequences that have sampled EOS (zeroed by the caller) */
+  int32_t* steps_run;          /* sampler 1: positions this launch consumed */
 } progen_decode_run_t;
 
 int progen_decode_run(const progen_decode_run_t* run, void* stream);

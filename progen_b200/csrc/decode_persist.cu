@@ -4,8 +4,10 @@
 // one cooperative kernel (one CTA per SM) generates every position of the
 // launch: the phases of a layer (LN + shift + QKV + rotary + cache | windowed attention | out-proj + residual | LN + shift +
 // FF-in + GLU/GELU | [gMLP: gate LN + causal spatial mix | SGU proj] | FF-out + residual) are separated by a grid barrier
-// (one atomic + one acquire poll per CTA), and the token loop, the sampler (top-k filter that keeps k-1 and zeroes the
-// rest, Gumbel-max, `seq[pos+1] += id` — quirks Q5/Q6) and the position counter stay on the device: no host round trip.
+// (one atomic + one acquire poll per CTA), and the token loop, the sampler and the position counter stay on the device: no
+// host round trip.  Sampler 0 is the reference's (top-k filter that keeps k-1 and zeroes the rest, Gumbel-max over host
+// noise, `seq[pos+1] += id` — quirks Q5/Q6); sampler 1 is the standard one (top-k, temperature, nucleus, in-kernel Philox
+// Gumbel noise, per-token log-probabilities, and an early exit once every sequence has sampled EOS).
 //
 // A position is ~65 dependent phases, so single-stream speed is LATENCY: a barrier is arrive -> prefetch -> wait, and between
 // the atomic and the poll every warp requests what does not depend on the other CTAs' output of the phase: its slice of the
@@ -23,6 +25,7 @@
 #include "common.cuh"
 #include "tc_ptx.cuh"
 #include "../../include/progen_b200.h"
+#include <cmath>
 #include <type_traits>
 
 namespace {
@@ -1134,7 +1137,8 @@ static __device__ void attention_phase_t(const progen_decode_run_t& r, const flo
 // running (max, sum, out) and the WP partials are merged through shared memory — no global partials, no atomics, no fences.
 // Two lanes per key for the logits (half a key row each: 32 registers at dim_head 64), lane = (key group, 4 channels) for
 // the value sum; every load of a slice is independent of the others.
-template <int NL>
+// PLAN: the number of sequences the work split is planned for (0: the launch's B; see run())
+template <int NL, int PLAN>
 static __device__ void attention_batch_t(const progen_decode_run_t& r, const float* kcache, const float* vcache, int pos, float* sq /* smem >= WPB * (2 dh + 4) */) {
   static_assert(NL >= 2, "two lanes share a key row");
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -1146,7 +1150,8 @@ static __device__ void attention_batch_t(const progen_decode_run_t& r, const flo
   const int nsl = (nreal + 15) / 16;
   const int npairs = r.B * r.heads;
   int WP = 8;
-  while (WP > 1 && (long long)npairs * WP > (long long)gridDim.x * WPB) WP >>= 1;
+  const int plan_pairs = PLAN > 0 ? PLAN * r.heads : npairs;
+  while (WP > 1 && (long long)plan_pairs * WP > (long long)gridDim.x * WPB) WP >>= 1;
   const int slots = WPB / WP, slot = warp / WP, sub = warp % WP;
   const int rounds = (npairs + gridDim.x * slots - 1) / (gridDim.x * slots);
   const float scale = rsqrtf((float)dh);
@@ -1242,12 +1247,13 @@ static __device__ void attention_batch_t(const progen_decode_run_t& r, const flo
     __syncthreads();
   }
 }
+template <int PLAN>
 static __device__ void attention_batch(const progen_decode_run_t& r, const float* kcache, const float* vcache, int pos, float* sq) {
   switch (r.dim_head) {
-    case 64: attention_batch_t<16>(r, kcache, vcache, pos, sq); break;
-    case 32: attention_batch_t<8>(r, kcache, vcache, pos, sq); break;
-    case 16: attention_batch_t<4>(r, kcache, vcache, pos, sq); break;
-    default: attention_batch_t<2>(r, kcache, vcache, pos, sq); break;
+    case 64: attention_batch_t<16, PLAN>(r, kcache, vcache, pos, sq); break;
+    case 32: attention_batch_t<8, PLAN>(r, kcache, vcache, pos, sq); break;
+    case 16: attention_batch_t<4, PLAN>(r, kcache, vcache, pos, sq); break;
+    default: attention_batch_t<2, PLAN>(r, kcache, vcache, pos, sq); break;
   }
 }
 
@@ -1266,16 +1272,18 @@ static __device__ void attention_phase(const progen_decode_run_t& r, const float
 // partial gate' goes to sg[split][b][c] (split 0 adds the current position's term and the bias); the SGU projection
 // phase multiplies xs with the sum of the partials while it stages its input (PRO_SGU).
 struct SguArgs { const float* ln_scale; const float* w; const float* b; float* hist; };
+template <int PLAN>
 static __device__ __forceinline__ int sgu_splits(const progen_decode_run_t& r) {
-  const int base = r.B * (r.hid / 2 / 128);
+  const int base = (PLAN > 0 ? PLAN : r.B) * (r.hid / 2 / 128);
   int s = (int)gridDim.x / (base > 0 ? base : 1);
   return s < 1 ? 1 : (s > MAXSPLIT ? MAXSPLIT : s);
 }
+template <int PLAN>
 static __device__ void sgu_phase(const progen_decode_run_t& r, const SguArgs& L, int pos, float* red /* smem [WPB][128] + stats */) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int C = r.hid / 2, n = r.n;
   const int cblocks = C / 128;
-  const int S = sgu_splits(r);
+  const int S = sgu_splits<PLAN>(r);
   const int tasks = r.B * cblocks * S;
   float* stat = red + WPB * 128;
   for (int t = blockIdx.x; t < tasks; t += gridDim.x) {
@@ -1426,6 +1434,171 @@ static __device__ void sample_phase(const progen_decode_run_t& r, int pos, float
   }
 }
 
+// ------------------------------------------------------------------------------------------------ standard sampler (sampler 1)
+// Philox4x32-10 (Salmon et al., SC'11): 10 rounds of the two 32 x 32 -> 64 multiplications, key bumped between rounds
+static __device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint32_t k0, uint32_t k1) {
+#pragma unroll
+  for (int i = 0; i < 10; ++i) {
+    if (i > 0) { k0 += 0x9E3779B9u; k1 += 0xBB67AE85u; }
+    const uint32_t lo0 = 0xD2511F53u * c.x, hi0 = __umulhi(0xD2511F53u, c.x);
+    const uint32_t lo1 = 0xCD9E8D57u * c.z, hi1 = __umulhi(0xCD9E8D57u, c.z);
+    c = make_uint4(hi1 ^ c.y ^ k0, lo1, hi0 ^ c.w ^ k1, lo0);
+  }
+  return c;
+}
+// Gumbel noise of token c at position p of the stream `sid` (the layout is spelled out in progen_b200.h; tests replay it)
+static __device__ __forceinline__ float philox_gumbel(unsigned long long seed, long long sid, int p, int c) {
+  const uint4 o = philox4x32_10(make_uint4((uint32_t)c >> 2, (uint32_t)p, (uint32_t)sid, (uint32_t)((unsigned long long)sid >> 32)),
+                                (uint32_t)seed, (uint32_t)(seed >> 32));
+  const uint32_t x = (c & 3) == 0 ? o.x : ((c & 3) == 1 ? o.y : ((c & 3) == 2 ? o.z : o.w));
+  const float u = (float)(2u * (x >> 9) + 1u) * 5.9604644775390625e-8f;        // (2 (x >> 9) + 1) 2^-24: exact, in (0, 1)
+  return -logf(-logf(u));
+}
+
+// Sampler 1 (one sequence per CTA, like sample_phase): top-k (ties at the k-th largest kept) -> softmax(l / T) -> nucleus
+// (smallest q-descending prefix reaching top_p) -> first maximal l / T + Gumbel over the kept ids; T == 0: first maximal raw
+// logit.  seq[p+1] = id (a write), token_logp = l[id] - logsumexp(l) (the unfiltered model at T = 1), id 0 ends the
+// sequence (end[b], one atomicAdd on n_ended).  Not inlined, and only reached through the uniform `sampler` branch, so its
+// registers stay out of the GEMV phases' allocation.  sv: shared memory [2 V]; red: the block-reduction scratch.
+static __device__ __noinline__ void sample_std_phase(const float* logits, int32_t* seq, const int32_t* start, int32_t* end, int32_t* n_ended,
+                                                     float* token_logp, float* logits_all, const float* embed, float* x,
+                                                     const int64_t* sample_id, int n, int V, int d, int B, int top_k, float temp,
+                                                     float top_p, unsigned long long seed, int pos, float* sv, float* red) {
+  static_assert(TPB >= 256, "V <= 512: at most two ids per thread");
+  const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  float* qv = sv + V;                                                          // kept ids: q; removed: -1
+  int* redi = reinterpret_cast<int*>(red + 32);
+  auto bsum = [&](float v) {                                                   // fixed order: independent of the grid
+    v = warp_sum(v);
+    __syncthreads();
+    if (lane == 0) red[warp] = v;
+    __syncthreads();
+    float s = 0.f;
+#pragma unroll
+    for (int k = 0; k < WPB; ++k) s += red[k];
+    return s;
+  };
+  auto bargmax = [&](float bv, int bi) {                                       // first maximal index
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) {
+      const float ov = __shfl_xor_sync(0xffffffffu, bv, off);
+      const int oi = __shfl_xor_sync(0xffffffffu, bi, off);
+      if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
+    }
+    __syncthreads();
+    if (lane == 0) { red[warp] = bv; redi[warp] = bi; }
+    __syncthreads();
+    float fv = red[0];
+    int fi = redi[0];
+#pragma unroll
+    for (int k = 1; k < WPB; ++k) {
+      const float ov = red[k];
+      const int oi = redi[k];
+      if (ov > fv || (ov == fv && oi < fi)) { fv = ov; fi = oi; }
+    }
+    return fi;
+  };
+  for (int b = blockIdx.x; b < B; b += gridDim.x) {
+    __syncthreads();
+    const float* lg = logits + (long long)b * V;
+    const long long row = (long long)b * n;
+    if (pos + 1 >= n) {
+      if (logits_all) for (int c = t; c < V; c += TPB) logits_all[(row + pos) * V + c] = __ldcg(lg + c);
+      continue;
+    }
+    int tok = seq[row + pos + 1];
+    const bool draw = pos + 1 >= start[b] && pos + 1 < end[b];                 // (after its EOS a sequence stays 0)
+    if (draw || logits_all) {
+      for (int c = t; c < V; c += TPB) {
+        const float v = __ldcg(lg + c);
+        sv[c] = v;
+        if (logits_all) logits_all[(row + pos) * V + c] = v;
+      }
+    }
+    if (draw) {
+      __syncthreads();
+      float m = -INFINITY;
+      for (int c = t; c < V; c += TPB) m = fmaxf(m, sv[c]);
+      m = warp_max(m);
+      __syncthreads();
+      if (lane == 0) red[warp] = m;
+      __syncthreads();
+      m = red[0];
+#pragma unroll
+      for (int k = 1; k < WPB; ++k) m = fmaxf(m, red[k]);
+      float s = 0.f;
+      for (int c = t; c < V; c += TPB) s += expf(sv[c] - m);
+      const float lse = m + logf(bsum(s));
+      int id;
+      if (temp == 0.f) {
+        float bv = -INFINITY;
+        int bi = 0x7fffffff;
+        for (int c = t; c < V; c += TPB) if (sv[c] > bv) { bv = sv[c]; bi = c; }
+        id = bargmax(bv, bi);
+      } else {
+        float kth = -INFINITY;
+        if (top_k > 0 && top_k < V) {
+          for (int c = t; c < V; c += TPB) {
+            const float v = sv[c];
+            int gt = 0, ge = 0;
+#pragma unroll 8
+            for (int j = 0; j < V; ++j) { const float u = sv[j]; gt += u > v; ge += u >= v; }
+            if (gt < top_k && top_k <= ge) red[48] = v;                        // the k-th largest value (with multiplicity)
+          }
+          __syncthreads();
+          kth = red[48];
+        }
+        const float mt = m / temp;                                              // the row maximum is always kept
+        float z = 0.f;
+        for (int c = t; c < V; c += TPB) if (sv[c] >= kth) z += expf(sv[c] / temp - mt);
+        z = bsum(z);
+        for (int c = t; c < V; c += TPB) qv[c] = sv[c] >= kth ? expf(sv[c] / temp - mt) / z : -1.f;
+        __syncthreads();
+        if (top_p < 1.f) {
+          // q-descending order = logit-descending order, ties by lower id; keep c iff the mass strictly before it < top_p
+          bool drop[2] = {false, false};
+#pragma unroll
+          for (int i = 0; i < 2; ++i) {
+            const int c = t + i * TPB;
+            if (c < V && qv[c] >= 0.f) {
+              const float v = sv[c];
+              float before = 0.f;
+              for (int j = 0; j < V; ++j) {
+                const float u = sv[j], qj = qv[j];
+                if (qj >= 0.f && (u > v || (u == v && j < c))) before += qj;
+              }
+              drop[i] = !(before < top_p);
+            }
+          }
+          __syncthreads();
+#pragma unroll
+          for (int i = 0; i < 2; ++i) if (drop[i]) qv[t + i * TPB] = -1.f;
+          __syncthreads();
+        }
+        float bv = -INFINITY;
+        int bi = 0x7fffffff;
+        const long long sid = sample_id[b];
+        for (int c = t; c < V; c += TPB) {
+          if (qv[c] < 0.f) continue;
+          const float sc = sv[c] / temp + philox_gumbel(seed, sid, pos + 1, c);
+          if (sc > bv) { bv = sc; bi = c; }
+        }
+        id = bargmax(bv, bi);
+      }
+      if (id >= V) id = 0;                                                      // no candidate compared (NaN logits): EOS
+      tok = id;
+      if (t == 0) {
+        seq[row + pos + 1] = id;
+        if (token_logp) token_logp[row + pos + 1] = sv[id] - lse;
+        if (id == 0) { end[b] = pos + 1; atomicAdd(n_ended, 1); }
+      }
+    }
+    const int id = tok < 0 ? 0 : (tok >= V ? V - 1 : tok);
+    for (int c = t * 4; c < d; c += TPB * 4)
+      *reinterpret_cast<float4*>(x + (long long)b * d + c) = *reinterpret_cast<const float4*>(embed + (long long)id * d + c);
+  }
+}
+
 enum { K_NONE = 0, K_GEMV = 1, K_ATT = 2, K_SGU = 3, K_SAMPLE = 4 };
 struct PhaseEnt { int kind, next; Phase ph; };     // next: table index of the following GEMV phase (weights to prefetch)
 static __host__ __device__ int num_phases(int depth) { return depth * 7 + 2; }
@@ -1500,7 +1673,8 @@ template <int BT, bool TCW> static constexpr size_t decode_smem_floats() {
   return (size_t)BT * TL::XP + TL::PART + TL::STATF + TL::WSM + WPB * 128 + 64;
 }
 
-template <int BT, typename TW>
+// STD: sampler 1 (a separate instantiation, so the sampler-0 kernels compile exactly as they do without it)
+template <int BT, typename TW, bool STD>
 static __device__ __forceinline__ void run(const progen_decode_run_t& r) {
   extern __shared__ __align__(16) float smem[];
   using TL = Tile<BT, sizeof(TW) == 2>;
@@ -1517,7 +1691,11 @@ static __device__ __forceinline__ void run(const progen_decode_run_t& r) {
   const int nph = num_phases(r.depth);
   constexpr bool MERGE_IN_ATT = BT > 1;
   const bool att_consumer = !MERGE_IN_ATT && r.inner <= 4 * TPB;
-  build_phase_table(r, tab, att_consumer, sgu_splits(r));
+  // The attention's warps per (sequence, head) and the SGU's split of the history range follow the number of sequences
+  // they are planned for.  Sampler 0 plans for the B of the launch.  Sampler 1 plans for the most sequences of the batch
+  // tile's class (1, 2-8, 9-64), so a row's arithmetic does not depend on how many rows share its launch.
+  constexpr int PLAN = STD ? (BT == 1 ? 1 : (BT <= 8 ? 8 : 64)) : 0;
+  build_phase_table(r, tab, att_consumer, sgu_splits<PLAN>(r));
   const bool use_tabs = BT == 1 && decode_smem_bytes<BT, sizeof(TW) == 2>(r.depth, true) <= MAX_SMEM;
   UnitEnt* utab = reinterpret_cast<UnitEnt*>((reinterpret_cast<uintptr_t>(tab + nph) + 15) & ~(uintptr_t)15);   // [nph][WSEGS]   (single stream only)
   FinEnt* ftab = reinterpret_cast<FinEnt*>(utab + (use_tabs ? nph * WSEGS : 0));
@@ -1579,11 +1757,14 @@ static __device__ __forceinline__ void run(const progen_decode_run_t& r) {
         prof_mark(pf, 3);
         have = fetch_next = !(e == nph - 2 && step + 1 == r.nsteps);
       } else if (kind == K_ATT) {
-        if (MERGE_IN_ATT || !att_consumer) attention_batch(r, tab[e].ph.kcache, tab[e].ph.vcache, pos, red);
+        if (MERGE_IN_ATT || !att_consumer) attention_batch<PLAN>(r, tab[e].ph.kcache, tab[e].ph.vcache, pos, red);
         else attention_phase(r, tab[e].ph.kcache, tab[e].ph.vcache, pos, red);
       } else if (kind == K_SGU) {
         const SguArgs sa{tab[e].ph.ln_scale, reinterpret_cast<const float*>(tab[e].ph.wt), tab[e].ph.bias, tab[e].ph.kcache};
-        sgu_phase(r, sa, pos, red);
+        sgu_phase<PLAN>(r, sa, pos, red);
+      } else if constexpr (STD) {
+        sample_std_phase(r.logits, r.seq, r.start, r.end, r.n_ended, r.token_logp, r.logits_all, r.embed, r.x, r.sample_id, r.n, r.V,
+                         d, B, r.top_k, r.temperature, r.top_p, r.seed, pos, xs, red);
       } else {
         sample_phase(r, pos, xs, red);
       }
@@ -1598,19 +1779,30 @@ static __device__ __forceinline__ void run(const progen_decode_run_t& r) {
         prof_mark(pf, 4);
       }
       grid_wait(r.grid_bar, round, pf, t0);
+      if (STD && kind == K_SAMPLE) {
+        // EOS early exit: the barrier above orders every CTA's count of this sampler phase before the read, and nothing
+        // writes the counter before the next sampler phase, so every CTA sees the same value and leaves together
+        int ended;
+        asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(ended) : "l"(r.n_ended) : "memory");
+        if (ended >= B) {
+          if (blockIdx.x == 0 && threadIdx.x == 0) *r.steps_run = step + 1;
+          return;
+        }
+      }
     }
   }
+  if (STD && blockIdx.x == 0 && threadIdx.x == 0) *r.steps_run = r.nsteps;
 }
 
 };  // struct Impl
 
-template <int BT, typename TW>
+template <int BT, typename TW, bool STD>
 __global__ void __launch_bounds__(threads_for(BT), 1) decode_persistent_kernel(const progen_decode_run_t r) {
-  Impl<threads_for(BT)>::template run<BT, TW>(r);
+  Impl<threads_for(BT)>::template run<BT, TW, STD>(r);
 }
 
-template <int BT, typename TW>
-int launch_run(const progen_decode_run_t& r, cudaStream_t s) {
+template <int BT, typename TW, bool STD>
+int launch_run_sampler(const progen_decode_run_t& r, cudaStream_t s) {
   using IM = Impl<threads_for(BT)>;
   using TL = typename IM::template Tile<BT, sizeof(TW) == 2>;
   constexpr int TPB = threads_for(BT);
@@ -1618,7 +1810,7 @@ int launch_run(const progen_decode_run_t& r, cudaStream_t s) {
   size_t smem = IM::template decode_smem_bytes<BT, sizeof(TW) == 2>(r.depth, BT == 1);
   if (smem > IM::MAX_SMEM) smem = IM::template decode_smem_bytes<BT, sizeof(TW) == 2>(r.depth, false);   // deep model: no unit tables
   PG_CHECK_ARG(smem <= IM::MAX_SMEM);                                  // (the phase table itself: depth * 7 + 2 entries)
-  auto kern = decode_persistent_kernel<BT, TW>;
+  auto kern = decode_persistent_kernel<BT, TW, STD>;
   static size_t set_for = 0;
   if (set_for < smem) {
     PG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -1632,6 +1824,10 @@ int launch_run(const progen_decode_run_t& r, cudaStream_t s) {
   PG_CUDA(cudaLaunchCooperativeKernel((void*)kern, dim3(grid), dim3(TPB), args, smem, s));
   __atomic_fetch_add(&g_progen_launches, 1ull, __ATOMIC_RELAXED);
   return PROGEN_OK;
+}
+template <int BT, typename TW>
+int launch_run(const progen_decode_run_t& r, cudaStream_t s) {
+  return r.sampler == 1 ? launch_run_sampler<BT, TW, true>(r, s) : launch_run_sampler<BT, TW, false>(r, s);
 }
 
 }  // namespace
@@ -1648,6 +1844,12 @@ int progen_decode_run(const progen_decode_run_t* r, void* stream) {
   PG_CHECK_ARG(r->window >= 1 && r->window <= 512);                    // <= 32 key slices per (sequence, head)
   PG_CHECK_ARG(r->pos0 >= 0 && r->pos0 + r->nsteps <= r->n);
   PG_CHECK_ARG(r->grid_bar != nullptr && r->att_count != nullptr && r->att_part != nullptr);
+  PG_CHECK_ARG(r->sampler == 0 || r->sampler == 1);
+  if (r->sampler == 1) {
+    PG_CHECK_ARG(std::isfinite(r->temperature) && r->temperature >= 0.f && r->top_p > 0.f && r->top_p <= 1.f);
+    PG_CHECK_ARG(r->top_k >= 0 && r->top_k <= r->V);
+    PG_CHECK_ARG(r->sample_id != nullptr && r->end != nullptr && r->n_ended != nullptr && r->steps_run != nullptr);
+  }
   if (r->nsteps == 0) return PROGEN_OK;
   cudaStream_t s = (cudaStream_t)stream;
   const bool bf = r->wdtype == PG_BF16;

@@ -33,7 +33,9 @@ class DecodeRun(C.Structure):
     _fields_ = [(k, _I) for k in ('n', 'd', 'heads', 'dim_head', 'inner', 'window', 'hid', 'V', 'depth', 'wdtype', 'shift_tokens',
                                   'top_k', 'B', 'pos0', 'nsteps', '_pad')] + \
                [(k, _P) for k in ('embed', 'lnf_scale', 'whead_t', 'bhead', 'rot_sin', 'rot_cos', 'layers', 'seq', 'start', 'noise',
-                                  'logits_all', 'x', 'q', 'att', 'att_part', 'att_count', 'u', 'sg', 'pj', 'logits', 'grid_bar', 'prof')]
+                                  'logits_all', 'x', 'q', 'att', 'att_part', 'att_count', 'u', 'sg', 'pj', 'logits', 'grid_bar', 'prof')] + \
+               [('sampler', _I), ('temperature', C.c_float), ('top_p', C.c_float), ('_pad1', _I), ('seed', C.c_uint64)] + \
+               [(k, _P) for k in ('sample_id', 'token_logp', 'end', 'n_ended', 'steps_run')]
 
 
 class BatchDecoder:
@@ -119,6 +121,7 @@ class BatchDecoder:
         m.u, m.sg, m.pj, m.logits = zeros(B, hid), zeros(8, B, hid // 2), zeros(B, hid // 2), zeros(B, self.V)
         self.grid_bar = torch.zeros(1, device=self.dev, dtype=torch.int32)
         m.grid_bar = self.grid_bar.data_ptr()
+        self._gen = None                                  # sampler-1 buffers, allocated by the first generate()
 
     def _hold(self, t):
         self.keep.append(t)
@@ -198,6 +201,78 @@ class BatchDecoder:
         out = seq * ~after_eos
         generated = int(sum(length - max(int(s), 1) for s in starts))
         return (out[0] if single else out), generated, e0.elapsed_time(e1) / 1e3
+
+    def generate(self, prompts, *, temperature=1.0, top_k=None, top_p=None, seed=0, sample_ids=None, max_length=None):
+        """The standard sampler (sampler 1 of csrc/decode_persist.cu) for up to B prompts (integer arrays of ids in [1, V)).
+        Each row is laid out as training data is, [0 (BOS), prompt..., 0...], and draws positions 1 + len(prompt) ..
+        max_length - 1 until it samples EOS (id 0).  Row b uses the Philox stream sample_ids[b] (default b); the
+        attention and SGU work splits are planned for the largest launch of the batch tile's class (1, 8 or 64 rows), so
+        a row's result depends on (seed, its sample id) and that class, not on the other rows of the launch.  Fewer prompts than B run on a prefix of the caches.
+        Returns a dict of numpy arrays: ids [R, n] int64, token_logp [R, n] float32 (log p(ids[t] | ids[:t]) at drawn t,
+        else 0), end [R] int32 (position of the EOS, n if none), start [R] int32; and steps_run (positions the last
+        launch consumed before every row had ended, or its full length) and device_s (that launch's device time)."""
+        n = self.n
+        max_length = n if max_length is None else int(max_length)
+        R = len(prompts)
+        if not 1 <= R <= self.B:
+            raise L.ProgenError(f'generate: 1 <= prompts <= {self.B}')
+        if not 2 <= max_length <= n:
+            raise L.ProgenError(f'generate: 2 <= max_length <= {n}')
+        if top_k is not None and not 1 <= int(top_k) <= self.V:
+            raise L.ProgenError(f'generate: 1 <= top_k <= {self.V}')
+        if top_p is not None and not 0.0 < float(top_p) <= 1.0:
+            raise L.ProgenError('generate: 0 < top_p <= 1')
+        if not (np.isfinite(temperature) and temperature >= 0):
+            raise L.ProgenError('generate: temperature must be finite and >= 0')
+        seq0 = np.zeros((R, n), np.int32)
+        starts = np.zeros(R, np.int32)
+        for b, pr in enumerate(prompts):
+            pr = np.asarray(pr, np.int64).reshape(-1)
+            if len(pr) + 1 >= max_length:
+                raise L.ProgenError(f'generate: a prompt of {len(pr)} ids leaves no position before max_length {max_length}')
+            if len(pr) and (pr.min() < 1 or pr.max() >= self.V):
+                raise L.ProgenError(f'generate: prompt ids must lie in [1, {self.V})')
+            seq0[b, 1:1 + len(pr)] = pr
+            starts[b] = 1 + len(pr)
+        sids = np.arange(R, dtype=np.int64) if sample_ids is None else np.asarray(sample_ids, np.int64).reshape(-1)
+        if sids.shape != (R,):
+            raise L.ProgenError('generate: one sample id per prompt')
+        if self._gen is None:
+            z = lambda *s, dtype: torch.zeros(*s, device=self.dev, dtype=dtype)
+            self._gen = dict(sample_id=z(self.B, dtype=torch.int64), token_logp=z(self.B, n, dtype=torch.float32),
+                             end=z(self.B, dtype=torch.int32), counters=z(2, dtype=torch.int32))
+        gb = self._gen
+        self.reset()
+        self.seq[:R].copy_(torch.as_tensor(seq0))
+        self.start[:R].copy_(torch.as_tensor(starts))
+        gb['sample_id'][:R].copy_(torch.as_tensor(sids))
+        gb['token_logp'].zero_()
+        gb['end'].fill_(n)
+        gb['counters'].zero_()                            # [n_ended, steps_run]
+        m = self.m
+        m.B, m.sampler = R, 1
+        m.temperature = float(temperature)
+        m.top_k = int(top_k) if top_k is not None else 0
+        m.top_p = float(top_p) if top_p is not None else 1.0
+        m.seed = int(seed) & 0xFFFFFFFFFFFFFFFF
+        m.sample_id, m.token_logp, m.end = gb['sample_id'].data_ptr(), gb['token_logp'].data_ptr(), gb['end'].data_ptr()
+        m.n_ended, m.steps_run = gb['counters'].data_ptr(), gb['counters'].data_ptr() + 4
+        try:
+            first = int(starts.min()) - 1                 # the first drawn position is start; it reads the logits of start - 1
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            if first > 0:
+                self.run(0, first)                        # prefill: only advances the caches
+            e0.record()
+            self.run(first, max_length - 1 - first)       # positions first .. max_length - 2 (the last writes max_length - 1)
+            e1.record()
+            torch.cuda.synchronize()
+        finally:
+            m.B, m.sampler, m.top_k = self.B, 0, 0
+            m.temperature, m.top_p, m.seed = 0.0, 0.0, 0
+            m.sample_id = m.token_logp = m.end = m.n_ended = m.steps_run = 0
+        return dict(ids=self.seq[:R].cpu().numpy().astype(np.int64), token_logp=gb['token_logp'][:R].cpu().numpy(),
+                    end=gb['end'][:R].cpu().numpy(), start=starts, steps_run=int(gb['counters'][1].item()),
+                    device_s=e0.elapsed_time(e1) / 1e3)
 
 
 class Decoder:

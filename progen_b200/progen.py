@@ -39,6 +39,7 @@ class ProGen:
         self.mixed_precision = bool(mixed_precision)
         self._engine = None
         self._loaded = None
+        self._gen_decoder = self._gen_params = None
 
     # ---- engine (created lazily so that constructing a model does not need a GPU; using it does)
     @property
@@ -131,6 +132,109 @@ class ProGen:
             pad = labels == 0
             out['token_mask'] = ~pad | ((np.cumsum(pad, axis=-1) == 1) & pad)
         return out
+
+    def generate(self, params, prompts, *, num_samples=1, temperature=1.0, top_k=None, top_p=None, max_length=None, seed=0,
+                 batch_size=64):
+        """Sample sequences with the standard sampler of the persistent decode kernel (temperature, top-k with ties kept,
+        nucleus top-p, in-kernel Philox Gumbel noise; csrc/decode_persist.cu), stopping each sequence at its EOS.
+        Unlike the reference sampler (utils.sample, sample.py), a prompt is laid out as training data is: BOS (0), the
+        prompt, then the generated residues; an empty prompt draws its first residue from the BOS logits.
+
+        prompts: a string, or a list of strings (encoded like training text) or of integer id arrays (ids in [1, V)).
+        Rows are prompt-major: row i * num_samples + j is sample j of prompt i and draws from Philox stream (seed, row).
+        Rows run min(batch_size, N) (<= 64) at a time in one persistent kernel.  The kernel's arithmetic depends on the
+        class of that launch size, 1, 2-8 or 9-64 rows, and on the GPU's SM count, but not on the size within the class:
+        on one GPU model a row is bitwise the same for every batch_size of the same class and every chunking (a ragged last
+        chunk is padded to the class).  Rows of different classes agree to fp32 round-off, so ids can differ where a draw
+        is that close.  max_length (default seq_len) bounds BOS + prompt + generated tokens;
+        temperature 0 is greedy (first maximal logit; top_k / top_p ignored).
+
+        Returns a dict of numpy arrays over the N = len(prompts) * num_samples rows:
+          tokens [N, seq_len] int64: BOS, prompt, generated tokens, EOS, zeros;
+          start [N] int64: position of the first generated token (1 + prompt length);
+          length [N] int64: generated tokens, EOS included;
+          finished [N] bool: an EOS was drawn before max_length;
+          log_likelihood [N] float64: sum of token_logp over the generated positions;
+          token_logp [N, seq_len] float32: log p(tokens[t] | tokens[:t]) under the unfiltered model (temperature 1) at
+            generated t, 0 elsewhere — the quantity `score` reports;
+          prompt_index [N] int64."""
+        cfg = self.config
+        V, n = cfg['num_tokens'], cfg['seq_len']
+
+        def integer(v, what, lo, hi):
+            if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, np.integer)) or not lo <= int(v) <= hi:
+                raise L.ProgenError(f'generate: {what} must be an integer in [{lo}, {hi}], got {v!r}')
+            return int(v)
+
+        max_length = n if max_length is None else integer(max_length, 'max_length', 2, n)
+        num_samples = integer(num_samples, 'num_samples', 1, 1 << 40)
+        batch_size = integer(batch_size, 'batch_size', 1, 64)
+        seed = integer(seed, 'seed', 0, (1 << 64) - 1)
+        top_k = None if top_k is None else integer(top_k, 'top_k', 1, V)
+        try:
+            temperature = float(temperature)
+            top_p = None if top_p is None else float(top_p)
+        except (TypeError, ValueError):
+            raise L.ProgenError('generate: temperature and top_p must be numbers') from None
+        if not (np.isfinite(temperature) and temperature >= 0.0):
+            raise L.ProgenError(f'generate: temperature must be finite and >= 0, got {temperature}')
+        if top_p is not None and not 0.0 < top_p <= 1.0:
+            raise L.ProgenError(f'generate: top_p must lie in (0, 1], got {top_p}')
+        from .data import encode_tokens
+        if isinstance(prompts, (str, bytes)):
+            prompts = [prompts]
+        if not isinstance(prompts, (list, tuple)) or len(prompts) == 0:
+            raise L.ProgenError('generate: prompts must be a string or a non-empty list of strings or id arrays')
+        ids = []
+        for p in prompts:
+            a = np.asarray(encode_tokens(p.decode() if isinstance(p, bytes) else p) if isinstance(p, (str, bytes)) else p)
+            if a.ndim != 1 or (a.size and not np.issubdtype(a.dtype, np.integer)):
+                raise L.ProgenError('generate: a prompt must be a string or a 1-D integer array')
+            a = a.astype(np.int64)
+            if a.size and (a.min() < 1 or a.max() >= V):
+                raise L.ProgenError(f'generate: prompt ids must lie in [1, {V}) (0 is BOS / EOS)')
+            if a.size + 1 >= max_length:
+                raise L.ProgenError(f'generate: a prompt of {a.size} ids leaves nothing to generate before max_length {max_length}')
+            ids.append(a)
+        N = len(ids) * num_samples
+        rows = [ids[r // num_samples] for r in range(N)]
+        per_launch = min(batch_size, N)
+        # a ragged last chunk is padded with copies of its last row (same prompt and stream, so it ends when that row does)
+        # up to the smallest size that runs the same GEMV formulation as the full chunks
+        min_rows = 9 if per_launch > 8 else (2 if per_launch > 1 else 1)
+        dec = self._generate_decoder(params, per_launch)
+        out = dict(tokens=np.zeros((N, n), np.int64), start=np.zeros(N, np.int64), end=np.zeros(N, np.int64),
+                   token_logp=np.zeros((N, n), np.float32))
+        for r0 in range(0, N, per_launch):
+            r1 = min(N, r0 + per_launch)
+            pad = max(0, min_rows - (r1 - r0))
+            chunk = rows[r0:r1] + [rows[r1 - 1]] * pad
+            sids = np.concatenate([np.arange(r0, r1), np.full(pad, r1 - 1)]).astype(np.int64)
+            res = dec.generate(chunk, temperature=temperature, top_k=top_k, top_p=top_p, seed=seed, sample_ids=sids,
+                               max_length=max_length)
+            out['tokens'][r0:r1] = res['ids'][:r1 - r0]
+            out['token_logp'][r0:r1] = res['token_logp'][:r1 - r0]
+            out['start'][r0:r1] = res['start'][:r1 - r0]
+            out['end'][r0:r1] = res['end'][:r1 - r0]
+        end = out.pop('end')
+        out['finished'] = end < max_length
+        out['length'] = np.where(out['finished'], end + 1, max_length) - out['start']
+        out['log_likelihood'] = out['token_logp'].astype(np.float64).sum(axis=-1)
+        out['prompt_index'] = np.arange(N, dtype=np.int64) // num_samples
+        return out
+
+    def _generate_decoder(self, params, batch):
+        """The BatchDecoder of `generate`, kept across calls with the same parameters (like `_ensure_loaded`); rebuilt when
+        a call needs more rows per launch than it holds."""
+        import torch
+        from .decode import BatchDecoder
+        dec = self._gen_decoder
+        if dec is None or self._gen_params is not params or dec.B < batch:
+            self._gen_decoder = None
+            dec = BatchDecoder(self.config, params, batch=batch,
+                               weights_dtype=torch.bfloat16 if self.mixed_precision else torch.float32)
+            self._gen_decoder, self._gen_params = dec, params
+        return dec
 
     def trainer(self, params, **optim_kwargs):
         from .trainer import Trainer

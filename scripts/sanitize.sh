@@ -12,6 +12,12 @@ timeout 900 compute-sanitizer --tool "$tool" --error-exitcode 9 --print-limit 20
   python -m pytest tests/test_gpu_decode.py -x -q -m gpu -k "test_decode_logits_match_oracle_forward" \
   -p no:cacheprovider > "$out/sanitize_${tool}_decode.log" 2>&1
 echo "decode: exit $? : $(grep -E 'ERROR SUMMARY|passed|failed' "$out/sanitize_${tool}_decode.log" | tail -n 2 | tr '\n' ' ')"
+# the standard sampler at 1, 2 and 24 rows (the BT 1, 8 and 32 kernels): shared-memory filter, Philox noise, the EOS
+# counter and the early exit (every row of the 24 ends)
+timeout 900 compute-sanitizer --tool "$tool" --error-exitcode 9 --print-limit 20 \
+  python -m pytest tests/test_gpu_generate.py -x -q -m gpu -k "test_reference_sampler_unaffected_by_generate or test_eos_ends_sequences_and_the_launch" \
+  -p no:cacheprovider > "$out/sanitize_${tool}_generate.log" 2>&1
+echo "generate: exit $? : $(grep -E 'ERROR SUMMARY|passed|failed' "$out/sanitize_${tool}_generate.log" | tail -n 2 | tr '\n' ' ')"
 # kernels the tiny model configs do not reach: many-tile / tail GEMMs (all epilogues), wgmma attention, streaming LN backward
 timeout 1200 compute-sanitizer --tool "$tool" --error-exitcode 9 --print-limit 20 \
   python -m pytest tests/test_gpu_gemm_tc.py tests/test_gpu_attn_tc.py tests/test_gpu_elementwise.py -x -q -m gpu \
