@@ -2,10 +2,14 @@
 
     python generate.py --checkpoint_path ./ckpts --prompt "[Tax=Mammalia] #" [--prompt ... | --prompts_file f.txt]
         --num_samples 100 --temperature 1.0 [--top_k K] [--top_p 0.95] --seed 0 --batch_size 64 [--max_length L]
+        [--alphabet ACDEFGHIKLMNPQRSTVWY] [--min_new_tokens N] [--repetition_penalty 1.2 --repetition_window 16]
         [--mixed_precision] --output samples.fasta
 
 Runs ProGen.generate: each prompt is laid out like training data (BOS, prompt), every sequence stops at its own EOS,
-temperature / top-k / nucleus (top-p) filtering happen in the persistent decode kernel.  Unlike sample.py (the reference
+temperature / top-k / nucleus (top-p) filtering happen in the persistent decode kernel.  --alphabet restricts every
+draw to those residues and EOS, --min_new_tokens forbids EOS for the first N generated tokens, and --repetition_penalty
+penalises the residues present in the last --repetition_window positions (0: the whole sequence); these act on the
+logits in the kernel and leave the reported log-likelihood that of the unconstrained model.  Unlike sample.py (the reference
 drop-in, one sequence, top_k=25 with the reference's quirks), the result of a row depends only on the seed and the row.
 The FASTA has one record per row (row = prompt index * num_samples + sample index):
     >{row} prompt={i} sample={j} log_likelihood={sum of log p of the generated tokens, EOS included} length={...} eos={0|1}
@@ -17,7 +21,8 @@ import numpy as np
 
 from progen_b200 import ProGen
 from progen_b200.checkpoint import get_checkpoint_fns
-from progen_b200.data import decode_tokens
+from progen_b200.data import decode_tokens, encode_tokens
+from progen_b200.lib import ProgenError
 
 
 def fasta_safe(residues):
@@ -25,6 +30,19 @@ def fasta_safe(residues):
     every record stays two lines"""
     s = ''.join(ch if ' ' <= ch <= '~' else '?' for ch in residues)
     return '?' + s[1:] if s.startswith('>') else s
+
+
+def alphabet_bias(alphabet, num_tokens):
+    """logit bias that leaves EOS and the characters of `alphabet` (encoded like training text) as the only candidates"""
+    ids = np.asarray(encode_tokens(alphabet), np.int64)
+    if ids.size == 0 or ids.min() < 1 or ids.max() >= num_tokens:
+        bad = [ch for ch in alphabet if not 1 <= ord(ch) + 1 < num_tokens]
+        raise ProgenError(f'--alphabet: characters outside the {num_tokens}-token vocabulary: {bad!r}' if bad else
+                          '--alphabet: empty')
+    bias = np.full(num_tokens, -np.inf, np.float32)
+    bias[0] = 0.0
+    bias[ids] = 0.0
+    return bias
 
 
 @click.command()
@@ -38,10 +56,14 @@ def fasta_safe(residues):
 @click.option('--seed', default=0)
 @click.option('--batch_size', default=64, help='sequences per kernel launch (<= 64)')
 @click.option('--max_length', default=None, type=int, help='BOS + prompt + generated tokens (default: seq_len)')
+@click.option('--alphabet', default=None, help='the only residue characters that may be drawn (EOS is always allowed)')
+@click.option('--min_new_tokens', default=0, help='generated tokens before EOS may be drawn')
+@click.option('--repetition_penalty', default=1.0, help='divide positive / multiply negative logits of recent ids (1 = off)')
+@click.option('--repetition_window', default=0, help='positions the repetition penalty looks back (0 = the whole sequence)')
 @click.option('--mixed_precision', default=False, is_flag=True, help='bf16 weights in the decode kernel')
 @click.option('--output', default='samples.fasta')
 def main(checkpoint_path, prompts, prompts_file, num_samples, temperature, top_k, top_p, seed, batch_size, max_length,
-         mixed_precision, output):
+         alphabet, min_new_tokens, repetition_penalty, repetition_window, mixed_precision, output):
     _, get_last_checkpoint, _ = get_checkpoint_fns(checkpoint_path)
     last_checkpoint = get_last_checkpoint()
     if last_checkpoint is None:
@@ -49,6 +71,7 @@ def main(checkpoint_path, prompts, prompts_file, num_samples, temperature, top_k
     params = last_checkpoint['params']
     model_kwargs = last_checkpoint['model_config']
     model = ProGen(**{**model_kwargs, 'mixed_precision': mixed_precision})
+    bias = None if alphabet is None else alphabet_bias(alphabet, model.config['num_tokens'])
     prompts = list(prompts)
     if prompts_file is not None:
         with open(prompts_file) as f:
@@ -58,7 +81,9 @@ def main(checkpoint_path, prompts, prompts_file, num_samples, temperature, top_k
     print(f'sequence length: {model_kwargs["seq_len"]}')
     t0 = time.perf_counter()
     res = model.generate(params, prompts, num_samples=num_samples, temperature=temperature, top_k=top_k, top_p=top_p,
-                         max_length=max_length, seed=seed, batch_size=batch_size)
+                         max_length=max_length, seed=seed, batch_size=batch_size, logit_bias=bias,
+                         min_new_tokens=min_new_tokens, repetition_penalty=repetition_penalty,
+                         repetition_window=repetition_window)
     secs = time.perf_counter() - t0
     N = len(res['length'])
     with open(output, 'w') as f:

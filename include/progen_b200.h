@@ -251,6 +251,19 @@ typedef struct progen_decode_run_t {
   int32_t* end;                /* [B] sampler 1: position of the sampled EOS, n if none (initialised to n by the caller) */
   int32_t* n_ended;            /* sampler 1: sequences that have sampled EOS (zeroed by the caller) */
   int32_t* steps_run;          /* sampler 1: positions this launch consumed */
+  /* Sampler-1 constraints, per-draw transforms of the logits l at p before the filter above (sampler 0: neutral only).
+   * token_logp stays l[id] - logsumexp(l) of the raw logits.  In fp32: a[c] = l[c] > 0 ? l[c] / repetition_penalty :
+   * l[c] * repetition_penalty for every id c present in seq[b] at positions max(1, p + 1 - W) .. p (W = repetition_window,
+   * 0 = the whole row; BOS excluded; each id counts once), else a[c] = l[c]; then a += logit_bias (-inf bans an id); then
+   * a[0] = -inf while p + 1 < start[b] + min_new_tokens.  The candidates are the ids whose a is neither -inf nor NaN; the
+   * filter and the draw above run on a over them (the softmax maximum is the candidates' maximum of a), and a row with
+   * none draws EOS.  Off (the unconstrained code) when logit_bias is NULL, repetition_penalty is 1 and min_new_tokens is
+   * 0; a zero-initialised struct must set repetition_penalty to 1. */
+  const float* logit_bias;     /* [V] or NULL */
+  float repetition_penalty;    /* finite, > 0; 1 = off */
+  int32_t repetition_window;   /* >= 0; 0 = every position since BOS */
+  int32_t min_new_tokens;      /* >= 0: the first min_new_tokens draws of a row are never EOS */
+  int32_t _pad2;
 } progen_decode_run_t;
 
 int progen_decode_run(const progen_decode_run_t* run, void* stream);

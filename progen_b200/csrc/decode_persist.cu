@@ -1460,14 +1460,28 @@ static __device__ __forceinline__ float philox_gumbel(unsigned long long seed, l
 // logit.  seq[p+1] = id (a write), token_logp = l[id] - logsumexp(l) (the unfiltered model at T = 1), id 0 ends the
 // sequence (end[b], one atomicAdd on n_ended).  Not inlined, and only reached through the uniform `sampler` branch, so its
 // registers stay out of the GEMV phases' allocation.  sv: shared memory [2 V]; red: the block-reduction scratch.
+// Constraints (progen_b200.h): after logsumexp of the raw logits, sv is overwritten with the adjusted logits a, and the
+// filter and draw below run on a unchanged: -inf and NaN never win a comparison, so only candidates can be drawn.
+struct SampleCons { const float* bias; float theta; int window, min_new; };  // one argument: fewer registers at the call
 static __device__ __noinline__ void sample_std_phase(const float* logits, int32_t* seq, const int32_t* start, int32_t* end, int32_t* n_ended,
                                                      float* token_logp, float* logits_all, const float* embed, float* x,
                                                      const int64_t* sample_id, int n, int V, int d, int B, int top_k, float temp,
-                                                     float top_p, unsigned long long seed, int pos, float* sv, float* red) {
+                                                     float top_p, unsigned long long seed, SampleCons cs, int pos, float* sv, float* red) {
   static_assert(TPB >= 256, "V <= 512: at most two ids per thread");
   const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
   float* qv = sv + V;                                                          // kept ids: q; removed: -1
   int* redi = reinterpret_cast<int*>(red + 32);
+  const bool cons = cs.bias != nullptr || cs.theta != 1.f || cs.min_new != 0;  // uniform
+  auto bmax = [&](float m) {
+    m = warp_max(m);
+    __syncthreads();
+    if (lane == 0) red[warp] = m;
+    __syncthreads();
+    m = red[0];
+#pragma unroll
+    for (int k = 1; k < WPB; ++k) m = fmaxf(m, red[k]);
+    return m;
+  };
   auto bsum = [&](float v) {                                                   // fixed order: independent of the grid
     v = warp_sum(v);
     __syncthreads();
@@ -1519,16 +1533,36 @@ static __device__ __noinline__ void sample_std_phase(const float* logits, int32_
       __syncthreads();
       float m = -INFINITY;
       for (int c = t; c < V; c += TPB) m = fmaxf(m, sv[c]);
-      m = warp_max(m);
-      __syncthreads();
-      if (lane == 0) red[warp] = m;
-      __syncthreads();
-      m = red[0];
-#pragma unroll
-      for (int k = 1; k < WPB; ++k) m = fmaxf(m, red[k]);
+      m = bmax(m);
       float s = 0.f;
       for (int c = t; c < V; c += TPB) s += expf(sv[c] - m);
       const float lse = m + logf(bsum(s));
+      if (cons) {
+        // presence flags of the ids at positions max(1, p + 1 - W) .. p, in the q half (filled only after this)
+        int* seen = reinterpret_cast<int*>(qv);
+        const bool pen = cs.theta != 1.f;
+        if (pen) {
+          for (int c = t; c < V; c += TPB) seen[c] = 0;
+          __syncthreads();
+          for (int j = (cs.window > 0 ? max(1, pos + 1 - cs.window) : 1) + t; j <= pos; j += TPB) {
+            const int c = __ldcg(seq + row + j);
+            if (c >= 0 && c < V) seen[c] = 1;
+          }
+          __syncthreads();
+        }
+        const bool no_eos = pos + 1 < start[b] + cs.min_new;
+        float ma = -INFINITY;
+        for (int c = t; c < V; c += TPB) {
+          float a = sv[c];
+          if (pen && seen[c]) a = a > 0.f ? __fdiv_rn(a, cs.theta) : __fmul_rn(a, cs.theta);
+          if (cs.bias) a = __fadd_rn(a, __ldg(cs.bias + c));                 // (no FMA with the penalty's product)
+          if (c == 0 && no_eos) a = -INFINITY;
+          sv[c] = a;
+          ma = fmaxf(ma, a);
+        }
+        if (t == 0) red[48] = -INFINITY;                                        // top-k over fewer candidates than k: keep all
+        m = bmax(ma);                                                           // the candidates' maximum (NaN skipped)
+      }
       int id;
       if (temp == 0.f) {
         float bv = -INFINITY;
@@ -1589,7 +1623,7 @@ static __device__ __noinline__ void sample_std_phase(const float* logits, int32_
       tok = id;
       if (t == 0) {
         seq[row + pos + 1] = id;
-        if (token_logp) token_logp[row + pos + 1] = sv[id] - lse;
+        if (token_logp) token_logp[row + pos + 1] = (cons ? __ldcg(lg + id) : sv[id]) - lse;   // the raw logit
         if (id == 0) { end[b] = pos + 1; atomicAdd(n_ended, 1); }
       }
     }
@@ -1764,7 +1798,8 @@ static __device__ __forceinline__ void run(const progen_decode_run_t& r) {
         sgu_phase<PLAN>(r, sa, pos, red);
       } else if constexpr (STD) {
         sample_std_phase(r.logits, r.seq, r.start, r.end, r.n_ended, r.token_logp, r.logits_all, r.embed, r.x, r.sample_id, r.n, r.V,
-                         d, B, r.top_k, r.temperature, r.top_p, r.seed, pos, xs, red);
+                         d, B, r.top_k, r.temperature, r.top_p, r.seed,
+                         SampleCons{r.logit_bias, r.repetition_penalty, r.repetition_window, r.min_new_tokens}, pos, xs, red);
       } else {
         sample_phase(r, pos, xs, red);
       }
@@ -1845,6 +1880,9 @@ int progen_decode_run(const progen_decode_run_t* r, void* stream) {
   PG_CHECK_ARG(r->pos0 >= 0 && r->pos0 + r->nsteps <= r->n);
   PG_CHECK_ARG(r->grid_bar != nullptr && r->att_count != nullptr && r->att_part != nullptr);
   PG_CHECK_ARG(r->sampler == 0 || r->sampler == 1);
+  PG_CHECK_ARG(std::isfinite(r->repetition_penalty) && r->repetition_penalty > 0.f);
+  PG_CHECK_ARG(r->repetition_window >= 0 && r->repetition_window <= r->n && r->min_new_tokens >= 0 && r->min_new_tokens <= r->n);
+  if (r->sampler == 0) PG_CHECK_ARG(r->logit_bias == nullptr && r->repetition_penalty == 1.f && r->min_new_tokens == 0);
   if (r->sampler == 1) {
     PG_CHECK_ARG(std::isfinite(r->temperature) && r->temperature >= 0.f && r->top_p > 0.f && r->top_p <= 1.f);
     PG_CHECK_ARG(r->top_k >= 0 && r->top_k <= r->V);

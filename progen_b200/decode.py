@@ -35,7 +35,8 @@ class DecodeRun(C.Structure):
                [(k, _P) for k in ('embed', 'lnf_scale', 'whead_t', 'bhead', 'rot_sin', 'rot_cos', 'layers', 'seq', 'start', 'noise',
                                   'logits_all', 'x', 'q', 'att', 'att_part', 'att_count', 'u', 'sg', 'pj', 'logits', 'grid_bar', 'prof')] + \
                [('sampler', _I), ('temperature', C.c_float), ('top_p', C.c_float), ('_pad1', _I), ('seed', C.c_uint64)] + \
-               [(k, _P) for k in ('sample_id', 'token_logp', 'end', 'n_ended', 'steps_run')]
+               [(k, _P) for k in ('sample_id', 'token_logp', 'end', 'n_ended', 'steps_run', 'logit_bias')] + \
+               [('repetition_penalty', C.c_float), ('repetition_window', _I), ('min_new_tokens', _I), ('_pad2', _I)]
 
 
 class BatchDecoder:
@@ -121,7 +122,9 @@ class BatchDecoder:
         m.u, m.sg, m.pj, m.logits = zeros(B, hid), zeros(8, B, hid // 2), zeros(B, hid // 2), zeros(B, self.V)
         self.grid_bar = torch.zeros(1, device=self.dev, dtype=torch.int32)
         m.grid_bar = self.grid_bar.data_ptr()
+        m.repetition_penalty = 1.0                        # constraints off
         self._gen = None                                  # sampler-1 buffers, allocated by the first generate()
+        self._bias = None                                 # [V] logit bias of generate(), allocated on first use
 
     def _hold(self, t):
         self.keep.append(t)
@@ -202,12 +205,17 @@ class BatchDecoder:
         generated = int(sum(length - max(int(s), 1) for s in starts))
         return (out[0] if single else out), generated, e0.elapsed_time(e1) / 1e3
 
-    def generate(self, prompts, *, temperature=1.0, top_k=None, top_p=None, seed=0, sample_ids=None, max_length=None):
+    def generate(self, prompts, *, temperature=1.0, top_k=None, top_p=None, seed=0, sample_ids=None, max_length=None,
+                 logit_bias=None, min_new_tokens=0, repetition_penalty=1.0, repetition_window=0):
         """The standard sampler (sampler 1 of csrc/decode_persist.cu) for up to B prompts (integer arrays of ids in [1, V)).
         Each row is laid out as training data is, [0 (BOS), prompt..., 0...], and draws positions 1 + len(prompt) ..
         max_length - 1 until it samples EOS (id 0).  Row b uses the Philox stream sample_ids[b] (default b); the
         attention and SGU work splits are planned for the largest launch of the batch tile's class (1, 8 or 64 rows), so
         a row's result depends on (seed, its sample id) and that class, not on the other rows of the launch.  Fewer prompts than B run on a prefix of the caches.
+        Constraints, applied to the logits of every draw before the filter (progen_b200.h, DESIGN.md §3.3): the ids present
+        in the last `repetition_window` positions (0: all since BOS) have positive logits divided and negative ones
+        multiplied by `repetition_penalty`; `logit_bias` ([V] floats, -inf bans an id) is added; EOS is banned for the
+        first `min_new_tokens` draws of a row.  They do not change token_logp, the unfiltered model's log-probability.
         Returns a dict of numpy arrays: ids [R, n] int64, token_logp [R, n] float32 (log p(ids[t] | ids[:t]) at drawn t,
         else 0), end [R] int32 (position of the EOS, n if none), start [R] int32; and steps_run (positions the last
         launch consumed before every row had ended, or its full length) and device_s (that launch's device time)."""
@@ -237,6 +245,14 @@ class BatchDecoder:
         sids = np.arange(R, dtype=np.int64) if sample_ids is None else np.asarray(sample_ids, np.int64).reshape(-1)
         if sids.shape != (R,):
             raise L.ProgenError('generate: one sample id per prompt')
+        if logit_bias is not None:
+            logit_bias = np.asarray(logit_bias, np.float32)
+            if logit_bias.shape != (self.V,) or np.isnan(logit_bias).any() or (logit_bias == np.inf).any():
+                raise L.ProgenError(f'generate: logit_bias must be {self.V} floats without NaN or +inf')
+        if not 0 <= int(min_new_tokens) <= n or not 0 <= int(repetition_window) <= n:
+            raise L.ProgenError(f'generate: min_new_tokens and repetition_window must lie in [0, {n}]')
+        if not (np.isfinite(repetition_penalty) and repetition_penalty > 0):
+            raise L.ProgenError('generate: repetition_penalty must be finite and > 0')
         if self._gen is None:
             z = lambda *s, dtype: torch.zeros(*s, device=self.dev, dtype=dtype)
             self._gen = dict(sample_id=z(self.B, dtype=torch.int64), token_logp=z(self.B, n, dtype=torch.float32),
@@ -257,6 +273,13 @@ class BatchDecoder:
         m.seed = int(seed) & 0xFFFFFFFFFFFFFFFF
         m.sample_id, m.token_logp, m.end = gb['sample_id'].data_ptr(), gb['token_logp'].data_ptr(), gb['end'].data_ptr()
         m.n_ended, m.steps_run = gb['counters'].data_ptr(), gb['counters'].data_ptr() + 4
+        if logit_bias is not None:
+            if self._bias is None:
+                self._bias = torch.zeros(self.V, device=self.dev, dtype=torch.float32)
+            self._bias.copy_(torch.from_numpy(logit_bias))
+            m.logit_bias = self._bias.data_ptr()
+        m.repetition_penalty = float(repetition_penalty)
+        m.repetition_window, m.min_new_tokens = int(repetition_window), int(min_new_tokens)
         try:
             first = int(starts.min()) - 1                 # the first drawn position is start; it reads the logits of start - 1
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -269,7 +292,8 @@ class BatchDecoder:
         finally:
             m.B, m.sampler, m.top_k = self.B, 0, 0
             m.temperature, m.top_p, m.seed = 0.0, 0.0, 0
-            m.sample_id = m.token_logp = m.end = m.n_ended = m.steps_run = 0
+            m.sample_id = m.token_logp = m.end = m.n_ended = m.steps_run = m.logit_bias = 0
+            m.repetition_penalty, m.repetition_window, m.min_new_tokens = 1.0, 0, 0
         return dict(ids=self.seq[:R].cpu().numpy().astype(np.int64), token_logp=gb['token_logp'][:R].cpu().numpy(),
                     end=gb['end'][:R].cpu().numpy(), start=starts, steps_run=int(gb['counters'][1].item()),
                     device_s=e0.elapsed_time(e1) / 1e3)

@@ -134,7 +134,7 @@ class ProGen:
         return out
 
     def generate(self, params, prompts, *, num_samples=1, temperature=1.0, top_k=None, top_p=None, max_length=None, seed=0,
-                 batch_size=64):
+                 batch_size=64, logit_bias=None, min_new_tokens=0, repetition_penalty=1.0, repetition_window=0):
         """Sample sequences with the standard sampler of the persistent decode kernel (temperature, top-k with ties kept,
         nucleus top-p, in-kernel Philox Gumbel noise; csrc/decode_persist.cu), stopping each sequence at its EOS.
         Unlike the reference sampler (utils.sample, sample.py), a prompt is laid out as training data is: BOS (0), the
@@ -148,6 +148,18 @@ class ProGen:
         chunk is padded to the class).  Rows of different classes agree to fp32 round-off, so ids can differ where a draw
         is that close.  max_length (default seq_len) bounds BOS + prompt + generated tokens;
         temperature 0 is greedy (first maximal logit; top_k / top_p ignored).
+
+        Constraints, applied in the kernel to the logits of every draw, in this order, before top-k / temperature / top-p
+        (DESIGN.md §3.3):
+          repetition_penalty θ (finite, > 0; 1 = off) and repetition_window W (integer in [0, seq_len]; 0 = the whole
+            row): each id present at least once among the last W positions before the draw (prompt and generated, BOS
+            excluded) has its logit l divided by θ if l > 0, else multiplied by θ;
+          logit_bias: None or V floats added to the logits; -inf bans an id, +inf and NaN are rejected, and some id in
+            [1, V) must stay allowed (EOS, id 0, may be banned);
+          min_new_tokens (integer in [0, max_length - 2]): the first min_new_tokens generated tokens of a row are never
+            EOS.  A row whose prompt leaves fewer positions before max_length simply runs to max_length unfinished.
+        Only the ids whose adjusted logit is not -inf can be drawn.  token_logp and log_likelihood do not see the
+        constraints: they stay the unfiltered model's at temperature 1, comparable with `score`.
 
         Returns a dict of numpy arrays over the N = len(prompts) * num_samples rows:
           tokens [N, seq_len] int64: BOS, prompt, generated tokens, EOS, zeros;
@@ -180,6 +192,26 @@ class ProGen:
             raise L.ProgenError(f'generate: temperature must be finite and >= 0, got {temperature}')
         if top_p is not None and not 0.0 < top_p <= 1.0:
             raise L.ProgenError(f'generate: top_p must lie in (0, 1], got {top_p}')
+        min_new_tokens = integer(min_new_tokens, 'min_new_tokens', 0, max_length - 2)
+        repetition_window = integer(repetition_window, 'repetition_window', 0, n)
+        try:
+            repetition_penalty = float(repetition_penalty)
+        except (TypeError, ValueError):
+            raise L.ProgenError('generate: repetition_penalty must be a number') from None
+        if not (np.isfinite(repetition_penalty) and repetition_penalty > 0.0):
+            raise L.ProgenError(f'generate: repetition_penalty must be finite and > 0, got {repetition_penalty}')
+        if logit_bias is not None:
+            try:
+                with np.errstate(over='ignore'):
+                    logit_bias = np.asarray(logit_bias, np.float64).astype(np.float32)   # the kernel adds fp32
+            except (TypeError, ValueError):
+                raise L.ProgenError('generate: logit_bias must be an array of floats') from None
+            if logit_bias.shape != (V,):
+                raise L.ProgenError(f'generate: logit_bias must have shape ({V},), got {logit_bias.shape}')
+            if np.isnan(logit_bias).any() or (logit_bias == np.inf).any():
+                raise L.ProgenError('generate: logit_bias must not contain NaN or +inf (in float32)')
+            if not np.isfinite(logit_bias[1:]).any():
+                raise L.ProgenError('generate: logit_bias bans every id in [1, V)')
         from .data import encode_tokens
         if isinstance(prompts, (str, bytes)):
             prompts = [prompts]
@@ -211,7 +243,8 @@ class ProGen:
             chunk = rows[r0:r1] + [rows[r1 - 1]] * pad
             sids = np.concatenate([np.arange(r0, r1), np.full(pad, r1 - 1)]).astype(np.int64)
             res = dec.generate(chunk, temperature=temperature, top_k=top_k, top_p=top_p, seed=seed, sample_ids=sids,
-                               max_length=max_length)
+                               max_length=max_length, logit_bias=logit_bias, min_new_tokens=min_new_tokens,
+                               repetition_penalty=repetition_penalty, repetition_window=repetition_window)
             out['tokens'][r0:r1] = res['ids'][:r1 - r0]
             out['token_logp'][r0:r1] = res['token_logp'][:r1 - r0]
             out['start'][r0:r1] = res['start'][:r1 - r0]

@@ -1,4 +1,4 @@
-"""Cost of the standard sampler (sampler 1) and gain of the EOS early exit, at the config-5 model.
+"""Cost of the standard sampler (sampler 1), of its constraints, and gain of the EOS early exit, at the config-5 model.
 
     python scripts/generate_bench.py [--rounds 3] [--samples 256]
 
@@ -8,7 +8,12 @@ bf16 weights in the persistent decode kernel; prompt '[Tax=Mammalia] #'.
     the reference sampler (BatchDecoder.sample, top_k 25, Gumbel noise: what bench.py --config cfg5 runs) and for sampler 1
     (BatchDecoder.generate, T 1, top_p 0.95; positions = steps_run, so an early exit is accounted for).  Sampler 1 plans
     the attention and SGU work splits for 1, 8 or 64 rows (the largest launch of the batch tile's class); B = 12 shows
-    what that costs a launch smaller than its class's largest.
+    what that costs a launch smaller than its class's largest.  `con` is sampler 1 with the constraints a protein user
+    sets: the 20 amino acids as the alphabet (a logit bias banning every other id but EOS), min_new_tokens 64,
+    repetition_penalty 1.2 over a 16-position window, against `std_full`, sampler 1 without them.  Both run with EOS
+    unreachable (the `no_eos` head bias below), so both consume every position: a position's cost grows with its index
+    (the gMLP layers' causal history sum), and the alphabet makes EOS so likely that a constrained launch would
+    otherwise stop after about a tenth of the positions of a plain one.
   end_to_end: wall clock of ProGen.generate(num_samples=`samples`, batch_size=64, T 1, top_p 0.95) including the host
     copies, for three parameter sets: as initialised (`model`), the head bias of token 0 raised so that EOS has probability
     about 1 % right after the prompt (`eos_1pct`), and EOS made unreachable by a -inf head bias (`no_eos`: every sequence
@@ -29,6 +34,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 from bench import gpu_info                                # noqa: E402
+from generate import alphabet_bias                        # noqa: E402
 from progen_b200 import ProGen                            # noqa: E402
 from progen_b200.data import encode_tokens                # noqa: E402
 from progen_b200.decode import BatchDecoder               # noqa: E402
@@ -37,6 +43,8 @@ from progen_b200.engine import P                          # noqa: E402
 KW = dict(num_tokens=256, dim=512, seq_len=1024, depth=12, heads=8, dim_head=64, window_size=256, global_mlp_depth=2,
           ff_glu=True)
 PROMPT = '[Tax=Mammalia] #'
+CONSTRAINED = dict(logit_bias=alphabet_bias('ACDEFGHIKLMNPQRSTVWY', KW['num_tokens']), min_new_tokens=64,
+                   repetition_penalty=1.2, repetition_window=16)
 
 
 def with_eos_bias(params, delta):
@@ -64,13 +72,14 @@ def main():
     psets = dict(model=params, eos_1pct=with_eos_bias(params, delta), no_eos=with_eos_bias(params, -np.inf))
     models = {k: ProGen(**KW, mixed_precision=True) for k in psets}
     decs = {B: BatchDecoder(models['model'].config, params, batch=B, weights_dtype=torch.bfloat16) for B in (1, 8, 12, 64)}
+    full = {B: BatchDecoder(models['model'].config, psets['no_eos'], batch=B, weights_dtype=torch.bfloat16) for B in decs}
 
     def quirk(B, seed):
         _, _, secs = decs[B].sample([prime] * B if B > 1 else prime, top_k=25, add_bos=True, greedy=False, seed=seed)
         return secs / (n - 1 - (len(prime) - 1))                # positions first .. n-2 of the timed launch
 
-    def std(B, seed):
-        r = decs[B].generate([prime] * B, temperature=1.0, top_p=0.95, seed=seed)
+    def std(B, seed, dec=decs, **cons):
+        r = dec[B].generate([prime] * B, temperature=1.0, top_p=0.95, seed=seed, **cons)
         return r['device_s'] / r['steps_run']
 
     def e2e(name, seed):
@@ -81,14 +90,17 @@ def main():
         torch.cuda.synchronize()
         return time.perf_counter() - t0, int(r['length'].sum()), int(r['finished'].sum())
 
-    per_pos = {f'{s}_B{B}': [] for B in decs for s in ('quirk', 'std')}
+    per_pos = {f'{s}_B{B}': [] for B in decs for s in ('quirk', 'std', 'std_full', 'con')}
     ends = {k: [] for k in psets}
     for rnd in range(args.rounds + 1):                          # round 0: warm-up
         for B in decs:
             q, s = quirk(B, 100 + rnd), std(B, 100 + rnd)
+            f, c = std(B, 100 + rnd, full), std(B, 100 + rnd, full, **CONSTRAINED)
             if rnd:
                 per_pos[f'quirk_B{B}'].append(q)
                 per_pos[f'std_B{B}'].append(s)
+                per_pos[f'std_full_B{B}'].append(f)
+                per_pos[f'con_B{B}'].append(c)
         for name in psets:
             r = e2e(name, rnd)
             if rnd:
@@ -96,6 +108,8 @@ def main():
     res = dict(per_position_us={k: dict(median=statistics.median(v) * 1e6, all=[x * 1e6 for x in v]) for k, v in per_pos.items()})
     res['std_over_quirk'] = {f'B{B}': statistics.median(per_pos[f'std_B{B}']) / statistics.median(per_pos[f'quirk_B{B}'])
                              for B in decs}
+    res['con_over_std'] = {f'B{B}': statistics.median(per_pos[f'con_B{B}']) / statistics.median(per_pos[f'std_full_B{B}'])
+                           for B in decs}
     e = {}
     for name, v in ends.items():
         secs = statistics.median([x[0] for x in v])
@@ -104,7 +118,7 @@ def main():
                        generated_tokens_per_s=tok / secs, finished=v[0][2])
     res['end_to_end'] = e
     res['early_exit_speedup_eos_1pct'] = e['no_eos']['s'] / e['eos_1pct']['s']
-    print(json.dumps(dict(metric='generation: sampler-1 cost per position and EOS early exit, config-5 model (bf16 weights)',
+    print(json.dumps(dict(metric='generation: sampler-1 and constraint cost per position and EOS early exit, config-5 model (bf16 weights)',
                           samples=args.samples, rounds=args.rounds, eos_bias_delta=delta, **res,
                           gpu=gpu_info(torch.cuda.current_device()))))
 

@@ -18,6 +18,11 @@ timeout 900 compute-sanitizer --tool "$tool" --error-exitcode 9 --print-limit 20
   python -m pytest tests/test_gpu_generate.py -x -q -m gpu -k "test_reference_sampler_unaffected_by_generate or test_eos_ends_sequences_and_the_launch" \
   -p no:cacheprovider > "$out/sanitize_${tool}_generate.log" 2>&1
 echo "generate: exit $? : $(grep -E 'ERROR SUMMARY|passed|failed' "$out/sanitize_${tool}_generate.log" | tail -n 2 | tr '\n' ' ')"
+# the constrained sampler at 1, 2 and 24 rows: presence flags in the q half, the bias, the minimum length and the early exit
+timeout 900 compute-sanitizer --tool "$tool" --error-exitcode 9 --print-limit 20 \
+  python -m pytest tests/test_gpu_generate_constraints.py -x -q -m gpu -k "test_reference_sampler_after_constrained_generate or test_min_length_binds_at_24_rows" \
+  -p no:cacheprovider > "$out/sanitize_${tool}_constraints.log" 2>&1
+echo "constraints: exit $? : $(grep -E 'ERROR SUMMARY|passed|failed' "$out/sanitize_${tool}_constraints.log" | tail -n 2 | tr '\n' ' ')"
 # kernels the tiny model configs do not reach: many-tile / tail GEMMs (all epilogues), wgmma attention, streaming LN backward
 timeout 1200 compute-sanitizer --tool "$tool" --error-exitcode 9 --print-limit 20 \
   python -m pytest tests/test_gpu_gemm_tc.py tests/test_gpu_attn_tc.py tests/test_gpu_elementwise.py -x -q -m gpu \
