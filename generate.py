@@ -3,13 +3,15 @@
     python generate.py --checkpoint_path ./ckpts --prompt "[Tax=Mammalia] #" [--prompt ... | --prompts_file f.txt]
         --num_samples 100 --temperature 1.0 [--top_k K] [--top_p 0.95] --seed 0 --batch_size 64 [--max_length L]
         [--alphabet ACDEFGHIKLMNPQRSTVWY] [--min_new_tokens N] [--repetition_penalty 1.2 --repetition_window 16]
-        [--mixed_precision] --output samples.fasta
+        [--mixed_precision] [--prefill forward] --output samples.fasta
 
 Runs ProGen.generate: each prompt is laid out like training data (BOS, prompt), every sequence stops at its own EOS,
 temperature / top-k / nucleus (top-p) filtering happen in the persistent decode kernel.  --alphabet restricts every
 draw to those residues and EOS, --min_new_tokens forbids EOS for the first N generated tokens, and --repetition_penalty
 penalises the residues present in the last --repetition_window positions (0: the whole sequence); these act on the
-logits in the kernel and leave the reported log-likelihood that of the unconstrained model.  Unlike sample.py (the reference
+logits in the kernel and leave the reported log-likelihood that of the unconstrained model.  --prefill forward fills
+the decoder's caches for the prompt with one forward pass per distinct prompt instead of one decode step per prompt
+position (faster for long prompts; bf16 models then differ from the default by round-off).  Unlike sample.py (the reference
 drop-in, one sequence, top_k=25 with the reference's quirks), the result of a row depends only on the seed and the row.
 The FASTA has one record per row (row = prompt index * num_samples + sample index):
     >{row} prompt={i} sample={j} log_likelihood={sum of log p of the generated tokens, EOS included} length={...} eos={0|1}
@@ -61,9 +63,11 @@ def alphabet_bias(alphabet, num_tokens):
 @click.option('--repetition_penalty', default=1.0, help='divide positive / multiply negative logits of recent ids (1 = off)')
 @click.option('--repetition_window', default=0, help='positions the repetition penalty looks back (0 = the whole sequence)')
 @click.option('--mixed_precision', default=False, is_flag=True, help='bf16 weights in the decode kernel')
+@click.option('--prefill', default='decode', type=click.Choice(['decode', 'forward']),
+              help='prompt positions: one decode step each, or one forward pass per distinct prompt')
 @click.option('--output', default='samples.fasta')
 def main(checkpoint_path, prompts, prompts_file, num_samples, temperature, top_k, top_p, seed, batch_size, max_length,
-         alphabet, min_new_tokens, repetition_penalty, repetition_window, mixed_precision, output):
+         alphabet, min_new_tokens, repetition_penalty, repetition_window, mixed_precision, prefill, output):
     _, get_last_checkpoint, _ = get_checkpoint_fns(checkpoint_path)
     last_checkpoint = get_last_checkpoint()
     if last_checkpoint is None:
@@ -83,7 +87,7 @@ def main(checkpoint_path, prompts, prompts_file, num_samples, temperature, top_k
     res = model.generate(params, prompts, num_samples=num_samples, temperature=temperature, top_k=top_k, top_p=top_p,
                          max_length=max_length, seed=seed, batch_size=batch_size, logit_bias=bias,
                          min_new_tokens=min_new_tokens, repetition_penalty=repetition_penalty,
-                         repetition_window=repetition_window)
+                         repetition_window=repetition_window, prefill=prefill)
     secs = time.perf_counter() - t0
     N = len(res['length'])
     with open(output, 'w') as f:

@@ -268,6 +268,21 @@ typedef struct progen_decode_run_t {
 
 int progen_decode_run(const progen_decode_run_t* run, void* stream);
 
+/* Prefill of the decoder's caches from an inference forward (generation with `prefill='forward'`): a strided row gather
+ * with conversion to fp32,
+ *   dst[b * dst_b_stride + g * dst_g_stride + r * dst_row_stride + c]
+ *     = fp32(src[(row_map[b] * src_seq_rows + row0 + r) * ld + col0 + g * cols + c])
+ * for b < B, g < groups, r < rows, c < cols.  src is a forward activation [src_seqs * src_seq_rows, ld] in src_dtype;
+ * row_map ([B] int32, device) names the forward sequence of each decoder row (entries are clamped to [0, src_seqs)), so one
+ * forward of a prompt fills every row that uses it.  With the caches of progen_decode_run_t: k / v rows 0..P-1 of the
+ * rotated q|k|v (col0 = inner or 2 inner, groups = heads, cols = dim_head) into kcache / vcache [B, heads, n, dim_head];
+ * LN-output row P, channels [0, d/2), which after the token shift holds position P-1's half, into slot P & 1 of
+ * shift1 / shift2 [B, 2, d/2]; normalised-gate rows 0..P-1 into gn_hist [B, n, hid/2].  16-byte source vectors: cols, col0
+ * and ld multiples of 4 (fp32) or 8 (bf16), src and dst 16-byte aligned, dst strides multiples of 4.  rows = 0 is a no-op. */
+int progen_gather_rows_f32(const void* src, long long ld, int src_dtype, int src_seqs, long long src_seq_rows,
+                           const int32_t* row_map, int B, int row0, int rows, int col0, int groups, int cols, float* dst,
+                           long long dst_b_stride, long long dst_g_stride, long long dst_row_stride, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

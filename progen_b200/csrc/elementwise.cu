@@ -1,5 +1,6 @@
 // HBM-bound kernels of the ProGen hot path: token embedding, LayerNorm(scale-only)+token-shift (fwd/bwd),
-// cross-entropy with the pad-as-EOS mask (fwd+bwd fused), rotary backward, SGU gating, GELU backward, column sums.
+// cross-entropy with the pad-as-EOS mask (fwd+bwd fused), rotary backward, SGU gating, GELU backward, column sums, and the
+// row gather that fills the decoder's caches from an inference forward (generation prefill).
 // All are coalesced, 8/16-byte vectorised, one warp per row where a row reduction is needed.
 #include "common.cuh"
 #include "../../include/progen_b200.h"
@@ -597,6 +598,32 @@ __global__ void tril_cast_kernel(const float* __restrict__ w, TO* __restrict__ o
   }
 }
 
+// decoder-cache prefill: dst[b, g, r, c] = fp32(src[(row_map[b] * src_seq_rows + row0 + r) * ld + col0 + g * cols + c]).
+// One thread moves 16 source bytes (4 fp32 or 8 bf16) to 16 or 32 destination bytes; consecutive threads take consecutive
+// column vectors of a row, so both sides coalesce.  The source (one forward row per distinct prompt) is read once per
+// decoder row that maps to it; the fp32 caches written are the bulk of the traffic.
+template <typename TI>
+__global__ void gather_rows_f32_kernel(const TI* __restrict__ src, long long ld, const int* __restrict__ row_map, int src_seqs,
+                                       long long src_seq_rows, int row0, int rows, int col0, int groups, int cols,
+                                       float* __restrict__ dst, long long dst_b, long long dst_g, long long dst_r,
+                                       long long total) {
+  constexpr int NV = 16 / sizeof(TI);
+  const int cv = cols / NV;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int c = (int)(i % cv) * NV;
+    long long t = i / cv;
+    const int r = (int)(t % rows);
+    t /= rows;
+    const int g = (int)(t % groups);
+    const int b = (int)(t / groups);
+    int s = row_map[b];
+    s = s < 0 ? 0 : (s >= src_seqs ? src_seqs - 1 : s);
+    float v[NV];
+    load_vec<NV>(src + (s * src_seq_rows + row0 + r) * ld + col0 + (long long)g * cols + c, v);
+    store_vec<NV>(dst + b * dst_b + g * dst_g + r * dst_r + c, v);
+  }
+}
+
 inline int ew_grid(long long work_items, int threads) {
   long long b = (work_items + threads - 1) / threads;
   const long long cap = (long long)pg_num_sms() * 8;
@@ -800,6 +827,32 @@ int progen_tril_cast(const float* w, void* out, int out_dtype, int n, void* stre
   const int grid = ew_grid((long long)n * (n / 4), 256);
   if (out_dtype == PG_F32) tril_cast_kernel<float><<<grid, 256, 0, s>>>(w, (float*)out, n);
   else tril_cast_kernel<bf16><<<grid, 256, 0, s>>>(w, (bf16*)out, n);
+  PG_LAUNCH_CHECK();
+  return PROGEN_OK;
+}
+
+int progen_gather_rows_f32(const void* src, long long ld, int src_dtype, int src_seqs, long long src_seq_rows,
+                           const int* row_map, int B, int row0, int rows, int col0, int groups, int cols, float* dst,
+                           long long dst_b_stride, long long dst_g_stride, long long dst_row_stride, void* stream) {
+  PG_CHECK_ARG(src != nullptr && row_map != nullptr && dst != nullptr);
+  PG_CHECK_ARG(src_dtype == PG_F32 || src_dtype == PG_BF16);
+  const int nv = src_dtype == PG_F32 ? 4 : 8;          // elements per 16-byte source vector
+  PG_CHECK_ARG(B > 0 && src_seqs > 0 && src_seq_rows > 0 && groups > 0 && cols > 0 && rows >= 0 && row0 >= 0 && col0 >= 0);
+  PG_CHECK_ARG(row0 + (long long)rows <= src_seq_rows && col0 + (long long)groups * cols <= ld);
+  PG_CHECK_ARG(cols % nv == 0 && col0 % nv == 0 && ld % nv == 0);
+  PG_CHECK_ARG(dst_b_stride >= 0 && dst_g_stride >= 0 && dst_row_stride >= 0);
+  PG_CHECK_ARG(dst_b_stride % 4 == 0 && dst_g_stride % 4 == 0 && dst_row_stride % 4 == 0);
+  PG_CHECK_ARG((uintptr_t)src % 16 == 0 && (uintptr_t)dst % 16 == 0);
+  if (rows == 0) return PROGEN_OK;
+  cudaStream_t s = (cudaStream_t)stream;
+  const long long total = (long long)B * groups * rows * (cols / nv);
+  const int grid = ew_grid(total, 256);
+  if (src_dtype == PG_F32)
+    gather_rows_f32_kernel<float><<<grid, 256, 0, s>>>((const float*)src, ld, row_map, src_seqs, src_seq_rows, row0, rows, col0,
+                                                       groups, cols, dst, dst_b_stride, dst_g_stride, dst_row_stride, total);
+  else
+    gather_rows_f32_kernel<bf16><<<grid, 256, 0, s>>>((const bf16*)src, ld, row_map, src_seqs, src_seq_rows, row0, rows, col0,
+                                                      groups, cols, dst, dst_b_stride, dst_g_stride, dst_row_stride, total);
   PG_LAUNCH_CHECK();
   return PROGEN_OK;
 }

@@ -65,9 +65,11 @@ class BatchDecoder:
         kinds = layer_kinds(cfg['depth'], cfg['global_mlp_depth'], cfg['ff_glu'])
         layers = (DecodeLayer * len(kinds))()
         self.state = []
+        self.caches = []                                  # per layer: name -> the cache tensor of the layer table
         for i, kind in enumerate(kinds):
             a, f = P + f'attn{i}/~/', P + f'ff{i}/~/'
             Lr = layers[i]
+            self.caches.append({})
             Lr.kind = {'glu': 0, 'gelu': 1, 'sgu': 2}[kind]
             Lr.ln1_scale = f32(params[a + 'layer_norm']['scale'])
             Lr.wqkv_t = wt(params[a + 'linear']['w'])
@@ -85,11 +87,11 @@ class BatchDecoder:
                 Lr.sgu_b = f32(np.asarray(params[g]['spatial_biases']).reshape(-1))
                 Lr.sgu_proj_t = wt(params[g + '/~/linear']['w'])
                 Lr.sgu_proj_b = f32(params[g + '/~/linear']['b'])
-                Lr.gn_hist = self._state(zeros(B, n, hid // 2))
-            Lr.kcache = self._state(zeros(B, n, I))
-            Lr.vcache = self._state(zeros(B, n, I))
-            Lr.shift1 = self._state(zeros(B, 2, d // 2))
-            Lr.shift2 = self._state(zeros(B, 2, d // 2))
+                Lr.gn_hist = self._state(zeros(B, n, hid // 2), 'gn_hist')
+            Lr.kcache = self._state(zeros(B, n, I), 'kcache')           # [B, heads, n, dim_head]
+            Lr.vcache = self._state(zeros(B, n, I), 'vcache')
+            Lr.shift1 = self._state(zeros(B, 2, d // 2), 'shift1')
+            Lr.shift2 = self._state(zeros(B, 2, d // 2), 'shift2')
         # the kernel reads the layer table from DEVICE memory
         raw = np.frombuffer(bytes(layers), dtype=np.uint8).copy()
         self.layers_dev = torch.from_numpy(raw).to(self.dev)
@@ -130,14 +132,66 @@ class BatchDecoder:
         self.keep.append(t)
         return t.data_ptr()
 
-    def _state(self, ptr):
+    def _state(self, ptr, name):
         self.state.append(self.keep[-1])
+        self.caches[-1][name] = self.keep[-1]
         return ptr
 
     def reset(self):
         for t in self.state:
             t.zero_()
         self.att_count.zero_()
+
+    def prefill(self, engine, prompts):
+        """Reset, then fill the caches of rows 0 .. len(prompts) - 1 for positions < P from ONE inference forward of
+        `engine` (an Engine with this decoder's config and parameters) over the distinct prompts, each laid out as
+        `generate` lays it out, [0 (BOS), prompt, 0...].  Every prompt must have the same length P; returns P, to pass to
+        `generate(prompts, prefilled=P)` with the same prompts.  P = 0 (empty prompts) prefills nothing.  The caches then
+        hold the forward's arithmetic (bf16 activations under mixed precision) rather than this kernel's."""
+        if not 1 <= len(prompts) <= self.B:
+            raise L.ProgenError(f'prefill: 1 <= prompts <= {self.B}')
+        seq0, starts = self._rows(prompts, self.n)
+        if len(set(starts.tolist())) != 1:
+            raise L.ProgenError('prefill: every prompt must have the same length')
+        keys = ('num_tokens', 'dim', 'seq_len', 'depth', 'window_size', 'global_mlp_depth', 'heads', 'dim_head', 'ff_mult',
+                'ff_glu', 'shift_tokens')
+        if any(engine.cfg[k] != self.cfg[k] for k in keys):
+            raise L.ProgenError('prefill: the engine and the decoder have different model configurations')
+        self.reset()
+        P = int(starts[0]) - 1
+        if P == 0:
+            return 0
+        distinct, row_map = {}, []
+        for row in seq0:
+            row_map.append(distinct.setdefault(row.tobytes(), len(distinct)))
+        ids = np.stack([np.frombuffer(k, np.int32) for k in distinct])
+        engine.prefill(ids, P, self._prefill_sink(torch.tensor(row_map, dtype=torch.int32, device=self.dev), len(distinct)))
+        return P
+
+    def _prefill_sink(self, row_map, nsrc):
+        """Engine.prefill sink: row b of every cache takes forward row row_map[b] (progen_gather_rows_f32)"""
+        cfg, n = self.cfg, self.n
+        h, dh, half_d = cfg['heads'], cfg['dim_head'], cfg['dim'] // 2
+        I = h * dh
+
+        def gather(buf, row0, rows, col0, groups, cols, dst, b_stride, g_stride, row_stride):
+            L.check(self.lib.progen_gather_rows_f32(buf.data_ptr(), buf.stride(0), L.dt(buf), nsrc, n, row_map.data_ptr(),
+                                                    row_map.numel(), row0, rows, col0, groups, cols, dst, b_stride, g_stride,
+                                                    row_stride, L.stream()), 'gather_rows_f32')
+
+        def sink(i, name, buf, P):
+            c = self.caches[i]
+            if name == 'qkv':                             # k, v rows 0..P-1 (rotated) -> [B, heads, n, dim_head]
+                for sec, cache in ((1, c['kcache']), (2, c['vcache'])):
+                    gather(buf, 0, P, sec * I, h, dh, cache.data_ptr(), h * n * dh, n * dh, dh)
+            elif name in ('y1', 'y2') and cfg['shift_tokens']:
+                # LN row P after the shift: its first half is position P-1's, the half the kernel reads at P (slot P & 1)
+                st = c['shift1' if name == 'y1' else 'shift2']
+                gather(buf, P, 1, 0, 1, half_d, st.data_ptr() + (P & 1) * half_d * 4, 2 * half_d, 0, 0)
+            elif name == 'gn':                            # normalised gate rows 0..P-1 -> [B, n, hid/2]
+                gh = c['gn_hist']
+                gather(buf, 0, P, 0, 1, gh.shape[-1], gh.data_ptr(), n * gh.shape[-1], 0, gh.shape[-1])
+        return sink
 
     def profile_barriers(self, pos0, nsteps):
         """Run, recording clock64 at entry / exit of every grid barrier of the LAST step on CTA 0 and the last CTA.
@@ -205,8 +259,22 @@ class BatchDecoder:
         generated = int(sum(length - max(int(s), 1) for s in starts))
         return (out[0] if single else out), generated, e0.elapsed_time(e1) / 1e3
 
+    def _rows(self, prompts, max_length):
+        """-> (seq0 [R, n] int32: [0 (BOS), prompt, 0...] per prompt, starts [R] int32: 1 + prompt length)"""
+        seq0 = np.zeros((len(prompts), self.n), np.int32)
+        starts = np.zeros(len(prompts), np.int32)
+        for b, pr in enumerate(prompts):
+            pr = np.asarray(pr, np.int64).reshape(-1)
+            if len(pr) + 1 >= max_length:
+                raise L.ProgenError(f'generate: a prompt of {len(pr)} ids leaves no position before max_length {max_length}')
+            if len(pr) and (pr.min() < 1 or pr.max() >= self.V):
+                raise L.ProgenError(f'generate: prompt ids must lie in [1, {self.V})')
+            seq0[b, 1:1 + len(pr)] = pr
+            starts[b] = 1 + len(pr)
+        return seq0, starts
+
     def generate(self, prompts, *, temperature=1.0, top_k=None, top_p=None, seed=0, sample_ids=None, max_length=None,
-                 logit_bias=None, min_new_tokens=0, repetition_penalty=1.0, repetition_window=0):
+                 logit_bias=None, min_new_tokens=0, repetition_penalty=1.0, repetition_window=0, prefilled=0):
         """The standard sampler (sampler 1 of csrc/decode_persist.cu) for up to B prompts (integer arrays of ids in [1, V)).
         Each row is laid out as training data is, [0 (BOS), prompt..., 0...], and draws positions 1 + len(prompt) ..
         max_length - 1 until it samples EOS (id 0).  Row b uses the Philox stream sample_ids[b] (default b); the
@@ -216,9 +284,12 @@ class BatchDecoder:
         in the last `repetition_window` positions (0: all since BOS) have positive logits divided and negative ones
         multiplied by `repetition_penalty`; `logit_bias` ([V] floats, -inf bans an id) is added; EOS is banned for the
         first `min_new_tokens` draws of a row.  They do not change token_logp, the unfiltered model's log-probability.
+        prefilled = P > 0: `prefill` has filled the caches of these prompts for positions < P (P <= every prompt's
+        length), so the caches are not reset and the kernel starts at position P instead of 0.
         Returns a dict of numpy arrays: ids [R, n] int64, token_logp [R, n] float32 (log p(ids[t] | ids[:t]) at drawn t,
         else 0), end [R] int32 (position of the EOS, n if none), start [R] int32; and steps_run (positions the last
-        launch consumed before every row had ended, or its full length) and device_s (that launch's device time)."""
+        launch consumed before every row had ended, or its full length), device_s (that launch's device time) and
+        prefill_s (device time of the launch that consumed the prompt positions before it, 0 when there was none)."""
         n = self.n
         max_length = n if max_length is None else int(max_length)
         R = len(prompts)
@@ -232,16 +303,11 @@ class BatchDecoder:
             raise L.ProgenError('generate: 0 < top_p <= 1')
         if not (np.isfinite(temperature) and temperature >= 0):
             raise L.ProgenError('generate: temperature must be finite and >= 0')
-        seq0 = np.zeros((R, n), np.int32)
-        starts = np.zeros(R, np.int32)
-        for b, pr in enumerate(prompts):
-            pr = np.asarray(pr, np.int64).reshape(-1)
-            if len(pr) + 1 >= max_length:
-                raise L.ProgenError(f'generate: a prompt of {len(pr)} ids leaves no position before max_length {max_length}')
-            if len(pr) and (pr.min() < 1 or pr.max() >= self.V):
-                raise L.ProgenError(f'generate: prompt ids must lie in [1, {self.V})')
-            seq0[b, 1:1 + len(pr)] = pr
-            starts[b] = 1 + len(pr)
+        seq0, starts = self._rows(prompts, max_length)
+        first = int(starts.min()) - 1                     # the first drawn position is start; it reads the logits of start - 1
+        if not 0 <= int(prefilled) <= first:
+            raise L.ProgenError(f'generate: prefilled must lie in [0, {first}] (the shortest prompt length)')
+        prefilled = int(prefilled)
         sids = np.arange(R, dtype=np.int64) if sample_ids is None else np.asarray(sample_ids, np.int64).reshape(-1)
         if sids.shape != (R,):
             raise L.ProgenError('generate: one sample id per prompt')
@@ -258,7 +324,8 @@ class BatchDecoder:
             self._gen = dict(sample_id=z(self.B, dtype=torch.int64), token_logp=z(self.B, n, dtype=torch.float32),
                              end=z(self.B, dtype=torch.int32), counters=z(2, dtype=torch.int32))
         gb = self._gen
-        self.reset()
+        if not prefilled:
+            self.reset()
         self.seq[:R].copy_(torch.as_tensor(seq0))
         self.start[:R].copy_(torch.as_tensor(starts))
         gb['sample_id'][:R].copy_(torch.as_tensor(sids))
@@ -281,10 +348,11 @@ class BatchDecoder:
         m.repetition_penalty = float(repetition_penalty)
         m.repetition_window, m.min_new_tokens = int(repetition_window), int(min_new_tokens)
         try:
-            first = int(starts.min()) - 1                 # the first drawn position is start; it reads the logits of start - 1
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            if first > 0:
-                self.run(0, first)                        # prefill: only advances the caches
+            ev = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
+            e0, e1 = ev[1], ev[2]
+            ev[0].record()
+            if first > prefilled:
+                self.run(prefilled, first - prefilled)    # prefill: only advances the caches
             e0.record()
             self.run(first, max_length - 1 - first)       # positions first .. max_length - 2 (the last writes max_length - 1)
             e1.record()
@@ -296,7 +364,7 @@ class BatchDecoder:
             m.repetition_penalty, m.repetition_window, m.min_new_tokens = 1.0, 0, 0
         return dict(ids=self.seq[:R].cpu().numpy().astype(np.int64), token_logp=gb['token_logp'][:R].cpu().numpy(),
                     end=gb['end'][:R].cpu().numpy(), start=starts, steps_run=int(gb['counters'][1].item()),
-                    device_s=e0.elapsed_time(e1) / 1e3)
+                    device_s=e0.elapsed_time(e1) / 1e3, prefill_s=ev[0].elapsed_time(e0) / 1e3)
 
 
 class Decoder:

@@ -355,8 +355,23 @@ class Engine:
         self._forward_device()
         return self.logits
 
-    def _forward_device(self, acts=None):
-        """forward pass on activation set `acts` (default: the training set, which keeps what the backward pass reads)"""
+    def prefill(self, ids, P, sink):
+        """Inference forward of ids [Bs, n] that hands every layer's state to `sink(layer, name, buf, P)` instead of
+        computing logits: name 'qkv' (the rotated q|k|v [T, 3 inner]) and 'y1' (the attention block's shifted LN output
+        [T, d]) after the QKV GEMM, 'y2' (the feed-forward block's) after its LayerNorm, and in gMLP layers 'gn' (the
+        normalised gate [T, hid/2]) after the spatial GEMM, before the gate overwrites it.  The sink must read what it
+        needs before it returns (the inference set reuses its buffers across layers).  Causality makes positions < P and
+        the shifted half of LN row P depend on ids[:, :P] alone.  Each row's result does not depend on the other rows."""
+        Bs = ids.shape[0]
+        if tuple(ids.shape[1:]) != (self.n,) or not 0 < P < self.n:
+            raise L.ProgenError(f'prefill: ids must be (B, {self.n}) and 0 < P < {self.n}')
+        acts = self.inference_acts(Bs)
+        acts.tok.copy_(torch.as_tensor(ids).reshape(-1).to(device=self.dev, dtype=torch.int32))
+        self._forward_device(acts, sink=lambda i, name, buf: sink(i, name, buf, P))
+
+    def _forward_device(self, acts=None, sink=None):
+        """forward pass on activation set `acts` (default: the training set, which keeps what the backward pass reads);
+        with a `sink` (Engine.prefill) the layers' state goes to it and the logits head is skipped"""
         acts = self.acts if acts is None else acts
         lib, st = self.lib, L.stream()
         cfg, d, I, hid, T, n = self.cfg, self.d, self.I, self.hid, acts.T, self.n
@@ -372,11 +387,16 @@ class Engine:
             self.ln_fwd(x0, d, self.Pf(a + 'layer_norm', 'scale'), s['y1'], d, s['mean1'], s['rstd1'], d, shift, acts=acts)
             self.fwd_gemm(s['y1'], d, self.W(a + 'linear', 'w'), 3 * I, s['qkv'], epi=L.EPI_ROTARY, rot_sin=self.rot_sin,
                           rot_cos=self.rot_cos, seq_len=n, dim_head=self.dh, acts=acts)
+            if sink is not None:
+                sink(i, 'qkv', s['qkv'])
+                sink(i, 'y1', s['y1'])
             self.attn_fwd(s['qkv'], s['att'], s['lse'], acts=acts)
             self.fwd_gemm(s['att'], I, self.W(a + 'linear_1', 'w'), d, x1, epi=L.EPI_RESIDUAL, bias=self.Pf(a + 'linear_1', 'b'),
                           aux=None if acts.inplace else x0, ldaux=d, acts=acts)
             # ---- FeedForward (progen.py:131-149); s['u'] is None in the inference set: no pre-activation store
             self.ln_fwd(x1, d, self.Pf(f + 'layer_norm', 'scale'), s['y2'], d, s['mean2'], s['rstd2'], d, shift, acts=acts)
+            if sink is not None:
+                sink(i, 'y2', s['y2'])
             if kind == 'glu':
                 self.fwd_gemm(s['y2'], d, self.W(f + 'linear', 'w'), 2 * hid, s['hact'], epi=L.EPI_GLU, ldo=hid, out2=s['u'],
                               ldo2=2 * hid, bias=self.Pf(f + 'linear', 'b'), acts=acts)
@@ -394,6 +414,8 @@ class Engine:
                 # gate_b = tril(W) @ gn_b for every sequence b; masked K tiles are skipped (causal=1)
                 self._mm(M=n, N=half, K=n, A=self.wm[i], lda=n, B=s['gn'], ldb=half, b_mn=True, out=s['gp'], ldo=half,
                          out_dtype=self.act_dt, batch=acts.B, b_batch_rows=n, d_batch_rows=n, causal=1)
+                if sink is not None:
+                    sink(i, 'gn', s['gn'])
                 L.check(lib.progen_sgu_gate_fwd(s['hact'].data_ptr(), hid, s['gp'].data_ptr(), half,
                                                 self.Pf(g, 'spatial_biases').data_ptr(), s['sg'].data_ptr(), half, self.act_dt,
                                                 T, half, n, st), 'sgu_gate_fwd')
@@ -402,6 +424,8 @@ class Engine:
                 last, last_k = s['pj'], half
             self.fwd_gemm(last, last_k, self.W(f + 'linear_1', 'w'), d, x2, epi=L.EPI_RESIDUAL, bias=self.Pf(f + 'linear_1', 'b'),
                           aux=None if acts.inplace else x1, ldaux=d, acts=acts)
+        if sink is not None:
+            return
         # ---- to_logits (progen.py:219-222)
         xl = acts.X[-1]
         self.ln_fwd(xl, d, self.Pf(P + 'layer_norm', 'scale'), acts.yf, d, acts.meanf, acts.rstdf, d, False, acts=acts)

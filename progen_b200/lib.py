@@ -66,6 +66,7 @@ PROTOTYPES = {
     'progen_tril_cast': [_P, _P, _I, _I, _P],
     'progen_decode_step': [_P, _I, _P],
     'progen_decode_run': [_P, _P],
+    'progen_gather_rows_f32': [_P, _LL, _I, _I, _LL, _P, _I, _I, _I, _I, _I, _I, _P, _LL, _LL, _LL, _P],
     'progen_optim_workspace_floats': [],
     'progen_grad_sqnorm': [_P, _LL, _P, _P, _P],
     'progen_adamw_step': [_P, _P, _P, _P, _P, _P, _LL, _LL, _P, _F, _F, _F, _F, _F, _F, _LL, _I, _P],

@@ -27,6 +27,28 @@ def _trunc_normal(rng, shape, std):
     return (r.reshape(shape) * std).astype(np.float32)
 
 
+def plan_launches(lengths, batch_size, by_length=False):
+    """The decoder launches of `ProGen.generate` for N = len(lengths) rows (lengths[r]: row r's prompt length).
+    Returns a list of (rows, real): rows is an int64 array of row indices, whose first `real` entries are the launch's rows
+    in row order and the rest padding.  Launches take up to per_launch = min(batch_size, N) rows; by_length (forward
+    prefill) runs only rows of one prompt length together, so every launch starts at the prefilled position of all its
+    rows.  A ragged launch is padded with copies of its last row (same prompt and stream, so it ends when that row does)
+    up to the smallest size of per_launch's class (1, 2-8 or 9-64 rows), which runs the same GEMV formulation and work
+    split as the full launches: a row's result depends only on the class, not on which rows share its launch."""
+    lengths = np.asarray(lengths, np.int64)
+    N = len(lengths)
+    per_launch = min(batch_size, N)
+    min_rows = 9 if per_launch > 8 else (2 if per_launch > 1 else 1)
+    groups = [np.flatnonzero(lengths == v) for v in np.unique(lengths)] if by_length else [np.arange(N)]
+    out = []
+    for g in groups:
+        for c0 in range(0, len(g), per_launch):
+            rows = g[c0:c0 + per_launch].astype(np.int64)
+            pad = max(0, min_rows - len(rows))
+            out.append((np.concatenate([rows, np.full(pad, rows[-1], np.int64)]), len(rows)))
+    return out
+
+
 class ProGen:
     def __init__(self, *, num_tokens, dim, seq_len, depth, window_size=256, global_mlp_depth=2, heads=8, dim_head=64,
                  ff_mult=4, ff_glu=True, attn_dim=None, clamp_gate=True, shift_tokens=True, mixed_precision=False,
@@ -134,7 +156,8 @@ class ProGen:
         return out
 
     def generate(self, params, prompts, *, num_samples=1, temperature=1.0, top_k=None, top_p=None, max_length=None, seed=0,
-                 batch_size=64, logit_bias=None, min_new_tokens=0, repetition_penalty=1.0, repetition_window=0):
+                 batch_size=64, logit_bias=None, min_new_tokens=0, repetition_penalty=1.0, repetition_window=0,
+                 prefill='decode'):
         """Sample sequences with the standard sampler of the persistent decode kernel (temperature, top-k with ties kept,
         nucleus top-p, in-kernel Philox Gumbel noise; csrc/decode_persist.cu), stopping each sequence at its EOS.
         Unlike the reference sampler (utils.sample, sample.py), a prompt is laid out as training data is: BOS (0), the
@@ -161,6 +184,15 @@ class ProGen:
         Only the ids whose adjusted logit is not -inf can be drawn.  token_logp and log_likelihood do not see the
         constraints: they stay the unfiltered model's at temperature 1, comparable with `score`.
 
+        prefill: how the positions before the first draw (BOS and the prompt but its last id) reach the decoder's caches.
+          'decode' (default): the decode kernel consumes them one position at a time, as it does generated positions.
+          'forward': one inference forward (the engine that `score` runs) over the distinct prompts of a launch fills the
+            caches, and the decode kernel starts at the last prompt id.  Faster for long prompts and for many samples of
+            one prompt; the caches carry the forward's arithmetic, so with mixed_precision (bf16 activations in the
+            forward, fp32 in the decoder) the results differ from 'decode' by round-off.  A launch then holds rows of one
+            prompt length only, so a row's result still depends only on (seed, row), the prompt and the launch class.
+          An empty prompt has nothing to prefill: both modes are the same there.
+
         Returns a dict of numpy arrays over the N = len(prompts) * num_samples rows:
           tokens [N, seq_len] int64: BOS, prompt, generated tokens, EOS, zeros;
           start [N] int64: position of the first generated token (1 + prompt length);
@@ -178,6 +210,8 @@ class ProGen:
                 raise L.ProgenError(f'generate: {what} must be an integer in [{lo}, {hi}], got {v!r}')
             return int(v)
 
+        if not isinstance(prefill, str) or prefill not in ('decode', 'forward'):
+            raise L.ProgenError(f"generate: prefill must be 'decode' or 'forward', got {prefill!r}")
         max_length = n if max_length is None else integer(max_length, 'max_length', 2, n)
         num_samples = integer(num_samples, 'num_samples', 1, 1 << 40)
         batch_size = integer(batch_size, 'batch_size', 1, 64)
@@ -230,25 +264,23 @@ class ProGen:
             ids.append(a)
         N = len(ids) * num_samples
         rows = [ids[r // num_samples] for r in range(N)]
-        per_launch = min(batch_size, N)
-        # a ragged last chunk is padded with copies of its last row (same prompt and stream, so it ends when that row does)
-        # up to the smallest size that runs the same GEMV formulation as the full chunks
-        min_rows = 9 if per_launch > 8 else (2 if per_launch > 1 else 1)
-        dec = self._generate_decoder(params, per_launch)
+        launches = plan_launches([len(a) for a in rows], batch_size, by_length=prefill == 'forward')
+        dec = self._generate_decoder(params, min(batch_size, N))
+        if prefill == 'forward':
+            self._ensure_loaded(params)
         out = dict(tokens=np.zeros((N, n), np.int64), start=np.zeros(N, np.int64), end=np.zeros(N, np.int64),
                    token_logp=np.zeros((N, n), np.float32))
-        for r0 in range(0, N, per_launch):
-            r1 = min(N, r0 + per_launch)
-            pad = max(0, min_rows - (r1 - r0))
-            chunk = rows[r0:r1] + [rows[r1 - 1]] * pad
-            sids = np.concatenate([np.arange(r0, r1), np.full(pad, r1 - 1)]).astype(np.int64)
+        for sids, real in launches:
+            chunk = [rows[r] for r in sids]
+            P = dec.prefill(self.engine, chunk) if prefill == 'forward' else 0
             res = dec.generate(chunk, temperature=temperature, top_k=top_k, top_p=top_p, seed=seed, sample_ids=sids,
                                max_length=max_length, logit_bias=logit_bias, min_new_tokens=min_new_tokens,
-                               repetition_penalty=repetition_penalty, repetition_window=repetition_window)
-            out['tokens'][r0:r1] = res['ids'][:r1 - r0]
-            out['token_logp'][r0:r1] = res['token_logp'][:r1 - r0]
-            out['start'][r0:r1] = res['start'][:r1 - r0]
-            out['end'][r0:r1] = res['end'][:r1 - r0]
+                               repetition_penalty=repetition_penalty, repetition_window=repetition_window, prefilled=P)
+            r = sids[:real]
+            out['tokens'][r] = res['ids'][:real]
+            out['token_logp'][r] = res['token_logp'][:real]
+            out['start'][r] = res['start'][:real]
+            out['end'][r] = res['end'][:real]
         end = out.pop('end')
         out['finished'] = end < max_length
         out['length'] = np.where(out['finished'], end + 1, max_length) - out['start']

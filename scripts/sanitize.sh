@@ -23,6 +23,11 @@ timeout 900 compute-sanitizer --tool "$tool" --error-exitcode 9 --print-limit 20
   python -m pytest tests/test_gpu_generate_constraints.py -x -q -m gpu -k "test_reference_sampler_after_constrained_generate or test_min_length_binds_at_24_rows" \
   -p no:cacheprovider > "$out/sanitize_${tool}_constraints.log" 2>&1
 echo "constraints: exit $? : $(grep -E 'ERROR SUMMARY|passed|failed' "$out/sanitize_${tool}_constraints.log" | tail -n 2 | tr '\n' ' ')"
+# forward prefill: the cache scatter from fp32 and bf16 forwards into 1 and 24 decoder rows, and the decode launch after it
+timeout 900 compute-sanitizer --tool "$tool" --error-exitcode 9 --print-limit 20 \
+  python -m pytest tests/test_gpu_generate_prefill.py -x -q -m gpu -k "test_scatter_at_1_and_24_rows" \
+  -p no:cacheprovider > "$out/sanitize_${tool}_prefill.log" 2>&1
+echo "prefill: exit $? : $(grep -E 'ERROR SUMMARY|passed|failed' "$out/sanitize_${tool}_prefill.log" | tail -n 2 | tr '\n' ' ')"
 # kernels the tiny model configs do not reach: many-tile / tail GEMMs (all epilogues), wgmma attention, streaming LN backward
 timeout 1200 compute-sanitizer --tool "$tool" --error-exitcode 9 --print-limit 20 \
   python -m pytest tests/test_gpu_gemm_tc.py tests/test_gpu_attn_tc.py tests/test_gpu_elementwise.py -x -q -m gpu \
