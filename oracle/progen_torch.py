@@ -8,6 +8,10 @@ intra-op threads), because the reference's Jax path cannot be installed here or 
 
 `operand_round` (optional) is applied to every GEMM / attention operand; passing a bf16 round-trip predicts the
 error of a bf16-operand / fp32-accumulate engine on CPU before spending GPU time.
+
+`device` (optional, default CPU) runs the same algorithm on another torch device, for shapes where float64 on the host is
+too slow (tests/test_gpu_large_configs.py).  Tables (rotary) are computed on the host in float64 either way and then moved,
+so only the GEMM / reduction order of the device differs.
 """
 import math
 import torch
@@ -15,12 +19,12 @@ import torch
 from .progen_ref import P, layer_kinds, ATTN_MASK_VALUE, LN_EPS
 
 
-def to_torch(params, dtype=torch.float64, requires_grad=False):
+def to_torch(params, dtype=torch.float64, requires_grad=False, device=None):
     out = {}
     for m, d in params.items():
         out[m] = {}
         for k, v in d.items():
-            t = torch.tensor(v, dtype=dtype)
+            t = torch.tensor(v, dtype=dtype, device=device)
             t.requires_grad_(requires_grad)
             out[m][k] = t
     return out
@@ -54,16 +58,18 @@ def _rot(x, sin, cos):
     return x * cos + x2 * sin
 
 
-def forward(prm, ids, cfg, operand_round=None):
-    """prm: nested dict of tensors; ids: (B, n) long -> logits (B, n, V)."""
+def forward(prm, ids, cfg, operand_round=None, device=None):
+    """prm: nested dict of tensors on `device` (default CPU); ids: (B, n) long -> logits (B, n, V)."""
     r = operand_round or (lambda t: t)
+    dev = torch.device('cpu') if device is None else torch.device(device)
+    ids = ids.to(dev)
     B, n = ids.shape
     h, dh, w = cfg['heads'], cfg['dim_head'], cfg['window_size']
     W = n // w
     x = prm[P + 'embed']['embeddings'][ids.clamp(0, cfg['num_tokens'] - 1)]     # jax gather clamps
     dtype = x.dtype
-    sin, cos = _rotary_tables(n, dh, dtype)
-    mask = torch.tril(torch.ones(w, 2 * w, dtype=torch.bool), w)
+    sin, cos = (t.to(dev) for t in _rotary_tables(n, dh, dtype))
+    mask = torch.tril(torch.ones(w, 2 * w, dtype=torch.bool, device=dev), w)
     for i, kind in enumerate(layer_kinds(cfg)):
         a = P + f'attn{i}/~/'
         y = _ln(x, prm[a + 'layer_norm']['scale'])
@@ -96,7 +102,7 @@ def forward(prm, ids, cfg, operand_round=None):
         if kind == 'sgu':
             xs, gate = u.chunk(2, dim=-1)
             gate = _ln(gate, prm[f + 'sgu/~/layer_norm']['scale'])
-            wts = prm[f + 'sgu']['spatial_weights'] * torch.tril(torch.ones(n, n, dtype=dtype))
+            wts = prm[f + 'sgu']['spatial_weights'] * torch.tril(torch.ones(n, n, dtype=dtype, device=dev))
             gate = torch.einsum('mk,bkd->bmd', r(wts), r(gate)) + prm[f + 'sgu']['spatial_biases']
             u = xs * gate
             u = r(u) @ r(prm[f + 'sgu/~/linear']['w']) + prm[f + 'sgu/~/linear']['b']
@@ -114,20 +120,22 @@ def cross_entropy(logits, targets, ignore_index=0):
     return -(nll * mask).sum(-1) / mask.sum(-1)
 
 
-def batch_loss(prm, data, cfg, operand_round=None):
+def batch_loss(prm, data, cfg, operand_round=None, device=None):
     """data: (B, n+1) long -> scalar (mean over rows of per-row CE), utils.py:61-76."""
     ids, labels = data[:, :-1], data[:, 1:]
-    return cross_entropy(forward(prm, ids, cfg, operand_round), labels).mean()
+    logits = forward(prm, ids, cfg, operand_round, device)
+    return cross_entropy(logits, labels.to(logits.device)).mean()
 
 
-def loss_and_grads(params_np, data_np, cfg, dtype=torch.float64, operand_round=None):
+def loss_and_grads(params_np, data_np, cfg, dtype=torch.float64, operand_round=None, device=None):
     """`operand_round=bf16_round` (with dtype=float32) is the CPU emulation of a bf16-operand / fp32-accumulate engine:
-    autograd sends the gradients through the same casts, so the backward GEMM operands are rounded as well."""
-    prm = to_torch(params_np, dtype, requires_grad=True)
+    autograd sends the gradients through the same casts, so the backward GEMM operands are rounded as well.
+    `device` (default CPU) is where the evaluation runs; the gradients come back as host numpy arrays."""
+    prm = to_torch(params_np, dtype, requires_grad=True, device=device)
     data = torch.as_tensor(data_np.astype('int64'))
-    loss = batch_loss(prm, data, cfg, operand_round)
+    loss = batch_loss(prm, data, cfg, operand_round, device)
     loss.backward()
-    grads = {m: {k: v.grad.numpy().copy() for k, v in d.items()} for m, d in prm.items()}
+    grads = {m: {k: v.grad.cpu().numpy().copy() for k, v in d.items()} for m, d in prm.items()}
     return float(loss.detach()), grads
 
 

@@ -302,7 +302,10 @@ int ln_shift_bwd_stream_launch(const void* dy, long long lddy, int act_dtype, co
   static int enabled = [] { const char* e = getenv("PROGEN_LN_STREAM"); return e ? atoi(e) : 1; }();
   if (!enabled) return 1;
   const int so = act_dtype == PG_BF16 ? 2 : 4, si = x_dtype == PG_BF16 ? 2 : 4;
-  const int rbt = d > 1024 ? 4 : RB;             // rows per stage: wide rows (config 4: d = 1536, gMLP 2d = 2048) take 4 so that >= 3 stages fit
+  // rows per stage: rows wider than 1024 take 4, so that >= 3 stages fit for config 4's residual rows (d = 1536) and
+  // config 3's gMLP gate rows (2d = 2048).  Config 4's gMLP gate rows (2d = 3072) are wider than 2048: the caller runs
+  // them on the row-per-warp kernel.
+  const int rbt = d > 1024 ? 4 : RB;
   if (T % RB != 0 || T % seq_len != 0 || d % 128 != 0 || d > 2048 || T < 8 * RB) return 1;
   // every bulk copy: 16-byte aligned addresses and sizes
   if ((lddy * so) % 16 || (ldx * si) % 16 || (ldo * so) % 16) return 1;

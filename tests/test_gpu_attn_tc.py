@@ -21,6 +21,11 @@ def _qkv(B, n, h, dh, seed):
 @pytest.mark.parametrize('cfg', SHAPES)
 def test_local_attn_tc_fwd(cfg):
     """forward vs the float64 reference, and output and log-sum-exp vs the fp32 simt kernel on the same bf16 input"""
+    check_fwd(cfg)
+
+
+def check_fwd(cfg):
+    """the checks of test_local_attn_tc_fwd at shape cfg = (B, n, w, h); returns (qkv, out, lse) for further checks"""
     from progen_b200 import lib as L
     L.require_device()
     B, n, w, h = cfg
@@ -40,6 +45,7 @@ def test_local_attn_tc_fwd(cfg):
     L.check(L.load().progen_local_attn_fwd_simt(qkv.data_ptr(), out2.data_ptr(), lse2.data_ptr(), L.BF16, B, n, w, h, dh, L.stream()))
     assert (lse - lse2).abs().max().item() < 2e-3
     assert (out.float() - out2.float()).abs().max().item() < 2e-2
+    return qkv, out, lse
 
 
 @pytest.mark.parametrize('cfg', SHAPES)
@@ -47,6 +53,11 @@ def test_local_attn_tc_fwd(cfg):
 def test_local_attn_tc_bwd(cfg, fused_rotary):
     """backward on the tensor-core forward's out and lse vs torch float64 autograd of the reference attention on the same
     bf16 q|k|v; with fused_rotary, also vs the unfused kernel's gradient with the rotary backward applied in torch"""
+    check_bwd(cfg, fused_rotary)
+
+
+def check_bwd(cfg, fused_rotary):
+    """the checks of test_local_attn_tc_bwd at shape cfg = (B, n, w, h)"""
     from progen_b200 import lib as L
     from gemm_cases import rotary_tables
     L.require_device()
