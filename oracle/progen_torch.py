@@ -58,8 +58,9 @@ def _rot(x, sin, cos):
     return x * cos + x2 * sin
 
 
-def forward(prm, ids, cfg, operand_round=None, device=None):
-    """prm: nested dict of tensors on `device` (default CPU); ids: (B, n) long -> logits (B, n, V)."""
+def forward(prm, ids, cfg, operand_round=None, device=None, return_hidden=False):
+    """prm: nested dict of tensors on `device` (default CPU); ids: (B, n) long -> logits (B, n, V), or with
+    `return_hidden` (logits, the final LayerNorm output (B, n, d): the head's input, which scoring pools)."""
     r = operand_round or (lambda t: t)
     dev = torch.device('cpu') if device is None else torch.device(device)
     ids = ids.to(dev)
@@ -108,7 +109,8 @@ def forward(prm, ids, cfg, operand_round=None, device=None):
             u = r(u) @ r(prm[f + 'sgu/~/linear']['w']) + prm[f + 'sgu/~/linear']['b']
         x = x + r(u) @ r(prm[f + 'linear_1']['w']) + prm[f + 'linear_1']['b']
     x = _ln(x, prm[P + 'layer_norm']['scale'])
-    return r(x) @ r(prm[P + 'linear']['w']) + prm[P + 'linear']['b']
+    logits = r(x) @ r(prm[P + 'linear']['w']) + prm[P + 'linear']['b']
+    return (logits, x) if return_hidden else logits
 
 
 def cross_entropy(logits, targets, ignore_index=0):

@@ -57,6 +57,23 @@ def test_torch_twin_matches_numpy_oracle_and_grad_fingerprints(name):
         np.testing.assert_allclose(np.resize(gr.ravel()[:8], 8), head, rtol=0, atol=1e-12)
 
 
+def test_torch_twin_hidden_state():
+    """return_hidden leaves the logits bit-identical and returns the head's input: the final LayerNorm output, which is
+    the [I | 0]-head read of the numpy oracle's hidden state"""
+    cfg, params, data, g = load_case('tiny_glu_sgu')
+    prm = T.to_torch(params)
+    ids = torch.as_tensor(data[:, :-1].astype(np.int64))
+    logits, hidden = T.forward(prm, ids, cfg, return_hidden=True)
+    assert torch.equal(logits, T.forward(prm, ids, cfg))
+    head = prm[O.P + 'linear']
+    assert torch.equal(hidden @ head['w'] + head['b'], logits)
+    d, V = cfg['dim'], cfg['num_tokens']
+    p = dict(params)
+    p[O.P + 'linear'] = {'w': np.eye(d, V, dtype=np.float32), 'b': np.zeros(V, np.float32)}
+    ref = np.stack([O.forward(p, r, cfg)[:, :d] for r in data[:, :-1]])
+    np.testing.assert_allclose(hidden.numpy(), ref, rtol=0, atol=1e-11)
+
+
 def test_torch_twin_gradients_match_finite_differences():
     cfg, params, data, g = load_case('tiny_glu_sgu')
     _, grads = T.loss_and_grads(params, data, cfg)
