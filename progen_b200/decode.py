@@ -57,6 +57,16 @@ class BatchDecoder:
         d, n = cfg['dim'], cfg['seq_len']
         I = cfg['heads'] * cfg['dim_head']
         hid = d * cfg['ff_mult']
+        # the shapes progen_decode_run accepts, refused here before any device buffer is allocated
+        limits = [(cfg['dim_head'] in (8, 16, 32, 64), f"dim_head in {{8, 16, 32, 64}} (got {cfg['dim_head']})"),
+                  (hid % 256 == 0, f"dim * ff_mult a multiple of 256 (got {hid})"),
+                  (d % 8 == 0 and I % 8 == 0, f'dim and heads * dim_head multiples of 8 (got {d}, {I})'),
+                  (max(d, I, hid) <= 8192, f'dim, heads * dim_head and dim * ff_mult <= 8192 (got {d}, {I}, {hid})'),
+                  (cfg['num_tokens'] % 2 == 0 and cfg['num_tokens'] <= 512, f"an even num_tokens <= 512 (got {cfg['num_tokens']})"),
+                  (1 <= cfg['window_size'] <= 512, f"window_size <= 512 (got {cfg['window_size']})")]
+        for ok, what in limits:
+            if not ok:
+                raise L.ProgenError(f'BatchDecoder: the persistent decode kernel needs {what}')
         self.n, self.V = n, cfg['num_tokens']
         self.keep = []
         f32 = lambda a: self._hold(torch.tensor(np.ascontiguousarray(np.asarray(a, np.float32)), device=self.dev))
