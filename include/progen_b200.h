@@ -264,6 +264,23 @@ typedef struct progen_decode_run_t {
   int32_t repetition_window;   /* >= 0; 0 = every position since BOS */
   int32_t min_new_tokens;      /* >= 0: the first min_new_tokens draws of a row are never EOS */
   int32_t _pad2;
+  /* Row queue (sampler 1, B >= 2; all NULL / 0 = no queue): the B sequences of the launch become slots that decode the
+   * Q = num_rows rows of a queue.  seq, start, end, token_logp and sample_id are then indexed by the queue row ([Q] /
+   * [Q, n]); caches and scratch stay per slot.  Slot b decodes row slot_row[b] (-1: idle) at position slot_pos[b], which
+   * it advances by one per step.  A row retires when it draws EOS or position max_length - 1; its slot counts it in
+   * `done` and claims q = next_row++: for q < Q the slot restarts at position 0 of row q (slot_pos = 0, token-shift
+   * slot 0 of every layer zeroed, x = embedding of seq[q][0]), otherwise it goes idle and writes nothing outside its own
+   * caches and scratch.  The launch ends after the sampler phase in which `done` reaches Q, or after nsteps steps
+   * (pos0 is not used: positions come from slot_pos).  A row's bits do not depend on its slot or on the other rows, so a
+   * queue gives the same rows as launches of B rows each (the attention and SGU plans are those of the batch tile's
+   * class).  The caller initialises slot_row[b] = b and slot_pos[b] in [0, max_length - 1) for every slot (Q >= B),
+   * next_row = B, done = 0, end[q] = n.  logits_all needs Q == B. */
+  int32_t* slot_row;           /* [B] device */
+  int32_t* slot_pos;           /* [B] device */
+  int32_t* next_row;           /* device: the next unclaimed queue row */
+  int32_t* done;               /* device: rows retired */
+  int32_t num_rows;            /* Q */
+  int32_t max_length;          /* in [2, n]: a row's last drawn position is max_length - 1 */
 } progen_decode_run_t;
 
 int progen_decode_run(const progen_decode_run_t* run, void* stream);

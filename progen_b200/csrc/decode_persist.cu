@@ -370,14 +370,19 @@ static __device__ __forceinline__ float4 merge_att(const Phase& ph, int k) {
 
 // One GEMV / skinny-GEMM phase over all B sequences.  BT = compile-time batch tile (B <= BT).  `w`, `pre` hold what
 // prefetch_phase loaded for THIS phase (the caller ran it before the previous grid barrier, or just now).
-template <int BT, typename TW>
+// SLOT (the queue kernels): sequence b is at position spos[b] (shared memory) instead of the shared ph.pos.
+template <int BT, typename TW, bool SLOT = false>
 static __device__ __forceinline__ void gemv_phase(const Phase& ph, int B, float* xs, float* part, float* stat, float* wsm, WRegs<TW>& w, const Pre& pre, const Prof& pf,
-                                           uint32_t sbar, uint32_t& sparity, bool reload_w0 = false) {
+                                           uint32_t sbar, uint32_t& sparity, bool reload_w0 = false, const int* spos = nullptr) {
   using TL = Tile<BT, sizeof(TW) == 2>;
   constexpr int KCB = TL::KCB, XP = TL::XP, BTP = TL::BTP;
   constexpr bool LANEB = TL::LANEB, TC = TL::TC;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const Geo g = ph.g;
+  auto pos_of = [&](int b) -> int {
+    if constexpr (SLOT) return spos[b];
+    else return ph.pos;
+  };
   const int nchunks = (ph.K + KCB - 1) / KCB;
   const int half = ph.K >> 1;
   bool staged = false;
@@ -457,7 +462,7 @@ static __device__ __forceinline__ void gemv_phase(const Phase& ph, int B, float*
       for (int j = 0; j < 2; ++j) {
         const int k = j * 128 + lane * 4;
         pvv[rr][j] = (ph.ln_prev && b < B && k < half)
-                         ? __ldcg(reinterpret_cast<const float4*>(ph.ln_prev + (long long)b * ph.K + (ph.pos & 1) * half + k)) : make_float4(0.f, 0.f, 0.f, 0.f);
+                         ? __ldcg(reinterpret_cast<const float4*>(ph.ln_prev + (long long)b * ph.K + (pos_of(b) & 1) * half + k)) : make_float4(0.f, 0.f, 0.f, 0.f);
       }
     }
     const float inv_k = 1.f / (float)ph.K;
@@ -506,7 +511,7 @@ static __device__ __forceinline__ void gemv_phase(const Phase& ph, int B, float*
           const int b = warp + rr * WPB;
           if (rr >= RPW || b >= B) continue;                 // warp-uniform
           float* xr = xs + b * XP + lane * 4;
-          float* st = ph.ln_prev ? ph.ln_prev + (long long)b * ph.K + ((ph.pos + 1) & 1) * half + lane * 4 : nullptr;
+          float* st = ph.ln_prev ? ph.ln_prev + (long long)b * ph.K + ((pos_of(b) + 1) & 1) * half + lane * 4 : nullptr;
 #pragma unroll
           for (int j = 0; j < NJ; ++j) {
             float4 t = make_float4(v[u][j].x * rstd[u] * sc[j].x, v[u][j].y * rstd[u] * sc[j].y, v[u][j].z * rstd[u] * sc[j].z, v[u][j].w * rstd[u] * sc[j].w);
@@ -546,7 +551,7 @@ static __device__ __forceinline__ void gemv_phase(const Phase& ph, int B, float*
           for (int j = 0; j < NJ / 2; ++j) {
             const int k = j * 128 + lane * 4;
             pvv[rr][j] = (ph.ln_prev && b < B && k < half)
-                             ? __ldcg(reinterpret_cast<const float4*>(ph.ln_prev + (long long)b * ph.K + (ph.pos & 1) * half + k)) : make_float4(0.f, 0.f, 0.f, 0.f);
+                             ? __ldcg(reinterpret_cast<const float4*>(ph.ln_prev + (long long)b * ph.K + (pos_of(b) & 1) * half + k)) : make_float4(0.f, 0.f, 0.f, 0.f);
           }
         }
 #pragma unroll
@@ -576,7 +581,7 @@ static __device__ __forceinline__ void gemv_phase(const Phase& ph, int B, float*
               t.x = (v[rr][j].x - mean) * rstd * sc.x; t.y = (v[rr][j].y - mean) * rstd * sc.y;
               t.z = (v[rr][j].z - mean) * rstd * sc.z; t.w = (v[rr][j].w - mean) * rstd * sc.w;
               if (st && k < half) {                         // k < half  =>  j < NJ / 2 (half = K / 2 <= NJ * 64)
-                if (blockIdx.x == 0) *reinterpret_cast<float4*>(st + ((ph.pos + 1) & 1) * half + k) = t;
+                if (blockIdx.x == 0) *reinterpret_cast<float4*>(st + ((pos_of(b) + 1) & 1) * half + k) = t;
                 t = pvv[rr][j < NJ / 2 ? j : 0];
               }
               *reinterpret_cast<float4*>(xs + b * XP + xs_off<BT>(k)) = t;
@@ -635,8 +640,8 @@ static __device__ __forceinline__ void gemv_phase(const Phase& ph, int B, float*
           v.z = (v.z - mean) * rstd * sc.z; v.w = (v.w - mean) * rstd * sc.w;
           if (ph.ln_prev && k0 + k < half) {
             float* st = ph.ln_prev + (long long)b * ph.K;            // [2][K/2]
-            const float4 pv = __ldcg(reinterpret_cast<const float4*>(st + (ph.pos & 1) * half + k0 + k));
-            if (blockIdx.x == 0) *reinterpret_cast<float4*>(st + ((ph.pos + 1) & 1) * half + k0 + k) = v;
+            const float4 pv = __ldcg(reinterpret_cast<const float4*>(st + (pos_of(b) & 1) * half + k0 + k));
+            if (blockIdx.x == 0) *reinterpret_cast<float4*>(st + ((pos_of(b) + 1) & 1) * half + k0 + k) = v;
             v = pv;
           }
         }
@@ -705,12 +710,12 @@ static __device__ __forceinline__ void gemv_phase(const Phase& ph, int B, float*
     else if (ph.epi == EP_GELU) { o[r0] = gelu_tanh(s0); o[r1] = gelu_tanh(s1); }
     else if (ph.epi == EP_GLU) { o[r0] = s0 * gelu_tanh(s1); }
     else {  // EP_ROTARY_CACHE: rotary on q, k AND v (progen.py:87); k, v rows go to the caches at position pos
-      const int hd = ph.dim_head >> 1, j = (r0 % ph.dim_head) >> 1;
-      const float sn = pf ? pre.sn : ph.rot_sin[ph.pos * hd + j], cs = pf ? pre.cs : ph.rot_cos[ph.pos * hd + j];
+      const int hd = ph.dim_head >> 1, j = (r0 % ph.dim_head) >> 1, p = pos_of(b);
+      const float sn = pf ? pre.sn : ph.rot_sin[p * hd + j], cs = pf ? pre.cs : ph.rot_cos[p * hd + j];
       const float o0 = s0 * cs - s1 * sn, o1 = s1 * cs + s0 * sn;
       const int sec = r0 / ph.inner, c = r0 % ph.inner;
       float* dst = sec == 0 ? o + c
-                            : (sec == 1 ? ph.kcache : ph.vcache) + (((long long)b * (ph.inner / ph.dim_head) + c / ph.dim_head) * ph.n + ph.pos) * ph.dim_head + c % ph.dim_head;
+                            : (sec == 1 ? ph.kcache : ph.vcache) + (((long long)b * (ph.inner / ph.dim_head) + c / ph.dim_head) * ph.n + p) * ph.dim_head + c % ph.dim_head;
       dst[0] = o0; dst[1] = o1;
     }
   };
@@ -843,7 +848,8 @@ static __device__ __forceinline__ void gemv_phase(const Phase& ph, int B, float*
         for (int nt = 0; nt < NTMAX; ++nt) { acc[nt][0] = acc[nt][1] = acc[nt][2] = acc[nt][3] = 0.f; }
         // epilogue operands of n-tiles n0, n0 + 1 for this lane's two sequences (b0, b0 + 8) and pair 4 nt + (lane & 3)
         const int b0 = mt * 16 + gr;
-        auto load_ops = [&](int n0, float (&bia)[2][2], float (&old)[2][4], float (&rot)[2][2]) {
+        constexpr int NRH = SLOT ? 2 : 1;                      // rotary entries per (n-tile, sequence): the two sequences' positions differ
+        auto load_ops = [&](int n0, float (&bia)[2][2], float (&old)[2][4], float (&rot)[2][NRH][2]) {
 #pragma unroll
           for (int u = 0; u < 2; ++u) {
             const int nt = n0 + u;
@@ -860,14 +866,18 @@ static __device__ __forceinline__ void gemv_phase(const Phase& ph, int B, float*
               old[u][0] = __ldcg(o0 + r0); old[u][1] = __ldcg(o0 + r1);
               old[u][2] = __ldcg(o1 + r0); old[u][3] = __ldcg(o1 + r1);
             }
-            rot[u][0] = rot[u][1] = 0.f;
-            if (ph.epi == EP_ROTARY_CACHE) {
-              const int hd = ph.dim_head >> 1, j = (r0 % ph.dim_head) >> 1;
-              rot[u][0] = ph.rot_sin[ph.pos * hd + j]; rot[u][1] = ph.rot_cos[ph.pos * hd + j];
+#pragma unroll
+            for (int hb = 0; hb < NRH; ++hb) {
+              rot[u][hb][0] = rot[u][hb][1] = 0.f;
+              if (ph.epi == EP_ROTARY_CACHE) {
+                const int hd = ph.dim_head >> 1, j = (r0 % ph.dim_head) >> 1;
+                const int p = pos_of(b0 + 8 * hb < B ? b0 + 8 * hb : 0);
+                rot[u][hb][0] = ph.rot_sin[p * hd + j]; rot[u][hb][1] = ph.rot_cos[p * hd + j];
+              }
             }
           }
         };
-        float bia0[2][2], old0[2][4], rot0[2][2];
+        float bia0[2][2], old0[2][4], rot0[2][NRH][2];
         load_ops(0, bia0, old0, rot0);                         // in flight under the MMA loop (every warp: kh is only known to be 0 later)
         for (int kc = 0; kc < nchunks; ++kc) {
           __syncthreads();                                     // wsm written (kc == 0) / the previous chunk's xs readers done
@@ -947,11 +957,13 @@ static __device__ __forceinline__ void gemv_phase(const Phase& ph, int B, float*
 #pragma unroll
           for (int n0 = 0; n0 < NTMAX; n0 += 2) {
             if (n0 >= NT) continue;                            // (no break: the loop must unroll, acc[] is indexed statically)
-            float bia[2][2], old[2][4], rot[2][2];
+            float bia[2][2], old[2][4], rot[2][NRH][2];
             if (n0 == 0) {
 #pragma unroll
               for (int u = 0; u < 2; ++u) {
-                bia[u][0] = bia0[u][0]; bia[u][1] = bia0[u][1]; rot[u][0] = rot0[u][0]; rot[u][1] = rot0[u][1];
+                bia[u][0] = bia0[u][0]; bia[u][1] = bia0[u][1];
+#pragma unroll
+                for (int hb = 0; hb < NRH; ++hb) { rot[u][hb][0] = rot0[u][hb][0]; rot[u][hb][1] = rot0[u][hb][1]; }
                 old[u][0] = old0[u][0]; old[u][1] = old0[u][1]; old[u][2] = old0[u][2]; old[u][3] = old0[u][3];
               }
             } else {
@@ -975,9 +987,9 @@ static __device__ __forceinline__ void gemv_phase(const Phase& ph, int B, float*
                   else if (ph.epi == EP_GELU) { o[r0] = gelu_tanh(s0); o[r1] = gelu_tanh(s1); }
                   else if (ph.epi == EP_GLU) { o[r0] = s0 * gelu_tanh(s1); }
                   else {
-                    const float sn = rot[u][0], cs = rot[u][1];
+                    const float sn = rot[u][SLOT ? hb : 0][0], cs = rot[u][SLOT ? hb : 0][1];
                     const int sec = r0 / ph.inner, c = r0 % ph.inner;
-                    float* dst = sec == 0 ? o + c : (sec == 1 ? ph.kcache : ph.vcache) + (((long long)b * (ph.inner / ph.dim_head) + c / ph.dim_head) * ph.n + ph.pos) * ph.dim_head + c % ph.dim_head;
+                    float* dst = sec == 0 ? o + c : (sec == 1 ? ph.kcache : ph.vcache) + (((long long)b * (ph.inner / ph.dim_head) + c / ph.dim_head) * ph.n + pos_of(b)) * ph.dim_head + c % ph.dim_head;
                     dst[0] = s0 * cs - s1 * sn; dst[1] = s1 * cs + s0 * sn;
                   }
                 }
@@ -1058,6 +1070,9 @@ static __device__ __forceinline__ void gemv_phase(const Phase& ph, int B, float*
 }
 
 // ------------------------------------------------------------------------------------------------ attention
+// the queue kernels' per-slot positions, passed as a pack of one pointer (empty in the other kernels)
+static __device__ __forceinline__ const int* slot_pos_of() { return nullptr; }
+static __device__ __forceinline__ const int* slot_pos_of(const int* p) { return p; }
 // task = (sequence, head, slice of 32 keys), one warp: partial (m, l, o[dh]) -> att_part[(b, head)][slice][dh + 4].  All of
 // the task's K and V loads are independent of each other (lane = key for the logits; lane = (key group, 4 channels) for
 // the value sum), so a task is ONE memory round trip.  The out-proj phase merges the partials (plus window 0's w zero keys
@@ -1138,16 +1153,19 @@ static __device__ void attention_phase_t(const progen_decode_run_t& r, const flo
 // Two lanes per key for the logits (half a key row each: 32 registers at dim_head 64), lane = (key group, 4 channels) for
 // the value sum; every load of a slice is independent of the others.
 // PLAN: the number of sequences the work split is planned for (0: the launch's B; see run())
-template <int NL, int PLAN>
-static __device__ void attention_batch_t(const progen_decode_run_t& r, const float* kcache, const float* vcache, int pos, float* sq /* smem >= WPB * (2 dh + 4) */) {
+// SLOT (the queue kernels): sequence b is at position spos[b] (shared memory); the window of each (sequence, head) follows it
+// (`spos` is a parameter pack, empty without SLOT, so the other kernels' calls stay as they were)
+template <int NL, int PLAN, bool SLOT, typename... SP>
+static __device__ void attention_batch_t(const progen_decode_run_t& r, const float* kcache, const float* vcache, int pos, float* sq /* smem >= WPB * (2 dh + 4) */,
+                                         SP... spos) {
   static_assert(NL >= 2, "two lanes share a key row");
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   constexpr int dh = NL * 4, HK = NL / 2, KG = 32 / NL, NV = 16 / KG;
   const int w = r.window, I = r.inner;
-  const int win = pos / w, i = pos % w;
-  const int key0 = win > 0 ? (win - 1) * w : 0;
-  const int nreal = (win > 0 ? w : 0) + i + 1;
-  const int nsl = (nreal + 15) / 16;
+  int win = pos / w, i = pos % w;
+  int key0 = win > 0 ? (win - 1) * w : 0;
+  int nreal = (win > 0 ? w : 0) + i + 1;
+  int nsl = (nreal + 15) / 16;
   const int npairs = r.B * r.heads;
   int WP = 8;
   const int plan_pairs = PLAN > 0 ? PLAN * r.heads : npairs;
@@ -1166,6 +1184,13 @@ static __device__ void attention_batch_t(const progen_decode_run_t& r, const flo
     float m = -INFINITY, lsum = 0.f;
     float4 o = make_float4(0.f, 0.f, 0.f, 0.f);
     if (on) {
+      if constexpr (SLOT) {
+        const int p = slot_pos_of(spos...)[b];
+        win = p / w; i = p % w;
+        key0 = win > 0 ? (win - 1) * w : 0;
+        nreal = (win > 0 ? w : 0) + i + 1;
+        nsl = (nreal + 15) / 16;
+      }
       const float* qv = r.q + (long long)b * I + hh * dh;
       if (lane < NL) *reinterpret_cast<float4*>(q_s + lane * 4) = __ldcg(reinterpret_cast<const float4*>(qv + lane * 4));
       __syncwarp();
@@ -1247,13 +1272,13 @@ static __device__ void attention_batch_t(const progen_decode_run_t& r, const flo
     __syncthreads();
   }
 }
-template <int PLAN>
-static __device__ void attention_batch(const progen_decode_run_t& r, const float* kcache, const float* vcache, int pos, float* sq) {
+template <int PLAN, bool SLOT, typename... SP>
+static __device__ void attention_batch(const progen_decode_run_t& r, const float* kcache, const float* vcache, int pos, float* sq, SP... spos) {
   switch (r.dim_head) {
-    case 64: attention_batch_t<16, PLAN>(r, kcache, vcache, pos, sq); break;
-    case 32: attention_batch_t<8, PLAN>(r, kcache, vcache, pos, sq); break;
-    case 16: attention_batch_t<4, PLAN>(r, kcache, vcache, pos, sq); break;
-    default: attention_batch_t<2, PLAN>(r, kcache, vcache, pos, sq); break;
+    case 64: attention_batch_t<16, PLAN, SLOT>(r, kcache, vcache, pos, sq, spos...); break;
+    case 32: attention_batch_t<8, PLAN, SLOT>(r, kcache, vcache, pos, sq, spos...); break;
+    case 16: attention_batch_t<4, PLAN, SLOT>(r, kcache, vcache, pos, sq, spos...); break;
+    default: attention_batch_t<2, PLAN, SLOT>(r, kcache, vcache, pos, sq, spos...); break;
   }
 }
 
@@ -1278,8 +1303,10 @@ static __device__ __forceinline__ int sgu_splits(const progen_decode_run_t& r) {
   int s = (int)gridDim.x / (base > 0 ? base : 1);
   return s < 1 ? 1 : (s > MAXSPLIT ? MAXSPLIT : s);
 }
-template <int PLAN>
-static __device__ void sgu_phase(const progen_decode_run_t& r, const SguArgs& L, int pos, float* red /* smem [WPB][128] + stats */) {
+// SLOT (the queue kernels): sequence b is at position spos[b] (shared memory); its split boundaries follow that position
+template <int PLAN, bool SLOT, typename... SP>
+static __device__ void sgu_phase(const progen_decode_run_t& r, const SguArgs& L, int pos_, float* red /* smem [WPB][128] + stats */,
+                                 SP... spos) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int C = r.hid / 2, n = r.n;
   const int cblocks = C / 128;
@@ -1288,6 +1315,8 @@ static __device__ void sgu_phase(const progen_decode_run_t& r, const SguArgs& L,
   float* stat = red + WPB * 128;
   for (int t = blockIdx.x; t < tasks; t += gridDim.x) {
     const int sp = t % S, cb = (t / S) % cblocks, b = t / (S * cblocks);
+    int pos = pos_;
+    if constexpr (SLOT) pos = slot_pos_of(spos...)[b];
     const int c0 = cb * 128 + lane * 4;
     float* hist = L.hist + (long long)b * n * C;
     const float* wrow = L.w + (long long)pos * n;
@@ -1463,11 +1492,25 @@ static __device__ __forceinline__ float philox_gumbel(unsigned long long seed, l
 // Constraints (progen_b200.h): after logsumexp of the raw logits, sv is overwritten with the adjusted logits a, and the
 // filter and draw below run on a unchanged: -inf and NaN never win a comparison, so only candidates can be drawn.
 struct SampleCons { const float* bias; float theta; int window, min_new; };  // one argument: fewer registers at the call
+// The queue kernels' view of the slots (SLOT): this step's row and position of every slot (shared memory), the queue's
+// device state and what a refill resets.  Without a queue (slot_row null) srow[b] = b and spos[b] = the launch's position.
+struct SlotArgs {
+  const int* srow; const int* spos;
+  int32_t* slot_row; int32_t* slot_pos; int32_t* next_row; int32_t* done;
+  const progen_decode_layer_t* layers;
+  int depth, num_rows, max_length, shift_tokens;
+};
+static __device__ __forceinline__ SlotArgs slot_args() { return SlotArgs{}; }
+static __device__ __forceinline__ SlotArgs slot_args(const SlotArgs& s) { return s; }
+// SLOT: the queue kernels pass one SlotArgs (`slot`); the single-stream kernels pass none, so their call is unchanged
+template <bool SLOT, typename... SA>
 static __device__ __noinline__ void sample_std_phase(const float* logits, int32_t* seq, const int32_t* start, int32_t* end, int32_t* n_ended,
                                                      float* token_logp, float* logits_all, const float* embed, float* x,
                                                      const int64_t* sample_id, int n, int V, int d, int B, int top_k, float temp,
-                                                     float top_p, unsigned long long seed, SampleCons cs, int pos, float* sv, float* red) {
+                                                     float top_p, unsigned long long seed, SampleCons cs, int pos_, float* sv, float* red,
+                                                     SA... slot) {
   static_assert(TPB >= 256, "V <= 512: at most two ids per thread");
+  static_assert(sizeof...(SA) == (SLOT ? 1 : 0), "one SlotArgs with SLOT");
   const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
   float* qv = sv + V;                                                          // kept ids: q; removed: -1
   int* redi = reinterpret_cast<int*>(red + 32);
@@ -1512,16 +1555,49 @@ static __device__ __noinline__ void sample_std_phase(const float* logits, int32_
     }
     return fi;
   };
+  const SlotArgs S = slot_args(slot...);
+  // queue: slot b retires its row (counted in `done`), then claims the next row of the queue, q = next_row++.  A claimed
+  // row starts at position 0: the slot's token-shift slot 0 of every layer (the only state read at position 0 before it
+  // is written) is zeroed and x takes the embedding of the row's BOS.  With no row left the slot goes idle.
+  auto refill = [&](int b) {
+    __syncthreads();                                                           // the draw's readers of red / redi are done
+    if (t == 0) { atomicAdd(S.done, 1); redi[0] = atomicAdd(S.next_row, 1); }
+    __syncthreads();
+    const int q = redi[0];
+    const bool got = q < S.num_rows;
+    if (t == 0) { S.slot_row[b] = got ? q : -1; S.slot_pos[b] = 0; }
+    if (got && S.shift_tokens) {
+      for (int li = 0; li < S.depth; ++li) {
+        float* s1 = S.layers[li].shift1 + (long long)b * d;                    // [B][2][d/2]: slot 0 of row b
+        float* s2 = S.layers[li].shift2 + (long long)b * d;
+        for (int c = t; c < (d >> 1); c += TPB) { s1[c] = 0.f; s2[c] = 0.f; }
+      }
+    }
+    int id = got ? seq[(long long)q * n] : 0;
+    id = id < 0 ? 0 : (id >= V ? V - 1 : id);
+    for (int c = t * 4; c < d; c += TPB * 4)
+      *reinterpret_cast<float4*>(x + (long long)b * d + c) = *reinterpret_cast<const float4*>(embed + (long long)id * d + c);
+  };
   for (int b = blockIdx.x; b < B; b += gridDim.x) {
     __syncthreads();
     const float* lg = logits + (long long)b * V;
-    const long long row = (long long)b * n;
+    int rb = b, pos = pos_;                                                    // the row slot b decodes, and its position
+    if constexpr (SLOT) {
+      rb = S.srow[b]; pos = S.spos[b];
+      if (rb < 0) {                                                            // idle: only the slot's own scratch (x stays finite)
+        for (int c = t * 4; c < d; c += TPB * 4)
+          *reinterpret_cast<float4*>(x + (long long)b * d + c) = *reinterpret_cast<const float4*>(embed + c);
+        continue;
+      }
+    }
+    const long long row = (long long)rb * n;
     if (pos + 1 >= n) {
       if (logits_all) for (int c = t; c < V; c += TPB) logits_all[(row + pos) * V + c] = __ldcg(lg + c);
+      if constexpr (SLOT) { if (S.slot_row) refill(b); }
       continue;
     }
     int tok = seq[row + pos + 1];
-    const bool draw = pos + 1 >= start[b] && pos + 1 < end[b];                 // (after its EOS a sequence stays 0)
+    const bool draw = pos + 1 >= start[rb] && pos + 1 < end[rb];               // (after its EOS a sequence stays 0)
     if (draw || logits_all) {
       for (int c = t; c < V; c += TPB) {
         const float v = __ldcg(lg + c);
@@ -1550,7 +1626,7 @@ static __device__ __noinline__ void sample_std_phase(const float* logits, int32_
           }
           __syncthreads();
         }
-        const bool no_eos = pos + 1 < start[b] + cs.min_new;
+        const bool no_eos = pos + 1 < start[rb] + cs.min_new;
         float ma = -INFINITY;
         for (int c = t; c < V; c += TPB) {
           float a = sv[c];
@@ -1611,7 +1687,7 @@ static __device__ __noinline__ void sample_std_phase(const float* logits, int32_
         }
         float bv = -INFINITY;
         int bi = 0x7fffffff;
-        const long long sid = sample_id[b];
+        const long long sid = sample_id[rb];
         for (int c = t; c < V; c += TPB) {
           if (qv[c] < 0.f) continue;
           const float sc = sv[c] / temp + philox_gumbel(seed, sid, pos + 1, c);
@@ -1624,7 +1700,13 @@ static __device__ __noinline__ void sample_std_phase(const float* logits, int32_
       if (t == 0) {
         seq[row + pos + 1] = id;
         if (token_logp) token_logp[row + pos + 1] = (cons ? __ldcg(lg + id) : sv[id]) - lse;   // the raw logit
-        if (id == 0) { end[b] = pos + 1; atomicAdd(n_ended, 1); }
+        if (id == 0) { end[rb] = pos + 1; atomicAdd(n_ended, 1); }
+      }
+    }
+    if constexpr (SLOT) {
+      if (S.slot_row) {                                                        // retire at EOS or at the last position
+        if ((draw && tok == 0) || pos + 1 >= S.max_length - 1) { refill(b); continue; }
+        if (t == 0) S.slot_pos[b] = pos + 1;
       }
     }
     const int id = tok < 0 ? 0 : (tok >= V ? V - 1 : tok);
@@ -1748,15 +1830,36 @@ static __device__ __forceinline__ void run(const progen_decode_run_t& r) {
   WRegs<TW> w;
   Pre pre{};
   bool have = false;                                   // `w`, `pre` hold the next GEMV phase's prefetch
+  // The queue kernels (sampler 1, B > 1) keep a row and a position per slot (DESIGN.md §3.3): every phase reads
+  // slot b's position from s_pos[b], copied at the top of each step from slot_pos (which the sampler phase advances), or
+  // the launch's position for every slot when the launch has no queue.
+  constexpr bool SLOT = STD && BT > 1;
+  const bool queue = SLOT && r.slot_row != nullptr;
+  int* s_row = nullptr;
+  int* s_pos = nullptr;
+  if constexpr (SLOT) {
+    __shared__ int slot_sh[2 * 64];
+    s_row = slot_sh;
+    s_pos = slot_sh + 64;
+  }
   for (int step = 0; step < r.nsteps; ++step) {
     const int pos = r.pos0 + step;
     pf.on = r.prof != nullptr && step == r.nsteps - 1 && (blockIdx.x == 0 || blockIdx.x == gridDim.x - 1);
     pf.ev = 0;
+    if constexpr (SLOT) {
+      if (threadIdx.x < B) {
+        s_row[threadIdx.x] = queue ? __ldcg(r.slot_row + threadIdx.x) : (int)threadIdx.x;
+        s_pos[threadIdx.x] = queue ? __ldcg(r.slot_pos + threadIdx.x) : pos;
+      }
+      __syncthreads();
+    }
     if (step == 0) {
       // embedding of the launch's first position (later ones are written by the sampler phase)
       for (int idx = blockIdx.x * TPB + threadIdx.x; idx < B * (d >> 2); idx += gridDim.x * TPB) {
         const int b = idx / (d >> 2), c = (idx % (d >> 2)) * 4;
-        int id = r.seq[(long long)b * r.n + pos];
+        int id;
+        if constexpr (SLOT) id = s_row[b] < 0 ? 0 : r.seq[(long long)s_row[b] * r.n + s_pos[b]];
+        else id = r.seq[(long long)b * r.n + pos];
         id = id < 0 ? 0 : (id >= r.V ? r.V - 1 : id);
         *reinterpret_cast<float4*>(r.x + (long long)b * d + c) = *reinterpret_cast<const float4*>(r.embed + (long long)id * d + c);
       }
@@ -1772,7 +1875,7 @@ static __device__ __forceinline__ void run(const progen_decode_run_t& r) {
         if (!have) prefetch_phase<BT, TW>(ph, w, pre, use_tabs ? utab + e * WSEGS : nullptr, use_tabs ? ftab + e * WSEGS : nullptr);
         prof_mark(pf, 0);
         if (B <= BT) {
-          gemv_phase<BT, TW>(ph, B, xs, part, stat, wsm, w, pre, pf, sbar, sparity);
+          gemv_phase<BT, TW, SLOT>(ph, B, xs, part, stat, wsm, w, pre, pf, sbar, sparity, false, s_pos);
         } else {
           // more sequences than the batch tile: sub-batches of BT sequences run through the phase one after the other with
           // the same weights (per warp, 32 sequences cost 4 LayerNorm rows and 8 k-steps; a 64-wide tile costs twice that
@@ -1785,21 +1888,32 @@ static __device__ __forceinline__ void run(const progen_decode_run_t& r) {
             if (ps.ln_prev) ps.ln_prev += (long long)b0 * ps.K;
             if (ps.kcache) { ps.kcache += (long long)b0 * ps.n * ps.inner; ps.vcache += (long long)b0 * ps.n * ps.inner; }
             if (ps.pro == PRO_SGU) ps.aux += (long long)b0 * ps.K;
-            gemv_phase<BT, TW>(ps, min(BT, B - b0), xs, part, stat, wsm, w, pre, pf, sbar, sparity, b0 > 0);
+            gemv_phase<BT, TW, SLOT>(ps, min(BT, B - b0), xs, part, stat, wsm, w, pre, pf, sbar, sparity, b0 > 0, SLOT ? s_pos + b0 : nullptr);
           }
         }
         prof_mark(pf, 3);
         have = fetch_next = !(e == nph - 2 && step + 1 == r.nsteps);
       } else if (kind == K_ATT) {
-        if (MERGE_IN_ATT || !att_consumer) attention_batch<PLAN>(r, tab[e].ph.kcache, tab[e].ph.vcache, pos, red);
-        else attention_phase(r, tab[e].ph.kcache, tab[e].ph.vcache, pos, red);
+        if (MERGE_IN_ATT || !att_consumer) {
+          if constexpr (SLOT) attention_batch<PLAN, true>(r, tab[e].ph.kcache, tab[e].ph.vcache, pos, red, (const int*)s_pos);
+          else attention_batch<PLAN, false>(r, tab[e].ph.kcache, tab[e].ph.vcache, pos, red);
+        } else {
+          attention_phase(r, tab[e].ph.kcache, tab[e].ph.vcache, pos, red);
+        }
       } else if (kind == K_SGU) {
         const SguArgs sa{tab[e].ph.ln_scale, reinterpret_cast<const float*>(tab[e].ph.wt), tab[e].ph.bias, tab[e].ph.kcache};
-        sgu_phase<PLAN>(r, sa, pos, red);
+        if constexpr (SLOT) sgu_phase<PLAN, true>(r, sa, pos, red, (const int*)s_pos);
+        else sgu_phase<PLAN, false>(r, sa, pos, red);
+      } else if constexpr (SLOT) {
+        sample_std_phase<true>(r.logits, r.seq, r.start, r.end, r.n_ended, r.token_logp, r.logits_all, r.embed, r.x, r.sample_id, r.n, r.V,
+                               d, B, r.top_k, r.temperature, r.top_p, r.seed,
+                               SampleCons{r.logit_bias, r.repetition_penalty, r.repetition_window, r.min_new_tokens}, pos, xs, red,
+                               SlotArgs{s_row, s_pos, r.slot_row, r.slot_pos, r.next_row, r.done, r.layers, r.depth, r.num_rows,
+                                        r.max_length, r.shift_tokens});
       } else if constexpr (STD) {
-        sample_std_phase(r.logits, r.seq, r.start, r.end, r.n_ended, r.token_logp, r.logits_all, r.embed, r.x, r.sample_id, r.n, r.V,
-                         d, B, r.top_k, r.temperature, r.top_p, r.seed,
-                         SampleCons{r.logit_bias, r.repetition_penalty, r.repetition_window, r.min_new_tokens}, pos, xs, red);
+        sample_std_phase<false>(r.logits, r.seq, r.start, r.end, r.n_ended, r.token_logp, r.logits_all, r.embed, r.x, r.sample_id, r.n, r.V,
+                                d, B, r.top_k, r.temperature, r.top_p, r.seed,
+                                SampleCons{r.logit_bias, r.repetition_penalty, r.repetition_window, r.min_new_tokens}, pos, xs, red);
       } else {
         sample_phase(r, pos, xs, red);
       }
@@ -1816,10 +1930,16 @@ static __device__ __forceinline__ void run(const progen_decode_run_t& r) {
       grid_wait(r.grid_bar, round, pf, t0);
       if (STD && kind == K_SAMPLE) {
         // EOS early exit: the barrier above orders every CTA's count of this sampler phase before the read, and nothing
-        // writes the counter before the next sampler phase, so every CTA sees the same value and leaves together
+        // writes the counter before the next sampler phase, so every CTA sees the same value and leaves together.  With a
+        // queue the count is of retired rows (EOS or the last position), and the launch ends when all Q have retired.
+        const int32_t* cnt = r.n_ended;
+        int goal = B;
+        if constexpr (SLOT) {
+          if (queue) { cnt = r.done; goal = r.num_rows; }
+        }
         int ended;
-        asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(ended) : "l"(r.n_ended) : "memory");
-        if (ended >= B) {
+        asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(ended) : "l"(cnt) : "memory");
+        if (ended >= goal) {
           if (blockIdx.x == 0 && threadIdx.x == 0) *r.steps_run = step + 1;
           return;
         }
@@ -1845,6 +1965,7 @@ int launch_run_sampler(const progen_decode_run_t& r, cudaStream_t s) {
   size_t smem = IM::template decode_smem_bytes<BT, sizeof(TW) == 2>(r.depth, BT == 1);
   if (smem > IM::MAX_SMEM) smem = IM::template decode_smem_bytes<BT, sizeof(TW) == 2>(r.depth, false);   // deep model: no unit tables
   PG_CHECK_ARG(smem <= IM::MAX_SMEM);                                  // (the phase table itself: depth * 7 + 2 entries)
+  if (STD && BT > 1) PG_CHECK_ARG(smem + 2 * 64 * sizeof(int) <= IM::MAX_SMEM);   // + the queue kernels' slot table (static)
   auto kern = decode_persistent_kernel<BT, TW, STD>;
   static size_t set_for = 0;
   if (set_for < smem) {
@@ -1877,7 +1998,15 @@ int progen_decode_run(const progen_decode_run_t* r, void* stream) {
   PG_CHECK_ARG(r->d <= 8192 && r->inner <= 8192 && r->hid <= 8192);   // K segments of one pair fit a wave (KS <= WSEGS)
   PG_CHECK_ARG(r->dim_head >= 8 && r->dim_head <= 64 && (r->dim_head & (r->dim_head - 1)) == 0);   // float4 lanes per value row
   PG_CHECK_ARG(r->window >= 1 && r->window <= 512);                    // <= 32 key slices per (sequence, head)
-  PG_CHECK_ARG(r->pos0 >= 0 && r->pos0 + r->nsteps <= r->n);
+  // row queue: every field or none; sampler 1 on a batched tile only; at least one row per slot
+  const bool queue = r->slot_row != nullptr || r->slot_pos != nullptr || r->next_row != nullptr || r->done != nullptr ||
+                     r->num_rows != 0 || r->max_length != 0;
+  if (queue) {
+    PG_CHECK_ARG(r->sampler == 1 && r->B >= 2 && r->num_rows >= r->B && r->max_length >= 2 && r->max_length <= r->n);
+    PG_CHECK_ARG(r->slot_row != nullptr && r->slot_pos != nullptr && r->next_row != nullptr && r->done != nullptr);
+    PG_CHECK_ARG(r->logits_all == nullptr || r->num_rows == r->B);
+  }
+  PG_CHECK_ARG(r->pos0 >= 0 && (queue || r->pos0 + r->nsteps <= r->n));
   PG_CHECK_ARG(r->grid_bar != nullptr && r->att_count != nullptr && r->att_part != nullptr);
   PG_CHECK_ARG(r->sampler == 0 || r->sampler == 1);
   PG_CHECK_ARG(std::isfinite(r->repetition_penalty) && r->repetition_penalty > 0.f);

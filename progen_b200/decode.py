@@ -36,7 +36,8 @@ class DecodeRun(C.Structure):
                                   'logits_all', 'x', 'q', 'att', 'att_part', 'att_count', 'u', 'sg', 'pj', 'logits', 'grid_bar', 'prof')] + \
                [('sampler', _I), ('temperature', C.c_float), ('top_p', C.c_float), ('_pad1', _I), ('seed', C.c_uint64)] + \
                [(k, _P) for k in ('sample_id', 'token_logp', 'end', 'n_ended', 'steps_run', 'logit_bias')] + \
-               [('repetition_penalty', C.c_float), ('repetition_window', _I), ('min_new_tokens', _I), ('_pad2', _I)]
+               [('repetition_penalty', C.c_float), ('repetition_window', _I), ('min_new_tokens', _I), ('_pad2', _I)] + \
+               [(k, _P) for k in ('slot_row', 'slot_pos', 'next_row', 'done')] + [('num_rows', _I), ('max_length', _I)]
 
 
 class BatchDecoder:
@@ -301,34 +302,16 @@ class BatchDecoder:
         launch consumed before every row had ended, or its full length), device_s (that launch's device time) and
         prefill_s (device time of the launch that consumed the prompt positions before it, 0 when there was none)."""
         n = self.n
-        max_length = n if max_length is None else int(max_length)
         R = len(prompts)
         if not 1 <= R <= self.B:
             raise L.ProgenError(f'generate: 1 <= prompts <= {self.B}')
-        if not 2 <= max_length <= n:
-            raise L.ProgenError(f'generate: 2 <= max_length <= {n}')
-        if top_k is not None and not 1 <= int(top_k) <= self.V:
-            raise L.ProgenError(f'generate: 1 <= top_k <= {self.V}')
-        if top_p is not None and not 0.0 < float(top_p) <= 1.0:
-            raise L.ProgenError('generate: 0 < top_p <= 1')
-        if not (np.isfinite(temperature) and temperature >= 0):
-            raise L.ProgenError('generate: temperature must be finite and >= 0')
-        seq0, starts = self._rows(prompts, max_length)
+        max_length, seq0, starts, sids = self._sampler_rows(prompts, sample_ids, max_length)
         first = int(starts.min()) - 1                     # the first drawn position is start; it reads the logits of start - 1
         if not 0 <= int(prefilled) <= first:
             raise L.ProgenError(f'generate: prefilled must lie in [0, {first}] (the shortest prompt length)')
         prefilled = int(prefilled)
-        sids = np.arange(R, dtype=np.int64) if sample_ids is None else np.asarray(sample_ids, np.int64).reshape(-1)
-        if sids.shape != (R,):
-            raise L.ProgenError('generate: one sample id per prompt')
-        if logit_bias is not None:
-            logit_bias = np.asarray(logit_bias, np.float32)
-            if logit_bias.shape != (self.V,) or np.isnan(logit_bias).any() or (logit_bias == np.inf).any():
-                raise L.ProgenError(f'generate: logit_bias must be {self.V} floats without NaN or +inf')
-        if not 0 <= int(min_new_tokens) <= n or not 0 <= int(repetition_window) <= n:
-            raise L.ProgenError(f'generate: min_new_tokens and repetition_window must lie in [0, {n}]')
-        if not (np.isfinite(repetition_penalty) and repetition_penalty > 0):
-            raise L.ProgenError('generate: repetition_penalty must be finite and > 0')
+        logit_bias = self._check_sampler(temperature, top_k, top_p, logit_bias, min_new_tokens, repetition_penalty,
+                                         repetition_window)
         if self._gen is None:
             z = lambda *s, dtype: torch.zeros(*s, device=self.dev, dtype=dtype)
             self._gen = dict(sample_id=z(self.B, dtype=torch.int64), token_logp=z(self.B, n, dtype=torch.float32),
@@ -343,20 +326,10 @@ class BatchDecoder:
         gb['end'].fill_(n)
         gb['counters'].zero_()                            # [n_ended, steps_run]
         m = self.m
-        m.B, m.sampler = R, 1
-        m.temperature = float(temperature)
-        m.top_k = int(top_k) if top_k is not None else 0
-        m.top_p = float(top_p) if top_p is not None else 1.0
-        m.seed = int(seed) & 0xFFFFFFFFFFFFFFFF
+        m.B = R
         m.sample_id, m.token_logp, m.end = gb['sample_id'].data_ptr(), gb['token_logp'].data_ptr(), gb['end'].data_ptr()
         m.n_ended, m.steps_run = gb['counters'].data_ptr(), gb['counters'].data_ptr() + 4
-        if logit_bias is not None:
-            if self._bias is None:
-                self._bias = torch.zeros(self.V, device=self.dev, dtype=torch.float32)
-            self._bias.copy_(torch.from_numpy(logit_bias))
-            m.logit_bias = self._bias.data_ptr()
-        m.repetition_penalty = float(repetition_penalty)
-        m.repetition_window, m.min_new_tokens = int(repetition_window), int(min_new_tokens)
+        self._set_sampler(temperature, top_k, top_p, seed, logit_bias, min_new_tokens, repetition_penalty, repetition_window)
         try:
             ev = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
             e0, e1 = ev[1], ev[2]
@@ -368,13 +341,118 @@ class BatchDecoder:
             e1.record()
             torch.cuda.synchronize()
         finally:
-            m.B, m.sampler, m.top_k = self.B, 0, 0
-            m.temperature, m.top_p, m.seed = 0.0, 0.0, 0
-            m.sample_id = m.token_logp = m.end = m.n_ended = m.steps_run = m.logit_bias = 0
-            m.repetition_penalty, m.repetition_window, m.min_new_tokens = 1.0, 0, 0
+            self._clear_sampler()
         return dict(ids=self.seq[:R].cpu().numpy().astype(np.int64), token_logp=gb['token_logp'][:R].cpu().numpy(),
                     end=gb['end'][:R].cpu().numpy(), start=starts, steps_run=int(gb['counters'][1].item()),
                     device_s=e0.elapsed_time(e1) / 1e3, prefill_s=ev[0].elapsed_time(e0) / 1e3)
+
+    def generate_queue(self, prompts, *, slots=None, temperature=1.0, top_k=None, top_p=None, seed=0, sample_ids=None,
+                       max_length=None, logit_bias=None, min_new_tokens=0, repetition_penalty=1.0, repetition_window=0):
+        """`generate` for Q = len(prompts) rows on `slots` (default min(B, Q), 2 <= slots <= min(B, Q)) sequences of ONE
+        persistent launch: the rows form a queue, and a slot whose row ends (EOS, or position max_length - 1) takes the
+        next row, which starts at position 0 with its prompt decoded like generated positions (csrc/decode_persist.cu,
+        progen_b200.h).  A row's bits depend on its seed, sample id, prompt, the class of `slots` (2-8 or 9-64) and
+        the GPU's SM count, not on its slot or the other rows, so each row equals what `generate` gives it in a launch of
+        that class; the launch merely has no slot waiting for its longest row.  Returns the arrays of `generate` over the
+        Q rows, steps_run (positions the launch ran) and device_s (its device time)."""
+        n = self.n
+        Q = len(prompts)
+        slots = min(self.B, Q) if slots is None else int(slots)
+        if not 2 <= slots <= min(self.B, Q):
+            raise L.ProgenError(f'generate_queue: 2 <= slots <= min(batch {self.B}, rows {Q})')
+        max_length, seq0, starts, sids = self._sampler_rows(prompts, sample_ids, max_length)
+        logit_bias = self._check_sampler(temperature, top_k, top_p, logit_bias, min_new_tokens, repetition_penalty,
+                                         repetition_window)
+        dev = self.dev
+        seq = torch.as_tensor(seq0).to(dev)
+        start = torch.as_tensor(starts).to(dev)
+        sample_id = torch.as_tensor(sids).to(dev)
+        token_logp = torch.zeros(Q, n, device=dev, dtype=torch.float32)
+        end = torch.full((Q,), n, device=dev, dtype=torch.int32)
+        slot_row = torch.arange(slots, device=dev, dtype=torch.int32)
+        slot_pos = torch.zeros(slots, device=dev, dtype=torch.int32)
+        counters = torch.tensor([0, 0, slots, 0], device=dev, dtype=torch.int32)   # [n_ended, steps_run, next_row, done]
+        self.reset()                                      # (token-shift slot 0 must be zero at position 0)
+        m = self.m
+        m.B, m.seq, m.start = slots, seq.data_ptr(), start.data_ptr()
+        m.sample_id, m.token_logp, m.end = sample_id.data_ptr(), token_logp.data_ptr(), end.data_ptr()
+        c = counters.data_ptr()
+        m.n_ended, m.steps_run, m.next_row, m.done = c, c + 4, c + 8, c + 12
+        m.slot_row, m.slot_pos, m.num_rows, m.max_length = slot_row.data_ptr(), slot_pos.data_ptr(), Q, max_length
+        self._set_sampler(temperature, top_k, top_p, seed, logit_bias, min_new_tokens, repetition_penalty, repetition_window)
+        # while rows wait in the queue every slot is busy, and a row consumes at most max_length - 1 positions
+        nsteps = -(-Q * (max_length - 1) // slots) + max_length - 1
+        try:
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            self.run(0, nsteps)
+            e1.record()
+            torch.cuda.synchronize()
+        finally:
+            self._clear_sampler()
+            m.seq, m.start = self.seq.data_ptr(), self.start.data_ptr()
+            m.slot_row = m.slot_pos = m.next_row = m.done = 0
+            m.num_rows = m.max_length = 0
+        cnt = counters.cpu().numpy()
+        if cnt[3] != Q:
+            raise L.ProgenError(f'generate_queue: {cnt[3]} of {Q} rows retired in {cnt[1]} steps')
+        return dict(ids=seq.cpu().numpy().astype(np.int64), token_logp=token_logp.cpu().numpy(), end=end.cpu().numpy(),
+                    start=starts, steps_run=int(cnt[1]), device_s=e0.elapsed_time(e1) / 1e3)
+
+    def _sampler_rows(self, prompts, sample_ids, max_length):
+        """-> (max_length, seq0, starts, sample ids) of generate / generate_queue, checked"""
+        n = self.n
+        max_length = n if max_length is None else int(max_length)
+        if not 2 <= max_length <= n:
+            raise L.ProgenError(f'generate: 2 <= max_length <= {n}')
+        seq0, starts = self._rows(prompts, max_length)
+        R = len(prompts)
+        sids = np.arange(R, dtype=np.int64) if sample_ids is None else np.asarray(sample_ids, np.int64).reshape(-1)
+        if sids.shape != (R,):
+            raise L.ProgenError('generate: one sample id per prompt')
+        return max_length, seq0, starts, sids
+
+    def _check_sampler(self, temperature, top_k, top_p, logit_bias, min_new_tokens, repetition_penalty, repetition_window):
+        """checks the sampler arguments of generate / generate_queue; -> logit_bias as float32 (or None)"""
+        n = self.n
+        if top_k is not None and not 1 <= int(top_k) <= self.V:
+            raise L.ProgenError(f'generate: 1 <= top_k <= {self.V}')
+        if top_p is not None and not 0.0 < float(top_p) <= 1.0:
+            raise L.ProgenError('generate: 0 < top_p <= 1')
+        if not (np.isfinite(temperature) and temperature >= 0):
+            raise L.ProgenError('generate: temperature must be finite and >= 0')
+        if logit_bias is not None:
+            logit_bias = np.asarray(logit_bias, np.float32)
+            if logit_bias.shape != (self.V,) or np.isnan(logit_bias).any() or (logit_bias == np.inf).any():
+                raise L.ProgenError(f'generate: logit_bias must be {self.V} floats without NaN or +inf')
+        if not 0 <= int(min_new_tokens) <= n or not 0 <= int(repetition_window) <= n:
+            raise L.ProgenError(f'generate: min_new_tokens and repetition_window must lie in [0, {n}]')
+        if not (np.isfinite(repetition_penalty) and repetition_penalty > 0):
+            raise L.ProgenError('generate: repetition_penalty must be finite and > 0')
+        return logit_bias
+
+    def _set_sampler(self, temperature, top_k, top_p, seed, logit_bias, min_new_tokens, repetition_penalty, repetition_window):
+        m = self.m
+        m.sampler = 1
+        m.temperature = float(temperature)
+        m.top_k = int(top_k) if top_k is not None else 0
+        m.top_p = float(top_p) if top_p is not None else 1.0
+        m.seed = int(seed) & 0xFFFFFFFFFFFFFFFF
+        if logit_bias is not None:
+            if self._bias is None:
+                self._bias = torch.zeros(self.V, device=self.dev, dtype=torch.float32)
+            self._bias.copy_(torch.from_numpy(logit_bias))
+            m.logit_bias = self._bias.data_ptr()
+        m.repetition_penalty = float(repetition_penalty)
+        m.repetition_window, m.min_new_tokens = int(repetition_window), int(min_new_tokens)
+
+    def _clear_sampler(self):
+        """back to the reference sampler's launch fields (sample() after generate() runs what it ran before)"""
+        m = self.m
+        m.B, m.sampler, m.top_k = self.B, 0, 0
+        m.temperature, m.top_p, m.seed = 0.0, 0.0, 0
+        m.sample_id = m.token_logp = m.end = m.n_ended = m.steps_run = m.logit_bias = 0
+        m.repetition_penalty, m.repetition_window, m.min_new_tokens = 1.0, 0, 0
 
 
 class Decoder:

@@ -49,6 +49,24 @@ def plan_launches(lengths, batch_size, by_length=False):
     return out
 
 
+# `ProGen.generate` feeds at most this many rows per slot to one queue launch: it bounds the launch's [rows, seq_len] ids
+# and log-probabilities in device memory and the time one launch holds the GPU
+QUEUE_ROWS_PER_SLOT = 64
+
+
+def plan_queue(n_rows, batch_size):
+    """The queue launches of `ProGen.generate` (prefill='decode') for n_rows rows: -> (slots, chunks), slots =
+    min(batch_size, n_rows) sequences per launch and chunks a list of int64 arrays of row indices in row order, each run
+    as the queue of one launch.  Rows are split into the fewest chunks of at most QUEUE_ROWS_PER_SLOT * slots rows, of
+    near-equal size, so every chunk holds at least `slots` rows.  None when slots < 2: the single-stream kernel keeps
+    one launch per row (`plan_launches`)."""
+    slots = min(batch_size, n_rows)
+    if slots < 2:
+        return None
+    k = -(-n_rows // (QUEUE_ROWS_PER_SLOT * slots))
+    return slots, [c.astype(np.int64) for c in np.array_split(np.arange(n_rows), k)]
+
+
 class ProGen:
     def __init__(self, *, num_tokens, dim, seq_len, depth, window_size=256, global_mlp_depth=2, heads=8, dim_head=64,
                  ff_mult=4, ff_glu=True, attn_dim=None, clamp_gate=True, shift_tokens=True, mixed_precision=False,
@@ -165,11 +183,14 @@ class ProGen:
 
         prompts: a string, or a list of strings (encoded like training text) or of integer id arrays (ids in [1, V)).
         Rows are prompt-major: row i * num_samples + j is sample j of prompt i and draws from Philox stream (seed, row).
-        Rows run min(batch_size, N) (<= 64) at a time in one persistent kernel.  The kernel's arithmetic depends on the
-        class of that launch size, 1, 2-8 or 9-64 rows, and on the GPU's SM count, but not on the size within the class:
-        on one GPU model a row is bitwise the same for every batch_size of the same class and every chunking (a ragged last
-        chunk is padded to the class).  Rows of different classes agree to fp32 round-off, so ids can differ where a draw
-        is that close.  max_length (default seq_len) bounds BOS + prompt + generated tokens;
+        Rows run min(batch_size, N) (<= 64) at a time in one persistent kernel.  With prefill='decode' and at least two
+        rows per launch, the rows form a queue (up to QUEUE_ROWS_PER_SLOT per slot and launch): a row that ends hands its
+        slot to the next row, so a launch does not wait for its longest row.  The kernel's arithmetic depends on the
+        class of the launch size, 1, 2-8 or 9-64 rows, and on the GPU's SM count, but not on the size within the class,
+        the slot or the other rows: on one GPU model a row is bitwise the same for every batch_size of the same class and
+        every chunking (with forward prefill a ragged last chunk is padded to the class).  Rows of different classes agree
+        to fp32 round-off, so ids can differ where a draw is that close.  max_length (default seq_len) bounds BOS + prompt
+        + generated tokens;
         temperature 0 is greedy (first maximal logit; top_k / top_p ignored).
 
         Constraints, applied in the kernel to the logits of every draw, in this order, before top-k / temperature / top-p
@@ -264,23 +285,30 @@ class ProGen:
             ids.append(a)
         N = len(ids) * num_samples
         rows = [ids[r // num_samples] for r in range(N)]
-        launches = plan_launches([len(a) for a in rows], batch_size, by_length=prefill == 'forward')
         dec = self._generate_decoder(params, min(batch_size, N))
         if prefill == 'forward':
             self._ensure_loaded(params)
         out = dict(tokens=np.zeros((N, n), np.int64), start=np.zeros(N, np.int64), end=np.zeros(N, np.int64),
                    token_logp=np.zeros((N, n), np.float32))
-        for sids, real in launches:
-            chunk = [rows[r] for r in sids]
-            P = dec.prefill(self.engine, chunk) if prefill == 'forward' else 0
-            res = dec.generate(chunk, temperature=temperature, top_k=top_k, top_p=top_p, seed=seed, sample_ids=sids,
-                               max_length=max_length, logit_bias=logit_bias, min_new_tokens=min_new_tokens,
-                               repetition_penalty=repetition_penalty, repetition_window=repetition_window, prefilled=P)
-            r = sids[:real]
-            out['tokens'][r] = res['ids'][:real]
-            out['token_logp'][r] = res['token_logp'][:real]
-            out['start'][r] = res['start'][:real]
-            out['end'][r] = res['end'][:real]
+        kw = dict(temperature=temperature, top_k=top_k, top_p=top_p, seed=seed, max_length=max_length, logit_bias=logit_bias,
+                  min_new_tokens=min_new_tokens, repetition_penalty=repetition_penalty, repetition_window=repetition_window)
+        def store(r, res):
+            out['tokens'][r] = res['ids'][:len(r)]
+            out['token_logp'][r] = res['token_logp'][:len(r)]
+            out['start'][r] = res['start'][:len(r)]
+            out['end'][r] = res['end'][:len(r)]
+
+        queue = plan_queue(N, batch_size) if prefill == 'decode' else None
+        if queue is not None:
+            # a slot whose row has ended takes the next row of the queue: no launch waits for its longest row
+            slots, chunks = queue
+            for sids in chunks:
+                store(sids, dec.generate_queue([rows[r] for r in sids], slots=slots, sample_ids=sids, **kw))
+        else:
+            for sids, real in plan_launches([len(a) for a in rows], batch_size, by_length=prefill == 'forward'):
+                chunk = [rows[r] for r in sids]
+                P = dec.prefill(self.engine, chunk) if prefill == 'forward' else 0
+                store(sids[:real], dec.generate(chunk, sample_ids=sids, prefilled=P, **kw))
         end = out.pop('end')
         out['finished'] = end < max_length
         out['length'] = np.where(out['finished'], end + 1, max_length) - out['start']
