@@ -156,7 +156,8 @@ int progen_adamw_step_dev(float* p, void* p_lp, const float* g, float* m, float*
 
 /* ---- KV-cached decode (BASELINE config 5; replaces the full re-forward per token of utils.py:115-117) ----
  * Weights are TRANSPOSED copies ([out, in], fp32 or bf16 per `wdtype`); caches and scratch are fp32 device buffers owned
- * by the caller.  `layers` is a HOST array of `depth` entries. */
+ * by the caller.  One layer of progen_decode_run_t's `layers`, a DEVICE array of `depth` entries; the cache and state
+ * pointers hold all B sequences of the launch, batch-major. */
 typedef struct progen_decode_layer_t {
   int32_t kind;                /* 0 GLU, 1 GELU, 2 gMLP/SGU  (progen.py:210-212) */
   int32_t _pad;
@@ -174,37 +175,17 @@ typedef struct progen_decode_layer_t {
   const float* sgu_b;          /* [n] */
   const void* sgu_proj_t;      /* [hid/2, hid/2] */
   const float* sgu_proj_b;
-  float* kcache;               /* [n, inner] rotated keys */
-  float* vcache;               /* [n, inner] rotated values */
-  float* shift1;               /* [2][d/2] previous position's LN half (attention block), indexed by position parity */
-  float* shift2;               /* [2][d/2] previous position's LN half (feed-forward block) */
-  float* gn_hist;              /* [n, hid/2] normalised gate history (gMLP layers) */
+  float* kcache;               /* [B, heads, n, dim_head] rotated keys (a head's keys are contiguous: the windowed read streams) */
+  float* vcache;               /* [B, heads, n, dim_head] rotated values */
+  float* shift1;               /* [B, 2, d/2] previous position's LN half (attention block), indexed by position parity */
+  float* shift2;               /* [B, 2, d/2] previous position's LN half (feed-forward block) */
+  float* gn_hist;              /* [B, n, hid/2] normalised gate history (gMLP layers) */
 } progen_decode_layer_t;
-
-typedef struct progen_decode_t {
-  int32_t n, d, heads, dim_head, inner, window, hid, V, depth, wdtype, shift_tokens, top_k;
-  const float* embed;          /* [V, d] */
-  const float* lnf_scale;      /* [d] */
-  const void* whead_t;         /* [V, d] */
-  const float* bhead;          /* [V] */
-  const float* rot_sin;        /* [n, dim_head/2] */
-  const float* rot_cos;
-  const progen_decode_layer_t* layers;
-  int32_t* seq;                /* [n] device: token ids; sampled ids are ADDED in place (utils.py:129) */
-  int32_t* pos;                /* device scalar: position consumed by the next step */
-  const float* noise;          /* [n, V] gumbel noise, or NULL for the greedy limit */
-  float* logits_all;           /* [n, V] every step's logits (may be NULL) */
-  float *x, *y, *q, *att, *u, *gn, *sg, *pj, *logits;   /* scratch: d, d, inner, inner, 2*hid, hid/2, hid/2, hid/2, V */
-} progen_decode_t;
-
-int progen_decode_step(const progen_decode_t* model, int do_sample, void* stream);
 
 /* Whole-generation decode in ONE persistent cooperative kernel (csrc/decode_persist.cu): consumes positions
  * pos0 .. pos0 + nsteps - 1 of B sequences in lock step (reference utils.py:106-135 per sequence; sample.py:66-71).
- * `layers` is a DEVICE array of `depth` progen_decode_layer_t whose cache / state pointers are batch-major:
- * kcache, vcache [B, heads, n, dim_head] (a head's keys are contiguous: the windowed read streams); shift1, shift2 [B, 2, d/2];
- * gn_hist [B, n, hid/2].  Sequence b keeps its prime before start[b]: position p+1 is sampled (seq[b][p+1] += id, quirk Q5)
- * iff p+1 >= start[b].  grid_bar (one uint32) must be zero on entry; att_count ([B * heads] int32) is reserved (the attention
+ * `layers` is a DEVICE array of `depth` progen_decode_layer_t (cache and state layouts above).  Sequence b keeps its
+ * prime before start[b]: position p+1 is sampled (seq[b][p+1] += id, quirk Q5) iff p+1 >= start[b].  grid_bar (one uint32) must be zero on entry; att_count ([B * heads] int32) is reserved (the attention
  * merges no longer use a global counter).  Limits: B <= 64, dim_head a power of two in [8, 64], window <= 512, V <= 512,
  * feature widths <= 8192. */
 typedef struct progen_decode_run_t {

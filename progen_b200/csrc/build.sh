@@ -8,7 +8,7 @@ mkdir -p "$OBJ"
 NVCC="${NVCC:-/usr/local/cuda/bin/nvcc}"
 FLAGS=(-gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC,-O3
        --expt-relaxed-constexpr -DCUDA_VERSION_STR="\"12.9\"" -I"$HERE" -I"$HERE/../../include")
-SRCS=(api gemm_tc gemm_simt elementwise ln_stream attn_simt attn_wgmma optim decode decode_persist)
+SRCS=(api gemm_tc gemm_simt elementwise ln_stream attn_simt attn_wgmma optim decode_persist)
 pids=()
 for s in "${SRCS[@]}"; do
   [ -f "$HERE/$s.cu" ] || continue

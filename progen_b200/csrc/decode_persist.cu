@@ -1,8 +1,7 @@
 // KV-cached autoregressive decode as ONE persistent kernel (BASELINE config 5; reference utils.py:106-135, sample.py:66-71).
 //
-// The per-step path (decode.cu) replays a CUDA graph of ~150 tiny kernels per token and is bound by launch latency.  Here
-// one cooperative kernel (one CTA per SM) generates every position of the
-// launch: the phases of a layer (LN + shift + QKV + rotary + cache | windowed attention | out-proj + residual | LN + shift +
+// One cooperative kernel (one CTA per SM) generates every position of the launch, with no kernel launch between its
+// steps: the phases of a layer (LN + shift + QKV + rotary + cache | windowed attention | out-proj + residual | LN + shift +
 // FF-in + GLU/GELU | [gMLP: gate LN + causal spatial mix | SGU proj] | FF-out + residual) are separated by a grid barrier
 // (one atomic + one acquire poll per CTA), and the token loop, the sampler and the position counter stay on the device: no
 // host round trip.  Sampler 0 is the reference's (top-k filter that keeps k-1 and zeroes the rest, Gumbel-max over host
@@ -35,17 +34,11 @@ using namespace tc;
 constexpr int WSEGS = 32;               // (row pair, 256-column segment) weight units of one CTA per wave
 constexpr int MAXEV = 160;              // profile events per sampled CTA (grid barriers of one step)
 constexpr int MAXSPLIT = 8;             // SGU: most splits of the history range
-// threads per CTA by batch tile.  A single sequence is a latency chain: 8 warps are enough.  For B > 8 the phases are bound by
-// L2 traffic of the activation staging and by memory latency, not by issue slots, so the default is 256 threads (no
-// spills) rather than 512.
-#ifndef PROGEN_DECODE_BATCH_THREADS
-#define PROGEN_DECODE_BATCH_THREADS 256
-#endif
-constexpr int threads_for(int BT) { return BT > 8 ? PROGEN_DECODE_BATCH_THREADS : 256; }
-
-template <int TPB> struct Impl {
-static constexpr int WPB = TPB / 32;
-static constexpr int MAXSEG = WSEGS / WPB;   // units a warp holds in registers
+// threads per CTA, every batch tile.  A single sequence is a latency chain: 8 warps are enough.  For B > 8 the phases are
+// bound by L2 traffic of the activation staging and by memory latency, not by issue slots, so 512 threads are no faster.
+constexpr int TPB = 256;
+constexpr int WPB = TPB / 32;
+constexpr int MAXSEG = WSEGS / WPB;     // units a warp holds in registers
 
 template <int BT, bool TCW = false> struct Tile {   // shared-memory geometry by batch tile; TCW: bf16 weights on the tensor pipe (BT > 8)
   static constexpr bool LANEB = BT > 8;                       // whole-batch formulations (B > 8)
@@ -590,7 +583,7 @@ static __device__ __forceinline__ void gemv_phase(const Phase& ph, int B, float*
         }
       }
     };
-    constexpr int RFW = TPB > 256 ? 2 : 4;                 // (128 registers per thread with 16 warps)
+    constexpr int RFW = 4;
     if (ph.K <= 512) ln_rows(std::integral_constant<int, RFW>{}, std::integral_constant<int, 4>{});
     else ln_rows(std::integral_constant<int, RFW / 2>{}, std::integral_constant<int, 8>{});
     __syncthreads();
@@ -1780,13 +1773,13 @@ static __device__ void build_phase_table(const progen_decode_run_t& r, PhaseEnt*
 }
 
 static constexpr size_t MAX_SMEM = 227 * 1024;
-// dynamic shared memory of a launch: the tile regions, the phase table and (single stream, when they fit) the unit tables
-template <int BT, bool TCW> static __host__ __device__ size_t decode_smem_bytes(int depth, bool with_unit_tables) {
-  return decode_smem_floats<BT, TCW>() * sizeof(float) + (size_t)num_phases(depth) * (sizeof(PhaseEnt) + (with_unit_tables ? WSEGS * (sizeof(UnitEnt) + sizeof(FinEnt)) : 0)) + 16;
-}
 template <int BT, bool TCW> static constexpr size_t decode_smem_floats() {
   using TL = Tile<BT, TCW>;
   return (size_t)BT * TL::XP + TL::PART + TL::STATF + TL::WSM + WPB * 128 + 64;
+}
+// dynamic shared memory of a launch: the tile regions, the phase table and (single stream, when they fit) the unit tables
+template <int BT, bool TCW> static __host__ __device__ size_t decode_smem_bytes(int depth, bool with_unit_tables) {
+  return decode_smem_floats<BT, TCW>() * sizeof(float) + (size_t)num_phases(depth) * (sizeof(PhaseEnt) + (with_unit_tables ? WSEGS * (sizeof(UnitEnt) + sizeof(FinEnt)) : 0)) + 16;
 }
 
 // STD: sampler 1 (a separate instantiation, so the sampler-0 kernels compile exactly as they do without it)
@@ -1949,23 +1942,19 @@ static __device__ __forceinline__ void run(const progen_decode_run_t& r) {
   if (STD && blockIdx.x == 0 && threadIdx.x == 0) *r.steps_run = r.nsteps;
 }
 
-};  // struct Impl
-
 template <int BT, typename TW, bool STD>
-__global__ void __launch_bounds__(threads_for(BT), 1) decode_persistent_kernel(const progen_decode_run_t r) {
-  Impl<threads_for(BT)>::template run<BT, TW, STD>(r);
+__global__ void __launch_bounds__(TPB, 1) decode_persistent_kernel(const progen_decode_run_t r) {
+  run<BT, TW, STD>(r);
 }
 
 template <int BT, typename TW, bool STD>
 int launch_run_sampler(const progen_decode_run_t& r, cudaStream_t s) {
-  using IM = Impl<threads_for(BT)>;
-  using TL = typename IM::template Tile<BT, sizeof(TW) == 2>;
-  constexpr int TPB = threads_for(BT);
+  using TL = Tile<BT, sizeof(TW) == 2>;
   static_assert((BT * TL::XP) % 4 == 0 && TL::PART % 4 == 0 && TL::WSM % 4 == 0, "the scratch regions must stay 16-byte aligned");
-  size_t smem = IM::template decode_smem_bytes<BT, sizeof(TW) == 2>(r.depth, BT == 1);
-  if (smem > IM::MAX_SMEM) smem = IM::template decode_smem_bytes<BT, sizeof(TW) == 2>(r.depth, false);   // deep model: no unit tables
-  PG_CHECK_ARG(smem <= IM::MAX_SMEM);                                  // (the phase table itself: depth * 7 + 2 entries)
-  if (STD && BT > 1) PG_CHECK_ARG(smem + 2 * 64 * sizeof(int) <= IM::MAX_SMEM);   // + the queue kernels' slot table (static)
+  size_t smem = decode_smem_bytes<BT, sizeof(TW) == 2>(r.depth, BT == 1);
+  if (smem > MAX_SMEM) smem = decode_smem_bytes<BT, sizeof(TW) == 2>(r.depth, false);   // deep model: no unit tables
+  PG_CHECK_ARG(smem <= MAX_SMEM);                                  // (the phase table itself: depth * 7 + 2 entries)
+  if (STD && BT > 1) PG_CHECK_ARG(smem + 2 * 64 * sizeof(int) <= MAX_SMEM);   // + the queue kernels' slot table (static)
   auto kern = decode_persistent_kernel<BT, TW, STD>;
   static size_t set_for = 0;
   if (set_for < smem) {
@@ -2022,10 +2011,8 @@ int progen_decode_run(const progen_decode_run_t* r, void* stream) {
   const bool bf = r->wdtype == PG_BF16;
   if (r->B == 1) return bf ? launch_run<1, bf16>(*r, s) : launch_run<1, float>(*r, s);
   if (r->B <= 8) return bf ? launch_run<8, bf16>(*r, s) : launch_run<8, float>(*r, s);
-  // 9 .. 64 sequences: the 32-sequence tile, twice per phase above 32 (PROGEN_DECODE_TILE64=1: one 64-wide tile, kept for A/B)
-  static const bool tile64 = [] { const char* e = getenv("PROGEN_DECODE_TILE64"); return e && atoi(e) != 0; }();
-  if (r->B <= 32 || !tile64) return bf ? launch_run<32, bf16>(*r, s) : launch_run<32, float>(*r, s);
-  return bf ? launch_run<64, bf16>(*r, s) : launch_run<64, float>(*r, s);
+  // 9 .. 64 sequences: the 32-sequence tile, twice per phase above 32
+  return bf ? launch_run<32, bf16>(*r, s) : launch_run<32, float>(*r, s);
 }
 
 }  // extern "C"

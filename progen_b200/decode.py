@@ -1,10 +1,12 @@
 """KV-cached sampler: the device-side equivalent of `progen_transformer.utils.sample` (utils.py:106-135).
 
-The reference re-runs the whole model over the full padded sequence for every generated token; here each step consumes
-one position (`progen_decode_step`, csrc/decode.cu), keeping rotated K/V rows, the token-shift halves and the SGU gate
-history per layer.  The position lives in device memory, so one captured CUDA graph is replayed for every token and the
-loop never synchronises with the host.  Quirks are kept: top-k keeps k-1 logits and zeroes the rest (Q6), `add_bos`
-adds the first sampled id to the last prime token (Q5), everything after the second pad is cleared (Q7)."""
+The reference re-runs the whole model over the full padded sequence for every generated token; here `BatchDecoder`
+consumes one position per step and keeps rotated K/V rows, the token-shift halves and the SGU gate history per layer
+and sequence.  Every position of a launch runs inside ONE persistent kernel (`progen_decode_run`,
+csrc/decode_persist.cu): the token loop, the sampler and the position counter stay on the device, and the loop never
+synchronises with the host.  `BatchDecoder.sample` keeps the reference's quirks: top-k keeps k-1 logits and zeroes the
+rest (Q6), `add_bos` adds the first sampled id to the last prime token (Q5), everything after the second pad is
+cleared (Q7).  `BatchDecoder.generate` / `generate_queue` run the standard sampler."""
 import ctypes as C
 
 import numpy as np
@@ -20,13 +22,6 @@ class DecodeLayer(C.Structure):
     _fields_ = [('kind', _I), ('_pad', _I)] + [(k, _P) for k in (
         'ln1_scale', 'wqkv_t', 'wo_t', 'bo', 'ln2_scale', 'win_t', 'bin', 'wout_t', 'bout', 'sgu_ln_scale', 'sgu_w', 'sgu_b',
         'sgu_proj_t', 'sgu_proj_b', 'kcache', 'vcache', 'shift1', 'shift2', 'gn_hist')]
-
-
-class DecodeModel(C.Structure):
-    _fields_ = [(k, _I) for k in ('n', 'd', 'heads', 'dim_head', 'inner', 'window', 'hid', 'V', 'depth', 'wdtype',
-                                  'shift_tokens', 'top_k')] + \
-               [(k, _P) for k in ('embed', 'lnf_scale', 'whead_t', 'bhead', 'rot_sin', 'rot_cos', 'layers', 'seq', 'pos', 'noise',
-                                  'logits_all', 'x', 'y', 'q', 'att', 'u', 'gn', 'sg', 'pj', 'logits')]
 
 
 class DecodeRun(C.Structure):
@@ -453,141 +448,3 @@ class BatchDecoder:
         m.temperature, m.top_p, m.seed = 0.0, 0.0, 0
         m.sample_id = m.token_logp = m.end = m.n_ended = m.steps_run = m.logit_bias = 0
         m.repetition_penalty, m.repetition_window, m.min_new_tokens = 1.0, 0, 0
-
-
-class Decoder:
-    def __init__(self, config, params, weights_dtype=torch.float32, keep_logits=False, device=None):
-        L.require_device()
-        self.lib = L.load()
-        self.cfg = cfg = config
-        self.dev = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
-        d, n = cfg['dim'], cfg['seq_len']
-        I = cfg['heads'] * cfg['dim_head']
-        hid = d * cfg['ff_mult']
-        self.n, self.V = n, cfg['num_tokens']
-        self.keep = []                       # every device tensor referenced by the C structs
-        f32 = lambda a: self._hold(torch.tensor(np.ascontiguousarray(np.asarray(a, np.float32)), device=self.dev))
-        wt = lambda a: self._hold(torch.tensor(np.ascontiguousarray(np.asarray(a, np.float32).T), device=self.dev).to(weights_dtype).contiguous())
-        zeros = lambda *s: self._hold(torch.zeros(*s, device=self.dev, dtype=torch.float32))
-        kinds = layer_kinds(cfg['depth'], cfg['global_mlp_depth'], cfg['ff_glu'])
-        self.layers = (DecodeLayer * len(kinds))()
-        self.state = []                      # caches to clear on reset
-        for i, kind in enumerate(kinds):
-            a, f = P + f'attn{i}/~/', P + f'ff{i}/~/'
-            Lr = self.layers[i]
-            Lr.kind = {'glu': 0, 'gelu': 1, 'sgu': 2}[kind]
-            Lr.ln1_scale = f32(params[a + 'layer_norm']['scale'])
-            Lr.wqkv_t = wt(params[a + 'linear']['w'])
-            Lr.wo_t = wt(params[a + 'linear_1']['w'])
-            Lr.bo = f32(params[a + 'linear_1']['b'])
-            Lr.ln2_scale = f32(params[f + 'layer_norm']['scale'])
-            Lr.win_t = wt(params[f + 'linear']['w'])
-            Lr.bin = f32(params[f + 'linear']['b'])
-            Lr.wout_t = wt(params[f + 'linear_1']['w'])
-            Lr.bout = f32(params[f + 'linear_1']['b'])
-            if kind == 'sgu':
-                g = f + 'sgu'
-                Lr.sgu_ln_scale = f32(params[g + '/~/layer_norm']['scale'])
-                Lr.sgu_w = f32(params[g]['spatial_weights'])
-                Lr.sgu_b = f32(np.asarray(params[g]['spatial_biases']).reshape(-1))
-                Lr.sgu_proj_t = wt(params[g + '/~/linear']['w'])
-                Lr.sgu_proj_b = f32(params[g + '/~/linear']['b'])
-                Lr.gn_hist = self._state(zeros(n, hid // 2))
-            Lr.kcache = self._state(zeros(n, I))
-            Lr.vcache = self._state(zeros(n, I))
-            Lr.shift1 = self._state(zeros(2, d // 2))       # double-buffered by position parity (read [pos&1], write [(pos+1)&1])
-            Lr.shift2 = self._state(zeros(2, d // 2))
-        m = self.m = DecodeModel()
-        m.n, m.d, m.heads, m.dim_head, m.inner, m.window, m.hid, m.V, m.depth = n, d, cfg['heads'], cfg['dim_head'], I, \
-            cfg['window_size'], hid, self.V, len(kinds)
-        m.wdtype = L.BF16 if weights_dtype == torch.bfloat16 else L.F32
-        m.shift_tokens = int(cfg['shift_tokens'])
-        m.embed = f32(params[P + 'embed']['embeddings'])
-        m.lnf_scale = f32(params[P + 'layer_norm']['scale'])
-        m.whead_t = wt(params[P + 'linear']['w'])
-        m.bhead = f32(params[P + 'linear']['b'])
-        inv_freq = 1.0 / (10000 ** (np.arange(0, cfg['dim_head'], 2, dtype=np.float64) / cfg['dim_head']))
-        ang = np.arange(n, dtype=np.float64)[:, None] * inv_freq[None, :]
-        m.rot_sin, m.rot_cos = f32(np.sin(ang)), f32(np.cos(ang))
-        m.layers = C.cast(self.layers, C.c_void_p)
-        self.seq = torch.zeros(n, device=self.dev, dtype=torch.int32)
-        self.pos = torch.zeros(1, device=self.dev, dtype=torch.int32)
-        m.seq, m.pos = self.seq.data_ptr(), self.pos.data_ptr()
-        self.logits_all = torch.zeros(n, self.V, device=self.dev) if keep_logits else None
-        m.logits_all = self.logits_all.data_ptr() if keep_logits else 0
-        self.noise = torch.zeros(n, self.V, device=self.dev)
-        m.noise = 0
-        for name, size in (('x', d), ('y', d), ('q', I), ('att', I), ('u', 2 * hid), ('gn', hid // 2), ('sg', hid // 2),
-                           ('pj', hid // 2), ('logits', self.V)):
-            setattr(m, name, zeros(size))
-        self.graph = None
-
-    def _hold(self, t):
-        self.keep.append(t)
-        return t.data_ptr()
-
-    def _state(self, ptr):
-        self.state.append(self.keep[-1])
-        return ptr
-
-    def reset(self):
-        for t in self.state:
-            t.zero_()
-        self.pos.zero_()
-
-    def step(self, do_sample):
-        L.check(self.lib.progen_decode_step(C.byref(self.m), int(do_sample), L.stream()), 'decode_step')
-
-    def sample(self, prime, length=None, top_k=None, add_bos=False, greedy=True, seed=0, use_graph=True):
-        """utils.py:106-135.  Returns (sampled ids as numpy int64 [length], generated-token count, device seconds)."""
-        length = self.n if length is None else length
-        assert length == self.n, 'the gMLP layers pin the sequence length (progen.py:175-181)'
-        prime = np.asarray(prime).astype(np.int64)
-        start_pos = prime.shape[-1]
-        pad_right = length - start_pos
-        padding = (0, pad_right) if not add_bos else (1, pad_right - 1)
-        seq0 = np.pad(prime, padding)
-        self.reset()
-        self.seq.copy_(torch.as_tensor(seq0.astype(np.int32)))
-        self.m.top_k = int(top_k) if top_k is not None else 0
-        if greedy:
-            self.m.noise = 0
-        else:
-            g = torch.Generator(device=self.dev).manual_seed(int(seed))
-            u = torch.rand(self.n, self.V, generator=g, device=self.dev)
-            self.noise.copy_(-torch.log(-torch.log(u + 1e-20) + 1e-20))           # utils.py:102-104
-            self.m.noise = self.noise.data_ptr()
-        # prefill: positions 0 .. start_pos-2 only advance the caches
-        for _ in range(max(0, start_pos - 1)):
-            self.step(False)
-        nsteps = length - start_pos                                                # curr_pos = start_pos .. length-1
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        if use_graph and nsteps > 1:
-            if self.graph is None or self._graph_key != (self.m.top_k, self.m.noise):
-                side = torch.cuda.Stream()
-                side.wait_stream(torch.cuda.current_stream())
-                with torch.cuda.stream(side):
-                    self.step(True)                                                # warm-up outside capture (counts as step 1)
-                    g_ = torch.cuda.CUDAGraph()
-                    with torch.cuda.graph(g_, stream=side):
-                        self.step(True)
-                torch.cuda.current_stream().wait_stream(side)
-                self.graph, self._graph_key = g_, (self.m.top_k, self.m.noise)
-                done = 1
-            else:
-                done = 0
-            e0.record()
-            for _ in range(nsteps - done):
-                self.graph.replay()
-            e1.record()
-            timed = nsteps - done
-        else:
-            e0.record()
-            for _ in range(nsteps):
-                self.step(True)
-            e1.record()
-            timed = nsteps
-        torch.cuda.synchronize()
-        seq = self.seq.cpu().numpy().astype(np.int64)
-        after_eos = np.cumsum(seq == 0) > 1                                        # utils.py:132-133
-        return seq * ~after_eos, timed, e0.elapsed_time(e1) / 1e3

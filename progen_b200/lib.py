@@ -64,7 +64,6 @@ PROTOTYPES = {
     'progen_gelu_bwd': [_P, _P, _I, _LL, _P],
     'progen_cast_f32': [_P, _P, _I, _LL, _P],
     'progen_tril_cast': [_P, _P, _I, _I, _P],
-    'progen_decode_step': [_P, _I, _P],
     'progen_decode_run': [_P, _P],
     'progen_gather_rows_f32': [_P, _LL, _I, _I, _LL, _P, _I, _I, _I, _I, _I, _I, _P, _LL, _LL, _LL, _P],
     'progen_optim_workspace_floats': [],

@@ -9,7 +9,7 @@ timeout 900 compute-sanitizer --tool "$tool" --error-exitcode 9 --print-limit 20
   -p no:cacheprovider > "$out/sanitize_${tool}_model.log" 2>&1
 echo "model: exit $? : $(grep -E 'ERROR SUMMARY|passed|failed' "$out/sanitize_${tool}_model.log" | tail -n 2 | tr '\n' ' ')"
 timeout 900 compute-sanitizer --tool "$tool" --error-exitcode 9 --print-limit 20 \
-  python -m pytest tests/test_gpu_decode.py -x -q -m gpu -k "test_decode_logits_match_oracle_forward" \
+  python -m pytest tests/test_gpu_decode.py -x -q -m gpu -k "test_persistent_logits_match_oracle_forward" \
   -p no:cacheprovider > "$out/sanitize_${tool}_decode.log" 2>&1
 echo "decode: exit $? : $(grep -E 'ERROR SUMMARY|passed|failed' "$out/sanitize_${tool}_decode.log" | tail -n 2 | tr '\n' ' ')"
 # the standard sampler at 1, 2 and 24 rows (the BT 1, 8 and 32 kernels): shared-memory filter, Philox noise, the EOS

@@ -53,7 +53,7 @@ def test_product_has_no_oracle_or_cpu_fallback():
             L.require_device()
 
 
-def test_ctypes_structs_match_the_header_layout(tmp_path):
+def test_ctypes_mirrors_match_the_header_layout(tmp_path):
     """Every ctypes mirror of a C-ABI struct has the size and the field offsets gcc gives the declaration in
     include/progen_b200.h (a field added on one side only would shift every pointer after it)."""
     import ctypes as C
@@ -63,8 +63,7 @@ def test_ctypes_structs_match_the_header_layout(tmp_path):
     from progen_b200 import decode as D
     if shutil.which('gcc') is None:
         pytest.skip('no gcc')
-    pairs = [('progen_gemm_t', L.GemmDesc), ('progen_decode_layer_t', D.DecodeLayer), ('progen_decode_t', D.DecodeModel),
-             ('progen_decode_run_t', D.DecodeRun)]
+    pairs = [('progen_gemm_t', L.GemmDesc), ('progen_decode_layer_t', D.DecodeLayer), ('progen_decode_run_t', D.DecodeRun)]
     lines = ['#include <stdio.h>', '#include <stddef.h>', '#include "progen_b200.h"', 'int main(void) {']
     for cname, cls in pairs:
         lines.append(f'  printf("{cname} size %zu\\n", sizeof({cname}));')

@@ -1,6 +1,7 @@
-"""KV-cached decode (csrc/decode.cu, progen_b200/decode.py) against the reference sampler: greedy token ids must match
-the golden samples produced by the reference's own `utils.sample` (tests/golden/make_golden.py) exactly, the per-position
-logits must match the oracle's full forward, and the cached path must agree with the engine's full re-forward sampler."""
+"""KV-cached decode (csrc/decode_persist.cu, progen_b200/decode.py::BatchDecoder) against the reference sampler: greedy
+token ids must match the golden samples produced by the reference's own `utils.sample` (tests/golden/make_golden.py)
+exactly, the per-position logits must match the oracle's full forward, the cached path must agree with the engine's full
+re-forward sampler, and B sequences decoded in lock step must agree with each decoded alone."""
 import numpy as np
 import pytest
 import torch
@@ -11,35 +12,10 @@ pytestmark = pytest.mark.gpu
 TINY = [n for n in CASES if n != 'cfg1']
 
 
-@pytest.mark.parametrize('name', TINY)
-@pytest.mark.parametrize('add_bos', [False, True])
-@pytest.mark.parametrize('use_graph', [False, True])
-def test_greedy_ids_match_reference_sampler(name, add_bos, use_graph):
-    from progen_b200.decode import Decoder
-    cfg, params, data, g = load_case(name)
-    dec = Decoder(cfg, params, keep_logits=True)
-    ids, steps, secs = dec.sample(g['prime'], top_k=25, add_bos=add_bos, greedy=True, use_graph=use_graph)
-    np.testing.assert_array_equal(ids, g[f'sample_bos{int(add_bos)}'])
-    assert steps > 0 and secs > 0
-
-
-def test_decode_logits_match_oracle_forward():
-    from progen_b200.decode import Decoder
-    from oracle import progen_ref as O
-    cfg, params, data, g = load_case('tiny_glu_sgu')
-    dec = Decoder(cfg, params, keep_logits=True)
-    dec.sample(g['prime'], top_k=25, add_bos=True, greedy=True, use_graph=False)
-    seq = dec.seq.cpu().numpy().astype(np.int64)                  # final ids BEFORE the post-hoc truncation
-    ref = O.forward(params, np.clip(seq, 0, 255), cfg)            # out-of-range ids clamp like a jax gather
-    got = dec.logits_all.cpu().numpy()
-    n = cfg['seq_len']
-    assert np.abs(got[:n - 1] - ref[:n - 1]).max() < 2e-5 * max(1.0, np.abs(ref).max())
-
-
-def test_stochastic_sampler_is_seeded_and_differs_from_greedy():
-    from progen_b200.decode import Decoder
+def test_persistent_stochastic_sampler_is_seeded_and_differs_from_greedy():
+    from progen_b200.decode import BatchDecoder
     cfg, params, data, g = load_case('tiny_all_glu')
-    dec = Decoder(cfg, params)
+    dec = BatchDecoder(cfg, params, batch=1)
     a, _, _ = dec.sample(g['prime'], top_k=25, add_bos=True, greedy=False, seed=1)
     b, _, _ = dec.sample(g['prime'], top_k=25, add_bos=True, greedy=False, seed=1)
     c, _, _ = dec.sample(g['prime'], top_k=25, add_bos=True, greedy=True)
@@ -47,33 +23,32 @@ def test_stochastic_sampler_is_seeded_and_differs_from_greedy():
     assert not np.array_equal(a, c)
 
 
-def test_cached_decode_equals_full_reforward_sampler_cfg1_size():
+def test_persistent_decode_equals_full_reforward_sampler_cfg1_size():
     """BASELINE config-5 shape (seq_len 1024, prime '[Tax=Mammalia] #', top_k=25, add_bos) on the config-1 model: the
     KV-cached path must reproduce the bug-compatible full re-forward sampler (utils.sample over ProGen.apply)."""
     from progen_b200 import ProGen
-    from progen_b200.decode import Decoder
+    from progen_b200.decode import BatchDecoder
     from progen_b200.data import encode_tokens
     from progen_b200.utils import sample
     cfg, params, data, g = load_case('cfg1')
     prime = np.array(encode_tokens('[Tax=Mammalia] #'), dtype=np.uint16)
-    dec = Decoder(cfg, params)
-    ids, steps, secs = dec.sample(prime, top_k=25, add_bos=True, greedy=True)
+    dec = BatchDecoder(cfg, params, batch=1)
+    ids, gen, secs = dec.sample(prime, top_k=25, add_bos=True, greedy=True)
     model = ProGen(**CASES['cfg1'])
     ref = sample(0, model.apply, params, prime, cfg['seq_len'], top_k=25, add_bos=True, greedy=True)
     np.testing.assert_array_equal(ids, ref)
-    assert steps >= cfg['seq_len'] - len(prime) - 1
+    assert gen >= cfg['seq_len'] - len(prime) - 1
+    print(f'persistent decode: {gen} tokens in {secs * 1e3:.1f} ms = {gen / secs:.0f} tokens/s')
 
 
-def test_bf16_weight_decode_runs_and_mostly_agrees():
-    from progen_b200.decode import Decoder
+def test_persistent_bf16_weight_decode_runs_and_mostly_agrees():
+    from progen_b200.decode import BatchDecoder
     cfg, params, data, g = load_case('tiny_all_glu')
-    a, _, _ = Decoder(cfg, params).sample(g['prime'], top_k=25, add_bos=True, greedy=True)
-    b, _, _ = Decoder(cfg, params, weights_dtype=torch.bfloat16).sample(g['prime'], top_k=25, add_bos=True, greedy=True)
+    a, _, _ = BatchDecoder(cfg, params, batch=1).sample(g['prime'], top_k=25, add_bos=True, greedy=True)
+    b, _, _ = BatchDecoder(cfg, params, batch=1, weights_dtype=torch.bfloat16).sample(g['prime'], top_k=25, add_bos=True,
+                                                                                      greedy=True)
     assert a.shape == b.shape and (a[:len(g['prime']) + 2] == b[:len(g['prime']) + 2]).all()
 
-
-# ---------------------------------------------------------------------------------------------------------------------
-# round 2: the whole generation in ONE persistent kernel (csrc/decode_persist.cu), single stream and batched
 
 @pytest.mark.parametrize('name', TINY)
 @pytest.mark.parametrize('add_bos', [False, True])
@@ -92,8 +67,8 @@ def test_persistent_logits_match_oracle_forward():
     cfg, params, data, g = load_case('tiny_glu_sgu')
     dec = BatchDecoder(cfg, params, batch=1, keep_logits=True)
     dec.sample(g['prime'], top_k=25, add_bos=True, greedy=True)
-    seq = dec.seq.cpu().numpy().astype(np.int64)[0]
-    ref = O.forward(params, np.clip(seq, 0, 255), cfg)
+    seq = dec.seq.cpu().numpy().astype(np.int64)[0]               # final ids BEFORE the post-hoc truncation
+    ref = O.forward(params, np.clip(seq, 0, 255), cfg)            # out-of-range ids clamp like a jax gather
     got = dec.logits_all.cpu().numpy()[0]
     n = cfg['seq_len']
     assert np.abs(got[:n - 1] - ref[:n - 1]).max() < 2e-5 * max(1.0, np.abs(ref).max())
@@ -214,19 +189,6 @@ def test_batched_decode_equals_single_stream(B):
         one, _, _ = single.sample(primes[b], top_k=25, add_bos=True, greedy=True)
         np.testing.assert_array_equal(batch[b], one)
     np.testing.assert_array_equal(batch[0], g['sample_bos1'])
-
-
-def test_persistent_decode_cfg1_size_matches_graph_decoder():
-    """BASELINE config-5 shape on the config-1 model: persistent kernel == round-1 per-step decoder (which is pinned to the
-    full re-forward sampler), fp32 and bit-equal"""
-    from progen_b200.decode import Decoder, BatchDecoder
-    from progen_b200.data import encode_tokens
-    cfg, params, data, g = load_case('cfg1')
-    prime = np.array(encode_tokens('[Tax=Mammalia] #'), dtype=np.uint16)
-    a, _, _ = Decoder(cfg, params).sample(prime, top_k=25, add_bos=True, greedy=True)
-    b, gen, secs = BatchDecoder(cfg, params, batch=1).sample(prime, top_k=25, add_bos=True, greedy=True)
-    np.testing.assert_array_equal(a, b)
-    print(f'persistent decode: {gen} tokens in {secs * 1e3:.1f} ms = {gen / secs:.0f} tokens/s')
 
 
 def test_gumbel_topk_sampler_distribution_chi_square():

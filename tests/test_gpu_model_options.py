@@ -24,7 +24,7 @@ Paths (T: tested here; R: a tested refusal; a, b, c: not run, for the reason giv
   training, apply and score, mixed precision   a    a     T     T        T     T    T    T         R      a
   persistent decoder, fp32 and bf16 weights    T    T     T     T        T     T    R    T         R      T
   standard sampler: host replay                T    T     T     b        b     b    R    b         R      b
-  reference sampler (Decoder, BatchDecoder 1)  c    T     c     c        c     c    c    T         T, R   c
+  reference sampler (BatchDecoder 1)           c    T     c     c        c     c    R    T         R      c
   forward prefill, fp32                        T    T     T     T        T     T    R    T         R      T
   forward prefill, mixed precision             a    a     T     T        T     T    R    T         R      a
 
@@ -32,8 +32,9 @@ Paths (T: tested here; R: a tested refusal; a, b, c: not run, for the reason giv
      refuses the rest (test_gpu_model.py::test_mixed_precision_refuses_shapes_without_a_tensor_core_kernel);
   b: the sampler reads only V and the logits: V = 24 (fewer ids than threads), 328 (a partial second id per thread) and
      384 cover its classes, 64 and 320 fall inside them, 256 is test_gpu_generate.py's;
-  c: the per-step decoder runs once per option it reads differently: V > 256 in its one-block sampler, no token shift
-     (its ln_shift flag), dim_head 128 (its attention);
+  c: the reference sampler is the persistent decoder's sampler 0 at one row, whose kernel the row above runs at every
+     option; it runs once per option the full re-forward reads differently: V > 256 (two ids per sampler thread) and no
+     token shift;
   R: ProGen.generate and BatchDecoder raise ProgenError naming the limit (hid % 256, dim_head <= 64) before allocating;
      the mixed-precision engine refuses dim_head 128.
 
@@ -344,31 +345,27 @@ def test_logit_bias_banning_every_id_below_256(name):
 
 
 # ------------------------------------------------------------------------------------------------ reference sampler
-@pytest.mark.parametrize('name', ['v328', 'no_shift', 'dh128'])
-def test_reference_sampler_equals_full_reforward(name):
-    """`Decoder` (the per-step decoder) and `BatchDecoder(batch=1)` greedy ids == the full re-forward `utils.sample` over
-    `ProGen.apply` (test_gpu_decode.py::test_cached_decode_equals_full_reforward_sampler_cfg1_size); `Decoder` logits at
-    every position within 2e-5 * max|logit| of the float64 oracle (::test_decode_logits_match_oracle_forward).  dim_head
-    128: `Decoder` only (the persistent decoder refuses it, test_decoders_refuse_what_they_cannot_run)."""
+@pytest.mark.parametrize('name', ['v328', 'no_shift'])
+def test_persistent_reference_sampler_equals_full_reforward(name):
+    """`BatchDecoder(batch=1)` greedy ids == the full re-forward `utils.sample` over `ProGen.apply`
+    (test_gpu_decode.py::test_persistent_decode_equals_full_reforward_sampler_cfg1_size), and its logits at every position
+    within 2e-5 * max|logit| of the float64 oracle (::test_persistent_logits_match_oracle_forward)."""
     from progen_b200 import ProGen
-    from progen_b200.decode import BatchDecoder, Decoder
+    from progen_b200.decode import BatchDecoder
     from progen_b200.utils import sample
     kw, cfg, params = _model(name)
     n, V = cfg['seq_len'], cfg['num_tokens']
     prime = _prompts(np.random.default_rng(V + n), [6], V)[0]
-    dec = Decoder(cfg, params, keep_logits=True)
+    dec = BatchDecoder(cfg, params, batch=1, keep_logits=True)
     ids, _, _ = dec.sample(prime, top_k=25, add_bos=True, greedy=True)
-    seq = dec.seq.cpu().numpy().astype(np.int64)                  # before the post-hoc truncation
-    got = dec.logits_all[:n - 1].double()
+    seq = dec.seq[0].cpu().numpy().astype(np.int64)               # before the post-hoc truncation
+    got = dec.logits_all[0, :n - 1].double()
     ref = _oracle(params, np.clip(seq, 0, V - 1)[None], cfg)[0, :n - 1]
     err, scale = _maxabs(got - ref), max(1.0, _maxabs(ref))
     want = sample(0, ProGen(**kw).apply, params, prime, n, top_k=25, add_bos=True, greedy=True)
     _report(case=f'reference_sampler_{name}', err=err, bound=2e-5 * scale, max_id=int(seq.max()))
     assert err < 2e-5 * scale
     np.testing.assert_array_equal(ids, want)
-    if name not in NO_DECODER:
-        one, _, _ = BatchDecoder(cfg, params, batch=1).sample(prime, top_k=25, add_bos=True, greedy=True)
-        np.testing.assert_array_equal(one, want)
 
 
 # ------------------------------------------------------------------------------------------------ forward prefill
