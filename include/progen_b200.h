@@ -113,7 +113,9 @@ int progen_rotary_bwd(void* dqkv, long long ld, int dtype, const float* sin_t, c
                       int seq_len, int dim_head, void* stream);
 
 /* sliding-window attention with one look-back window — progen.py:88-102 (q,k,v already rotated, [T, 3*heads*dim_head]).
- * `_simt`: fp32-exact CUDA-core kernels.  lse / delta: [T, heads] fp32. */
+ * `_simt`: fp32-exact CUDA-core kernels.  lse / delta: [T, heads] fp32.  The backward needs seq_len % window == 0; the
+ * forward takes a partial last window (any seq_len for `_simt`, seq_len % 64 == 0 for `_tc`) and then computes the first
+ * seq_len rows of the forward at a longer length, bitwise (causality: no key at or beyond seq_len is read). */
 int progen_local_attn_fwd_simt(const void* qkv, void* out, float* lse, int dtype, int B, int seq_len, int window, int heads,
                                int dim_head, void* stream);
 int progen_local_attn_bwd_simt(const void* qkv, const void* out, const void* dout, const float* lse, void* dqkv,

@@ -234,9 +234,12 @@ int launch_bwd(const void* qkv, const void* out, const void* dout, const float* 
 
 extern "C" {
 
+// The forward takes any seq_len: the last window may be partial.  A query at pos reads keys (win - 1) * w .. pos only, so
+// a forward cut short of the model's sequence length computes the first seq_len rows of the full one, bitwise.  The
+// backward keeps whole windows (a key's gradient reads the whole next window).
 int progen_local_attn_fwd_simt(const void* qkv, void* out, float* lse, int dtype, int B, int seq_len, int window,
                                int heads, int dim_head, void* stream) {
-  PG_CHECK_ARG(B > 0 && seq_len > 0 && window > 0 && seq_len % window == 0 && heads > 0);
+  PG_CHECK_ARG(B > 0 && seq_len > 0 && window > 0 && heads > 0);
   AttnDims dm{(long long)B * seq_len, seq_len, window, heads, dim_head, 3LL * heads * dim_head};
   ATTN_DISPATCH(launch_fwd, qkv, out, lse, dm, (cudaStream_t)stream);
 }

@@ -427,8 +427,12 @@ template <typename K> int prepare(K kern) {
   return PROGEN_OK;
 }
 
-int check_dims(const void* qkv, int B, int seq_len, int window, int heads, int dim_head) {
-  PG_CHECK_ARG(qkv != nullptr && B > 0 && heads > 0 && dim_head == DH && window % TILE == 0 && seq_len % window == 0);
+// full_windows: seq_len must be whole windows (the backward kernels stream the whole next window of every key tile).
+// The forward only needs whole 64-row tiles: a query tile of a partial last window reads the previous window and its own
+// keys up to the diagonal, the same key tiles it reads at full length, so no key at or beyond seq_len is touched.
+int check_dims(const void* qkv, int B, int seq_len, int window, int heads, int dim_head, bool full_windows) {
+  PG_CHECK_ARG(qkv != nullptr && B > 0 && heads > 0 && dim_head == DH && window % TILE == 0 && seq_len > 0 &&
+               seq_len % (full_windows ? window : TILE) == 0);
   PG_CHECK_ARG((long long)B * seq_len < (1ll << 31));
   return PROGEN_OK;
 }
@@ -437,11 +441,12 @@ int check_dims(const void* qkv, int B, int seq_len, int window, int heads, int d
 
 extern "C" {
 
-// bf16, dim_head == 64, window % 64 == 0 (every tile lies inside one window).  qkv [T, 3*heads*64] (rotated),
-// out [T, heads*64], lse [T, heads].
+// bf16, dim_head == 64, window % 64 == 0 (every tile lies inside one window), seq_len % 64 == 0: the last window may be
+// partial (a forward cut short of the model's sequence length computes the first seq_len rows of the full one, bitwise).
+// qkv [T, 3*heads*64] (rotated), out [T, heads*64], lse [T, heads].
 int progen_local_attn_fwd_tc(const void* qkv, void* out, float* lse, int B, int seq_len, int window, int heads, int dim_head,
                              void* stream) {
-  int rc = check_dims(qkv, B, seq_len, window, heads, dim_head);
+  int rc = check_dims(qkv, B, seq_len, window, heads, dim_head, false);
   if (rc) return rc;
   const int I = heads * DH;
   const uint64_t T = (uint64_t)B * seq_len;
@@ -459,7 +464,7 @@ int progen_local_attn_fwd_tc(const void* qkv, void* out, float* lse, int B, int 
 int progen_local_attn_bwd_tc(const void* qkv, const void* out, const void* dout, const float* lse, void* dqkv, float* delta,
                              const float* rot_sin, const float* rot_cos, int B, int seq_len, int window, int heads, int dim_head,
                              void* stream) {
-  int rc = check_dims(qkv, B, seq_len, window, heads, dim_head);
+  int rc = check_dims(qkv, B, seq_len, window, heads, dim_head, true);
   if (rc) return rc;
   const int I = heads * DH;
   const uint64_t T = (uint64_t)B * seq_len;

@@ -23,6 +23,28 @@ P = 'pro_gen_base/~/'      # haiku module-path prefix of the reference parameter
 ALIGN = 64                 # every parameter segment starts on a 64-element boundary (TMA needs 16-byte bases)
 
 
+CUT_ALIGN = 128            # a cut forward's row length: whole 128-row GEMM tiles, and every SGU row tile keeps its k-blocks
+
+
+def counted_length(labels):
+    """labels [N, n] -> [N]: 1 + the last position the loss mask counts (non-pad labels plus the first pad, quirk Q8).
+    Positions at or beyond it add nothing to a row's log-likelihood."""
+    labels = np.asarray(labels)
+    n = labels.shape[1]
+    pad = labels == 0
+    first = np.where(pad.any(1), pad.argmax(1), n)
+    last = np.where((~pad).any(1), n - 1 - (~pad)[:, ::-1].argmax(1), -1)
+    return np.minimum(n, np.maximum(first, last) + 1)
+
+
+def cut_length(labels):
+    """the row length of a forward that covers every counted position of labels [N, n]: their largest counted length
+    rounded up to CUT_ALIGN, at most n"""
+    n = np.asarray(labels).shape[1]
+    need = int(counted_length(labels).max()) if len(labels) else 1
+    return min(n, -(-need // CUT_ALIGN) * CUT_ALIGN)
+
+
 def layer_kinds(depth, global_mlp_depth, ff_glu):
     """reference progen.py:210-212"""
     out = []
@@ -342,9 +364,10 @@ class Engine:
     def colsum(self, t, N, out, ld=None):
         L.check(self.lib.progen_colsum(t.data_ptr(), N if ld is None else ld, L.dt(t), out.data_ptr(), self.T, N, L.stream()), 'colsum')
 
-    def ln_fwd(self, x, ldx, scale, y, ldy, mean, rstd, dcols, shift, acts=None):
+    def ln_fwd(self, x, ldx, scale, y, ldy, mean, rstd, dcols, shift, acts=None, seq_len=None):
         L.check(self.lib.progen_ln_shift_fwd(x.data_ptr(), ldx, L.dt(x), scale.data_ptr(), y.data_ptr(), ldy, L.dt(y),
-                                             mean.data_ptr(), rstd.data_ptr(), (acts or self.acts).T, dcols, self.n, int(shift), L.stream()), 'ln_fwd')
+                                             mean.data_ptr(), rstd.data_ptr(), (acts or self.acts).T, dcols,
+                                             self.n if seq_len is None else seq_len, int(shift), L.stream()), 'ln_fwd')
 
     # ------------------------------------------------------------------------------------------ forward
     def forward(self, ids):
@@ -369,12 +392,17 @@ class Engine:
         acts.tok.copy_(torch.as_tensor(ids).reshape(-1).to(device=self.dev, dtype=torch.int32))
         self._forward_device(acts, sink=lambda i, name, buf: sink(i, name, buf, P))
 
-    def _forward_device(self, acts=None, sink=None):
+    def _forward_device(self, acts=None, sink=None, length=None):
         """forward pass on activation set `acts` (default: the training set, which keeps what the backward pass reads);
-        with a `sink` (Engine.prefill) the layers' state goes to it and the logits head is skipped"""
+        with a `sink` (Engine.prefill) the layers' state goes to it and the logits head is skipped.
+        `length` (default seq_len): the positions per row, acts.T = acts.B * length.  Every mixing op is causal, so a
+        forward cut to the first `length` positions computes exactly those positions of the full one (DESIGN.md §3.6)."""
         acts = self.acts if acts is None else acts
         lib, st = self.lib, L.stream()
-        cfg, d, I, hid, T, n = self.cfg, self.d, self.I, self.hid, acts.T, self.n
+        cfg, d, I, hid, T = self.cfg, self.d, self.I, self.hid, acts.T
+        n = self.n if length is None else length
+        if T != acts.B * n:
+            raise L.ProgenError(f'forward: {T} token rows are not {acts.B} rows of length {n}')
         shift = cfg['shift_tokens']
         L.check(lib.progen_embed_fwd(acts.tok.data_ptr(), self.Pf(P + 'embed', 'embeddings').data_ptr(), acts.X[0].data_ptr(),
                                      T, d, self.V, st), 'embed_fwd')
@@ -384,17 +412,17 @@ class Engine:
             # in place (inference): x0 = x1 = x2 is one buffer, and the residual epilogue without aux reads its output
             x0, x1, x2 = acts.X[2 * i], acts.X[2 * i + 1], acts.X[2 * i + 2]
             # ---- LocalAttention (progen.py:73-103)
-            self.ln_fwd(x0, d, self.Pf(a + 'layer_norm', 'scale'), s['y1'], d, s['mean1'], s['rstd1'], d, shift, acts=acts)
+            self.ln_fwd(x0, d, self.Pf(a + 'layer_norm', 'scale'), s['y1'], d, s['mean1'], s['rstd1'], d, shift, acts=acts, seq_len=n)
             self.fwd_gemm(s['y1'], d, self.W(a + 'linear', 'w'), 3 * I, s['qkv'], epi=L.EPI_ROTARY, rot_sin=self.rot_sin,
                           rot_cos=self.rot_cos, seq_len=n, dim_head=self.dh, acts=acts)
             if sink is not None:
                 sink(i, 'qkv', s['qkv'])
                 sink(i, 'y1', s['y1'])
-            self.attn_fwd(s['qkv'], s['att'], s['lse'], acts=acts)
+            self.attn_fwd(s['qkv'], s['att'], s['lse'], acts=acts, seq_len=n)
             self.fwd_gemm(s['att'], I, self.W(a + 'linear_1', 'w'), d, x1, epi=L.EPI_RESIDUAL, bias=self.Pf(a + 'linear_1', 'b'),
                           aux=None if acts.inplace else x0, ldaux=d, acts=acts)
             # ---- FeedForward (progen.py:131-149); s['u'] is None in the inference set: no pre-activation store
-            self.ln_fwd(x1, d, self.Pf(f + 'layer_norm', 'scale'), s['y2'], d, s['mean2'], s['rstd2'], d, shift, acts=acts)
+            self.ln_fwd(x1, d, self.Pf(f + 'layer_norm', 'scale'), s['y2'], d, s['mean2'], s['rstd2'], d, shift, acts=acts, seq_len=n)
             if sink is not None:
                 sink(i, 'y2', s['y2'])
             if kind == 'glu':
@@ -410,9 +438,9 @@ class Engine:
                 g = f + 'sgu'
                 gate = s['hact'][:, half:]
                 self.ln_fwd(gate, hid, self.Pf(g + '/~/layer_norm', 'scale'), s['gn'], half, s['mean3'], s['rstd3'], half, False,
-                            acts=acts)
+                            acts=acts, seq_len=n)
                 # gate_b = tril(W) @ gn_b for every sequence b; masked K tiles are skipped (causal=1)
-                self._mm(M=n, N=half, K=n, A=self.wm[i], lda=n, B=s['gn'], ldb=half, b_mn=True, out=s['gp'], ldo=half,
+                self._mm(M=n, N=half, K=n, A=self.wm[i], lda=self.n, B=s['gn'], ldb=half, b_mn=True, out=s['gp'], ldo=half,
                          out_dtype=self.act_dt, batch=acts.B, b_batch_rows=n, d_batch_rows=n, causal=1)
                 if sink is not None:
                     sink(i, 'gn', s['gn'])
@@ -428,17 +456,18 @@ class Engine:
             return
         # ---- to_logits (progen.py:219-222)
         xl = acts.X[-1]
-        self.ln_fwd(xl, d, self.Pf(P + 'layer_norm', 'scale'), acts.yf, d, acts.meanf, acts.rstdf, d, False, acts=acts)
+        self.ln_fwd(xl, d, self.Pf(P + 'layer_norm', 'scale'), acts.yf, d, acts.meanf, acts.rstdf, d, False, acts=acts, seq_len=n)
         self.fwd_gemm(acts.yf, d, self.W(P + 'linear', 'w'), self.V, acts.logits, bias=self.Pf(P + 'linear', 'b'), out_dtype=L.F32,
                       acts=acts)
 
-    def attn_fwd(self, qkv, out, lse, acts=None):
+    def attn_fwd(self, qkv, out, lse, acts=None, seq_len=None):
         B = (acts or self.acts).B
+        n = self.n if seq_len is None else seq_len
         if self.attn_tc:
-            L.check(self.lib.progen_local_attn_fwd_tc(qkv.data_ptr(), out.data_ptr(), lse.data_ptr(), B, self.n, self.w, self.h,
+            L.check(self.lib.progen_local_attn_fwd_tc(qkv.data_ptr(), out.data_ptr(), lse.data_ptr(), B, n, self.w, self.h,
                                                       self.dh, L.stream()), 'local_attn_fwd')
             return
-        L.check(self.lib.progen_local_attn_fwd_simt(qkv.data_ptr(), out.data_ptr(), lse.data_ptr(), self.act_dt, B, self.n,
+        L.check(self.lib.progen_local_attn_fwd_simt(qkv.data_ptr(), out.data_ptr(), lse.data_ptr(), self.act_dt, B, n,
                                                     self.w, self.h, self.dh, L.stream()), 'local_attn_fwd')
 
     def attn_bwd(self, qkv, out, dout, lse, dqkv):
@@ -452,12 +481,16 @@ class Engine:
                                                     L.stream()), 'local_attn_bwd')
 
     # ------------------------------------------------------------------------------------------ scoring (inference)
-    def score(self, data, batch_size=64, tokens=False, embeddings=False):
+    def score(self, data, batch_size=64, tokens=False, embeddings=False, length=None):
         """data: (N, n+1) integer rows (ids = data[:, :-1], labels = data[:, 1:], as in loss_and_grad) -> dict of numpy
         arrays: log_likelihood [N] (sum of the label log-probabilities under the loss mask), num_tokens [N] (mask size);
         token_logp [N, n] with `tokens`; embedding [N, d] (masked mean of the final LayerNorm output) with `embeddings`.
         Runs the forward on the inference activation set, `batch_size` rows at a time: one H2D copy of the rows, the
-        forward, progen_token_logprob (+ progen_masked_mean_pool) and one D2H copy of the results per chunk."""
+        forward, progen_token_logprob (+ progen_masked_mean_pool) and one D2H copy of the results per chunk.
+        `length` (default seq_len): run the forward over the first `length` positions of every row only, on a
+        (B, length) view of the same activation set.  It must be seq_len or a multiple of CUT_ALIGN that covers every
+        counted position of every row (`cut_length`); the results are then bitwise those of the full-length forward, and
+        token_logp is zero beyond `length`."""
         rows = torch.as_tensor(np.asarray(data).astype(np.int32)) if not isinstance(data, torch.Tensor) else data
         rows = rows.to(device='cpu', dtype=torch.int32)
         if rows.dim() != 2 or rows.shape[1] != self.n + 1:
@@ -465,6 +498,14 @@ class Engine:
         if batch_size < 1:
             raise L.ProgenError(f'score: batch_size must be >= 1, got {batch_size}')
         N, n, d = rows.shape[0], self.n, self.d
+        cut = n if length is None else length
+        if length is not None:
+            if not isinstance(length, (int, np.integer)) or not (length == n or (0 < length < n and length % CUT_ALIGN == 0)):
+                raise L.ProgenError(f'score: length must be seq_len ({n}) or a multiple of {CUT_ALIGN} below it, got {length!r}')
+            if N and int(counted_length(rows[:, 1:].numpy()).max()) > length:
+                raise L.ProgenError(f'score: length {length} cuts off counted positions (cut_length of these rows: '
+                                    f'{cut_length(rows[:, 1:].numpy())})')
+            cut = int(length)
         out = dict(log_likelihood=np.zeros(N, np.float32), num_tokens=np.zeros(N, np.int64))
         if tokens:
             out['token_logp'] = np.zeros((N, n), np.float32)
@@ -477,25 +518,27 @@ class Engine:
         for r0 in range(0, N, batch_size):
             chunk = rows[r0:r0 + batch_size]
             B = chunk.shape[0]
-            acts = full if B == full.B else full.view(B, n)
+            acts = full if B == full.B and cut == n else full.view(B, cut)
             T = acts.T
-            acts.rows.copy_(chunk)
-            acts.tok.view(B, n).copy_(acts.rows[:, :-1])
-            acts.labels.view(B, n).copy_(acts.rows[:, 1:])
-            self._forward_device(acts)
+            # the rows staged as one contiguous (B, cut + 1) block: one H2D copy of what the cut forward reads
+            staged = acts.rows if cut == n else full.rows.view(-1)[:B * (cut + 1)].view(B, cut + 1)
+            staged.copy_(chunk if cut == n else chunk[:, :cut + 1])
+            acts.tok.view(B, cut).copy_(staged[:, :-1])
+            acts.labels.view(B, cut).copy_(staged[:, 1:])
+            self._forward_device(acts, length=length)
             # results, packed for one D2H copy: seq_ll [B] | seq_count [B] | logp [T] | embedding [B, d]
             ll, cnt, lp, emb = full.res[:B], full.res[B:2 * B], full.res[2 * B:2 * B + T], full.res[2 * B + T:2 * B + T + B * d]
             L.check(lib.progen_token_logprob(acts.logits.data_ptr(), L.F32, acts.labels.data_ptr(), lp.data_ptr(), ll.data_ptr(),
-                                             cnt.data_ptr(), B, n, self.V, st), 'token_logprob')
+                                             cnt.data_ptr(), B, cut, self.V, st), 'token_logprob')
             if embeddings:
                 L.check(lib.progen_masked_mean_pool(acts.yf.data_ptr(), d, self.act_dt, acts.labels.data_ptr(), emb.data_ptr(),
-                                                    B, n, d, st), 'masked_mean_pool')
+                                                    B, cut, d, st), 'masked_mean_pool')
             used = 2 * B + (T + B * d if embeddings else T if tokens else 0)
             host = full.res[:used].cpu().numpy()
             out['log_likelihood'][r0:r0 + B] = host[:B]
             out['num_tokens'][r0:r0 + B] = host[B:2 * B].astype(np.int64)
             if tokens:
-                out['token_logp'][r0:r0 + B] = host[2 * B:2 * B + T].reshape(B, n)
+                out['token_logp'][r0:r0 + B, :cut] = host[2 * B:2 * B + T].reshape(B, cut)
             if embeddings:
                 out['embedding'][r0:r0 + B] = host[2 * B + T:].reshape(B, d)
         return out

@@ -9,7 +9,8 @@ Beyond the reference surface: `.apply` also accepts a batch (B, n); `.loss_and_g
 equivalent of `value_and_grad(get_loss_fn(model))` (utils.py:61-93); `.trainer(...)` owns device-resident training
 state (parameters, Adam moments, apply_every accumulator) for the train.py loop; `.score(params, data)` is an
 inference-only forward returning per-sequence log-likelihoods (and optionally per-token log-probabilities and pooled
-embeddings).
+embeddings); `.score_variants` / `.mutational_scan` score substitutions against a wild type on that forward, cut to the
+positions that count.
 """
 import numpy as np
 import torch
@@ -172,6 +173,60 @@ class ProGen:
             pad = labels == 0
             out['token_mask'] = ~pad | ((np.cumsum(pad, axis=-1) == 1) & pad)
         return out
+
+    def score_variants(self, params, wild_type, mutations, *, prefix='', batch_size=64, return_tokens=False):
+        """Zero-shot variant effects: log p(variant) - log p(wild type) under the model, for each mutation set.
+
+        wild_type: residue string.  prefix: optional prompt / tag string placed before the residues (e.g.
+        '[Tax=Mammalia] #').  Each row is `data.collate([prefix + residues], seq_len)`, exactly what `score` receives.
+        mutations: non-empty list of ProteinGym-style sets, 'A23G', 'A23G:K45R', or '' for the wild type; positions are
+        1-based over the residues (not the prefix).  Rejected with ProgenError naming the set: a wild-type letter that does
+        not match, a position out of range or cut off by seq_len, the same position twice in one set, a new letter that
+        is not one printable ASCII character.  Identity substitutions (A23A) are allowed.
+
+        The wild type and every variant run through the scoring forward cut to L = min(seq_len, counted length rounded up
+        to 128) positions: every mixing op is causal, so positions < L depend on ids < L only, and the cut forward
+        computes them bitwise as the full-length one does (DESIGN.md §3.6).  The wild type is scored once per call.
+
+        Returns a dict:
+          delta [M] float64: sum over positions of (variant - wild type) token log-probabilities, in float64, so
+            identical positions cancel exactly (0.0 for '' and for identity substitutions);
+          log_likelihood [M] float32 and num_tokens [M] int64: as `score` reports them for the variant rows;
+          wt_log_likelihood (float32): `score`'s log-likelihood of the wild-type row;
+          token_logp [M, seq_len] float32 (with return_tokens): as `score` reports it (zero beyond L).
+        Rows run batch_size at a time; results do not depend on batch_size or on the other sets in the call."""
+        from .engine import cut_length
+        from .variants import parse_mutations, variant_rows
+        n = self.config['seq_len']
+        subs = parse_mutations(wild_type, mutations, n, prefix)
+        if isinstance(batch_size, (bool, np.bool_)) or not isinstance(batch_size, (int, np.integer)) or batch_size < 1:
+            raise L.ProgenError(f'score_variants: batch_size must be an integer >= 1, got {batch_size!r}')
+        rows = variant_rows(wild_type, subs, n, prefix)
+        length = cut_length(rows[:, 1:])
+        self._ensure_loaded(params)
+        sc = self.engine.score(rows, batch_size=batch_size, tokens=True, length=length)
+        lp = sc['token_logp'][:, :length].astype(np.float64)
+        out = dict(delta=(lp[1:] - lp[0]).sum(axis=-1), log_likelihood=sc['log_likelihood'][1:],
+                   num_tokens=sc['num_tokens'][1:], wt_log_likelihood=sc['log_likelihood'][0])
+        if return_tokens:
+            out['token_logp'] = sc['token_logp'][1:]
+        return out
+
+    def mutational_scan(self, params, wild_type, *, positions=None, alphabet='ACDEFGHIKLMNPQRSTVWY', prefix='', batch_size=64):
+        """Deep mutational scan: every single substitution at `positions` (1-based, default every residue) to each letter
+        of `alphabet`, scored by `score_variants` in one call.  Returns a dict: delta [P, |alphabet|] float64 (0.0 at
+        the wild-type letter, which is not run), positions [P] int64, alphabet, wt_log_likelihood."""
+        from .variants import check_scan, scan_sets
+        pos = check_scan(wild_type, positions, alphabet)
+        sets, index = scan_sets(wild_type, pos, alphabet)
+        delta = np.zeros(index.shape, np.float64)
+        if sets:
+            res = self.score_variants(params, wild_type, sets, prefix=prefix, batch_size=batch_size)
+            delta[index >= 0] = res['delta'][index[index >= 0]]
+            wt = res['wt_log_likelihood']
+        else:                          # an alphabet of the wild-type letter alone: nothing to run but the wild type
+            wt = self.score_variants(params, wild_type, [''], prefix=prefix, batch_size=batch_size)['wt_log_likelihood']
+        return dict(delta=delta, positions=pos, alphabet=alphabet, wt_log_likelihood=wt)
 
     def generate(self, params, prompts, *, num_samples=1, temperature=1.0, top_k=None, top_p=None, max_length=None, seed=0,
                  batch_size=64, logit_bias=None, min_new_tokens=0, repetition_penalty=1.0, repetition_window=0,
