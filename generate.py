@@ -3,13 +3,17 @@
     python generate.py --checkpoint_path ./ckpts --prompt "[Tax=Mammalia] #" [--prompt ... | --prompts_file f.txt]
         --num_samples 100 --temperature 1.0 [--top_k K] [--top_p 0.95] --seed 0 --batch_size 64 [--max_length L]
         [--alphabet ACDEFGHIKLMNPQRSTVWY] [--min_new_tokens N] [--repetition_penalty 1.2 --repetition_window 16]
-        [--mixed_precision] [--prefill forward] --output samples.fasta
+        [--fix 12=H,57=D,102=S] [--position_bias bias.npy] [--mixed_precision] [--prefill forward] --output samples.fasta
 
 Runs ProGen.generate: each prompt is laid out like training data (BOS, prompt), every sequence stops at its own EOS,
 temperature / top-k / nucleus (top-p) filtering happen in the persistent decode kernel.  --alphabet restricts every
 draw to those residues and EOS, --min_new_tokens forbids EOS for the first N generated tokens, and --repetition_penalty
 penalises the residues present in the last --repetition_window positions (0: the whole sequence); these act on the
-logits in the kernel and leave the reported log-likelihood that of the unconstrained model.  --prefill forward fills
+logits in the kernel and leave the reported log-likelihood that of the unconstrained model.  --fix K=R,... makes
+generated residue K (1-based) of every sequence R, and no sequence ends before its last fixed residue; --position_bias
+adds row j of a float32 [T, V] .npy array to the logits of generated token j + 1 (-inf bans an id there).  A
+contradiction between these constraints (a fixed residue outside --alphabet, say) stops with the library's error
+message before anything runs.  --prefill forward fills
 the decoder's caches for the prompt with one forward pass per distinct prompt instead of one decode step per prompt
 position (faster for long prompts; bf16 models then differ from the default by round-off).  Unlike sample.py (the reference
 drop-in, one sequence, top_k=25 with the reference's quirks), the result of a row depends only on the seed and the row.
@@ -47,6 +51,31 @@ def alphabet_bias(alphabet, num_tokens):
     return bias
 
 
+def parse_fix(text):
+    """--fix '12=H,57=D' -> {12: 'H', 57: 'D'}: 1-based generated offsets and one residue character each"""
+    out = {}
+    for item in text.split(','):
+        k, sep, res = item.strip().partition('=')
+        if not sep or not k.strip().isdigit() or len(res.strip()) != 1:
+            raise ProgenError(f'--fix: expected OFFSET=RESIDUE items separated by commas (e.g. 12=H,57=D), got {item!r}')
+        k = int(k)
+        if k in out:
+            raise ProgenError(f'--fix: offset {k} given twice')
+        out[k] = res.strip()
+    return out
+
+
+def load_position_bias(path):
+    """--position_bias: a [T, V] float32 array from a .npy file"""
+    try:
+        a = np.load(path, allow_pickle=False)
+    except (OSError, ValueError) as e:
+        raise ProgenError(f'--position_bias: cannot read {path}: {e}') from None
+    if a.dtype != np.float32 or a.ndim != 2:
+        raise ProgenError(f'--position_bias: {path} must hold a float32 [T, V] array, got {a.dtype} {a.shape}')
+    return a
+
+
 @click.command()
 @click.option('--checkpoint_path', default='./ckpts')
 @click.option('--prompt', 'prompts', multiple=True, help='prompt text (repeatable)')
@@ -62,12 +91,15 @@ def alphabet_bias(alphabet, num_tokens):
 @click.option('--min_new_tokens', default=0, help='generated tokens before EOS may be drawn')
 @click.option('--repetition_penalty', default=1.0, help='divide positive / multiply negative logits of recent ids (1 = off)')
 @click.option('--repetition_window', default=0, help='positions the repetition penalty looks back (0 = the whole sequence)')
+@click.option('--fix', default=None, help='fixed residues by 1-based generated offset, e.g. 12=H,57=D,102=S')
+@click.option('--position_bias', default=None, help='.npy float32 [T, V]: row j is added to the logits of generated token j+1')
 @click.option('--mixed_precision', default=False, is_flag=True, help='bf16 weights in the decode kernel')
 @click.option('--prefill', default='decode', type=click.Choice(['decode', 'forward']),
               help='prompt positions: one decode step each, or one forward pass per distinct prompt')
 @click.option('--output', default='samples.fasta')
 def main(checkpoint_path, prompts, prompts_file, num_samples, temperature, top_k, top_p, seed, batch_size, max_length,
-         alphabet, min_new_tokens, repetition_penalty, repetition_window, mixed_precision, prefill, output):
+         alphabet, min_new_tokens, repetition_penalty, repetition_window, fix, position_bias, mixed_precision, prefill,
+         output):
     _, get_last_checkpoint, _ = get_checkpoint_fns(checkpoint_path)
     last_checkpoint = get_last_checkpoint()
     if last_checkpoint is None:
@@ -76,6 +108,11 @@ def main(checkpoint_path, prompts, prompts_file, num_samples, temperature, top_k
     model_kwargs = last_checkpoint['model_config']
     model = ProGen(**{**model_kwargs, 'mixed_precision': mixed_precision})
     bias = None if alphabet is None else alphabet_bias(alphabet, model.config['num_tokens'])
+    try:
+        fixed = None if fix is None else parse_fix(fix)
+        pbias = None if position_bias is None else load_position_bias(position_bias)
+    except ProgenError as e:
+        exit(f'ProgenError: {e}')
     prompts = list(prompts)
     if prompts_file is not None:
         with open(prompts_file) as f:
@@ -84,10 +121,16 @@ def main(checkpoint_path, prompts, prompts_file, num_samples, temperature, top_k
         prompts = ['']
     print(f'sequence length: {model_kwargs["seq_len"]}')
     t0 = time.perf_counter()
-    res = model.generate(params, prompts, num_samples=num_samples, temperature=temperature, top_k=top_k, top_p=top_p,
-                         max_length=max_length, seed=seed, batch_size=batch_size, logit_bias=bias,
-                         min_new_tokens=min_new_tokens, repetition_penalty=repetition_penalty,
-                         repetition_window=repetition_window, prefill=prefill)
+    kw = dict(num_samples=num_samples, temperature=temperature, top_k=top_k, top_p=top_p, max_length=max_length, seed=seed,
+              batch_size=batch_size, logit_bias=bias, min_new_tokens=min_new_tokens, repetition_penalty=repetition_penalty,
+              repetition_window=repetition_window, prefill=prefill)
+    if fixed is None and pbias is None:
+        res = model.generate(params, prompts, **kw)
+    else:
+        try:                                             # contradictory constraints: the library's message, no traceback
+            res = model.generate(params, prompts, position_bias=pbias, fixed=fixed, **kw)
+        except ProgenError as e:
+            exit(f'ProgenError: {e}')
     secs = time.perf_counter() - t0
     N = len(res['length'])
     with open(output, 'w') as f:

@@ -240,8 +240,8 @@ typedef struct progen_decode_run_t {
    * 0 = the whole row; BOS excluded; each id counts once), else a[c] = l[c]; then a += logit_bias (-inf bans an id); then
    * a[0] = -inf while p + 1 < start[b] + min_new_tokens.  The candidates are the ids whose a is neither -inf nor NaN; the
    * filter and the draw above run on a over them (the softmax maximum is the candidates' maximum of a), and a row with
-   * none draws EOS.  Off (the unconstrained code) when logit_bias is NULL, repetition_penalty is 1 and min_new_tokens is
-   * 0; a zero-initialised struct must set repetition_penalty to 1. */
+   * none draws EOS.  Off (the unconstrained code) when logit_bias and position_bias (below) are NULL, repetition_penalty
+   * is 1 and min_new_tokens is 0; a zero-initialised struct must set repetition_penalty to 1. */
   const float* logit_bias;     /* [V] or NULL */
   float repetition_penalty;    /* finite, > 0; 1 = off */
   int32_t repetition_window;   /* >= 0; 0 = every position since BOS */
@@ -264,6 +264,15 @@ typedef struct progen_decode_run_t {
   int32_t* done;               /* device: rows retired */
   int32_t num_rows;            /* Q */
   int32_t max_length;          /* in [2, n]: a row's last drawn position is max_length - 1 */
+  /* Position-specific bias (sampler 1; both pointers NULL = off): tables of per-offset logit biases.  For the draw of
+   * position p + 1 of row r (the queue row when there is a queue), j = p + 1 - start[r] is the 0-based generated offset;
+   * if t = position_bias_table[r] >= 0 and j < position_bias_len, a[c] += position_bias[(t * position_bias_len + j) * V
+   * + c] in fp32 (its own rounding, no FMA), after the logit bias and before the min_new_tokens EOS ban above.  -inf bans
+   * an id at that offset; an offset whose only candidate is one id forces it.  token_logp is unchanged. */
+  const float* position_bias;        /* [tables, position_bias_len, V] or NULL */
+  const int32_t* position_bias_table;/* [rows]: the table of each row, -1 = none */
+  int32_t position_bias_len;         /* in [1, n] when position_bias is set */
+  int32_t _pad3;
 } progen_decode_run_t;
 
 int progen_decode_run(const progen_decode_run_t* run, void* stream);

@@ -1484,7 +1484,9 @@ static __device__ __forceinline__ float philox_gumbel(unsigned long long seed, l
 // registers stay out of the GEMV phases' allocation.  sv: shared memory [2 V]; red: the block-reduction scratch.
 // Constraints (progen_b200.h): after logsumexp of the raw logits, sv is overwritten with the adjusted logits a, and the
 // filter and draw below run on a unchanged: -inf and NaN never win a comparison, so only candidates can be drawn.
-struct SampleCons { const float* bias; float theta; int window, min_new; };  // one argument: fewer registers at the call
+// One argument (fewer registers at the call): the logit bias, the repetition penalty, min_new_tokens and the position
+// tables (pbias [tables, plen, V], ptable [rows]: each row's table or -1; pbias null = none)
+struct SampleCons { const float* bias; float theta; int window, min_new; const float* pbias; const int32_t* ptable; int plen; };
 // The queue kernels' view of the slots (SLOT): this step's row and position of every slot (shared memory), the queue's
 // device state and what a refill resets.  Without a queue (slot_row null) srow[b] = b and spos[b] = the launch's position.
 struct SlotArgs {
@@ -1507,7 +1509,7 @@ static __device__ __noinline__ void sample_std_phase(const float* logits, int32_
   const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
   float* qv = sv + V;                                                          // kept ids: q; removed: -1
   int* redi = reinterpret_cast<int*>(red + 32);
-  const bool cons = cs.bias != nullptr || cs.theta != 1.f || cs.min_new != 0;  // uniform
+  const bool cons = cs.bias != nullptr || cs.theta != 1.f || cs.min_new != 0 || cs.pbias != nullptr;  // uniform
   auto bmax = [&](float m) {
     m = warp_max(m);
     __syncthreads();
@@ -1620,11 +1622,17 @@ static __device__ __noinline__ void sample_std_phase(const float* logits, int32_
           __syncthreads();
         }
         const bool no_eos = pos + 1 < start[rb] + cs.min_new;
+        const float* pb = nullptr;                                              // the row's table row at offset j
+        if (cs.pbias) {
+          const int tb = __ldg(cs.ptable + rb), j = pos + 1 - start[rb];       // (j >= 0: a drawn position)
+          if (tb >= 0 && j < cs.plen) pb = cs.pbias + ((long long)tb * cs.plen + j) * V;
+        }
         float ma = -INFINITY;
         for (int c = t; c < V; c += TPB) {
           float a = sv[c];
           if (pen && seen[c]) a = a > 0.f ? __fdiv_rn(a, cs.theta) : __fmul_rn(a, cs.theta);
           if (cs.bias) a = __fadd_rn(a, __ldg(cs.bias + c));                 // (no FMA with the penalty's product)
+          if (pb) a = __fadd_rn(a, __ldg(pb + c));                            // a separate rounding after the bias
           if (c == 0 && no_eos) a = -INFINITY;
           sv[c] = a;
           ma = fmaxf(ma, a);
@@ -1900,13 +1908,15 @@ static __device__ __forceinline__ void run(const progen_decode_run_t& r) {
       } else if constexpr (SLOT) {
         sample_std_phase<true>(r.logits, r.seq, r.start, r.end, r.n_ended, r.token_logp, r.logits_all, r.embed, r.x, r.sample_id, r.n, r.V,
                                d, B, r.top_k, r.temperature, r.top_p, r.seed,
-                               SampleCons{r.logit_bias, r.repetition_penalty, r.repetition_window, r.min_new_tokens}, pos, xs, red,
+                               SampleCons{r.logit_bias, r.repetition_penalty, r.repetition_window, r.min_new_tokens, r.position_bias,
+                                          r.position_bias_table, r.position_bias_len}, pos, xs, red,
                                SlotArgs{s_row, s_pos, r.slot_row, r.slot_pos, r.next_row, r.done, r.layers, r.depth, r.num_rows,
                                         r.max_length, r.shift_tokens});
       } else if constexpr (STD) {
         sample_std_phase<false>(r.logits, r.seq, r.start, r.end, r.n_ended, r.token_logp, r.logits_all, r.embed, r.x, r.sample_id, r.n, r.V,
                                 d, B, r.top_k, r.temperature, r.top_p, r.seed,
-                                SampleCons{r.logit_bias, r.repetition_penalty, r.repetition_window, r.min_new_tokens}, pos, xs, red);
+                                SampleCons{r.logit_bias, r.repetition_penalty, r.repetition_window, r.min_new_tokens, r.position_bias,
+                                          r.position_bias_table, r.position_bias_len}, pos, xs, red);
       } else {
         sample_phase(r, pos, xs, red);
       }
@@ -2001,6 +2011,9 @@ int progen_decode_run(const progen_decode_run_t* r, void* stream) {
   PG_CHECK_ARG(std::isfinite(r->repetition_penalty) && r->repetition_penalty > 0.f);
   PG_CHECK_ARG(r->repetition_window >= 0 && r->repetition_window <= r->n && r->min_new_tokens >= 0 && r->min_new_tokens <= r->n);
   if (r->sampler == 0) PG_CHECK_ARG(r->logit_bias == nullptr && r->repetition_penalty == 1.f && r->min_new_tokens == 0);
+  // position tables: both pointers or neither, a length in [1, n], sampler 1 only
+  PG_CHECK_ARG((r->position_bias == nullptr) == (r->position_bias_table == nullptr));
+  if (r->position_bias) PG_CHECK_ARG(r->sampler == 1 && r->position_bias_len >= 1 && r->position_bias_len <= r->n);
   if (r->sampler == 1) {
     PG_CHECK_ARG(std::isfinite(r->temperature) && r->temperature >= 0.f && r->top_p > 0.f && r->top_p <= 1.f);
     PG_CHECK_ARG(r->top_k >= 0 && r->top_k <= r->V);

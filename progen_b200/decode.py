@@ -32,7 +32,8 @@ class DecodeRun(C.Structure):
                [('sampler', _I), ('temperature', C.c_float), ('top_p', C.c_float), ('_pad1', _I), ('seed', C.c_uint64)] + \
                [(k, _P) for k in ('sample_id', 'token_logp', 'end', 'n_ended', 'steps_run', 'logit_bias')] + \
                [('repetition_penalty', C.c_float), ('repetition_window', _I), ('min_new_tokens', _I), ('_pad2', _I)] + \
-               [(k, _P) for k in ('slot_row', 'slot_pos', 'next_row', 'done')] + [('num_rows', _I), ('max_length', _I)]
+               [(k, _P) for k in ('slot_row', 'slot_pos', 'next_row', 'done')] + [('num_rows', _I), ('max_length', _I)] + \
+               [(k, _P) for k in ('position_bias', 'position_bias_table')] + [('position_bias_len', _I), ('_pad3', _I)]
 
 
 class BatchDecoder:
@@ -133,6 +134,7 @@ class BatchDecoder:
         m.repetition_penalty = 1.0                        # constraints off
         self._gen = None                                  # sampler-1 buffers, allocated by the first generate()
         self._bias = None                                 # [V] logit bias of generate(), allocated on first use
+        self._pos = None                                  # position tables and row map of the running launch
 
     def _hold(self, t):
         self.keep.append(t)
@@ -280,7 +282,8 @@ class BatchDecoder:
         return seq0, starts
 
     def generate(self, prompts, *, temperature=1.0, top_k=None, top_p=None, seed=0, sample_ids=None, max_length=None,
-                 logit_bias=None, min_new_tokens=0, repetition_penalty=1.0, repetition_window=0, prefilled=0):
+                 logit_bias=None, min_new_tokens=0, repetition_penalty=1.0, repetition_window=0, position_bias=None,
+                 prefilled=0):
         """The standard sampler (sampler 1 of csrc/decode_persist.cu) for up to B prompts (integer arrays of ids in [1, V)).
         Each row is laid out as training data is, [0 (BOS), prompt..., 0...], and draws positions 1 + len(prompt) ..
         max_length - 1 until it samples EOS (id 0).  Row b uses the Philox stream sample_ids[b] (default b); the
@@ -290,6 +293,9 @@ class BatchDecoder:
         in the last `repetition_window` positions (0: all since BOS) have positive logits divided and negative ones
         multiplied by `repetition_penalty`; `logit_bias` ([V] floats, -inf bans an id) is added; EOS is banned for the
         first `min_new_tokens` draws of a row.  They do not change token_logp, the unfiltered model's log-probability.
+        position_bias = (tables [Tb, Lb, V] float32, table_of_row [R] ints in [-1, Tb)): the draw of a row's generated
+        offset j (0 = its first generated token) adds tables[table_of_row[r], j] to the logits after logit_bias and
+        before the EOS ban, for j < Lb (-1: no table; -inf bans an id at that offset).
         prefilled = P > 0: `prefill` has filled the caches of these prompts for positions < P (P <= every prompt's
         length), so the caches are not reset and the kernel starts at position P instead of 0.
         Returns a dict of numpy arrays: ids [R, n] int64, token_logp [R, n] float32 (log p(ids[t] | ids[:t]) at drawn t,
@@ -305,8 +311,8 @@ class BatchDecoder:
         if not 0 <= int(prefilled) <= first:
             raise L.ProgenError(f'generate: prefilled must lie in [0, {first}] (the shortest prompt length)')
         prefilled = int(prefilled)
-        logit_bias = self._check_sampler(temperature, top_k, top_p, logit_bias, min_new_tokens, repetition_penalty,
-                                         repetition_window)
+        logit_bias, position_bias = self._check_sampler(temperature, top_k, top_p, logit_bias, min_new_tokens,
+                                                        repetition_penalty, repetition_window, position_bias, R)
         if self._gen is None:
             z = lambda *s, dtype: torch.zeros(*s, device=self.dev, dtype=dtype)
             self._gen = dict(sample_id=z(self.B, dtype=torch.int64), token_logp=z(self.B, n, dtype=torch.float32),
@@ -324,7 +330,8 @@ class BatchDecoder:
         m.B = R
         m.sample_id, m.token_logp, m.end = gb['sample_id'].data_ptr(), gb['token_logp'].data_ptr(), gb['end'].data_ptr()
         m.n_ended, m.steps_run = gb['counters'].data_ptr(), gb['counters'].data_ptr() + 4
-        self._set_sampler(temperature, top_k, top_p, seed, logit_bias, min_new_tokens, repetition_penalty, repetition_window)
+        self._set_sampler(temperature, top_k, top_p, seed, logit_bias, min_new_tokens, repetition_penalty, repetition_window,
+                          position_bias)
         try:
             ev = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
             e0, e1 = ev[1], ev[2]
@@ -342,22 +349,24 @@ class BatchDecoder:
                     device_s=e0.elapsed_time(e1) / 1e3, prefill_s=ev[0].elapsed_time(e0) / 1e3)
 
     def generate_queue(self, prompts, *, slots=None, temperature=1.0, top_k=None, top_p=None, seed=0, sample_ids=None,
-                       max_length=None, logit_bias=None, min_new_tokens=0, repetition_penalty=1.0, repetition_window=0):
+                       max_length=None, logit_bias=None, min_new_tokens=0, repetition_penalty=1.0, repetition_window=0,
+                       position_bias=None):
         """`generate` for Q = len(prompts) rows on `slots` (default min(B, Q), 2 <= slots <= min(B, Q)) sequences of ONE
         persistent launch: the rows form a queue, and a slot whose row ends (EOS, or position max_length - 1) takes the
         next row, which starts at position 0 with its prompt decoded like generated positions (csrc/decode_persist.cu,
         progen_b200.h).  A row's bits depend on its seed, sample id, prompt, the class of `slots` (2-8 or 9-64) and
         the GPU's SM count, not on its slot or the other rows, so each row equals what `generate` gives it in a launch of
-        that class; the launch merely has no slot waiting for its longest row.  Returns the arrays of `generate` over the
-        Q rows, steps_run (positions the launch ran) and device_s (its device time)."""
+        that class; the launch merely has no slot waiting for its longest row.  position_bias's table_of_row is indexed
+        by queue row ([Q]).  Returns the arrays of `generate` over the Q rows, steps_run (positions the launch ran) and
+        device_s (its device time)."""
         n = self.n
         Q = len(prompts)
         slots = min(self.B, Q) if slots is None else int(slots)
         if not 2 <= slots <= min(self.B, Q):
             raise L.ProgenError(f'generate_queue: 2 <= slots <= min(batch {self.B}, rows {Q})')
         max_length, seq0, starts, sids = self._sampler_rows(prompts, sample_ids, max_length)
-        logit_bias = self._check_sampler(temperature, top_k, top_p, logit_bias, min_new_tokens, repetition_penalty,
-                                         repetition_window)
+        logit_bias, position_bias = self._check_sampler(temperature, top_k, top_p, logit_bias, min_new_tokens,
+                                                        repetition_penalty, repetition_window, position_bias, Q)
         dev = self.dev
         seq = torch.as_tensor(seq0).to(dev)
         start = torch.as_tensor(starts).to(dev)
@@ -374,7 +383,8 @@ class BatchDecoder:
         c = counters.data_ptr()
         m.n_ended, m.steps_run, m.next_row, m.done = c, c + 4, c + 8, c + 12
         m.slot_row, m.slot_pos, m.num_rows, m.max_length = slot_row.data_ptr(), slot_pos.data_ptr(), Q, max_length
-        self._set_sampler(temperature, top_k, top_p, seed, logit_bias, min_new_tokens, repetition_penalty, repetition_window)
+        self._set_sampler(temperature, top_k, top_p, seed, logit_bias, min_new_tokens, repetition_penalty, repetition_window,
+                          position_bias)
         # while rows wait in the queue every slot is busy, and a row consumes at most max_length - 1 positions
         nsteps = -(-Q * (max_length - 1) // slots) + max_length - 1
         try:
@@ -407,8 +417,10 @@ class BatchDecoder:
             raise L.ProgenError('generate: one sample id per prompt')
         return max_length, seq0, starts, sids
 
-    def _check_sampler(self, temperature, top_k, top_p, logit_bias, min_new_tokens, repetition_penalty, repetition_window):
-        """checks the sampler arguments of generate / generate_queue; -> logit_bias as float32 (or None)"""
+    def _check_sampler(self, temperature, top_k, top_p, logit_bias, min_new_tokens, repetition_penalty, repetition_window,
+                       position_bias=None, rows=0):
+        """checks the sampler arguments of generate / generate_queue (`rows` rows); -> (logit_bias as float32 or None,
+        position_bias as (float32 tables, int32 map) or None)"""
         n = self.n
         if top_k is not None and not 1 <= int(top_k) <= self.V:
             raise L.ProgenError(f'generate: 1 <= top_k <= {self.V}')
@@ -424,9 +436,27 @@ class BatchDecoder:
             raise L.ProgenError(f'generate: min_new_tokens and repetition_window must lie in [0, {n}]')
         if not (np.isfinite(repetition_penalty) and repetition_penalty > 0):
             raise L.ProgenError('generate: repetition_penalty must be finite and > 0')
-        return logit_bias
+        if position_bias is not None:
+            try:
+                tables, table_of_row = position_bias
+                tables = np.ascontiguousarray(np.asarray(tables, np.float32))
+                table_of_row = np.asarray(table_of_row)
+            except (TypeError, ValueError):
+                raise L.ProgenError('generate: position_bias must be a pair (tables [Tb, Lb, V], table_of_row [rows])') from None
+            if tables.ndim != 3 or tables.shape[0] < 1 or not 1 <= tables.shape[1] <= n or tables.shape[2] != self.V:
+                raise L.ProgenError(f'generate: position_bias tables must have shape [Tb >= 1, 1..{n}, {self.V}], '
+                                    f'got {tables.shape}')
+            if np.isnan(tables).any() or (tables == np.inf).any():
+                raise L.ProgenError('generate: position_bias tables must not contain NaN or +inf')
+            if table_of_row.shape != (rows,) or (rows and not np.issubdtype(table_of_row.dtype, np.integer)):
+                raise L.ProgenError(f'generate: position_bias needs one integer table index per row ({rows})')
+            if rows and (table_of_row.min() < -1 or table_of_row.max() >= tables.shape[0]):
+                raise L.ProgenError(f'generate: position_bias table indices must lie in [-1, {tables.shape[0]})')
+            position_bias = tables, table_of_row.astype(np.int32)
+        return logit_bias, position_bias
 
-    def _set_sampler(self, temperature, top_k, top_p, seed, logit_bias, min_new_tokens, repetition_penalty, repetition_window):
+    def _set_sampler(self, temperature, top_k, top_p, seed, logit_bias, min_new_tokens, repetition_penalty, repetition_window,
+                     position_bias=None):
         m = self.m
         m.sampler = 1
         m.temperature = float(temperature)
@@ -440,6 +470,11 @@ class BatchDecoder:
             m.logit_bias = self._bias.data_ptr()
         m.repetition_penalty = float(repetition_penalty)
         m.repetition_window, m.min_new_tokens = int(repetition_window), int(min_new_tokens)
+        if position_bias is not None:                     # uploaded per launch, held until _clear_sampler
+            tables, table_of_row = position_bias
+            self._pos = (torch.from_numpy(tables).to(self.dev), torch.from_numpy(table_of_row).to(self.dev))
+            m.position_bias, m.position_bias_table = self._pos[0].data_ptr(), self._pos[1].data_ptr()
+            m.position_bias_len = tables.shape[1]
 
     def _clear_sampler(self):
         """back to the reference sampler's launch fields (sample() after generate() runs what it ran before)"""
@@ -448,3 +483,6 @@ class BatchDecoder:
         m.temperature, m.top_p, m.seed = 0.0, 0.0, 0
         m.sample_id = m.token_logp = m.end = m.n_ended = m.steps_run = m.logit_bias = 0
         m.repetition_penalty, m.repetition_window, m.min_new_tokens = 1.0, 0, 0
+        m.position_bias = m.position_bias_table = 0
+        m.position_bias_len = 0
+        self._pos = None

@@ -53,19 +53,154 @@ def plan_launches(lengths, batch_size, by_length=False):
 # `ProGen.generate` feeds at most this many rows per slot to one queue launch: it bounds the launch's [rows, seq_len] ids
 # and log-probabilities in device memory and the time one launch holds the GPU
 QUEUE_ROWS_PER_SLOT = 64
+# ... and position-bias tables (`generate(position_bias=, fixed=)`) of at most this many bytes: one [seq_len, V] table is
+# 1 MiB at seq_len 1024 and V 256, and a queue launch of distinct prompts could otherwise hold thousands of them
+QUEUE_TABLE_BYTES = 256 << 20
 
 
-def plan_queue(n_rows, batch_size):
+def plan_queue(n_rows, batch_size, row_table=None, table_bytes=0):
     """The queue launches of `ProGen.generate` (prefill='decode') for n_rows rows: -> (slots, chunks), slots =
     min(batch_size, n_rows) sequences per launch and chunks a list of int64 arrays of row indices in row order, each run
     as the queue of one launch.  Rows are split into the fewest chunks of at most QUEUE_ROWS_PER_SLOT * slots rows, of
-    near-equal size, so every chunk holds at least `slots` rows.  None when slots < 2: the single-stream kernel keeps
-    one launch per row (`plan_launches`)."""
+    near-equal size, so every chunk holds at least `slots` rows.  With row_table ([n_rows] ints: each row's position
+    table, -1 = none) and table_bytes (the bytes of one table), a chunk is further cut, in row order, before the row
+    whose table would take its distinct tables past QUEUE_TABLE_BYTES, but never below `slots` rows (a last piece that
+    short joins the one before it).  None when slots < 2: the single-stream kernel keeps one launch per row
+    (`plan_launches`)."""
     slots = min(batch_size, n_rows)
     if slots < 2:
         return None
     k = -(-n_rows // (QUEUE_ROWS_PER_SLOT * slots))
-    return slots, [c.astype(np.int64) for c in np.array_split(np.arange(n_rows), k)]
+    chunks = [c.astype(np.int64) for c in np.array_split(np.arange(n_rows), k)]
+    if row_table is None or table_bytes <= 0:
+        return slots, chunks
+    row_table = np.asarray(row_table, np.int64)
+    cap = max(1, QUEUE_TABLE_BYTES // table_bytes)           # distinct tables per launch
+    out = []
+    for c in chunks:
+        pieces, cur, seen = [], [], set()
+        for r in c.tolist():
+            t = int(row_table[r])
+            if t >= 0 and t not in seen and len(seen) >= cap and len(cur) >= slots:
+                pieces.append(cur)
+                cur, seen = [], set()
+            cur.append(r)
+            if t >= 0:
+                seen.add(t)
+        if pieces and len(cur) < slots:
+            pieces[-1] += cur
+        else:
+            pieces.append(cur)
+        out += [np.asarray(q, np.int64) for q in pieces]
+    return slots, out
+
+
+def _per_prompt(arg, n_prompts, what, single):
+    """`arg` for every prompt: one value (single(arg) true) for all, or a list with one entry (or None) per prompt"""
+    if arg is None:
+        return [None] * n_prompts
+    if single(arg):
+        return [arg] * n_prompts
+    if not isinstance(arg, (list, tuple)) or len(arg) != n_prompts:
+        raise L.ProgenError(f'generate: {what} must be one value for every prompt or a list of {n_prompts} (one per prompt)')
+    return list(arg)
+
+
+def position_tables(starts, V, n, max_length, position_bias=None, fixed=None, logit_bias=None, min_new_tokens=0):
+    """The position tables of `ProGen.generate` for prompts whose first generated position is starts[i] (1 + prompt
+    length).  position_bias: None, a [T, V] array for every prompt, or a list of one array or None per prompt; fixed:
+    None, a dict {k: residue} for every prompt, or a list of one dict or None per prompt (k: 1-based generated offset;
+    residue: one character, encoded like training text, or an id in [1, V)).  A prompt's table row j is the bias of its
+    generated offset j + 1: its position_bias row (0 past its end) plus, for fixed residues, 0 at the fixed id and -inf
+    elsewhere at offset k, and -inf on EOS at every offset before its last fixed offset.  Checked, with ProgenError naming
+    the prompt and the offset: offsets in [1, max_length - starts[i]], residues in the vocabulary, and every reachable
+    offset keeps a candidate (an id with logit_bias + row finite; EOS not counted at offsets <= min_new_tokens).
+    Returns (tables, prompt_table): the distinct tables (float32 [L, V], L <= n; equal tables stored once) and an int64
+    array with each prompt's table index (-1: none)."""
+    from .data import encode_tokens
+    P = len(starts)
+    biases = _per_prompt(position_bias, P, 'position_bias', lambda a: not isinstance(a, (list, tuple)))
+    fixes = _per_prompt(fixed, P, 'fixed', lambda a: isinstance(a, dict))
+    lb = np.zeros(V, np.float32) if logit_bias is None else np.asarray(logit_bias, np.float32)
+    tables, index, prompt_table = [], {}, np.full(P, -1, np.int64)
+    for i in range(P):
+        reach = max_length - int(starts[i])              # generated offsets 1 .. reach fit before max_length
+        b, f = biases[i], fixes[i]
+        rows = None
+        if b is not None:
+            try:
+                with np.errstate(over='ignore'):
+                    rows = np.asarray(b, np.float64).astype(np.float32)
+            except (TypeError, ValueError):
+                raise L.ProgenError(f'generate: position_bias of prompt {i} must be an array of floats') from None
+            if rows.ndim != 2 or not 1 <= rows.shape[0] <= n or rows.shape[1] != V:
+                raise L.ProgenError(f'generate: position_bias of prompt {i} must have shape [T, {V}] with 1 <= T <= {n}, '
+                                    f'got {rows.shape}')
+            if np.isnan(rows).any() or (rows == np.inf).any():
+                raise L.ProgenError(f'generate: position_bias of prompt {i} must not contain NaN or +inf (in float32)')
+        if f is not None:
+            if not isinstance(f, dict):
+                raise L.ProgenError(f'generate: fixed of prompt {i} must be a dict {{offset: residue}} or None')
+            ids = {}
+            for k, res in f.items():
+                if isinstance(k, (bool, np.bool_)) or not isinstance(k, (int, np.integer)) or not 1 <= int(k) <= reach:
+                    raise L.ProgenError(f'generate: fixed offset {k!r} of prompt {i} must be an integer in [1, {reach}] '
+                                        f'(1-based, reachable before max_length {max_length})')
+                if isinstance(res, str) and len(res) == 1:
+                    c = encode_tokens(res)[0]
+                elif isinstance(res, (int, np.integer)) and not isinstance(res, (bool, np.bool_)):
+                    c = int(res)
+                else:
+                    raise L.ProgenError(f'generate: fixed residue at offset {k} of prompt {i} must be one character or an id')
+                if not 1 <= c < V:
+                    raise L.ProgenError(f'generate: fixed residue {res!r} at offset {k} of prompt {i} is outside the '
+                                        f'vocabulary (ids in [1, {V}))')
+                ids[int(k)] = c
+            if ids:
+                last = max(ids)
+                fx = np.zeros((last, V), np.float32)
+                fx[:, 0] = -np.inf                       # no EOS before the last fixed residue
+                for k, c in ids.items():
+                    fx[k - 1] = -np.inf
+                    fx[k - 1, c] = 0.0
+                if rows is None:
+                    rows = fx
+                else:
+                    L_ = max(len(rows), last)
+                    t = np.zeros((L_, V), np.float32)
+                    t[:len(rows)] = rows
+                    t[:last] += fx
+                    rows = t
+        if rows is None:
+            continue
+        for j in range(min(len(rows), reach)):
+            ok = np.isfinite(lb + rows[j])
+            if j < min_new_tokens:
+                ok[0] = False
+            if not ok.any():
+                raise L.ProgenError(f'generate: prompt {i} has no id left to draw at generated offset {j + 1} (the logit '
+                                    f'bias, position bias, fixed residues and min_new_tokens together ban every id)')
+        key = (rows.shape, rows.tobytes())
+        if key not in index:
+            index[key] = len(tables)
+            tables.append(rows)
+        prompt_table[i] = index[key]
+    return tables, prompt_table
+
+
+def launch_tables(tables, row_table, rows):
+    """position_bias of one decoder launch over `rows` (row indices), for BatchDecoder.generate / generate_queue: the
+    distinct tables its rows use, stacked and zero-padded to the longest (a zero row changes no logit), and each launch
+    row's index into them.  None when no row has a table."""
+    t = np.asarray(row_table, np.int64)[np.asarray(rows, np.int64)]
+    used = np.unique(t[t >= 0])
+    if used.size == 0:
+        return None
+    Lb = max(len(tables[u]) for u in used)
+    stack = np.zeros((len(used), Lb, tables[used[0]].shape[1]), np.float32)
+    for i, u in enumerate(used):
+        stack[i, :len(tables[u])] = tables[u]
+    return stack, np.where(t >= 0, np.searchsorted(used, t), -1).astype(np.int32)
 
 
 class ProGen:
@@ -230,7 +365,7 @@ class ProGen:
 
     def generate(self, params, prompts, *, num_samples=1, temperature=1.0, top_k=None, top_p=None, max_length=None, seed=0,
                  batch_size=64, logit_bias=None, min_new_tokens=0, repetition_penalty=1.0, repetition_window=0,
-                 prefill='decode'):
+                 prefill='decode', position_bias=None, fixed=None):
         """Sample sequences with the standard sampler of the persistent decode kernel (temperature, top-k with ties kept,
         nucleus top-p, in-kernel Philox Gumbel noise; csrc/decode_persist.cu), stopping each sequence at its EOS.
         Unlike the reference sampler (utils.sample, sample.py), a prompt is laid out as training data is: BOS (0), the
@@ -257,8 +392,21 @@ class ProGen:
             [1, V) must stay allowed (EOS, id 0, may be banned);
           min_new_tokens (integer in [0, max_length - 2]): the first min_new_tokens generated tokens of a row are never
             EOS.  A row whose prompt leaves fewer positions before max_length simply runs to max_length unfinished.
+          position_bias (after logit_bias, before the min_new_tokens EOS ban): None, a float array [T, V] (1 <= T <=
+            seq_len) for every prompt, or a list with one array or None per prompt.  Row j is added to the logits of
+            generated token j + 1, whatever the prompt's length; -inf bans an id at that offset; offsets past T are
+            unconstrained.
+          fixed: None, a dict {k: residue} for every prompt, or a list with one dict or None per prompt: generated token k
+            (1-based, at position start + k - 1) is `residue`, one character encoded like training text or an id in
+            [1, V).  It becomes position-bias rows (`position_tables`): 0 at the id and -inf elsewhere at offset k, and
+            -inf on EOS at every earlier offset, so no row ends before its last fixed residue; added to the prompt's
+            position_bias.  Offsets a prompt cannot reach before max_length, residues outside the vocabulary, and any
+            reachable offset left with no candidate (say a fixed residue banned by logit_bias) raise ProgenError naming
+            the prompt and the offset; an offset that allows only EOS ends the row there.
         Only the ids whose adjusted logit is not -inf can be drawn.  token_logp and log_likelihood do not see the
-        constraints: they stay the unfiltered model's at temperature 1, comparable with `score`.
+        constraints: they stay the unfiltered model's at temperature 1, comparable with `score`.  With position tables a
+        row's bits depend only on (seed, row), its prompt, its table and the launch class, not on the other rows' tables
+        or on how the rows are split into launches (QUEUE_TABLE_BYTES bounds the tables of one launch).
 
         prefill: how the positions before the first draw (BOS and the prompt but its last id) reach the decoder's caches.
           'decode' (default): the decode kernel consumes them one position at a time, as it does generated positions.
@@ -338,8 +486,11 @@ class ProGen:
             if a.size + 1 >= max_length:
                 raise L.ProgenError(f'generate: a prompt of {a.size} ids leaves nothing to generate before max_length {max_length}')
             ids.append(a)
+        tables, prompt_table = position_tables([1 + len(a) for a in ids], V, n, max_length, position_bias, fixed,
+                                               logit_bias, min_new_tokens)
         N = len(ids) * num_samples
         rows = [ids[r // num_samples] for r in range(N)]
+        row_table = prompt_table[np.arange(N) // num_samples]
         dec = self._generate_decoder(params, min(batch_size, N))
         if prefill == 'forward':
             self._ensure_loaded(params)
@@ -353,17 +504,20 @@ class ProGen:
             out['start'][r] = res['start'][:len(r)]
             out['end'][r] = res['end'][:len(r)]
 
-        queue = plan_queue(N, batch_size) if prefill == 'decode' else None
+        table_bytes = max((t.nbytes for t in tables), default=0)
+        queue = plan_queue(N, batch_size, row_table, table_bytes) if prefill == 'decode' else None
         if queue is not None:
             # a slot whose row has ended takes the next row of the queue: no launch waits for its longest row
             slots, chunks = queue
             for sids in chunks:
-                store(sids, dec.generate_queue([rows[r] for r in sids], slots=slots, sample_ids=sids, **kw))
+                store(sids, dec.generate_queue([rows[r] for r in sids], slots=slots, sample_ids=sids,
+                                               position_bias=launch_tables(tables, row_table, sids), **kw))
         else:
             for sids, real in plan_launches([len(a) for a in rows], batch_size, by_length=prefill == 'forward'):
                 chunk = [rows[r] for r in sids]
                 P = dec.prefill(self.engine, chunk) if prefill == 'forward' else 0
-                store(sids[:real], dec.generate(chunk, sample_ids=sids, prefilled=P, **kw))
+                store(sids[:real], dec.generate(chunk, sample_ids=sids, prefilled=P,
+                                                position_bias=launch_tables(tables, row_table, sids), **kw))
         end = out.pop('end')
         out['finished'] = end < max_length
         out['length'] = np.where(out['finished'], end + 1, max_length) - out['start']

@@ -1,6 +1,6 @@
 """Cost of the standard sampler (sampler 1), of its constraints, and gain of the EOS early exit, at the config-5 model.
 
-    python scripts/generate_bench.py [--rounds 3] [--samples 256]
+    python scripts/generate_bench.py [--rounds 3] [--samples 256] [--skip_end_to_end]
 
 Model: d512 L12 n1024 w256 h8 (10 GLU + 2 gMLP layers), seeded parameters (ProGen.init(1234), as bench.py --config cfg5),
 bf16 weights in the persistent decode kernel; prompt '[Tax=Mammalia] #'.
@@ -13,7 +13,9 @@ bf16 weights in the persistent decode kernel; prompt '[Tax=Mammalia] #'.
     repetition_penalty 1.2 over a 16-position window, against `std_full`, sampler 1 without them.  Both run with EOS
     unreachable (the `no_eos` head bias below), so both consume every position: a position's cost grows with its index
     (the gMLP layers' causal history sum), and the alphabet makes EOS so likely that a constrained launch would
-    otherwise stop after about a tenth of the positions of a plain one.
+    otherwise stop after about a tenth of the positions of a plain one.  `pos` is sampler 1 with a full-length position
+    table (`position_bias`, one [seq_len, V] table for every row): a random finite profile over the 20 amino acids
+    (every other id but EOS at -inf) with a fixed residue (a one-hot row) every 50 positions, against `std_full` too.
   end_to_end: wall clock of ProGen.generate(num_samples=`samples`, batch_size=64, T 1, top_p 0.95) including the host
     copies, for three parameter sets: as initialised (`model`), the head bias of token 0 raised so that EOS has probability
     about 1 % right after the prompt (`eos_1pct`), and EOS made unreachable by a -inf head bias (`no_eos`: every sequence
@@ -55,10 +57,25 @@ def with_eos_bias(params, delta):
     return out
 
 
+def position_table(n, V, seed=7):
+    """[1, n, V]: a random finite profile over the 20 amino acids at every generated offset, EOS left at 0, and every
+    50th offset a fixed residue (0 at one amino acid, -inf everywhere else)"""
+    rng = np.random.default_rng(seed)
+    aa = np.array(encode_tokens('ACDEFGHIKLMNPQRSTVWY'), np.int64)
+    t = np.full((n, V), -np.inf, np.float32)
+    t[:, 0] = 0.0
+    t[:, aa] = rng.normal(0.0, 1.0, (n, len(aa))).astype(np.float32)
+    for j in range(49, n, 50):
+        t[j] = -np.inf
+        t[j, rng.choice(aa)] = 0.0
+    return t[None]
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--rounds', type=int, default=3)
     ap.add_argument('--samples', type=int, default=256)
+    ap.add_argument('--skip_end_to_end', action='store_true', help='per-position launches only')
     args = ap.parse_args()
     n = KW['seq_len']
     params = ProGen(**KW).init(1234)
@@ -90,18 +107,21 @@ def main():
         torch.cuda.synchronize()
         return time.perf_counter() - t0, int(r['length'].sum()), int(r['finished'].sum())
 
-    per_pos = {f'{s}_B{B}': [] for B in decs for s in ('quirk', 'std', 'std_full', 'con')}
+    table = position_table(n, KW['num_tokens'])
+    per_pos = {f'{s}_B{B}': [] for B in decs for s in ('quirk', 'std', 'std_full', 'con', 'pos')}
     ends = {k: [] for k in psets}
     for rnd in range(args.rounds + 1):                          # round 0: warm-up
         for B in decs:
             q, s = quirk(B, 100 + rnd), std(B, 100 + rnd)
             f, c = std(B, 100 + rnd, full), std(B, 100 + rnd, full, **CONSTRAINED)
+            pt = std(B, 100 + rnd, full, position_bias=(table, np.zeros(B, np.int64)))
             if rnd:
                 per_pos[f'quirk_B{B}'].append(q)
                 per_pos[f'std_B{B}'].append(s)
                 per_pos[f'std_full_B{B}'].append(f)
                 per_pos[f'con_B{B}'].append(c)
-        for name in psets:
+                per_pos[f'pos_B{B}'].append(pt)
+        for name in ([] if args.skip_end_to_end else psets):
             r = e2e(name, rnd)
             if rnd:
                 ends[name].append(r)
@@ -110,14 +130,19 @@ def main():
                              for B in decs}
     res['con_over_std'] = {f'B{B}': statistics.median(per_pos[f'con_B{B}']) / statistics.median(per_pos[f'std_full_B{B}'])
                            for B in decs}
+    res['pos_over_std'] = {f'B{B}': statistics.median(per_pos[f'pos_B{B}']) / statistics.median(per_pos[f'std_full_B{B}'])
+                           for B in decs}
     e = {}
     for name, v in ends.items():
+        if not v:
+            continue
         secs = statistics.median([x[0] for x in v])
         tok = v[0][1]
         e[name] = dict(s=secs, s_all=[x[0] for x in v], seqs_per_s=args.samples / secs, generated_tokens=tok,
                        generated_tokens_per_s=tok / secs, finished=v[0][2])
     res['end_to_end'] = e
-    res['early_exit_speedup_eos_1pct'] = e['no_eos']['s'] / e['eos_1pct']['s']
+    if e:
+        res['early_exit_speedup_eos_1pct'] = e['no_eos']['s'] / e['eos_1pct']['s']
     print(json.dumps(dict(metric='generation: sampler-1 and constraint cost per position and EOS early exit, config-5 model (bf16 weights)',
                           samples=args.samples, rounds=args.rounds, eos_bias_delta=delta, **res,
                           gpu=gpu_info(torch.cuda.current_device()))))
