@@ -6,8 +6,9 @@ and sequence.  Every position of a launch runs inside ONE persistent kernel (`pr
 csrc/decode_persist.cu): the token loop, the sampler and the position counter stay on the device, and the loop never
 synchronises with the host.  `BatchDecoder.sample` keeps the reference's quirks: top-k keeps k-1 logits and zeroes the
 rest (Q6), `add_bos` adds the first sampled id to the last prime token (Q5), everything after the second pad is
-cleared (Q7).  `BatchDecoder.generate` / `generate_queue` run the standard sampler."""
+cleared (Q7).  `BatchDecoder.generate` / `generate_queue` run the standard sampler with the settings of a `Sampling`."""
 import ctypes as C
+from dataclasses import dataclass
 
 import numpy as np
 import torch
@@ -16,6 +17,84 @@ from . import lib as L
 from .engine import P, layer_kinds
 
 _P, _I = C.c_void_p, C.c_int32
+
+
+def integer(v, what, lo, hi):
+    """v as an int; ProgenError unless it is an integer (not a bool) in [lo, hi]"""
+    if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, np.integer)) or not lo <= int(v) <= hi:
+        raise L.ProgenError(f'generate: {what} must be an integer in [{lo}, {hi}], got {v!r}')
+    return int(v)
+
+
+def prompt_ids(prompts, V, max_length):
+    """each prompt as an int64 array; ProgenError unless it is 1-D, of integer ids in [1, V), and leaves a position to
+    draw before max_length"""
+    out = []
+    for p in prompts:
+        a = np.asarray(p)
+        if a.ndim != 1 or (a.size and not np.issubdtype(a.dtype, np.integer)):
+            raise L.ProgenError('generate: a prompt must be a string or a 1-D integer array')
+        a = a.astype(np.int64)
+        if a.size and (a.min() < 1 or a.max() >= V):
+            raise L.ProgenError(f'generate: prompt ids must lie in [1, {V}) (0 is BOS / EOS)')
+        if a.size + 1 >= max_length:
+            raise L.ProgenError(f'generate: a prompt of {a.size} ids leaves nothing to generate before max_length {max_length}')
+        out.append(a)
+    return out
+
+
+@dataclass(frozen=True, eq=False)
+class Sampling:
+    """The settings of the standard sampler (sampler 1 of csrc/decode_persist.cu) for one generate call, checked by
+    `Sampling.check`; `ProGen.generate` documents each of them"""
+    temperature: float
+    top_k: int | None
+    top_p: float | None
+    seed: int
+    logit_bias: np.ndarray | None                    # [V] float32
+    min_new_tokens: int
+    repetition_penalty: float
+    repetition_window: int
+
+    @classmethod
+    def check(cls, V, n, min_new_max, keep_an_id, *, temperature=1.0, top_k=None, top_p=None, seed=0, logit_bias=None,
+              min_new_tokens=0, repetition_penalty=1.0, repetition_window=0):
+        """The settings for a model of V ids and seq_len n, or ProgenError before any device work.  The two rules the
+        callers set: min_new_tokens lies in [0, min_new_max], and with keep_an_id logit_bias must leave some id of
+        [1, V) allowed.  `ProGen.generate` passes max_length - 2 and True; `BatchDecoder` passes n and False, the
+        kernel's own limits (min_new_tokens = n bans EOS for the whole row)."""
+        seed = integer(seed, 'seed', 0, (1 << 64) - 1)
+        top_k = None if top_k is None else integer(top_k, 'top_k', 1, V)
+        try:
+            temperature = float(temperature)
+            top_p = None if top_p is None else float(top_p)
+        except (TypeError, ValueError):
+            raise L.ProgenError('generate: temperature and top_p must be numbers') from None
+        if not (np.isfinite(temperature) and temperature >= 0.0):
+            raise L.ProgenError(f'generate: temperature must be finite and >= 0, got {temperature}')
+        if top_p is not None and not 0.0 < top_p <= 1.0:
+            raise L.ProgenError(f'generate: top_p must lie in (0, 1], got {top_p}')
+        min_new_tokens = integer(min_new_tokens, 'min_new_tokens', 0, min_new_max)
+        repetition_window = integer(repetition_window, 'repetition_window', 0, n)
+        try:
+            repetition_penalty = float(repetition_penalty)
+        except (TypeError, ValueError):
+            raise L.ProgenError('generate: repetition_penalty must be a number') from None
+        if not (np.isfinite(repetition_penalty) and repetition_penalty > 0.0):
+            raise L.ProgenError(f'generate: repetition_penalty must be finite and > 0, got {repetition_penalty}')
+        if logit_bias is not None:
+            try:
+                with np.errstate(over='ignore'):
+                    logit_bias = np.asarray(logit_bias, np.float64).astype(np.float32)   # the kernel adds fp32
+            except (TypeError, ValueError):
+                raise L.ProgenError('generate: logit_bias must be an array of floats') from None
+            if logit_bias.shape != (V,):
+                raise L.ProgenError(f'generate: logit_bias must have shape ({V},), got {logit_bias.shape}')
+            if np.isnan(logit_bias).any() or (logit_bias == np.inf).any():
+                raise L.ProgenError('generate: logit_bias must not contain NaN or +inf (in float32)')
+            if keep_an_id and not np.isfinite(logit_bias[1:]).any():
+                raise L.ProgenError('generate: logit_bias bans every id in [1, V)')
+        return cls(temperature, top_k, top_p, seed, logit_bias, min_new_tokens, repetition_penalty, repetition_window)
 
 
 class DecodeLayer(C.Structure):
@@ -132,9 +211,6 @@ class BatchDecoder:
         self.grid_bar = torch.zeros(1, device=self.dev, dtype=torch.int32)
         m.grid_bar = self.grid_bar.data_ptr()
         m.repetition_penalty = 1.0                        # constraints off
-        self._gen = None                                  # sampler-1 buffers, allocated by the first generate()
-        self._bias = None                                 # [V] logit bias of generate(), allocated on first use
-        self._pos = None                                  # position tables and row map of the running launch
 
     def _hold(self, t):
         self.keep.append(t)
@@ -217,10 +293,12 @@ class BatchDecoder:
         self.last_marks = raw[640:].reshape(160, 8)[:ev]      # clock64 inside CTA 0's phases (0 = not recorded)
         return p[:, :ev]
 
-    def run(self, pos0, nsteps):
+    def run(self, pos0, nsteps, m=None):
+        """launch the struct m (default self.m, the reference sampler's) for positions pos0 .. pos0 + nsteps - 1"""
+        m = self.m if m is None else m
         self.grid_bar.zero_()
-        self.m.pos0, self.m.nsteps = int(pos0), int(nsteps)
-        L.check(self.lib.progen_decode_run(C.byref(self.m), L.stream()), 'decode_run')
+        m.pos0, m.nsteps = int(pos0), int(nsteps)
+        L.check(self.lib.progen_decode_run(C.byref(m), L.stream()), 'decode_run')
 
     def sample(self, primes, length=None, top_k=None, add_bos=False, greedy=True, seed=0):
         """utils.py:106-135 for every prime of `primes` (a list of integer arrays, or one array for B = 1).
@@ -268,18 +346,13 @@ class BatchDecoder:
         return (out[0] if single else out), generated, e0.elapsed_time(e1) / 1e3
 
     def _rows(self, prompts, max_length):
-        """-> (seq0 [R, n] int32: [0 (BOS), prompt, 0...] per prompt, starts [R] int32: 1 + prompt length)"""
-        seq0 = np.zeros((len(prompts), self.n), np.int32)
-        starts = np.zeros(len(prompts), np.int32)
-        for b, pr in enumerate(prompts):
-            pr = np.asarray(pr, np.int64).reshape(-1)
-            if len(pr) + 1 >= max_length:
-                raise L.ProgenError(f'generate: a prompt of {len(pr)} ids leaves no position before max_length {max_length}')
-            if len(pr) and (pr.min() < 1 or pr.max() >= self.V):
-                raise L.ProgenError(f'generate: prompt ids must lie in [1, {self.V})')
-            seq0[b, 1:1 + len(pr)] = pr
-            starts[b] = 1 + len(pr)
-        return seq0, starts
+        """-> (seq0 [R, n] int32: [0 (BOS), prompt, 0...] per prompt, starts [R] int32: 1 + prompt length), checked by
+        `prompt_ids`"""
+        ids = prompt_ids(prompts, self.V, max_length)
+        seq0 = np.zeros((len(ids), self.n), np.int32)
+        for b, a in enumerate(ids):
+            seq0[b, 1:1 + len(a)] = a
+        return seq0, np.array([1 + len(a) for a in ids], np.int32)
 
     def generate(self, prompts, *, temperature=1.0, top_k=None, top_p=None, seed=0, sample_ids=None, max_length=None,
                  logit_bias=None, min_new_tokens=0, repetition_penalty=1.0, repetition_window=0, position_bias=None,
@@ -293,6 +366,8 @@ class BatchDecoder:
         in the last `repetition_window` positions (0: all since BOS) have positive logits divided and negative ones
         multiplied by `repetition_penalty`; `logit_bias` ([V] floats, -inf bans an id) is added; EOS is banned for the
         first `min_new_tokens` draws of a row.  They do not change token_logp, the unfiltered model's log-probability.
+        The settings are checked as `ProGen.generate` checks them (`Sampling.check`), except that min_new_tokens may be
+        up to n and logit_bias may ban every id of [1, V).
         position_bias = (tables [Tb, Lb, V] float32, table_of_row [R] ints in [-1, Tb)): the draw of a row's generated
         offset j (0 = its first generated token) adds tables[table_of_row[r], j] to the logits after logit_bias and
         before the EOS ban, for j < Lb (-1: no table; -inf bans an id at that offset).
@@ -302,51 +377,12 @@ class BatchDecoder:
         else 0), end [R] int32 (position of the EOS, n if none), start [R] int32; and steps_run (positions the last
         launch consumed before every row had ended, or its full length), device_s (that launch's device time) and
         prefill_s (device time of the launch that consumed the prompt positions before it, 0 when there was none)."""
-        n = self.n
-        R = len(prompts)
-        if not 1 <= R <= self.B:
+        if not 1 <= len(prompts) <= self.B:
             raise L.ProgenError(f'generate: 1 <= prompts <= {self.B}')
-        max_length, seq0, starts, sids = self._sampler_rows(prompts, sample_ids, max_length)
-        first = int(starts.min()) - 1                     # the first drawn position is start; it reads the logits of start - 1
-        if not 0 <= int(prefilled) <= first:
-            raise L.ProgenError(f'generate: prefilled must lie in [0, {first}] (the shortest prompt length)')
-        prefilled = int(prefilled)
-        logit_bias, position_bias = self._check_sampler(temperature, top_k, top_p, logit_bias, min_new_tokens,
-                                                        repetition_penalty, repetition_window, position_bias, R)
-        if self._gen is None:
-            z = lambda *s, dtype: torch.zeros(*s, device=self.dev, dtype=dtype)
-            self._gen = dict(sample_id=z(self.B, dtype=torch.int64), token_logp=z(self.B, n, dtype=torch.float32),
-                             end=z(self.B, dtype=torch.int32), counters=z(2, dtype=torch.int32))
-        gb = self._gen
-        if not prefilled:
-            self.reset()
-        self.seq[:R].copy_(torch.as_tensor(seq0))
-        self.start[:R].copy_(torch.as_tensor(starts))
-        gb['sample_id'][:R].copy_(torch.as_tensor(sids))
-        gb['token_logp'].zero_()
-        gb['end'].fill_(n)
-        gb['counters'].zero_()                            # [n_ended, steps_run]
-        m = self.m
-        m.B = R
-        m.sample_id, m.token_logp, m.end = gb['sample_id'].data_ptr(), gb['token_logp'].data_ptr(), gb['end'].data_ptr()
-        m.n_ended, m.steps_run = gb['counters'].data_ptr(), gb['counters'].data_ptr() + 4
-        self._set_sampler(temperature, top_k, top_p, seed, logit_bias, min_new_tokens, repetition_penalty, repetition_window,
-                          position_bias)
-        try:
-            ev = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
-            e0, e1 = ev[1], ev[2]
-            ev[0].record()
-            if first > prefilled:
-                self.run(prefilled, first - prefilled)    # prefill: only advances the caches
-            e0.record()
-            self.run(first, max_length - 1 - first)       # positions first .. max_length - 2 (the last writes max_length - 1)
-            e1.record()
-            torch.cuda.synchronize()
-        finally:
-            self._clear_sampler()
-        return dict(ids=self.seq[:R].cpu().numpy().astype(np.int64), token_logp=gb['token_logp'][:R].cpu().numpy(),
-                    end=gb['end'][:R].cpu().numpy(), start=starts, steps_run=int(gb['counters'][1].item()),
-                    device_s=e0.elapsed_time(e1) / 1e3, prefill_s=ev[0].elapsed_time(e0) / 1e3)
+        s = Sampling.check(self.V, self.n, self.n, False, temperature=temperature, top_k=top_k, top_p=top_p, seed=seed,
+                           logit_bias=logit_bias, min_new_tokens=min_new_tokens, repetition_penalty=repetition_penalty,
+                           repetition_window=repetition_window)
+        return self._generate(prompts, s, sample_ids, max_length, position_bias, prefilled=prefilled)
 
     def generate_queue(self, prompts, *, slots=None, temperature=1.0, top_k=None, top_p=None, seed=0, sample_ids=None,
                        max_length=None, logit_bias=None, min_new_tokens=0, repetition_penalty=1.0, repetition_window=0,
@@ -357,132 +393,97 @@ class BatchDecoder:
         progen_b200.h).  A row's bits depend on its seed, sample id, prompt, the class of `slots` (2-8 or 9-64) and
         the GPU's SM count, not on its slot or the other rows, so each row equals what `generate` gives it in a launch of
         that class; the launch merely has no slot waiting for its longest row.  position_bias's table_of_row is indexed
-        by queue row ([Q]).  Returns the arrays of `generate` over the Q rows, steps_run (positions the launch ran) and
-        device_s (its device time)."""
-        n = self.n
+        by queue row ([Q]).  Returns the dict of `generate` over the Q rows; steps_run is the positions the launch ran
+        and prefill_s is 0."""
         Q = len(prompts)
         slots = min(self.B, Q) if slots is None else int(slots)
         if not 2 <= slots <= min(self.B, Q):
             raise L.ProgenError(f'generate_queue: 2 <= slots <= min(batch {self.B}, rows {Q})')
-        max_length, seq0, starts, sids = self._sampler_rows(prompts, sample_ids, max_length)
-        logit_bias, position_bias = self._check_sampler(temperature, top_k, top_p, logit_bias, min_new_tokens,
-                                                        repetition_penalty, repetition_window, position_bias, Q)
-        dev = self.dev
-        seq = torch.as_tensor(seq0).to(dev)
-        start = torch.as_tensor(starts).to(dev)
-        sample_id = torch.as_tensor(sids).to(dev)
-        token_logp = torch.zeros(Q, n, device=dev, dtype=torch.float32)
-        end = torch.full((Q,), n, device=dev, dtype=torch.int32)
-        slot_row = torch.arange(slots, device=dev, dtype=torch.int32)
-        slot_pos = torch.zeros(slots, device=dev, dtype=torch.int32)
-        counters = torch.tensor([0, 0, slots, 0], device=dev, dtype=torch.int32)   # [n_ended, steps_run, next_row, done]
-        self.reset()                                      # (token-shift slot 0 must be zero at position 0)
-        m = self.m
-        m.B, m.seq, m.start = slots, seq.data_ptr(), start.data_ptr()
-        m.sample_id, m.token_logp, m.end = sample_id.data_ptr(), token_logp.data_ptr(), end.data_ptr()
-        c = counters.data_ptr()
-        m.n_ended, m.steps_run, m.next_row, m.done = c, c + 4, c + 8, c + 12
-        m.slot_row, m.slot_pos, m.num_rows, m.max_length = slot_row.data_ptr(), slot_pos.data_ptr(), Q, max_length
-        self._set_sampler(temperature, top_k, top_p, seed, logit_bias, min_new_tokens, repetition_penalty, repetition_window,
-                          position_bias)
-        # while rows wait in the queue every slot is busy, and a row consumes at most max_length - 1 positions
-        nsteps = -(-Q * (max_length - 1) // slots) + max_length - 1
-        try:
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            self.run(0, nsteps)
-            e1.record()
-            torch.cuda.synchronize()
-        finally:
-            self._clear_sampler()
-            m.seq, m.start = self.seq.data_ptr(), self.start.data_ptr()
-            m.slot_row = m.slot_pos = m.next_row = m.done = 0
-            m.num_rows = m.max_length = 0
-        cnt = counters.cpu().numpy()
-        if cnt[3] != Q:
-            raise L.ProgenError(f'generate_queue: {cnt[3]} of {Q} rows retired in {cnt[1]} steps')
-        return dict(ids=seq.cpu().numpy().astype(np.int64), token_logp=token_logp.cpu().numpy(), end=end.cpu().numpy(),
-                    start=starts, steps_run=int(cnt[1]), device_s=e0.elapsed_time(e1) / 1e3)
+        s = Sampling.check(self.V, self.n, self.n, False, temperature=temperature, top_k=top_k, top_p=top_p, seed=seed,
+                           logit_bias=logit_bias, min_new_tokens=min_new_tokens, repetition_penalty=repetition_penalty,
+                           repetition_window=repetition_window)
+        return self._generate(prompts, s, sample_ids, max_length, position_bias, slots=slots)
 
-    def _sampler_rows(self, prompts, sample_ids, max_length):
-        """-> (max_length, seq0, starts, sample ids) of generate / generate_queue, checked"""
-        n = self.n
-        max_length = n if max_length is None else int(max_length)
-        if not 2 <= max_length <= n:
-            raise L.ProgenError(f'generate: 2 <= max_length <= {n}')
+    def _generate(self, prompts, s, sample_ids, max_length, position_bias, prefilled=0, slots=None):
+        """One sampler-1 launch with the checked settings s (a Sampling).  slots None: row b runs on sequence b, after a
+        launch that consumes the prompt positions from `prefilled` on; else the rows form the queue of `slots` sequences.
+        It launches a copy of self.m with this call's buffers and sampler fields, so self.m keeps what `sample` runs."""
+        n, dev, R = self.n, self.dev, len(prompts)
+        max_length = n if max_length is None else integer(max_length, 'max_length', 2, n)
         seq0, starts = self._rows(prompts, max_length)
-        R = len(prompts)
         sids = np.arange(R, dtype=np.int64) if sample_ids is None else np.asarray(sample_ids, np.int64).reshape(-1)
         if sids.shape != (R,):
             raise L.ProgenError('generate: one sample id per prompt')
-        return max_length, seq0, starts, sids
-
-    def _check_sampler(self, temperature, top_k, top_p, logit_bias, min_new_tokens, repetition_penalty, repetition_window,
-                       position_bias=None, rows=0):
-        """checks the sampler arguments of generate / generate_queue (`rows` rows); -> (logit_bias as float32 or None,
-        position_bias as (float32 tables, int32 map) or None)"""
-        n = self.n
-        if top_k is not None and not 1 <= int(top_k) <= self.V:
-            raise L.ProgenError(f'generate: 1 <= top_k <= {self.V}')
-        if top_p is not None and not 0.0 < float(top_p) <= 1.0:
-            raise L.ProgenError('generate: 0 < top_p <= 1')
-        if not (np.isfinite(temperature) and temperature >= 0):
-            raise L.ProgenError('generate: temperature must be finite and >= 0')
-        if logit_bias is not None:
-            logit_bias = np.asarray(logit_bias, np.float32)
-            if logit_bias.shape != (self.V,) or np.isnan(logit_bias).any() or (logit_bias == np.inf).any():
-                raise L.ProgenError(f'generate: logit_bias must be {self.V} floats without NaN or +inf')
-        if not 0 <= int(min_new_tokens) <= n or not 0 <= int(repetition_window) <= n:
-            raise L.ProgenError(f'generate: min_new_tokens and repetition_window must lie in [0, {n}]')
-        if not (np.isfinite(repetition_penalty) and repetition_penalty > 0):
-            raise L.ProgenError('generate: repetition_penalty must be finite and > 0')
+        first = int(starts.min()) - 1                     # the first drawn position is start; it reads the logits of start - 1
+        if not 0 <= int(prefilled) <= first:
+            raise L.ProgenError(f'generate: prefilled must lie in [0, {first}] (the shortest prompt length)')
+        prefilled = int(prefilled)
+        position_bias = self._position_bias(position_bias, R)
+        to_dev = lambda a: torch.as_tensor(a).to(dev)
+        seq, start, sample_id = to_dev(seq0), to_dev(starts), to_dev(sids)
+        token_logp = torch.zeros(R, n, device=dev, dtype=torch.float32)
+        end = torch.full((R,), n, device=dev, dtype=torch.int32)
+        counters = torch.tensor([0, 0, slots or 0, 0], device=dev, dtype=torch.int32)   # [n_ended, steps_run, next_row, done]
+        m = DecodeRun.from_buffer_copy(self.m)
+        m.B = R if slots is None else slots
+        m.seq, m.start, m.sample_id, m.token_logp, m.end = (t.data_ptr() for t in (seq, start, sample_id, token_logp, end))
+        c = counters.data_ptr()
+        m.n_ended, m.steps_run = c, c + 4
+        m.sampler, m.temperature, m.seed = 1, s.temperature, s.seed
+        m.top_k, m.top_p = s.top_k or 0, 1.0 if s.top_p is None else s.top_p
+        m.repetition_penalty, m.repetition_window, m.min_new_tokens = s.repetition_penalty, s.repetition_window, s.min_new_tokens
+        if s.logit_bias is not None:                      # the device copies below live until the launch has synchronised
+            bias = to_dev(s.logit_bias)
+            m.logit_bias = bias.data_ptr()
         if position_bias is not None:
-            try:
-                tables, table_of_row = position_bias
-                tables = np.ascontiguousarray(np.asarray(tables, np.float32))
-                table_of_row = np.asarray(table_of_row)
-            except (TypeError, ValueError):
-                raise L.ProgenError('generate: position_bias must be a pair (tables [Tb, Lb, V], table_of_row [rows])') from None
-            if tables.ndim != 3 or tables.shape[0] < 1 or not 1 <= tables.shape[1] <= n or tables.shape[2] != self.V:
-                raise L.ProgenError(f'generate: position_bias tables must have shape [Tb >= 1, 1..{n}, {self.V}], '
-                                    f'got {tables.shape}')
-            if np.isnan(tables).any() or (tables == np.inf).any():
-                raise L.ProgenError('generate: position_bias tables must not contain NaN or +inf')
-            if table_of_row.shape != (rows,) or (rows and not np.issubdtype(table_of_row.dtype, np.integer)):
-                raise L.ProgenError(f'generate: position_bias needs one integer table index per row ({rows})')
-            if rows and (table_of_row.min() < -1 or table_of_row.max() >= tables.shape[0]):
-                raise L.ProgenError(f'generate: position_bias table indices must lie in [-1, {tables.shape[0]})')
-            position_bias = tables, table_of_row.astype(np.int32)
-        return logit_bias, position_bias
-
-    def _set_sampler(self, temperature, top_k, top_p, seed, logit_bias, min_new_tokens, repetition_penalty, repetition_window,
-                     position_bias=None):
-        m = self.m
-        m.sampler = 1
-        m.temperature = float(temperature)
-        m.top_k = int(top_k) if top_k is not None else 0
-        m.top_p = float(top_p) if top_p is not None else 1.0
-        m.seed = int(seed) & 0xFFFFFFFFFFFFFFFF
-        if logit_bias is not None:
-            if self._bias is None:
-                self._bias = torch.zeros(self.V, device=self.dev, dtype=torch.float32)
-            self._bias.copy_(torch.from_numpy(logit_bias))
-            m.logit_bias = self._bias.data_ptr()
-        m.repetition_penalty = float(repetition_penalty)
-        m.repetition_window, m.min_new_tokens = int(repetition_window), int(min_new_tokens)
-        if position_bias is not None:                     # uploaded per launch, held until _clear_sampler
-            tables, table_of_row = position_bias
-            self._pos = (torch.from_numpy(tables).to(self.dev), torch.from_numpy(table_of_row).to(self.dev))
-            m.position_bias, m.position_bias_table = self._pos[0].data_ptr(), self._pos[1].data_ptr()
+            tables, table_of_row = map(to_dev, position_bias)
+            m.position_bias, m.position_bias_table = tables.data_ptr(), table_of_row.data_ptr()
             m.position_bias_len = tables.shape[1]
+        if slots is None:
+            pre = (prefilled, first - prefilled)          # prefill: only advances the caches
+            main = (first, max_length - 1 - first)        # positions first .. max_length - 2 (the last writes max_length - 1)
+        else:
+            slot_row = torch.arange(slots, device=dev, dtype=torch.int32)
+            slot_pos = torch.zeros(slots, device=dev, dtype=torch.int32)
+            m.next_row, m.done = c + 8, c + 12
+            m.slot_row, m.slot_pos, m.num_rows, m.max_length = slot_row.data_ptr(), slot_pos.data_ptr(), R, max_length
+            # while rows wait in the queue every slot is busy, and a row consumes at most max_length - 1 positions
+            pre, main = (0, 0), (0, -(-R * (max_length - 1) // slots) + max_length - 1)
+        if not prefilled:
+            self.reset()                                  # (a queue row needs token-shift slot 0 zero at position 0)
+        ev = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
+        ev[0].record()
+        if pre[1] > 0:
+            self.run(*pre, m)
+        ev[1].record()
+        self.run(*main, m)
+        ev[2].record()
+        torch.cuda.synchronize()
+        cnt = counters.cpu().numpy()
+        if slots is not None and cnt[3] != R:
+            raise L.ProgenError(f'generate_queue: {cnt[3]} of {R} rows retired in {cnt[1]} steps')
+        return dict(ids=seq.cpu().numpy().astype(np.int64), token_logp=token_logp.cpu().numpy(), end=end.cpu().numpy(),
+                    start=starts, steps_run=int(cnt[1]), device_s=ev[1].elapsed_time(ev[2]) / 1e3,
+                    prefill_s=ev[0].elapsed_time(ev[1]) / 1e3 if pre[1] > 0 else 0.0)
 
-    def _clear_sampler(self):
-        """back to the reference sampler's launch fields (sample() after generate() runs what it ran before)"""
-        m = self.m
-        m.B, m.sampler, m.top_k = self.B, 0, 0
-        m.temperature, m.top_p, m.seed = 0.0, 0.0, 0
-        m.sample_id = m.token_logp = m.end = m.n_ended = m.steps_run = m.logit_bias = 0
-        m.repetition_penalty, m.repetition_window, m.min_new_tokens = 1.0, 0, 0
-        m.position_bias = m.position_bias_table = 0
-        m.position_bias_len = 0
-        self._pos = None
+    def _position_bias(self, position_bias, rows):
+        """checks position_bias of generate / generate_queue (`rows` rows); -> (float32 tables, int32 map) or None"""
+        if position_bias is None:
+            return None
+        n = self.n
+        try:
+            tables, table_of_row = position_bias
+            tables = np.ascontiguousarray(np.asarray(tables, np.float32))
+            table_of_row = np.asarray(table_of_row)
+        except (TypeError, ValueError):
+            raise L.ProgenError('generate: position_bias must be a pair (tables [Tb, Lb, V], table_of_row [rows])') from None
+        if tables.ndim != 3 or tables.shape[0] < 1 or not 1 <= tables.shape[1] <= n or tables.shape[2] != self.V:
+            raise L.ProgenError(f'generate: position_bias tables must have shape [Tb >= 1, 1..{n}, {self.V}], '
+                                f'got {tables.shape}')
+        if np.isnan(tables).any() or (tables == np.inf).any():
+            raise L.ProgenError('generate: position_bias tables must not contain NaN or +inf')
+        if table_of_row.shape != (rows,) or (rows and not np.issubdtype(table_of_row.dtype, np.integer)):
+            raise L.ProgenError(f'generate: position_bias needs one integer table index per row ({rows})')
+        if rows and (table_of_row.min() < -1 or table_of_row.max() >= tables.shape[0]):
+            raise L.ProgenError(f'generate: position_bias table indices must lie in [-1, {tables.shape[0]})')
+        return tables, table_of_row.astype(np.int32)

@@ -95,6 +95,17 @@ def plan_queue(n_rows, batch_size, row_table=None, table_bytes=0):
     return slots, out
 
 
+def plan_generate(lengths, batch_size, prefill='decode', row_table=None, table_bytes=0):
+    """The decoder launches of `ProGen.generate` for N = len(lengths) rows: a list of (rows, real, slots).  With
+    prefill='decode' and at least two rows per launch each chunk of `plan_queue` is the queue of one launch on `slots`
+    sequences (real = len(rows)); otherwise the launches of `plan_launches` keep rows fixed to sequences (slots None)."""
+    queue = plan_queue(len(lengths), batch_size, row_table, table_bytes) if prefill == 'decode' else None
+    if queue is not None:
+        slots, chunks = queue
+        return [(c, len(c), slots) for c in chunks]
+    return [(rows, real, None) for rows, real in plan_launches(lengths, batch_size, by_length=prefill == 'forward')]
+
+
 def _per_prompt(arg, n_prompts, what, single):
     """`arg` for every prompt: one value (single(arg) true) for all, or a list with one entry (or None) per prompt"""
     if arg is None:
@@ -426,68 +437,26 @@ class ProGen:
           token_logp [N, seq_len] float32: log p(tokens[t] | tokens[:t]) under the unfiltered model (temperature 1) at
             generated t, 0 elsewhere — the quantity `score` reports;
           prompt_index [N] int64."""
+        from .data import encode_tokens
+        from .decode import Sampling, integer, prompt_ids
         cfg = self.config
         V, n = cfg['num_tokens'], cfg['seq_len']
-
-        def integer(v, what, lo, hi):
-            if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, np.integer)) or not lo <= int(v) <= hi:
-                raise L.ProgenError(f'generate: {what} must be an integer in [{lo}, {hi}], got {v!r}')
-            return int(v)
-
         if not isinstance(prefill, str) or prefill not in ('decode', 'forward'):
             raise L.ProgenError(f"generate: prefill must be 'decode' or 'forward', got {prefill!r}")
         max_length = n if max_length is None else integer(max_length, 'max_length', 2, n)
         num_samples = integer(num_samples, 'num_samples', 1, 1 << 40)
         batch_size = integer(batch_size, 'batch_size', 1, 64)
-        seed = integer(seed, 'seed', 0, (1 << 64) - 1)
-        top_k = None if top_k is None else integer(top_k, 'top_k', 1, V)
-        try:
-            temperature = float(temperature)
-            top_p = None if top_p is None else float(top_p)
-        except (TypeError, ValueError):
-            raise L.ProgenError('generate: temperature and top_p must be numbers') from None
-        if not (np.isfinite(temperature) and temperature >= 0.0):
-            raise L.ProgenError(f'generate: temperature must be finite and >= 0, got {temperature}')
-        if top_p is not None and not 0.0 < top_p <= 1.0:
-            raise L.ProgenError(f'generate: top_p must lie in (0, 1], got {top_p}')
-        min_new_tokens = integer(min_new_tokens, 'min_new_tokens', 0, max_length - 2)
-        repetition_window = integer(repetition_window, 'repetition_window', 0, n)
-        try:
-            repetition_penalty = float(repetition_penalty)
-        except (TypeError, ValueError):
-            raise L.ProgenError('generate: repetition_penalty must be a number') from None
-        if not (np.isfinite(repetition_penalty) and repetition_penalty > 0.0):
-            raise L.ProgenError(f'generate: repetition_penalty must be finite and > 0, got {repetition_penalty}')
-        if logit_bias is not None:
-            try:
-                with np.errstate(over='ignore'):
-                    logit_bias = np.asarray(logit_bias, np.float64).astype(np.float32)   # the kernel adds fp32
-            except (TypeError, ValueError):
-                raise L.ProgenError('generate: logit_bias must be an array of floats') from None
-            if logit_bias.shape != (V,):
-                raise L.ProgenError(f'generate: logit_bias must have shape ({V},), got {logit_bias.shape}')
-            if np.isnan(logit_bias).any() or (logit_bias == np.inf).any():
-                raise L.ProgenError('generate: logit_bias must not contain NaN or +inf (in float32)')
-            if not np.isfinite(logit_bias[1:]).any():
-                raise L.ProgenError('generate: logit_bias bans every id in [1, V)')
-        from .data import encode_tokens
+        sampling = Sampling.check(V, n, max_length - 2, True, temperature=temperature, top_k=top_k, top_p=top_p, seed=seed,
+                                  logit_bias=logit_bias, min_new_tokens=min_new_tokens,
+                                  repetition_penalty=repetition_penalty, repetition_window=repetition_window)
         if isinstance(prompts, (str, bytes)):
             prompts = [prompts]
         if not isinstance(prompts, (list, tuple)) or len(prompts) == 0:
             raise L.ProgenError('generate: prompts must be a string or a non-empty list of strings or id arrays')
-        ids = []
-        for p in prompts:
-            a = np.asarray(encode_tokens(p.decode() if isinstance(p, bytes) else p) if isinstance(p, (str, bytes)) else p)
-            if a.ndim != 1 or (a.size and not np.issubdtype(a.dtype, np.integer)):
-                raise L.ProgenError('generate: a prompt must be a string or a 1-D integer array')
-            a = a.astype(np.int64)
-            if a.size and (a.min() < 1 or a.max() >= V):
-                raise L.ProgenError(f'generate: prompt ids must lie in [1, {V}) (0 is BOS / EOS)')
-            if a.size + 1 >= max_length:
-                raise L.ProgenError(f'generate: a prompt of {a.size} ids leaves nothing to generate before max_length {max_length}')
-            ids.append(a)
+        ids = prompt_ids([encode_tokens(p.decode() if isinstance(p, bytes) else p) if isinstance(p, (str, bytes)) else p
+                          for p in prompts], V, max_length)
         tables, prompt_table = position_tables([1 + len(a) for a in ids], V, n, max_length, position_bias, fixed,
-                                               logit_bias, min_new_tokens)
+                                               sampling.logit_bias, sampling.min_new_tokens)
         N = len(ids) * num_samples
         rows = [ids[r // num_samples] for r in range(N)]
         row_table = prompt_table[np.arange(N) // num_samples]
@@ -496,28 +465,14 @@ class ProGen:
             self._ensure_loaded(params)
         out = dict(tokens=np.zeros((N, n), np.int64), start=np.zeros(N, np.int64), end=np.zeros(N, np.int64),
                    token_logp=np.zeros((N, n), np.float32))
-        kw = dict(temperature=temperature, top_k=top_k, top_p=top_p, seed=seed, max_length=max_length, logit_bias=logit_bias,
-                  min_new_tokens=min_new_tokens, repetition_penalty=repetition_penalty, repetition_window=repetition_window)
-        def store(r, res):
-            out['tokens'][r] = res['ids'][:len(r)]
-            out['token_logp'][r] = res['token_logp'][:len(r)]
-            out['start'][r] = res['start'][:len(r)]
-            out['end'][r] = res['end'][:len(r)]
-
         table_bytes = max((t.nbytes for t in tables), default=0)
-        queue = plan_queue(N, batch_size, row_table, table_bytes) if prefill == 'decode' else None
-        if queue is not None:
-            # a slot whose row has ended takes the next row of the queue: no launch waits for its longest row
-            slots, chunks = queue
-            for sids in chunks:
-                store(sids, dec.generate_queue([rows[r] for r in sids], slots=slots, sample_ids=sids,
-                                               position_bias=launch_tables(tables, row_table, sids), **kw))
-        else:
-            for sids, real in plan_launches([len(a) for a in rows], batch_size, by_length=prefill == 'forward'):
-                chunk = [rows[r] for r in sids]
-                P = dec.prefill(self.engine, chunk) if prefill == 'forward' else 0
-                store(sids[:real], dec.generate(chunk, sample_ids=sids, prefilled=P,
-                                                position_bias=launch_tables(tables, row_table, sids), **kw))
+        for sids, real, slots in plan_generate([len(a) for a in rows], batch_size, prefill, row_table, table_bytes):
+            chunk = [rows[r] for r in sids]
+            P = dec.prefill(self.engine, chunk) if prefill == 'forward' else 0
+            res = dec._generate(chunk, sampling, sids, max_length, launch_tables(tables, row_table, sids), prefilled=P,
+                                slots=slots)
+            for k, key in (('tokens', 'ids'), ('token_logp', 'token_logp'), ('start', 'start'), ('end', 'end')):
+                out[k][sids[:real]] = res[key][:real]
         end = out.pop('end')
         out['finished'] = end < max_length
         out['length'] = np.where(out['finished'], end + 1, max_length) - out['start']

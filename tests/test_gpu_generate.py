@@ -358,6 +358,37 @@ def test_reference_sampler_unaffected_by_generate():
     np.testing.assert_array_equal(a, b)
 
 
+def test_generate_leaves_the_launch_struct_unchanged():
+    """generate / generate_queue launch a copy of dec.m, so the struct sample() launches keeps every byte through a static,
+    a queue, a forward-prefilled and a refused call, with every constraint field set"""
+    from progen_b200 import ProGen
+    from progen_b200.decode import BatchDecoder
+    from progen_b200.lib import ProgenError
+    cfg, params, data, g = load_case('tiny_glu_sgu')
+    V = cfg['num_tokens']
+    model = ProGen(**CASES['tiny_glu_sgu'])
+    model._ensure_loaded(params)
+    dec = BatchDecoder(cfg, params, batch=4)
+    prompts = _prompts(np.random.default_rng(12), [3, 3, 5, 1])
+    bias = np.where(np.arange(V) % 5 == 2, -np.inf, 0.1).astype(np.float32)
+    kw = dict(temperature=0.8, top_k=20, top_p=0.9, seed=7, logit_bias=bias, min_new_tokens=2, repetition_penalty=1.2,
+              repetition_window=8)
+    table = lambda rows: (np.zeros((1, 4, V), np.float32), np.zeros(rows, np.int64))
+    before = bytes(dec.m)
+    dec.generate(prompts, position_bias=table(4), **kw)
+    assert bytes(dec.m) == before, 'static generate'
+    dec.generate_queue(prompts * 2, slots=3, position_bias=table(8), **kw)
+    assert bytes(dec.m) == before, 'generate_queue'
+    P = dec.prefill(model.engine, prompts[:2])
+    res = dec.generate(prompts[:2], prefilled=P, position_bias=table(2), **kw)
+    assert P == 3 and res['prefill_s'] == 0.0
+    assert bytes(dec.m) == before, 'forward-prefilled generate'
+    for bad in (dict(top_k=0), dict(position_bias=table(3)), dict(prefilled=4)):
+        with pytest.raises(ProgenError):
+            dec.generate(prompts, **{**kw, **bad})
+    assert bytes(dec.m) == before, 'refused generate'
+
+
 def test_bf16_weights_generate_and_mostly_agree():
     from progen_b200 import ProGen
     cfg, params, data, g = load_case('tiny_all_glu')
