@@ -103,6 +103,17 @@ int progen_ce_fwd_bwd(const void* logits, int dtype, const int* labels, float* w
  * -seq_ll / seq_count is the per-sequence cross_entropy of utils.py:45-59. */
 int progen_token_logprob(const void* logits, int dtype, const int* labels, float* logp, float* seq_ll, float* seq_count,
                          int B, int n, int V, void* stream);
+/* preference (DPO) head over B = 2 * pairs rows: rows 0..pairs-1 are chosen, row i + pairs is the rejected row of pair i;
+ * ref_ll [B] holds the frozen reference's sums in the same order.  Runs progen_token_logprob (logp [B*n], seq_ll and
+ * seq_count [B] as there: s(row) = seq_ll), then per pair, in double, z = beta * ((s(c) - ref_c) - (s(r) - ref_r)) and
+ * loss_i = softplus(-z), and the per-token weights [B*n] w_t = -(d loss / d s(row)) * mask_t = +-beta * sigma(-z) *
+ * inv_pairs * mask_t, then the CE kernel of progen_ce_fwd_bwd with those weights: dlogits = w_t * (softmax - onehot).
+ * stats [pairs, 4] = (s(c), s(r), z, loss_i); *loss = inv_pairs * sum_i loss_i (written, not accumulated).  ce_scratch is
+ * one float the CE kernel accumulates its unused weighted NLL into.  No float atomics reach stats, loss or weights: they
+ * are the same bits in every launch.  Refused: null pointers, pairs < 1, beta or inv_pairs not finite and > 0. */
+int progen_preference_head(const void* logits, int dtype, const int* labels, const float* ref_ll, float* logp, float* seq_ll,
+                           float* seq_count, float* weights, float* stats, float* loss, float* ce_scratch, void* dlogits,
+                           int dlogits_dtype, int pairs, int n, int V, float beta, float inv_pairs, void* stream);
 /* out[b, :] = sum_t mask_t x[b, t, :] / sum_t mask_t (fp32, fixed order) over rows of x [B*n, d] (stride ldx), with the
  * same mask as above: for a sequence of L residues, input positions 0..L (BOS and every residue). */
 int progen_masked_mean_pool(const void* x, long long ldx, int dtype, const int* labels, float* out, int B, int n, int d,

@@ -2,6 +2,7 @@
 // cross-entropy with the pad-as-EOS mask (fwd+bwd fused), rotary backward, SGU gating, GELU backward, column sums, and the
 // row gather that fills the decoder's caches from an inference forward (generation prefill).
 // All are coalesced, 8/16-byte vectorised, one warp per row where a row reduction is needed.
+#include <cmath>
 #include "common.cuh"
 #include "../../include/progen_b200.h"
 
@@ -454,6 +455,61 @@ __global__ void seq_logprob_sum_kernel(const int* __restrict__ labels, float* __
   }
 }
 
+// ------------------------------------------------------------------------------------------ preference (DPO) head
+// Pair i of a preference batch is (chosen row i, rejected row i + pairs).  Its margin z = beta * ((s_c - ref_c) -
+// (s_r - ref_r)), its loss softplus(-z) and sigma(-z), in double.  The per-pair blocks and the loss sum both call this, so
+// they see the same bits.
+__device__ __forceinline__ void preference_pair(const float* __restrict__ seq_ll, const float* __restrict__ ref_ll, int i,
+                                                int pairs, double beta, double& z, double& loss, double& sig) {
+  z = beta * (((double)seq_ll[i] - (double)ref_ll[i]) - ((double)seq_ll[i + pairs] - (double)ref_ll[i + pairs]));
+  const double e = exp(-fabs(z));
+  loss = fmax(-z, 0.0) + log1p(e);
+  sig = z >= 0.0 ? e / (1.0 + e) : 1.0 / (1.0 + e);
+}
+
+constexpr int PREF_THREADS = 256;
+
+// Grid (pairs, 2), PREF_THREADS threads: block (i, side) writes the per-token CE weights of row i + side * pairs,
+// w_t = -(d loss / d s(row)) * mask_t = +-beta * sigma(-z) * inv_pairs under the loss mask (Q8), and block (i, 0) its
+// stats row.  Block (0, 0) also sums the pair losses in a fixed order (strided per-thread partials, then the partials in
+// thread order): no float atomics, so stats, loss and weights are the same bits in every launch.
+__global__ void preference_weights_kernel(const int* __restrict__ labels, const float* __restrict__ seq_ll,
+                                          const float* __restrict__ ref_ll, float* __restrict__ w, float* __restrict__ stats,
+                                          float* __restrict__ loss, int pairs, int n, float beta, float inv_pairs) {
+  const int i = blockIdx.x, side = blockIdx.y;
+  const long long row = i + (long long)side * pairs;
+  double z, l, sig;
+  preference_pair(seq_ll, ref_ll, i, pairs, beta, z, l, sig);
+  const float g = (float)((double)beta * sig * (double)inv_pairs);
+  const float wv = side == 0 ? g : -g;
+  const int* lb = labels + row * n;
+  int first, count;
+  seq_loss_mask(lb, n, first, count);
+  for (int t = threadIdx.x; t < n; t += blockDim.x) w[row * n + t] = (lb[t] != 0 || t == first) ? wv : 0.f;
+  if (side == 0 && threadIdx.x == 0) {
+    float* st = stats + 4LL * i;
+    st[0] = seq_ll[i];
+    st[1] = seq_ll[i + pairs];
+    st[2] = (float)z;
+    st[3] = (float)l;
+  }
+  if (i == 0 && side == 0) {
+    __shared__ double part[PREF_THREADS];
+    double acc = 0.0;
+    for (int j = threadIdx.x; j < pairs; j += PREF_THREADS) {
+      preference_pair(seq_ll, ref_ll, j, pairs, beta, z, l, sig);
+      acc += l;
+    }
+    part[threadIdx.x] = acc;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      double s = 0.0;
+      for (int k = 0; k < PREF_THREADS; ++k) s += part[k];
+      *loss = (float)(s * (double)inv_pairs);
+    }
+  }
+}
+
 // out[b, :] = sum_t mask_t x[b, t, :] / sum_t mask_t.  Grid (ceil(d / 128), B), 256 threads: lane owns 4 columns, warp w sums
 // rows t = w, w + 8, ... in order, then the 8 warp partials are added in order: fixed order, fp32 accumulation.
 template <typename TX>
@@ -752,6 +808,36 @@ int progen_token_logprob(const void* logits, int dtype, const int* labels, float
   else { progen_set_error("token_logprob: unsupported dtype %d", dtype); return PROGEN_ERR_UNSUPPORTED; }
   PG_LAUNCH_CHECK();
   seq_logprob_sum_kernel<<<B, 256, 0, s>>>(labels, logp, seq_ll, seq_count, n);
+  PG_LAUNCH_CHECK();
+  return PROGEN_OK;
+}
+
+int progen_preference_head(const void* logits, int dtype, const int* labels, const float* ref_ll, float* logp, float* seq_ll,
+                           float* seq_count, float* weights, float* stats, float* loss, float* ce_scratch, void* dlogits,
+                           int dlogits_dtype, int pairs, int n, int V, float beta, float inv_pairs, void* stream) {
+  PG_CHECK_ARG(logits && labels && ref_ll && logp && seq_ll && seq_count && weights && stats && loss && ce_scratch && dlogits);
+  PG_CHECK_ARG(pairs >= 1 && pairs <= (1 << 30) && n > 0 && V % 4 == 0);
+  PG_CHECK_ARG(std::isfinite(beta) && beta > 0.f && std::isfinite(inv_pairs) && inv_pairs > 0.f);
+  const bool f32_f32 = dtype == PG_F32 && dlogits_dtype == PG_F32, f32_bf16 = dtype == PG_F32 && dlogits_dtype == PG_BF16,
+             bf16_bf16 = dtype == PG_BF16 && dlogits_dtype == PG_BF16;
+  if (!(f32_f32 || f32_bf16 || bf16_bf16)) {
+    progen_set_error("preference_head: unsupported dtypes %d / %d", dtype, dlogits_dtype);
+    return PROGEN_ERR_UNSUPPORTED;
+  }
+  cudaStream_t s = (cudaStream_t)stream;
+  const int B = 2 * pairs;
+  const long long T = (long long)B * n;
+  const int rc = progen_token_logprob(logits, dtype, labels, logp, seq_ll, seq_count, B, n, V, stream);
+  if (rc != PROGEN_OK) return rc;
+  preference_weights_kernel<<<dim3(pairs, 2), PREF_THREADS, 0, s>>>(labels, seq_ll, ref_ll, weights, stats, loss, pairs, n,
+                                                                    beta, inv_pairs);
+  PG_LAUNCH_CHECK();
+  const int grid = row_grid(T);
+#define CE_CASE(TL, TD) ce_fwd_bwd_kernel<TL, TD><<<grid, 256, 0, s>>>((const TL*)logits, labels, weights, ce_scratch, (TD*)dlogits, T, V)
+  if (f32_f32) CE_CASE(float, float);
+  else if (f32_bf16) CE_CASE(float, bf16);
+  else CE_CASE(bf16, bf16);
+#undef CE_CASE
   PG_LAUNCH_CHECK();
   return PROGEN_OK;
 }

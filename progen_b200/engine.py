@@ -290,6 +290,10 @@ class Engine:
         self.logits = F(T, self.V)
         self.dlogits = A(T, self.V)
         self.ce_w = F(T)
+        # preference (DPO) head (preference_step_device): B = 2 * pairs rows; allocated here so a captured step's pointers
+        # stay valid
+        self.logp, self.seq_ll, self.seq_count, self.ref = F(T), F(B), F(B), F(B)
+        self.stats, self.ce_scratch = F(max(1, B // 2), 4), F(1)
         # backward temporaries (shared by all layers)
         self.dres = F(T, d)
         self.dres_lp = A(T, d) if self.mp else self.dres
@@ -573,6 +577,36 @@ class Engine:
                                       self.loss.data_ptr(), self.dlogits.data_ptr(), self.act_dt, self.B, self.n, self.V,
                                       1.0 / global_batch, st), 'ce_fwd_bwd')
         self._backward_device()
+
+    def load_preference(self, rows, ref):
+        """rows (2P, n+1): the chosen rows, then their rejected rows; ref [2P] float32: the reference log-likelihoods in
+        the same order -> self.tok / self.labels / self.ref; returns P"""
+        B = self.load_batch(rows)
+        self.ref.copy_(torch.as_tensor(np.asarray(ref, np.float32)), non_blocking=True)
+        return B // 2
+
+    def preference_step_device(self, pairs, beta, global_pairs, zero_grads=True):
+        """forward + preference (DPO) head + backward on 2 * pairs rows already resident in self.tok / self.labels (rows
+        0..P-1 chosen, row i + P the rejected row of pair i) and their reference log-likelihoods in self.ref.  The loss is
+        the sum of the pair losses softplus(-z) over 1/global_pairs (DESIGN.md §3.7); self.stats [P, 4] holds each pair's
+        (s(chosen), s(rejected), z, loss)."""
+        if 2 * pairs != self.B:
+            raise L.ProgenError(f'preference step: {pairs} pairs need {2 * pairs} resident rows, have {self.B}')
+        self._forward_device()
+        if zero_grads:
+            self.grads.zero_()
+        L.check(self.lib.progen_preference_head(self.logits.data_ptr(), L.F32, self.labels.data_ptr(), self.ref.data_ptr(),
+                                                self.logp.data_ptr(), self.seq_ll.data_ptr(), self.seq_count.data_ptr(),
+                                                self.ce_w.data_ptr(), self.stats.data_ptr(), self.loss.data_ptr(),
+                                                self.ce_scratch.data_ptr(), self.dlogits.data_ptr(), self.act_dt, pairs, self.n,
+                                                self.V, beta, 1.0 / global_pairs, L.stream()), 'preference_head')
+        self._backward_device()
+
+    def preference_stats(self, pairs):
+        """the last preference step's per-pair statistics as numpy float32 [pairs]"""
+        st = self.stats[:pairs].cpu().numpy() if pairs else np.zeros((0, 4), np.float32)
+        return dict(policy_chosen=st[:, 0].copy(), policy_rejected=st[:, 1].copy(), margin=st[:, 2].copy(),
+                    loss=st[:, 3].copy())
 
     def ln_bwd_res(self, dy, x, scale, mean, rstd, dscale, shift, next_bias_grad=None):
         """LN(+shift) backward into the residual-gradient stream; `next_bias_grad` (+= column sums of the updated dres) is

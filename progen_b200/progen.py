@@ -6,7 +6,8 @@ Same constructor keywords (including the accepted-and-ignored `attn_dim`, `clamp
 interchange.  Everything below `.apply` runs as sm_90a kernels behind the C ABI (include/progen_b200.h).
 
 Beyond the reference surface: `.apply` also accepts a batch (B, n); `.loss_and_grad(params, data)` is the fused
-equivalent of `value_and_grad(get_loss_fn(model))` (utils.py:61-93); `.trainer(...)` owns device-resident training
+equivalent of `value_and_grad(get_loss_fn(model))` (utils.py:61-93) and `.preference_loss_and_grad` its preference
+(DPO) twin over chosen / rejected pairs; `.trainer(...)` owns device-resident training
 state (parameters, Adam moments, apply_every accumulator) for the train.py loop; `.score(params, data)` is an
 inference-only forward returning per-sequence log-likelihoods (and optionally per-token log-probabilities and pooled
 embeddings); `.score_variants` / `.mutational_scan` score substitutions against a wild type on that forward, cut to the
@@ -292,6 +293,22 @@ class ProGen:
         self._ensure_loaded(params)
         loss = self.engine.loss_and_grad(data)
         return float(loss.item()), self.engine.export_grads()
+
+    def preference_loss_and_grad(self, params, chosen, rejected, ref_chosen, ref_rejected, *, beta=0.1):
+        """The preference (DPO, Rafailov et al. 2023) twin of `loss_and_grad`.  Pair i is (chosen[i], rejected[i]), each a
+        (P, n+1) integer row of the `collate` / `loss_and_grad` contract; ref_chosen / ref_rejected [P] are the rows'
+        log-likelihoods under the frozen reference parameters, as `score` returns them.  With s(x) the policy's
+        log-likelihood (what `score` reports, bitwise), z_i = beta * ((s(c_i) - ref_c_i) - (s(r_i) - ref_r_i)) and
+        loss = mean_i softplus(-z_i).  Inputs are checked before any device work (ProgenError).
+        Returns (python float loss, haiku-shaped dict of numpy fp32 gradients, stats), stats a dict of float32 [P] arrays:
+        policy_chosen, policy_rejected (s), margin (z) and loss (each pair's)."""
+        from .preference import check_pairs
+        rows, ref, beta, _ = check_pairs(chosen, rejected, ref_chosen, ref_rejected, beta, None, self.config['seq_len'])
+        self._ensure_loaded(params)
+        eng = self.engine
+        P = eng.load_preference(rows, ref)
+        eng.preference_step_device(P, beta, P)
+        return float(eng.loss.item()), eng.export_grads(), eng.preference_stats(P)
 
     def score(self, params, data, *, batch_size=64, return_tokens=False, return_embeddings=False):
         """Log-likelihood of sequences under the model, without keeping any training state.

@@ -88,23 +88,71 @@ class Trainer:
         of the gradient buffer is part of the graph (issued on the capture stream between backward and the norm).  Call
         after at least one eager step of the same shape (kernel attributes, tensor maps, buffers and the NCCL communicator
         must exist before capture).  `install=False` returns the graph without making it the one `step` replays."""
+        gb = global_batch or batch_rows * self.world
+        return self._capture(batch_rows, (batch_rows, gb), lambda: self.eng.step_device(gb), install)
+
+    def _capture(self, batch_rows, key, step_device, install=True):
+        """capture step_device() + gradient exchange + optimizer for batches of `batch_rows` rows; `key` is what a later
+        step must match to replay it"""
         if self.world > 1 and self.overlap:
             raise L.ProgenError('capture_graph: PROGEN_DDP_OVERLAP=1 launches its bucketed all-reduces eagerly')
         eng = self.eng
         eng.ensure_batch(batch_rows)
-        gb = global_batch or batch_rows * self.world
         if self._adam_state is None:
             self._adam_state = torch.zeros(4, dtype=torch.int64, device=eng.dev)   # AdamDevState: count | bc1, bc2 | emit, pad
         self._adam_state[0] = self.count
         torch.cuda.synchronize()
         g = torch.cuda.CUDAGraph()
         with torch.cuda.graph(g):
-            eng.step_device(gb)
+            step_device()
             self._allreduce_grads()
             self._update_captured()
         if install:
-            self._graph, self._graph_key, self._graph_epoch = g, (batch_rows, gb), getattr(eng, 'alloc_epoch', 0)
+            self._graph, self._graph_key, self._graph_epoch = g, key, getattr(eng, 'alloc_epoch', 0)
         return g
+
+    # ---- preference (DPO) fine-tuning
+    def preference_step(self, chosen, rejected, ref_chosen, ref_rejected, beta=0.1, sync_loss=False, global_pairs=None):
+        """One micro-step of preference (DPO) fine-tuning on this rank's pairs: the loss and gradient of
+        `ProGen.preference_loss_and_grad`, then the same clip / AdamW / apply_every update as `step`.  chosen / rejected:
+        (P, n+1) integer rows; ref_chosen / ref_rejected [P]: their log-likelihoods under the frozen reference (`score`).
+        Data parallel: give each rank `parallel.shard_rows(P_global, rank, world)` of the pairs and global_pairs =
+        P_global (default: equal shards, P * world); a rank without pairs contributes zeros but joins the all-reduce.
+        With cuda_graph=True the step is captured after two eager steps of one (P, global_pairs, beta) and replayed from
+        then on.  Returns the device scalar loss (global mean when sync_loss); `preference_stats()` has the per-pair
+        statistics."""
+        from .preference import check_pairs
+        gp = global_pairs
+        if gp is None and self.world > 1:
+            gp = len(chosen) * self.world
+        rows, ref, beta, gp = check_pairs(chosen, rejected, ref_chosen, ref_rejected, beta, gp, self.eng.n,
+                                          what='preference_step', allow_empty=True)
+        P = rows.shape[0] // 2
+        self._pref_pairs = P
+        if P == 0:
+            self.eng.grads.zero_()
+            self.eng.loss.zero_()
+            return self._update(sync_loss)
+        key = (2 * P, gp, 'preference', beta)
+        self._drop_graph_unless(2 * P)
+        if self._graph is not None and self._graph_key == key:
+            self.eng.load_preference(rows, ref)            # H2D copies stay outside the graph
+            return self._replay(sync_loss)
+        self.eng.load_preference(rows, ref)
+        self.eng.preference_step_device(P, beta, gp)
+        loss = self._update(sync_loss)
+        if self._auto_graph and not self.overlap:
+            self._eager_run = self._eager_run + 1 if key == self._eager_key else 1
+            self._eager_key = key
+            if self._eager_run >= 2:
+                self._capture(2 * P, key, lambda: self.eng.preference_step_device(P, beta, gp))
+                self._eager_run = 0
+        return loss
+
+    def preference_stats(self):
+        """this rank's statistics of its last `preference_step` as numpy float32 [P] arrays: policy_chosen and
+        policy_rejected (the policy's log-likelihoods s), margin (z) and loss (each pair's softplus(-z))"""
+        return self.eng.preference_stats(getattr(self, '_pref_pairs', 0))
 
     def _allreduce_grads(self):
         """SUM of the per-rank gradients (each already scaled by 1/global_rows): the reference's pmap mean, utils.py:78-91"""
