@@ -58,9 +58,12 @@ def _rot(x, sin, cos):
     return x * cos + x2 * sin
 
 
-def forward(prm, ids, cfg, operand_round=None, device=None, return_hidden=False):
+def forward(prm, ids, cfg, operand_round=None, device=None, return_hidden=False, probe=None):
     """prm: nested dict of tensors on `device` (default CPU); ids: (B, n) long -> logits (B, n, V), or with
-    `return_hidden` (logits, the final LayerNorm output (B, n, d): the head's input, which scoring pools)."""
+    `return_hidden` (logits, the final LayerNorm output (B, n, d): the head's input, which scoring pools).
+    `probe` (optional dict) receives, per layer, lists of intermediate tensors without changing any result: 'resid' the
+    residual stream entering the layer (and, last, the stream entering the final LayerNorm), 'attn' the attention
+    probabilities (B, h, W, w, 2w), 'gelu_in' the GELU input (the gate half for GLU layers)."""
     r = operand_round or (lambda t: t)
     dev = torch.device('cpu') if device is None else torch.device(device)
     ids = ids.to(dev)
@@ -71,8 +74,10 @@ def forward(prm, ids, cfg, operand_round=None, device=None, return_hidden=False)
     dtype = x.dtype
     sin, cos = (t.to(dev) for t in _rotary_tables(n, dh, dtype))
     mask = torch.tril(torch.ones(w, 2 * w, dtype=torch.bool, device=dev), w)
+    keep = (lambda key, t: probe.setdefault(key, []).append(t.detach())) if probe is not None else (lambda key, t: None)
     for i, kind in enumerate(layer_kinds(cfg)):
         a = P + f'attn{i}/~/'
+        keep('resid', x)
         y = _ln(x, prm[a + 'layer_norm']['scale'])
         if cfg['shift_tokens']:
             y = _shift(y)
@@ -86,6 +91,7 @@ def forward(prm, ids, cfg, operand_round=None, device=None, return_hidden=False)
         sim = torch.einsum('bhwid,bhwjd->bhwij', q, k) * (dh ** -0.5)
         sim = torch.where(mask, sim, torch.full_like(sim, ATTN_MASK_VALUE))
         attn = torch.softmax(sim, dim=-1)
+        keep('attn', attn)
         o = torch.einsum('bhwij,bhwjd->bhwid', r(attn), v)
         o = o.reshape(B, h, n, dh).transpose(1, 2).reshape(B, n, h * dh)
         x = x + r(o) @ r(prm[a + 'linear_1']['w']) + prm[a + 'linear_1']['b']
@@ -97,8 +103,10 @@ def forward(prm, ids, cfg, operand_round=None, device=None, return_hidden=False)
         u = r(y) @ r(prm[f + 'linear']['w']) + prm[f + 'linear']['b']
         if kind == 'glu':
             val, gate = u.chunk(2, dim=-1)
+            keep('gelu_in', gate)
             u = val * _gelu(gate)
         else:
+            keep('gelu_in', u)
             u = _gelu(u)
         if kind == 'sgu':
             xs, gate = u.chunk(2, dim=-1)
@@ -108,6 +116,7 @@ def forward(prm, ids, cfg, operand_round=None, device=None, return_hidden=False)
             u = xs * gate
             u = r(u) @ r(prm[f + 'sgu/~/linear']['w']) + prm[f + 'sgu/~/linear']['b']
         x = x + r(u) @ r(prm[f + 'linear_1']['w']) + prm[f + 'linear_1']['b']
+    keep('resid', x)
     x = _ln(x, prm[P + 'layer_norm']['scale'])
     logits = r(x) @ r(prm[P + 'linear']['w']) + prm[P + 'linear']['b']
     return (logits, x) if return_hidden else logits

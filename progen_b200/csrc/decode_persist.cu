@@ -1641,7 +1641,8 @@ static __device__ __noinline__ void sample_std_phase(const float* logits, int32_
         m = bmax(ma);                                                           // the candidates' maximum (NaN skipped)
       }
       int id;
-      if (temp == 0.f) {
+      // a temperature so small that max / T overflows (e.g. 1e-39, subnormal) is the T -> 0 limit: the greedy draw
+      if (temp == 0.f || isinf(m / temp)) {
         float bv = -INFINITY;
         int bi = 0x7fffffff;
         for (int c = t; c < V; c += TPB) if (sv[c] > bv) { bv = sv[c]; bi = c; }

@@ -409,7 +409,8 @@ class ProGen:
         every chunking (with forward prefill a ragged last chunk is padded to the class).  Rows of different classes agree
         to fp32 round-off, so ids can differ where a draw is that close.  max_length (default seq_len) bounds BOS + prompt
         + generated tokens;
-        temperature 0 is greedy (first maximal logit; top_k / top_p ignored).
+        temperature 0 is greedy (first maximal logit; top_k / top_p ignored), and so is a positive temperature so small
+        that the largest logit divided by it overflows float32 (e.g. 1e-39).
 
         Constraints, applied in the kernel to the logits of every draw, in this order, before top-k / temperature / top-p
         (DESIGN.md §3.3):
