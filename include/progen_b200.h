@@ -68,6 +68,8 @@ typedef struct progen_gemm_t {
   const void* aux;
   const float* rot_sin;   /* [seq_len, dim_head/2], fixed_pos_embedding progen.py:24-28 */
   const float* rot_cos;
+  float* colsum;          /* EPI_GLU_BWD / EPI_GELU_BWD, nullable: colsum[c] += sum over rows of the stored out[., c]
+                             (the pre-activation Linear's bias gradient; 16-byte aligned on the TC backend) */
 } progen_gemm_t;
 
 int progen_gemm(const progen_gemm_t* desc, void* stream);

@@ -50,8 +50,10 @@ int progen_gemm(const progen_gemm_t* d, void* stream) {
   g.epi.rot_sin = d->rot_sin; g.epi.rot_cos = d->rot_cos;
   g.epi.seq_len = d->seq_len > 0 ? d->seq_len : 1; g.epi.dim_head = d->dim_head > 0 ? d->dim_head : 2;
   g.epi.atomic = d->atomic; g.epi.tril = d->tril; g.epi.tril_rows = d->tril_rows > 0 ? d->tril_rows : 1;
+  g.epi.colsum = d->colsum;
   PG_CHECK_ARG(g.epi_kind >= 0 && g.epi_kind < EPI_NUM_KINDS);
   PG_CHECK_ARG(g.epi.out != nullptr);
+  PG_CHECK_ARG(!g.epi.colsum || g.epi_kind == EPI_GLU_BWD || g.epi_kind == EPI_GELU_BWD);
   if (g.epi_kind == EPI_GLU || g.epi_kind == EPI_GELU) PG_CHECK_ARG(g.epi.bias != nullptr);   // out2 may be null (inference)
   if (g.epi_kind == EPI_GLU_BWD || g.epi_kind == EPI_GELU_BWD) PG_CHECK_ARG(g.epi.aux != nullptr);
   if (g.epi_kind == EPI_ROTARY) PG_CHECK_ARG(g.epi.rot_sin && g.epi.rot_cos && d->seq_len > 0 && d->dim_head > 0 && d->dim_head % 2 == 0);

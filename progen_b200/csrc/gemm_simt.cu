@@ -75,12 +75,26 @@ __global__ void __launch_bounds__(256) gemm_simt_kernel(const TI* __restrict__ A
 
   const int col = n0 + tx * 8;
   if (col >= g.N) return;
+  using CS = EpiColsum<KIND, 8>;
+  EpiCol<8> cb;
+  epi_load_col<KIND, 8>(g.epi, col, true, cb);
+  float csum[CS::REGS];
+#pragma unroll
+  for (int k = 0; k < CS::REGS; ++k) csum[k] = 0.f;
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
     const int m = m0 + ty * 8 + i;
     if (m >= g.M) break;
     const long long row = (g.batch_reduce ? 0 : (long long)z * g.d_batch_rows) + m;
-    epi_apply<KIND, TO, 8>(g.epi, DirectIO{}, row, col, acc[i], true);
+    EpiPre<KIND, TO, 8> pre;
+    epi_load<KIND, TO, 8>(g.epi, row, col, true, pre);
+    epi_finish<KIND, TO, 8>(g.epi, row, col, acc[i], cb, pre, true, csum);
+  }
+  if constexpr (CS::W > 0) {
+    if (g.epi.colsum) {
+#pragma unroll
+      for (int k = 0; k < CS::W; ++k) atomicAdd(g.epi.colsum + CS::OUT_SCALE * col + k, csum[k]);
+    }
   }
 }
 
@@ -116,8 +130,7 @@ int gemm_simt_launch(const GemmArgs& a, cudaStream_t stream) {
   PG_CHECK_ARG(a.M > 0 && a.N > 0 && a.K > 0 && a.batch >= 1);
   PG_CHECK_ARG(a.N % 8 == 0);
   PG_CHECK_ARG(a.split_k == 1);
-  PG_CHECK_ARG(!a.batch_reduce || (a.epi_kind == EPI_ACCUM && a.epi.atomic));
-  SimtDev gd;
+  PG_CHECK_ARG(!a.batch_reduce || (a.epi_kind == EPI_ACCUM && a.epi.atomic));  SimtDev gd;
   gd.M = a.M; gd.N = a.N; gd.K = a.K;
   gd.a_rs = a.a_mn_major ? 1 : a.lda; gd.a_cs = a.a_mn_major ? a.lda : 1;
   gd.b_rs = a.b_mn_major ? 1 : a.ldb; gd.b_cs = a.b_mn_major ? a.ldb : 1;

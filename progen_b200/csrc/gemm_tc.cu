@@ -34,6 +34,7 @@ constexpr int B_BYTES = BN * BK * 2;   // 16 KiB
 constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
 constexpr int STAGES = 4;                // a fifth stage fits only with epilogue passes of 64 x 64; measured slower on the step
 constexpr int EPI_ROWS = 64;           // the epilogue stages and applies the tile in two passes of 64 rows
+constexpr int EPI_ITEMS = EPI_ROWS * (BN / 8) / 128;   // row slices of 8 columns per consumer thread and pass
 constexpr int CS_LD = BN + 4;          // fp32 row stride of the staged accumulator rows
 constexpr int CS_BYTES = EPI_ROWS * CS_LD * 4;
 constexpr int SMEM_TOTAL = 1024 /*align slack*/ + STAGES * STAGE_BYTES + 2 * CS_BYTES + 2 * STAGES * 8;
@@ -196,15 +197,39 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
       advance(1);
     }
     if (t + (int)gridDim.x < tiles) named_bar_arrive(BAR_TURN + (c ^ 1), 256);   // tile p + 1 may issue its MMAs
+
+    // ---- epilogue, 64 rows per pass: stage the fp32 rows in this warpgroup's buffer, then 8 consecutive columns of
+    // one row per thread, 16 threads per row.  Item i of pass h is tile row 64 h + 8 i + tid / 16, columns
+    // 8 (tid % 16) .. + 7: a thread keeps its columns for the whole tile.  The global reads of a pass (epi_load) all go
+    // out before its first item is finished, so a thread has EPI_ITEMS of them in flight instead of one.
+    const int w = tid >> 5, lane = tid & 31;
+    const int r0 = 16 * w + (lane >> 2), c0 = 2 * (lane & 3);
+    const int cc = 8 * (tid & 15), col = ti.n0 + cc;
+    const bool col_ok = col < g.N;
+    const int m_first = ti.m0 + (tid >> 4);
+    const long long row_first = (g.batch_reduce ? 0 : (long long)ti.z * g.d_batch_rows) + m_first;
+    using CS = EpiColsum<KIND, 8>;
+    EpiCol<8> cb;
+    EpiPre<KIND, TO, 8> pre[EPI_ITEMS];
+    epi_load_col<KIND, 8>(g.epi, col, col_ok, cb);
+    // pass 0's load phase does not read the accumulators: it overlaps the last k-block's MMAs.  The residual kind
+    // (64 prefetch registers and the bias) does not fit next to all 128 accumulators without spilling: it issues pass
+    // 0's loads once acc[0] is staged.
+    constexpr bool LOAD_BEFORE_WAIT = KIND != EPI_RESIDUAL;
+    auto load_pass0 = [&] {
+#pragma unroll
+      for (int i = 0; i < EPI_ITEMS; ++i)
+        epi_load<KIND, TO, 8>(g.epi, row_first + 8 * i, col, col_ok && m_first + 8 * i < g.M, pre[i]);
+    };
+    if constexpr (LOAD_BEFORE_WAIT) load_pass0();
     wgmma_wait<0>();
     fence_regs(acc[0]);
     fence_regs(acc[1]);
     if (prev >= 0 && tid == 0) mbar_arrive(empty_bar(prev));
 
-    // ---- epilogue, 64 rows per pass: stage the fp32 rows in this warpgroup's buffer, then 8 consecutive columns of
-    // one row per thread, 16 threads per row
-    const int w = tid >> 5, lane = tid & 31;
-    const int r0 = 16 * w + (lane >> 2), c0 = 2 * (lane & 3);
+    float csum[CS::REGS];
+#pragma unroll
+    for (int k = 0; k < CS::REGS; ++k) csum[k] = 0.f;
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       named_bar_sync(BAR_EPI + c, 128);         // every thread has read the rows staged before
@@ -213,18 +238,51 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
         *reinterpret_cast<float2*>(cs + r0 * CS_LD + 8 * j + c0) = make_float2(acc[h][4 * j], acc[h][4 * j + 1]);
         *reinterpret_cast<float2*>(cs + (r0 + 8) * CS_LD + 8 * j + c0) = make_float2(acc[h][4 * j + 2], acc[h][4 * j + 3]);
       }
+      if constexpr (!LOAD_BEFORE_WAIT) {
+        if (h == 0) load_pass0();
+      }
       named_bar_sync(BAR_EPI + c, 128);
-#pragma unroll 1
-      for (int idx = tid; idx < EPI_ROWS * (BN / 8); idx += 128) {
-        const int r = idx / (BN / 8), cc = (idx % (BN / 8)) * 8;
-        const int m = ti.m0 + EPI_ROWS * h + r, col = ti.n0 + cc;
-        if (m >= g.M || col >= g.N) continue;
+#pragma unroll
+      for (int i = 0; i < EPI_ITEMS; ++i) {
+        const int r = 8 * i + (tid >> 4);
+        const int m = m_first + EPI_ROWS * h + 8 * i;
         float v[8];
         const float4 x0 = *reinterpret_cast<const float4*>(cs + r * CS_LD + cc);
         const float4 x1 = *reinterpret_cast<const float4*>(cs + r * CS_LD + cc + 4);
         v[0] = x0.x; v[1] = x0.y; v[2] = x0.z; v[3] = x0.w; v[4] = x1.x; v[5] = x1.y; v[6] = x1.z; v[7] = x1.w;
-        const long long row = (g.batch_reduce ? 0 : (long long)ti.z * g.d_batch_rows) + m;
-        epi_apply<KIND, TO, 8>(g.epi, DirectIO{}, row, col, v, true);
+        epi_finish<KIND, TO, 8>(g.epi, row_first + EPI_ROWS * h + 8 * i, col, v, cb, pre[i], col_ok && m < g.M, csum);
+        // pass 1's load phase, one slot at a time as pass 0 frees it: in flight while pass 0 finishes and pass 1 stages
+        if (h == 0)
+          epi_load<KIND, TO, 8>(g.epi, row_first + EPI_ROWS + 8 * i, col, col_ok && m + EPI_ROWS < g.M, pre[i]);
+      }
+    }
+    if constexpr (CS::W > 0) {
+      if (g.epi.colsum) {                       // uniform
+        // the tile's column sums: lanes l and l ^ 16 own the same columns; the four warps meet in the staging buffer,
+        // then one red.global.add.v4 per 4 output columns
+        constexpr int TW = 16 * CS::W;          // output columns of the tile
+#pragma unroll
+        for (int k = 0; k < CS::W; ++k) csum[k] += __shfl_xor_sync(0xffffffffu, csum[k], 16);
+        named_bar_sync(BAR_EPI + c, 128);       // every thread has read the staged rows
+        if (lane < 16) {
+#pragma unroll
+          for (int k = 0; k < CS::W; k += 4)
+            *reinterpret_cast<float4*>(cs + w * TW + lane * CS::W + k) = make_float4(csum[k], csum[k + 1], csum[k + 2], csum[k + 3]);
+        }
+        named_bar_sync(BAR_EPI + c, 128);
+        const int out0 = CS::OUT_SCALE * ti.n0, out_cols = CS::OUT_SCALE * g.N;
+#pragma unroll
+        for (int q = tid; q < TW / 4; q += 128) {
+          float4 s = *reinterpret_cast<const float4*>(cs + 4 * q);
+#pragma unroll
+          for (int ww = 1; ww < 4; ++ww) {
+            const float4 x = *reinterpret_cast<const float4*>(cs + ww * TW + 4 * q);
+            s.x += x.x; s.y += x.y; s.z += x.z; s.w += x.w;
+          }
+          if (out0 + 4 * q < out_cols)
+            asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(g.epi.colsum + out0 + 4 * q), "f"(s.x),
+                         "f"(s.y), "f"(s.z), "f"(s.w) : "memory");
+        }
       }
     }
   }
@@ -329,6 +387,7 @@ int gemm_tc_launch(const GemmArgs& a, cudaStream_t stream) {
   PG_CHECK_ARG((reinterpret_cast<uintptr_t>(a.A) & 15) == 0 && (reinterpret_cast<uintptr_t>(a.B) & 15) == 0);
   PG_CHECK_ARG(!(a.split_k > 1 && a.causal));
   if (a.epi_kind == EPI_ROTARY) PG_CHECK_ARG(a.epi.seq_len % 32 == 0);
+  PG_CHECK_ARG((reinterpret_cast<uintptr_t>(a.epi.colsum) & 15) == 0);    // red.global.add.v4
   PG_CHECK_ARG(!(a.split_k > 1 || a.batch_reduce) || (a.epi_kind == EPI_ACCUM && a.epi.atomic));
 
   // stored 2D extents of each operand

@@ -662,16 +662,18 @@ class Engine:
                                                 self.G(g + '/~/layer_norm', 'scale').data_ptr(), 0, T, half, n, 0, 0, st), 'ln_bwd_sgu')
                 L.check(lib.progen_gelu_bwd(da.data_ptr(), s['u'].data_ptr(), self.act_dt, T * hid, st), 'gelu_bwd')
                 du, n_in = da, hid
+                self.colsum(du, n_in, self.G(f + 'linear', 'b'))
             elif kind == 'glu':
+                # the epilogue also adds the column sums of du into the proj_in bias gradient (interleaved like du)
                 self.wgrad_gemm(s['hact'], hid, dres_lp, d, self.G(f + 'linear_1', 'w'))
                 self.dgrad_gemm(dres_lp, d, self.W(f + 'linear_1', 'w'), hid, self.du, epi=L.EPI_GLU_BWD, ldo=2 * hid,
-                                aux=s['u'], ldaux=2 * hid)
+                                aux=s['u'], ldaux=2 * hid, colsum=self.G(f + 'linear', 'b'))
                 du, n_in = self.du, 2 * hid
             else:
                 self.wgrad_gemm(s['hact'], hid, dres_lp, d, self.G(f + 'linear_1', 'w'))
-                self.dgrad_gemm(dres_lp, d, self.W(f + 'linear_1', 'w'), hid, self.dh_, epi=L.EPI_GELU_BWD, aux=s['u'], ldaux=hid)
+                self.dgrad_gemm(dres_lp, d, self.W(f + 'linear_1', 'w'), hid, self.dh_, epi=L.EPI_GELU_BWD, aux=s['u'], ldaux=hid,
+                                colsum=self.G(f + 'linear', 'b'))
                 du, n_in = self.dh_, hid
-            self.colsum(du, n_in, self.G(f + 'linear', 'b'))
             self.wgrad_gemm(s['y2'], d, du, n_in, self.G(f + 'linear', 'w'))
             self.dgrad_gemm(du, n_in, self.W(f + 'linear', 'w'), d, self.dy)
             self.ln_bwd_res(self.dy, x1, self.Pf(f + 'layer_norm', 'scale'), s['mean2'], s['rstd2'], self.G(f + 'layer_norm', 'scale'), shift,

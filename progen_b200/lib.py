@@ -32,6 +32,7 @@ class GemmDesc(C.Structure):
         ('ldo', C.c_int64), ('ldo2', C.c_int64), ('ldaux', C.c_int64),
         ('A', C.c_void_p), ('B', C.c_void_p), ('out', C.c_void_p), ('out2', C.c_void_p),
         ('bias', C.c_void_p), ('aux', C.c_void_p), ('rot_sin', C.c_void_p), ('rot_cos', C.c_void_p),
+        ('colsum', C.c_void_p),
     ]
 
 
@@ -126,7 +127,7 @@ def stream():
 def gemm(*, M, N, K, A, lda, B, ldb, out, ldo, epi=EPI_STORE, backend, a_mn=False, b_mn=False, in_dtype, out_dtype=F32,
          batch=1, a_batch_rows=0, b_batch_rows=0, d_batch_rows=0, batch_reduce=False, causal=0, split_k=1,
          out2=None, ldo2=0, bias=None, aux=None, ldaux=0, rot_sin=None, rot_cos=None, seq_len=0, dim_head=0,
-         atomic=False, tril=False, tril_rows=0):
+         atomic=False, tril=False, tril_rows=0, colsum=None):
     """Thin wrapper over progen_gemm; tensors are passed as torch tensors (or raw ints for sub-views)."""
     d = GemmDesc()
     d.M, d.N, d.K = M, N, K
@@ -141,4 +142,5 @@ def gemm(*, M, N, K, A, lda, B, ldb, out, ldo, epi=EPI_STORE, backend, a_mn=Fals
     as_ptr = lambda x: x if isinstance(x, int) else ptr(x)
     d.A, d.B, d.out, d.out2 = as_ptr(A), as_ptr(B), as_ptr(out), as_ptr(out2)
     d.bias, d.aux, d.rot_sin, d.rot_cos = as_ptr(bias), as_ptr(aux), as_ptr(rot_sin), as_ptr(rot_cos)
+    d.colsum = as_ptr(colsum)
     check(load().progen_gemm(C.byref(d), stream()), 'progen_gemm')
