@@ -212,6 +212,19 @@ static __device__ __forceinline__ void load_wave(const Phase& ph, const Geo& g, 
 // phase time whenever it exceeds the barrier's own latency.
 struct __align__(16) UnitEnt { int off0, off1; short pl, ks; int kmax; };   // weight offsets of the unit's two rows (-1: no unit), columns left in its segment
 struct FinEnt { int r0, r1, d0, sel, rj; };                    // rows, store offset (sel: 0 out, 1 K cache, 2 V cache), rotary index
+// the finalizer entry of `pair` (single stream: built into the unit tables, or in the prefetch when they do not fit)
+static __device__ __forceinline__ FinEnt fin_entry(const Phase& ph, int pair) {
+  FinEnt f;
+  f.r0 = ph.epi == EP_GLU ? pair : 2 * pair; f.r1 = ph.epi == EP_GLU ? pair + ph.N : 2 * pair + 1;
+  f.d0 = f.r0; f.sel = 0; f.rj = 0;
+  if (ph.epi == EP_ROTARY_CACHE) {
+    const int sec = f.r0 / ph.inner, c = f.r0 % ph.inner;
+    f.rj = (f.r0 % ph.dim_head) >> 1;
+    f.sel = sec;
+    f.d0 = sec == 0 ? c : (c / ph.dim_head) * ph.n * ph.dim_head + c % ph.dim_head;
+  }
+  return f;
+}
 static __device__ void build_unit_tables(const Phase& ph, UnitEnt* ut, FinEnt* ft, int u /* 0 .. WSEGS-1 */) {
   const Geo& g = ph.g;
   const int pw = min(g.PW, g.np);
@@ -226,21 +239,7 @@ static __device__ void build_unit_tables(const Phase& ph, UnitEnt* ut, FinEnt* f
     }
     ut[u] = e;
   }
-  {
-    FinEnt f{0, 0, 0, 0, 0};
-    if (u < pw) {
-      const int pair = g.p_lo + u;
-      f.r0 = ph.epi == EP_GLU ? pair : 2 * pair; f.r1 = ph.epi == EP_GLU ? pair + ph.N : 2 * pair + 1;
-      f.d0 = f.r0;
-      if (ph.epi == EP_ROTARY_CACHE) {
-        const int sec = f.r0 / ph.inner, c = f.r0 % ph.inner;
-        f.rj = (f.r0 % ph.dim_head) >> 1;
-        f.sel = sec;
-        f.d0 = sec == 0 ? c : (c / ph.dim_head) * ph.n * ph.dim_head + c % ph.dim_head;
-      }
-    }
-    ft[u] = f;
-  }
+  ft[u] = u < pw ? fin_entry(ph, g.p_lo + u) : FinEnt{0, 0, 0, 0, 0};
 }
 
 // everything of phase `ph` (pos filled in) that can be loaded before the barrier in front of it.  ut / ft: this phase's
@@ -268,20 +267,7 @@ static __device__ __forceinline__ void prefetch_phase(const Phase& ph, WRegs<TW>
       load_wave<TW>(ph, g, 0, w);                                // (deep models: the per-launch tables do not fit shared memory)
     }
     if (t < min(g.PW, g.np)) {                                  // this thread finalizes pair t of wave 0
-      FinEnt f;
-      if (ft != nullptr) {
-        f = ft[t];
-      } else {
-        const int pair = g.p_lo + t;
-        f.r0 = ph.epi == EP_GLU ? pair : 2 * pair; f.r1 = ph.epi == EP_GLU ? pair + ph.N : 2 * pair + 1;
-        f.d0 = f.r0; f.sel = 0; f.rj = 0;
-        if (ph.epi == EP_ROTARY_CACHE) {
-          const int sec = f.r0 / ph.inner, c = f.r0 % ph.inner;
-          f.rj = (f.r0 % ph.dim_head) >> 1;
-          f.sel = sec;
-          f.d0 = sec == 0 ? c : (c / ph.dim_head) * ph.n * ph.dim_head + c % ph.dim_head;
-        }
-      }
+      const FinEnt f = ft != nullptr ? ft[t] : fin_entry(ph, g.p_lo + t);
       pre.b0 = ph.bias ? ph.bias[f.r0] : 0.f;
       pre.b1 = ph.bias ? ph.bias[f.r1] : 0.f;
       pre.d0 = ph.out + f.r0; pre.d1 = ph.out + f.r1;
@@ -690,21 +676,17 @@ static __device__ __forceinline__ void gemv_phase(const Phase& ph, int B, float*
     }
   };
   // bias + activation / residual / rotary + cache for the two rows of `pair` of sequence b
-  auto epilogue = [&](int b, int pair, float s0, float s1, bool pf /* operands in `pre` */) {
+  auto epilogue = [&](int b, int pair, float s0, float s1) {
     const int r0 = ph.epi == EP_GLU ? pair : 2 * pair, r1 = ph.epi == EP_GLU ? pair + ph.N : 2 * pair + 1;
-    if (pf) { s0 += pre.b0; s1 += pre.b1; }
-    else if (ph.bias) { s0 += ph.bias[r0]; s1 += ph.bias[r1]; }
+    if (ph.bias) { s0 += ph.bias[r0]; s1 += ph.bias[r1]; }
     float* o = ph.out + (long long)b * ph.ldo;
     if (ph.epi == EP_BIAS) { o[r0] = s0; o[r1] = s1; }
-    else if (ph.epi == EP_RESIDUAL) {
-      if (pf) { o[r0] = pre.o0 + s0; o[r1] = pre.o1 + s1; }
-      else { o[r0] = __ldcg(o + r0) + s0; o[r1] = __ldcg(o + r1) + s1; }
-    }
+    else if (ph.epi == EP_RESIDUAL) { o[r0] = __ldcg(o + r0) + s0; o[r1] = __ldcg(o + r1) + s1; }
     else if (ph.epi == EP_GELU) { o[r0] = gelu_tanh(s0); o[r1] = gelu_tanh(s1); }
     else if (ph.epi == EP_GLU) { o[r0] = s0 * gelu_tanh(s1); }
     else {  // EP_ROTARY_CACHE: rotary on q, k AND v (progen.py:87); k, v rows go to the caches at position pos
       const int hd = ph.dim_head >> 1, j = (r0 % ph.dim_head) >> 1, p = pos_of(b);
-      const float sn = pf ? pre.sn : ph.rot_sin[p * hd + j], cs = pf ? pre.cs : ph.rot_cos[p * hd + j];
+      const float sn = ph.rot_sin[p * hd + j], cs = ph.rot_cos[p * hd + j];
       const float o0 = s0 * cs - s1 * sn, o1 = s1 * cs + s0 * sn;
       const int sec = r0 / ph.inner, c = r0 % ph.inner;
       float* dst = sec == 0 ? o + c
@@ -811,7 +793,7 @@ static __device__ __forceinline__ void gemv_phase(const Phase& ph, int B, float*
             const float* pp = part + ((pl * g.KS + ks) * 2) * BTP + b;
             s0 += pp[0]; s1 += pp[BTP];
           }
-          epilogue(b, g.p_lo + pbase + pl, s0, s1, false);
+          epilogue(b, g.p_lo + pbase + pl, s0, s1);
         }
       }
       if (wave + 1 < g.nwaves) __syncthreads();
@@ -1054,7 +1036,7 @@ static __device__ __forceinline__ void gemv_phase(const Phase& ph, int B, float*
 #pragma unroll
         for (int lp = 0; lp < MAXLP; ++lp) {
           const int pl = q + NRQ * lp;
-          if (pl < pw) epilogue(b, g.p_lo + pbase + pl, acc[lp][0][0] + acc[lp][0][1], acc[lp][1][0] + acc[lp][1][1], false);
+          if (pl < pw) epilogue(b, g.p_lo + pbase + pl, acc[lp][0][0] + acc[lp][0][1], acc[lp][1][0] + acc[lp][1][1]);
         }
       }
       }
@@ -1063,9 +1045,6 @@ static __device__ __forceinline__ void gemv_phase(const Phase& ph, int B, float*
 }
 
 // ------------------------------------------------------------------------------------------------ attention
-// the queue kernels' per-slot positions, passed as a pack of one pointer (empty in the other kernels)
-static __device__ __forceinline__ const int* slot_pos_of() { return nullptr; }
-static __device__ __forceinline__ const int* slot_pos_of(const int* p) { return p; }
 // task = (sequence, head, slice of 32 keys), one warp: partial (m, l, o[dh]) -> att_part[(b, head)][slice][dh + 4].  All of
 // the task's K and V loads are independent of each other (lane = key for the logits; lane = (key group, 4 channels) for
 // the value sum), so a task is ONE memory round trip.  The out-proj phase merges the partials (plus window 0's w zero keys
@@ -1147,10 +1126,9 @@ static __device__ void attention_phase_t(const progen_decode_run_t& r, const flo
 // the value sum; every load of a slice is independent of the others.
 // PLAN: the number of sequences the work split is planned for (0: the launch's B; see run())
 // SLOT (the queue kernels): sequence b is at position spos[b] (shared memory); the window of each (sequence, head) follows it
-// (`spos` is a parameter pack, empty without SLOT, so the other kernels' calls stay as they were)
-template <int NL, int PLAN, bool SLOT, typename... SP>
+template <int NL, int PLAN, bool SLOT>
 static __device__ void attention_batch_t(const progen_decode_run_t& r, const float* kcache, const float* vcache, int pos, float* sq /* smem >= WPB * (2 dh + 4) */,
-                                         SP... spos) {
+                                         const int* spos) {
   static_assert(NL >= 2, "two lanes share a key row");
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   constexpr int dh = NL * 4, HK = NL / 2, KG = 32 / NL, NV = 16 / KG;
@@ -1178,7 +1156,7 @@ static __device__ void attention_batch_t(const progen_decode_run_t& r, const flo
     float4 o = make_float4(0.f, 0.f, 0.f, 0.f);
     if (on) {
       if constexpr (SLOT) {
-        const int p = slot_pos_of(spos...)[b];
+        const int p = spos[b];
         win = p / w; i = p % w;
         key0 = win > 0 ? (win - 1) * w : 0;
         nreal = (win > 0 ? w : 0) + i + 1;
@@ -1265,13 +1243,13 @@ static __device__ void attention_batch_t(const progen_decode_run_t& r, const flo
     __syncthreads();
   }
 }
-template <int PLAN, bool SLOT, typename... SP>
-static __device__ void attention_batch(const progen_decode_run_t& r, const float* kcache, const float* vcache, int pos, float* sq, SP... spos) {
+template <int PLAN, bool SLOT>
+static __device__ void attention_batch(const progen_decode_run_t& r, const float* kcache, const float* vcache, int pos, float* sq, const int* spos) {
   switch (r.dim_head) {
-    case 64: attention_batch_t<16, PLAN, SLOT>(r, kcache, vcache, pos, sq, spos...); break;
-    case 32: attention_batch_t<8, PLAN, SLOT>(r, kcache, vcache, pos, sq, spos...); break;
-    case 16: attention_batch_t<4, PLAN, SLOT>(r, kcache, vcache, pos, sq, spos...); break;
-    default: attention_batch_t<2, PLAN, SLOT>(r, kcache, vcache, pos, sq, spos...); break;
+    case 64: attention_batch_t<16, PLAN, SLOT>(r, kcache, vcache, pos, sq, spos); break;
+    case 32: attention_batch_t<8, PLAN, SLOT>(r, kcache, vcache, pos, sq, spos); break;
+    case 16: attention_batch_t<4, PLAN, SLOT>(r, kcache, vcache, pos, sq, spos); break;
+    default: attention_batch_t<2, PLAN, SLOT>(r, kcache, vcache, pos, sq, spos); break;
   }
 }
 
@@ -1297,9 +1275,9 @@ static __device__ __forceinline__ int sgu_splits(const progen_decode_run_t& r) {
   return s < 1 ? 1 : (s > MAXSPLIT ? MAXSPLIT : s);
 }
 // SLOT (the queue kernels): sequence b is at position spos[b] (shared memory); its split boundaries follow that position
-template <int PLAN, bool SLOT, typename... SP>
+template <int PLAN, bool SLOT>
 static __device__ void sgu_phase(const progen_decode_run_t& r, const SguArgs& L, int pos_, float* red /* smem [WPB][128] + stats */,
-                                 SP... spos) {
+                                 const int* spos) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int C = r.hid / 2, n = r.n;
   const int cblocks = C / 128;
@@ -1309,7 +1287,7 @@ static __device__ void sgu_phase(const progen_decode_run_t& r, const SguArgs& L,
   for (int t = blockIdx.x; t < tasks; t += gridDim.x) {
     const int sp = t % S, cb = (t / S) % cblocks, b = t / (S * cblocks);
     int pos = pos_;
-    if constexpr (SLOT) pos = slot_pos_of(spos...)[b];
+    if constexpr (SLOT) pos = spos[b];
     const int c0 = cb * 128 + lane * 4;
     float* hist = L.hist + (long long)b * n * C;
     const float* wrow = L.w + (long long)pos * n;
@@ -1338,26 +1316,14 @@ static __device__ void sgu_phase(const progen_decode_run_t& r, const SguArgs& L,
       const float* gate = r.u + (long long)b * r.hid + C;
       float s = 0.f;
       for (int c = threadIdx.x * 4; c < C; c += TPB * 4) { const float4 v = __ldcg(reinterpret_cast<const float4*>(gate + c)); s += (v.x + v.y) + (v.z + v.w); }
-      s = warp_sum(s);
-      if (lane == 0) stat[warp] = s;
-      __syncthreads();
-      float tt = 0.f;
-#pragma unroll
-      for (int k = 0; k < WPB; ++k) tt += stat[k];
-      const float mean = tt / C;
+      const float mean = block_sum(s, stat) / C;
       float qq = 0.f;
       for (int c = threadIdx.x * 4; c < C; c += TPB * 4) {
         const float4 v = __ldcg(reinterpret_cast<const float4*>(gate + c));
         const float a0 = v.x - mean, a1 = v.y - mean, a2 = v.z - mean, a3 = v.w - mean;
         qq += (a0 * a0 + a1 * a1) + (a2 * a2 + a3 * a3);
       }
-      qq = warp_sum(qq);
-      if (lane == 0) stat[WPB + warp] = qq;
-      __syncthreads();
-      tt = 0.f;
-#pragma unroll
-      for (int k = 0; k < WPB; ++k) tt += stat[WPB + k];
-      const float rstd = rsqrtf(tt / C + 1e-5f);
+      const float rstd = rsqrtf(block_sum(qq, stat + WPB) / C + 1e-5f);
       const float4 gv = __ldcg(reinterpret_cast<const float4*>(gate + c0));
       const float4 sc = *reinterpret_cast<const float4*>(L.ln_scale + c0);
       gnow.x = (gv.x - mean) * rstd * sc.x; gnow.y = (gv.y - mean) * rstd * sc.y;
@@ -1384,11 +1350,76 @@ static __device__ void sgu_phase(const progen_decode_run_t& r, const SguArgs& L,
 }
 
 // ------------------------------------------------------------------------------------------------ sampler (one sequence per CTA)
+// Block reductions of the samplers: every thread gets the result.  red: [WPB] floats, then [WPB] ints at red + 32; the
+// barrier in front lets the caller reuse `red` right after it read the previous result.
+static __device__ __forceinline__ float bmax(float m, float* red) {
+  m = warp_max(m);
+  __syncthreads();
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = m;
+  __syncthreads();
+  m = red[0];
+#pragma unroll
+  for (int k = 1; k < WPB; ++k) m = fmaxf(m, red[k]);
+  return m;
+}
+static __device__ __forceinline__ float bsum(float v, float* red) {                 // fixed order: independent of the grid
+  v = warp_sum(v);
+  __syncthreads();
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  float s = 0.f;
+#pragma unroll
+  for (int k = 0; k < WPB; ++k) s += red[k];
+  return s;
+}
+// the first maximal index over the CTA of (bv, bi) (ties go to the lower index)
+static __device__ __forceinline__ int bargmax(float bv, int bi, float* red) {
+  int* redi = reinterpret_cast<int*>(red + 32);
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) {
+    const float ov = __shfl_xor_sync(0xffffffffu, bv, off);
+    const int oi = __shfl_xor_sync(0xffffffffu, bi, off);
+    if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
+  }
+  __syncthreads();
+  if ((threadIdx.x & 31) == 0) { red[threadIdx.x >> 5] = bv; redi[threadIdx.x >> 5] = bi; }
+  __syncthreads();
+  float fv = red[0];
+  int fi = redi[0];
+#pragma unroll
+  for (int k = 1; k < WPB; ++k) {
+    const float ov = red[k];
+    const int oi = redi[k];
+    if (ov > fv || (ov == fv && oi < fi)) { fv = ov; fi = oi; }
+  }
+  return fi;
+}
+// The k-th largest of sv[0 .. V) with multiplicity, by an O(V^2) rank count over shared memory.  The thread that finds it
+// writes red[48].  Where none does (NaN logits), red[48] keeps what the caller put there: sampler 1 seeds it with -inf
+// under constraints; otherwise (sampler 0 always) it is whatever the scratch last held, i.e. undefined.
+static __device__ __forceinline__ float kth_largest(const float* sv, int V, int k, float* red) {
+  for (int c = threadIdx.x; c < V; c += TPB) {
+    const float v = sv[c];
+    int gt = 0, ge = 0;
+#pragma unroll 8
+    for (int j = 0; j < V; ++j) { const float u = sv[j]; gt += u > v; ge += u >= v; }
+    if (gt < k && k <= ge) red[48] = v;
+  }
+  __syncthreads();
+  return red[48];
+}
+static __device__ __forceinline__ int clamp_id(int id, int V) { return id < 0 ? 0 : (id >= V ? V - 1 : id); }
+// x[b] = the embedding row of token id (clamped into the vocabulary), by the whole CTA
+static __device__ __forceinline__ void embed_row(float* x, const float* embed, int b, int id, int V, int d) {
+  id = clamp_id(id, V);
+  for (int c = threadIdx.x * 4; c < d; c += TPB * 4)
+    *reinterpret_cast<float4*>(x + (long long)b * d + c) = *reinterpret_cast<const float4*>(embed + (long long)id * d + c);
+}
+
 // utils.py:97-129: top-k filter keeps logits > (k-th largest), the rest become 0.0 and lose their noise; argmax(logits +
 // gumbel) (first maximal index); seq[pos + 1] += index (ADD, quirk Q5).  Then the next position's embedding row.
 static __device__ void sample_phase(const progen_decode_run_t& r, int pos, float* sv /* smem [V] */, float* red) {
-  const int t = threadIdx.x, V = r.V, lane = t & 31, warp = t >> 5;
-  int* redi = reinterpret_cast<int*>(red + 32);
+  const int t = threadIdx.x, V = r.V;
   for (int b = blockIdx.x; b < r.B; b += gridDim.x) {
     __syncthreads();
     const float* lg = r.logits + (long long)b * V;
@@ -1407,19 +1438,8 @@ static __device__ void sample_phase(const progen_decode_run_t& r, int pos, float
     }
     if (draw) {
       __syncthreads();
-      float kth = -INFINITY;
-      if (r.top_k > 0) {
-        for (int c = t; c < V; c += TPB) {
-          const float v = sv[c];
-          int gt = 0, ge = 0;
-#pragma unroll 8
-          for (int j = 0; j < V; ++j) { const float u = sv[j]; gt += u > v; ge += u >= v; }
-          if (gt < r.top_k && r.top_k <= ge) red[0] = v;                       // the k-th largest value (with multiplicity)
-        }
-        __syncthreads();
-        kth = red[0];
-      }
-      // first maximal index of (kept logit + noise | 0.0): thread-strided scan, then warp / block arg-max with index ties
+      const float kth = r.top_k > 0 ? kth_largest(sv, V, r.top_k, red) : -INFINITY;
+      // first maximal index of (kept logit + noise | 0.0): thread-strided scan, then the block arg-max
       float bv = -INFINITY;
       int bi = 0x7fffffff;
       for (int c = t; c < V; c += TPB) {
@@ -1429,30 +1449,11 @@ static __device__ void sample_phase(const progen_decode_run_t& r, int pos, float
         const float x = keep ? v + nz : 0.f;
         if (x > bv) { bv = x; bi = c; }                                        // ascending c: keeps the first maximum
       }
-#pragma unroll
-      for (int off = 16; off > 0; off >>= 1) {
-        const float ov = __shfl_xor_sync(0xffffffffu, bv, off);
-        const int oi = __shfl_xor_sync(0xffffffffu, bi, off);
-        if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
-      }
-      __syncthreads();                                                          // red[0] (kth) has been read by everyone
-      if (lane == 0) { red[1 + warp] = bv; redi[warp] = bi; }
-      __syncthreads();
-      float fv = red[1];
-      int fi = redi[0];
-#pragma unroll
-      for (int k = 1; k < WPB; ++k) {
-        const float ov = red[1 + k];
-        const int oi = redi[k];
-        if (ov > fv || (ov == fv && oi < fi)) { fv = ov; fi = oi; }
-      }
-      tok += fi;
+      tok += bargmax(bv, bi, red);
       if (t == 0) r.seq[(long long)b * r.n + pos + 1] = tok;
     }
     // the next position's embedding row (its token is final now), so the next step starts at layer 0 without a phase
-    const int id = tok < 0 ? 0 : (tok >= V ? V - 1 : tok);
-    for (int c = t * 4; c < r.d; c += TPB * 4)
-      *reinterpret_cast<float4*>(r.x + (long long)b * r.d + c) = *reinterpret_cast<const float4*>(r.embed + (long long)id * r.d + c);
+    embed_row(r.x, r.embed, b, tok, V, r.d);
   }
 }
 
@@ -1506,50 +1507,10 @@ static __device__ __noinline__ void sample_std_phase(const float* logits, int32_
                                                      SA... slot) {
   static_assert(TPB >= 256, "V <= 512: at most two ids per thread");
   static_assert(sizeof...(SA) == (SLOT ? 1 : 0), "one SlotArgs with SLOT");
-  const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  const int t = threadIdx.x;
   float* qv = sv + V;                                                          // kept ids: q; removed: -1
   int* redi = reinterpret_cast<int*>(red + 32);
   const bool cons = cs.bias != nullptr || cs.theta != 1.f || cs.min_new != 0 || cs.pbias != nullptr;  // uniform
-  auto bmax = [&](float m) {
-    m = warp_max(m);
-    __syncthreads();
-    if (lane == 0) red[warp] = m;
-    __syncthreads();
-    m = red[0];
-#pragma unroll
-    for (int k = 1; k < WPB; ++k) m = fmaxf(m, red[k]);
-    return m;
-  };
-  auto bsum = [&](float v) {                                                   // fixed order: independent of the grid
-    v = warp_sum(v);
-    __syncthreads();
-    if (lane == 0) red[warp] = v;
-    __syncthreads();
-    float s = 0.f;
-#pragma unroll
-    for (int k = 0; k < WPB; ++k) s += red[k];
-    return s;
-  };
-  auto bargmax = [&](float bv, int bi) {                                       // first maximal index
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) {
-      const float ov = __shfl_xor_sync(0xffffffffu, bv, off);
-      const int oi = __shfl_xor_sync(0xffffffffu, bi, off);
-      if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
-    }
-    __syncthreads();
-    if (lane == 0) { red[warp] = bv; redi[warp] = bi; }
-    __syncthreads();
-    float fv = red[0];
-    int fi = redi[0];
-#pragma unroll
-    for (int k = 1; k < WPB; ++k) {
-      const float ov = red[k];
-      const int oi = redi[k];
-      if (ov > fv || (ov == fv && oi < fi)) { fv = ov; fi = oi; }
-    }
-    return fi;
-  };
   const SlotArgs S = slot_args(slot...);
   // queue: slot b retires its row (counted in `done`), then claims the next row of the queue, q = next_row++.  A claimed
   // row starts at position 0: the slot's token-shift slot 0 of every layer (the only state read at position 0 before it
@@ -1568,8 +1529,7 @@ static __device__ __noinline__ void sample_std_phase(const float* logits, int32_
         for (int c = t; c < (d >> 1); c += TPB) { s1[c] = 0.f; s2[c] = 0.f; }
       }
     }
-    int id = got ? seq[(long long)q * n] : 0;
-    id = id < 0 ? 0 : (id >= V ? V - 1 : id);
+    const int id = clamp_id(got ? seq[(long long)q * n] : 0, V);
     for (int c = t * 4; c < d; c += TPB * 4)
       *reinterpret_cast<float4*>(x + (long long)b * d + c) = *reinterpret_cast<const float4*>(embed + (long long)id * d + c);
   };
@@ -1604,10 +1564,10 @@ static __device__ __noinline__ void sample_std_phase(const float* logits, int32_
       __syncthreads();
       float m = -INFINITY;
       for (int c = t; c < V; c += TPB) m = fmaxf(m, sv[c]);
-      m = bmax(m);
+      m = bmax(m, red);
       float s = 0.f;
       for (int c = t; c < V; c += TPB) s += expf(sv[c] - m);
-      const float lse = m + logf(bsum(s));
+      const float lse = m + logf(bsum(s, red));
       if (cons) {
         // presence flags of the ids at positions max(1, p + 1 - W) .. p, in the q half (filled only after this)
         int* seen = reinterpret_cast<int*>(qv);
@@ -1638,7 +1598,7 @@ static __device__ __noinline__ void sample_std_phase(const float* logits, int32_
           ma = fmaxf(ma, a);
         }
         if (t == 0) red[48] = -INFINITY;                                        // top-k over fewer candidates than k: keep all
-        m = bmax(ma);                                                           // the candidates' maximum (NaN skipped)
+        m = bmax(ma, red);                                                      // the candidates' maximum (NaN skipped)
       }
       int id;
       // a temperature so small that max / T overflows (e.g. 1e-39, subnormal) is the T -> 0 limit: the greedy draw
@@ -1646,24 +1606,13 @@ static __device__ __noinline__ void sample_std_phase(const float* logits, int32_
         float bv = -INFINITY;
         int bi = 0x7fffffff;
         for (int c = t; c < V; c += TPB) if (sv[c] > bv) { bv = sv[c]; bi = c; }
-        id = bargmax(bv, bi);
+        id = bargmax(bv, bi, red);
       } else {
-        float kth = -INFINITY;
-        if (top_k > 0 && top_k < V) {
-          for (int c = t; c < V; c += TPB) {
-            const float v = sv[c];
-            int gt = 0, ge = 0;
-#pragma unroll 8
-            for (int j = 0; j < V; ++j) { const float u = sv[j]; gt += u > v; ge += u >= v; }
-            if (gt < top_k && top_k <= ge) red[48] = v;                        // the k-th largest value (with multiplicity)
-          }
-          __syncthreads();
-          kth = red[48];
-        }
+        const float kth = top_k > 0 && top_k < V ? kth_largest(sv, V, top_k, red) : -INFINITY;
         const float mt = m / temp;                                              // the row maximum is always kept
         float z = 0.f;
         for (int c = t; c < V; c += TPB) if (sv[c] >= kth) z += expf(sv[c] / temp - mt);
-        z = bsum(z);
+        z = bsum(z, red);
         for (int c = t; c < V; c += TPB) qv[c] = sv[c] >= kth ? expf(sv[c] / temp - mt) / z : -1.f;
         __syncthreads();
         if (top_p < 1.f) {
@@ -1695,7 +1644,7 @@ static __device__ __noinline__ void sample_std_phase(const float* logits, int32_
           const float sc = sv[c] / temp + philox_gumbel(seed, sid, pos + 1, c);
           if (sc > bv) { bv = sc; bi = c; }
         }
-        id = bargmax(bv, bi);
+        id = bargmax(bv, bi, red);
       }
       if (id >= V) id = 0;                                                      // no candidate compared (NaN logits): EOS
       tok = id;
@@ -1711,7 +1660,7 @@ static __device__ __noinline__ void sample_std_phase(const float* logits, int32_
         if (t == 0) S.slot_pos[b] = pos + 1;
       }
     }
-    const int id = tok < 0 ? 0 : (tok >= V ? V - 1 : tok);
+    const int id = clamp_id(tok, V);
     for (int c = t * 4; c < d; c += TPB * 4)
       *reinterpret_cast<float4*>(x + (long long)b * d + c) = *reinterpret_cast<const float4*>(embed + (long long)id * d + c);
   }
@@ -1862,7 +1811,7 @@ static __device__ __forceinline__ void run(const progen_decode_run_t& r) {
         int id;
         if constexpr (SLOT) id = s_row[b] < 0 ? 0 : r.seq[(long long)s_row[b] * r.n + s_pos[b]];
         else id = r.seq[(long long)b * r.n + pos];
-        id = id < 0 ? 0 : (id >= r.V ? r.V - 1 : id);
+        id = clamp_id(id, r.V);
         *reinterpret_cast<float4*>(r.x + (long long)b * d + c) = *reinterpret_cast<const float4*>(r.embed + (long long)id * d + c);
       }
       grid_sync(r.grid_bar, round, pf);
@@ -1897,15 +1846,13 @@ static __device__ __forceinline__ void run(const progen_decode_run_t& r) {
         have = fetch_next = !(e == nph - 2 && step + 1 == r.nsteps);
       } else if (kind == K_ATT) {
         if (MERGE_IN_ATT || !att_consumer) {
-          if constexpr (SLOT) attention_batch<PLAN, true>(r, tab[e].ph.kcache, tab[e].ph.vcache, pos, red, (const int*)s_pos);
-          else attention_batch<PLAN, false>(r, tab[e].ph.kcache, tab[e].ph.vcache, pos, red);
+          attention_batch<PLAN, SLOT>(r, tab[e].ph.kcache, tab[e].ph.vcache, pos, red, s_pos);
         } else {
           attention_phase(r, tab[e].ph.kcache, tab[e].ph.vcache, pos, red);
         }
       } else if (kind == K_SGU) {
         const SguArgs sa{tab[e].ph.ln_scale, reinterpret_cast<const float*>(tab[e].ph.wt), tab[e].ph.bias, tab[e].ph.kcache};
-        if constexpr (SLOT) sgu_phase<PLAN, true>(r, sa, pos, red, (const int*)s_pos);
-        else sgu_phase<PLAN, false>(r, sa, pos, red);
+        sgu_phase<PLAN, SLOT>(r, sa, pos, red, s_pos);
       } else if constexpr (SLOT) {
         sample_std_phase<true>(r.logits, r.seq, r.start, r.end, r.n_ended, r.token_logp, r.logits_all, r.embed, r.x, r.sample_id, r.n, r.V,
                                d, B, r.top_k, r.temperature, r.top_p, r.seed,
