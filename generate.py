@@ -26,7 +26,7 @@ import click
 import numpy as np
 
 from progen_b200 import ProGen
-from progen_b200.checkpoint import get_checkpoint_fns
+from progen_b200.checkpoint import get_checkpoint_fns, package_params
 from progen_b200.data import decode_tokens, encode_tokens
 from progen_b200.lib import ProgenError
 
@@ -104,7 +104,7 @@ def main(checkpoint_path, prompts, prompts_file, num_samples, temperature, top_k
     last_checkpoint = get_last_checkpoint()
     if last_checkpoint is None:
         exit(f'no checkpoints found at {checkpoint_path}')
-    params = last_checkpoint['params']
+    params = package_params(last_checkpoint)             # plain params, or base + merged adapters
     model_kwargs = last_checkpoint['model_config']
     model = ProGen(**{**model_kwargs, 'mixed_precision': mixed_precision})
     bias = None if alphabet is None else alphabet_bias(alphabet, model.config['num_tokens'])

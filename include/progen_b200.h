@@ -70,6 +70,16 @@ typedef struct progen_gemm_t {
   const float* rot_cos;
   float* colsum;          /* EPI_GLU_BWD / EPI_GELU_BWD, nullable: colsum[c] += sum over rows of the stored out[., c]
                              (the pre-activation Linear's bias gradient; 16-byte aligned on the TC backend) */
+  /* Optional tail operand pair (K2 = 0: none): the accumulator is A*B^T + A2*B2^T, with A2(m,k) / B2(n,k) for k < K2
+   * addressed like A / B through lda2 / ldb2 and their own major flags, before the unchanged epilogue.  The tail's
+   * k-blocks run after the K loop of (A, B), in order, as if [A | A2] and [B | B2] were one operand pair (the TC backend
+   * zero-fills the tail's last k-block).  This is a low-rank adapter's x*A*B folded into its projection's GEMM.  TC:
+   * K2 % 8 == 0, a2/b2 major flags equal to a/b's, 16-byte aligned A2 / B2 and lda2 / ldb2 % 8 == 0.  Refused with a
+   * tail: split_k > 1, causal, batch > 1, batch_reduce and EPI_ACCUM. */
+  int64_t lda2, ldb2;
+  const void* A2;
+  const void* B2;
+  int32_t K2, a2_mn_major, b2_mn_major, _pad_tail;
 } progen_gemm_t;
 
 int progen_gemm(const progen_gemm_t* desc, void* stream);
@@ -83,7 +93,7 @@ int progen_embed_bwd(const int* tokens, const float* dx, float* dtable, long lon
  * Saves mean / rstd per row for the backward pass. */
 int progen_ln_shift_fwd(const void* x, long long ldx, int x_dtype, const float* scale, void* y, long long ldy, int y_dtype,
                         float* mean, float* rstd, long long T, int d, int seq_len, int shift, void* stream);
-/* backward of the above; residual=1 accumulates into the fp32 residual gradient `dres` [T,d] and mirrors it to `dout`;
+/* backward of the above (dscale nullable: a frozen scale); residual=1 accumulates into the fp32 residual gradient `dres` [T,d] and mirrors it to `dout`;
  * `dres_colsum` (nullable, residual only) += column sums of the updated dres = the bias gradient of the Linear that
  * produced this residual branch's input (saves a separate pass over dres). */
 int progen_ln_shift_bwd(const void* dy, long long lddy, int act_dtype, const void* x, long long ldx, int x_dtype,
@@ -144,7 +154,7 @@ int progen_local_attn_bwd_tc(const void* qkv, const void* out, const void* dout,
                              const float* rot_sin, const float* rot_cos, int B, int seq_len, int window, int heads, int dim_head,
                              void* stream);
 
-/* SGU gating — progen.py:182-184: out = xs * (Gp + spatial_biases[m]) and its backward (dxs, dGp, dbias) */
+/* SGU gating — progen.py:182-184: out = xs * (Gp + spatial_biases[m]) and its backward (dxs, dGp, dbias; dbias nullable) */
 int progen_sgu_gate_fwd(const void* xs, long long ldx, const void* gp, long long ldg, const float* bias, void* out,
                         long long ldo, int dtype, long long T, int C, int seq_len, void* stream);
 int progen_sgu_gate_bwd(const void* ds, long long ldds, const void* xs, long long ldx, const void* gp, long long ldg,
@@ -153,6 +163,9 @@ int progen_sgu_gate_bwd(const void* ds, long long ldds, const void* xs, long lon
 /* da *= gelu'(u) (tanh-approximate GELU, jax.nn.gelu default — progen.py:143) */
 int progen_gelu_bwd(void* da, const void* u, int dtype, long long numel, void* stream);
 int progen_cast_f32(const float* in, void* out, int out_dtype, long long numel, void* stream);
+/* out = scale * in, cast to out_dtype (in == out allowed for PROGEN_F32): the scaled compute copy s*B of a low-rank adapter
+ * and the scale of its gradient.  numel % 4 == 0, 16-byte aligned buffers. */
+int progen_scale_cast_f32(const float* in, void* out, int out_dtype, float scale, long long numel, void* stream);
 /* out = tril(spatial_weights) in the act dtype — the mask of progen.py:178-179 applied once per parameter update */
 int progen_tril_cast(const float* w, void* out, int out_dtype, int n, void* stream);
 

@@ -51,6 +51,9 @@ int progen_gemm(const progen_gemm_t* d, void* stream) {
   g.epi.seq_len = d->seq_len > 0 ? d->seq_len : 1; g.epi.dim_head = d->dim_head > 0 ? d->dim_head : 2;
   g.epi.atomic = d->atomic; g.epi.tril = d->tril; g.epi.tril_rows = d->tril_rows > 0 ? d->tril_rows : 1;
   g.epi.colsum = d->colsum;
+  g.K2 = d->K2;
+  g.A2 = d->A2; g.lda2 = d->lda2; g.a2_mn_major = d->a2_mn_major;
+  g.B2 = d->B2; g.ldb2 = d->ldb2; g.b2_mn_major = d->b2_mn_major;
   PG_CHECK_ARG(g.epi_kind >= 0 && g.epi_kind < EPI_NUM_KINDS);
   PG_CHECK_ARG(g.epi.out != nullptr);
   PG_CHECK_ARG(!g.epi.colsum || g.epi_kind == EPI_GLU_BWD || g.epi_kind == EPI_GELU_BWD);

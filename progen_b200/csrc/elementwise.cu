@@ -241,22 +241,25 @@ __global__ void ln_shift_bwd_kernel(const TO* __restrict__ dy, long long lddy, c
       }
     }
   }
-  // dscale: reduce the 8 warps of the block through shared memory (128 columns at a time), one atomic per column per block
+  // dscale (nullable: a frozen scale): reduce the 8 warps of the block through shared memory (128 columns at a time),
+  // one atomic per column per block
   __shared__ float red[ROWS_PER_BLOCK][128];
 #pragma unroll
   for (int ch = 0; ch < NCH; ++ch) {
     if (ch * 128 >= d) break;
+    if (dscale) {                              // block-uniform
 #pragma unroll
-    for (int i = 0; i < 4; ++i) red[warp][lane * 4 + i] = ds_acc[ch][i];
-    __syncthreads();
-    if (threadIdx.x < 128) {
-      float s = 0.f;
+      for (int i = 0; i < 4; ++i) red[warp][lane * 4 + i] = ds_acc[ch][i];
+      __syncthreads();
+      if (threadIdx.x < 128) {
+        float s = 0.f;
 #pragma unroll
-      for (int w = 0; w < ROWS_PER_BLOCK; ++w) s += red[w][threadIdx.x];
-      const int c = ch * 128 + threadIdx.x;
-      if (c < d) atomicAdd(dscale + c, s);
+        for (int w = 0; w < ROWS_PER_BLOCK; ++w) s += red[w][threadIdx.x];
+        const int c = ch * 128 + threadIdx.x;
+        if (c < d) atomicAdd(dscale + c, s);
+      }
+      __syncthreads();
     }
-    __syncthreads();
     if constexpr (RESIDUAL) {
       if (dres_colsum) {                       // block-uniform
 #pragma unroll
@@ -612,7 +615,7 @@ __global__ void sgu_gate_bwd_kernel(const TO* __restrict__ ds, long long ldds, c
       store4(dgp + t * lddg + c, o2);
     }
     acc = warp_sum(acc);
-    if (lane == 0) atomicAdd(dbias + m, acc);
+    if (lane == 0 && dbias) atomicAdd(dbias + m, acc);      // dbias nullable: frozen spatial biases
   }
 }
 
@@ -635,6 +638,18 @@ __global__ void cast_kernel(const float* __restrict__ in, TO* __restrict__ out, 
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total4; i += (long long)gridDim.x * blockDim.x) {
     float v[4];
     load4<float>(in + i * 4, v);
+    store4(out + i * 4, v);
+  }
+}
+
+// out = scale * in: a low-rank adapter's scaled compute copy (s B) and its scaled gradient (in place for fp32)
+template <typename TO>
+__global__ void scale_cast_kernel(const float* in, TO* out, float scale, long long total4) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total4; i += (long long)gridDim.x * blockDim.x) {
+    float v[4];
+    load4<float>(in + i * 4, v);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) v[j] *= scale;
     store4(out + i * 4, v);
   }
 }
@@ -903,6 +918,16 @@ int progen_cast_f32(const float* in, void* out, int out_dtype, long long numel, 
   const int grid = ew_grid(numel / 4, 256);
   if (out_dtype == PG_F32) cast_kernel<float><<<grid, 256, 0, s>>>(in, (float*)out, numel / 4);
   else cast_kernel<bf16><<<grid, 256, 0, s>>>(in, (bf16*)out, numel / 4);
+  PG_LAUNCH_CHECK();
+  return PROGEN_OK;
+}
+
+int progen_scale_cast_f32(const float* in, void* out, int out_dtype, float scale, long long numel, void* stream) {
+  PG_CHECK_ARG(numel > 0 && numel % 4 == 0 && in != nullptr && out != nullptr);
+  cudaStream_t s = (cudaStream_t)stream;
+  const int grid = ew_grid(numel / 4, 256);
+  if (out_dtype == PG_F32) scale_cast_kernel<float><<<grid, 256, 0, s>>>(in, (float*)out, scale, numel / 4);
+  else scale_cast_kernel<bf16><<<grid, 256, 0, s>>>(in, (bf16*)out, scale, numel / 4);
   PG_LAUNCH_CHECK();
   return PROGEN_OK;
 }

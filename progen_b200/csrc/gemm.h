@@ -20,7 +20,21 @@ struct GemmArgs {
   int out_dtype;    // PG_F32 | PG_BF16 (ignored by EPI_RESIDUAL / EPI_ACCUM which are fp32)
   int epi_kind;
   EpiArgs epi;
+  // tail operand pair (K2 = 0: none): acc += A2[M,K2] * B2[N,K2]^T after the K loop of (A, B), same addressing rules
+  const void* A2; long long lda2; int a2_mn_major;
+  const void* B2; long long ldb2; int b2_mn_major;
+  int K2;
 };
+
+// the tail's refusals, shared by both backends
+#define PG_CHECK_TAIL(a)                                                                                               \
+  do {                                                                                                                 \
+    PG_CHECK_ARG((a).K2 >= 0);                                                                                         \
+    if ((a).K2 > 0) {                                                                                                  \
+      PG_CHECK_ARG((a).A2 != nullptr && (a).B2 != nullptr);                                                            \
+      PG_CHECK_ARG((a).split_k == 1 && !(a).causal && (a).batch == 1 && !(a).batch_reduce && (a).epi_kind != EPI_ACCUM); \
+    }                                                                                                                  \
+  } while (0)
 
 int gemm_tc_launch(const GemmArgs& g, cudaStream_t stream);
 int gemm_simt_launch(const GemmArgs& g, cudaStream_t stream);

@@ -56,12 +56,15 @@ struct GemmDev {
   long long d_batch_rows;
   int causal, split_k;
   EpiArgs epi;
+  int K2;                              // tail operand pair: k-blocks of (A2, B2) after those of (A, B)
 };
 
 struct TileInfo {
   int z, m0, n0, kb_begin, kb_end;
+  int kb_main;                         // TAIL: k-blocks kb_main .. kb_end - 1 are the tail's
 };
 
+template <bool TAIL>
 __device__ __forceinline__ void decode_tile(const GemmDev& g, int t, TileInfo& ti) {
   const int m_tiles = (g.M + BM - 1) / BM;
   const int n_tiles = (g.N + BN - 1) / BN;
@@ -83,11 +86,16 @@ __device__ __forceinline__ void decode_tile(const GemmDev& g, int t, TileInfo& t
   }
   ti.kb_begin = b;
   ti.kb_end = e;
+  if constexpr (TAIL) {                // no split / causal / batch with a tail: (b, e) = (0, kb_total)
+    ti.kb_main = e;
+    ti.kb_end = e + (g.K2 + BK - 1) / BK;
+  }
 }
 
-template <bool A_MN, bool B_MN, int KIND, typename TO>
+template <bool A_MN, bool B_MN, int KIND, typename TO, bool TAIL>
 __global__ void __launch_bounds__(THREADS, 1)
-gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b, const GemmDev g,
+gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,
+               const __grid_constant__ CUtensorMap tma_a2, const __grid_constant__ CUtensorMap tma_b2, const GemmDev g,
                const int tiles) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_u32 = smem_u32(smem_raw);
@@ -101,6 +109,10 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
   if (threadIdx.x == 0) {
     prefetch_tensormap(&tma_a);
     prefetch_tensormap(&tma_b);
+    if constexpr (TAIL) {
+      prefetch_tensormap(&tma_a2);
+      prefetch_tensormap(&tma_b2);
+    }
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full_bar(s), 1);
       mbar_init(empty_bar(s), 1);                 // released by the one consumer warpgroup that read the stage
@@ -125,7 +137,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
     if (threadIdx.x == 0) {
       for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
         TileInfo ti;
-        decode_tile(g, t, ti);
+        decode_tile<TAIL>(g, t, ti);
         const int a_row0 = ti.z * g.a_batch_rows;
         const int b_row0 = ti.z * g.b_batch_rows;
         for (int kb = ti.kb_begin; kb < ti.kb_end; ++kb) {
@@ -133,6 +145,24 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
           const uint32_t sa = smem_base + stage * STAGE_BYTES;
           const uint32_t sb = sa + A_BYTES;
           mbar_expect_tx(full_bar(stage), STAGE_BYTES);
+          if (TAIL && kb >= ti.kb_main) {
+            // the tail pair (batch 1: row offset 0); TMA zero-fills the k-block beyond K2
+            const int k0 = (kb - ti.kb_main) * BK;
+            if constexpr (!A_MN) {
+              tma_load_2d(sa, &tma_a2, full_bar(stage), k0, ti.m0);
+            } else {
+#pragma unroll
+              for (int i = 0; i < BM / 64; ++i) tma_load_2d(sa + i * 8192, &tma_a2, full_bar(stage), ti.m0 + 64 * i, k0);
+            }
+            if constexpr (!B_MN) {
+              tma_load_2d(sb, &tma_b2, full_bar(stage), k0, ti.n0);
+            } else {
+#pragma unroll
+              for (int i = 0; i < BN / 64; ++i) tma_load_2d(sb + i * 8192, &tma_b2, full_bar(stage), ti.n0 + 64 * i, k0);
+            }
+            advance(1);
+            continue;
+          }
           const int k0 = kb * BK;
           if constexpr (!A_MN) {
             tma_load_2d(sa, &tma_a, full_bar(stage), k0, a_row0 + ti.m0);                   // box {64 k, 128 m}
@@ -162,7 +192,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
   float* cs = reinterpret_cast<float*>(smem_raw + (cs_base - raw_u32)) + c * (CS_BYTES / 4);
   for (int p = 0, t = blockIdx.x; t < tiles; ++p, t += gridDim.x) {
     TileInfo ti;
-    decode_tile(g, t, ti);
+    decode_tile<TAIL>(g, t, ti);
     if ((p & 1) != c) {
       advance(ti.kb_end - ti.kb_begin);
       continue;
@@ -357,15 +387,16 @@ int get_tensor_map(const void* ptr, uint64_t inner, uint64_t outer, uint64_t row
 }
 
 
-template <bool A_MN, bool B_MN, int KIND, typename TO>
-int launch_inst(const CUtensorMap& ta, const CUtensorMap& tb, const GemmDev& gd, int tiles, cudaStream_t stream) {
-  auto kern = gemm_tc_kernel<A_MN, B_MN, KIND, TO>;
+template <bool A_MN, bool B_MN, int KIND, typename TO, bool TAIL>
+int launch_inst(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& ta2, const CUtensorMap& tb2,
+                const GemmDev& gd, int tiles, cudaStream_t stream) {
+  auto kern = gemm_tc_kernel<A_MN, B_MN, KIND, TO, TAIL>;
   static bool attr_set = false;
   if (!attr_set) {
     PG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL));
     attr_set = true;
   }
-  kern<<<std::min(tiles, pg_num_sms()), THREADS, SMEM_TOTAL, stream>>>(ta, tb, gd, tiles);
+  kern<<<std::min(tiles, pg_num_sms()), THREADS, SMEM_TOTAL, stream>>>(ta, tb, ta2, tb2, gd, tiles);
   PG_LAUNCH_CHECK();
   return PROGEN_OK;
 }
@@ -381,7 +412,7 @@ int pg_tensor_map_2d_bf16(const void* ptr, uint64_t inner, uint64_t outer, uint6
 int gemm_tc_launch(const GemmArgs& a, cudaStream_t stream) {
   PG_CHECK_ARG(a.in_dtype == PG_BF16);
   PG_CHECK_ARG(a.M > 0 && a.N > 0 && a.K > 0 && a.batch >= 1 && a.split_k >= 1);
-  PG_CHECK_ARG(a.N % 32 == 0);
+  PG_CHECK_ARG(a.N % 8 == 0);                        // 8-column epilogue items (an adapter's rank can be 8 .. 64)
   PG_CHECK_ARG(a.K % BK == 0);                       // TMA would zero-fill a K tail, but batched operands must not bleed
   PG_CHECK_ARG(a.lda % 8 == 0 && a.ldb % 8 == 0);    // 16-byte global strides for TMA
   PG_CHECK_ARG((reinterpret_cast<uintptr_t>(a.A) & 15) == 0 && (reinterpret_cast<uintptr_t>(a.B) & 15) == 0);
@@ -389,6 +420,13 @@ int gemm_tc_launch(const GemmArgs& a, cudaStream_t stream) {
   if (a.epi_kind == EPI_ROTARY) PG_CHECK_ARG(a.epi.seq_len % 32 == 0);
   PG_CHECK_ARG((reinterpret_cast<uintptr_t>(a.epi.colsum) & 15) == 0);    // red.global.add.v4
   PG_CHECK_ARG(!(a.split_k > 1 || a.batch_reduce) || (a.epi_kind == EPI_ACCUM && a.epi.atomic));
+  PG_CHECK_TAIL(a);
+  const bool tail = a.K2 > 0;
+  if (tail) {
+    PG_CHECK_ARG(a.K2 % 8 == 0 && a.lda2 % 8 == 0 && a.ldb2 % 8 == 0);
+    PG_CHECK_ARG(a.a2_mn_major == a.a_mn_major && a.b2_mn_major == a.b_mn_major);
+    PG_CHECK_ARG((reinterpret_cast<uintptr_t>(a.A2) & 15) == 0 && (reinterpret_cast<uintptr_t>(a.B2) & 15) == 0);
+  }
 
   // stored 2D extents of each operand
   const uint64_t a_rows = (a.batch > 1 && a.a_batch_rows > 0) ? (uint64_t)a.a_batch_rows * a.batch
@@ -403,6 +441,15 @@ int gemm_tc_launch(const GemmArgs& a, cudaStream_t stream) {
   if (!a.b_mn_major) rc = get_tensor_map(a.B, a.K, b_rows, a.ldb, BK, BN, &tb);
   else               rc = get_tensor_map(a.B, a.N, b_rows, a.ldb, 64, BK, &tb);
   if (rc) return rc;
+  CUtensorMap ta2 = ta, tb2 = tb;            // unused without a tail
+  if (tail) {
+    if (!a.a_mn_major) rc = get_tensor_map(a.A2, a.K2, a.M, a.lda2, BK, BM, &ta2);
+    else               rc = get_tensor_map(a.A2, a.M, a.K2, a.lda2, 64, BK, &ta2);
+    if (rc) return rc;
+    if (!a.b_mn_major) rc = get_tensor_map(a.B2, a.K2, a.N, a.ldb2, BK, BN, &tb2);
+    else               rc = get_tensor_map(a.B2, a.N, a.K2, a.ldb2, 64, BK, &tb2);
+    if (rc) return rc;
+  }
 
   GemmDev gd;
   gd.M = a.M; gd.N = a.N; gd.K = a.K;
@@ -410,12 +457,15 @@ int gemm_tc_launch(const GemmArgs& a, cudaStream_t stream) {
   gd.a_batch_rows = (int)a.a_batch_rows; gd.b_batch_rows = (int)a.b_batch_rows; gd.d_batch_rows = a.d_batch_rows;
   gd.causal = a.causal; gd.split_k = a.split_k;
   gd.epi = a.epi;
+  gd.K2 = a.K2;
   const long long tiles = (long long)a.batch * a.split_k * ((a.M + BM - 1) / BM) * ((a.N + BN - 1) / BN);
   PG_CHECK_ARG(tiles < (1ll << 31));
 
   const int am = a.a_mn_major ? 1 : 0, bm = a.b_mn_major ? 1 : 0;
   const bool obf = a.out_dtype == PG_BF16;
-#define TC_CASE(AM, BMJ, KIND, TO) return launch_inst<AM, BMJ, KIND, TO>(ta, tb, gd, (int)tiles, stream)
+#define TC_CASE(AM, BMJ, KIND, TO)                                                                       \
+  return tail ? launch_inst<AM, BMJ, KIND, TO, true>(ta, tb, ta2, tb2, gd, (int)tiles, stream)            \
+              : launch_inst<AM, BMJ, KIND, TO, false>(ta, tb, ta2, tb2, gd, (int)tiles, stream)
   switch (a.epi_kind) {
     case EPI_STORE:
       if (!am && bm) { if (obf) TC_CASE(false, true, EPI_STORE, bf16); else TC_CASE(false, true, EPI_STORE, float); }
@@ -441,8 +491,9 @@ int gemm_tc_launch(const GemmArgs& a, cudaStream_t stream) {
       if (!am && !bm && obf) TC_CASE(false, false, EPI_GELU_BWD, bf16);
       break;
     case EPI_ACCUM:
-      if (am && bm) TC_CASE(true, true, EPI_ACCUM, float);
-      if (!am && !bm) TC_CASE(false, false, EPI_ACCUM, float);
+      // weight gradients take no tail (PG_CHECK_TAIL)
+      if (am && bm) return launch_inst<true, true, EPI_ACCUM, float, false>(ta, tb, ta2, tb2, gd, (int)tiles, stream);
+      if (!am && !bm) return launch_inst<false, false, EPI_ACCUM, float, false>(ta, tb, ta2, tb2, gd, (int)tiles, stream);
       break;
     default: break;
   }

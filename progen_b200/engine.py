@@ -188,6 +188,7 @@ class Engine:
         self.loss = torch.zeros(1, device=self.dev)       # exists before the first batch: a rank without rows still reports 0
         self.loaded_token = None
         self.on_layer_grads = None        # optional callback(layer_index) fired when a layer's weight gradients are final
+        self.lora = None                  # lora.Adapters: the training set runs the adapted model with a frozen base
         self.lib = L.load()
         self.num_sms = torch.cuda.get_device_properties(self.dev).multi_processor_count
 
@@ -231,7 +232,14 @@ class Engine:
         return self.export_tree(self.params)
 
     def export_grads(self):
-        return self.export_tree(self.grads)
+        return self.export_tree(self.base_grads())
+
+    def base_grads(self):
+        """the flat fp32 gradient of every parameter; released while adapters train (a LoRA Trainer) and allocated
+        again, zeroed, by the next full-gradient path"""
+        if self.grads is None:
+            self.grads = torch.zeros(self.n_params_padded, device=self.dev, dtype=torch.float32)
+        return self.grads
 
     def refresh_compute_copies(self):
         """bf16 mirror of all parameters + tril-masked SGU matrices; call after every parameter change."""
@@ -255,7 +263,7 @@ class Engine:
         return self.seg(self.params, module, name)
 
     def G(self, module, name):
-        return self.seg(self.grads, module, name)
+        return self.seg(self.base_grads(), module, name)
 
     # ------------------------------------------------------------------------------------------ workspaces
     def ensure_batch(self, B):
@@ -341,6 +349,27 @@ class Engine:
     def _mm(self, **kw):
         L.gemm(backend=self.backend, in_dtype=self.act_dt, **kw)
 
+    def lora_fwd(self, x, K, module, N):
+        """adapters: u = x A of projection `module` (input x [T, K], N outputs) -> the tail (u, s B) of its GEMM"""
+        lo = self.lora
+        if lo is None:
+            return {}
+        u = lo.u[module]
+        self.fwd_gemm(x, K, lo.seg(lo.lp, module, 'lora_a'), lo.r, u)
+        return dict(A2=u, lda2=lo.r, B2=lo.seg(lo.lp, module, 'lora_b'), ldb2=N, K2=lo.r)
+
+    def lora_bwd(self, x, K, module, dy, N):
+        """adapters: from the projection's output gradient dy [T, N], g' = s g = dy (s B)^T, dB += u^T dy (scaled by s
+        after the backward pass), dA += x^T g' -> the tail (g', A^T) of its input-gradient GEMM"""
+        lo = self.lora
+        if lo is None:
+            return {}
+        g, A = lo.g, lo.seg(lo.lp, module, 'lora_a')
+        self.dgrad_gemm(dy, N, lo.seg(lo.lp, module, 'lora_b'), lo.r, g)
+        self.wgrad_gemm(lo.u[module], lo.r, dy, N, lo.seg(lo.grads, module, 'lora_b'))
+        self.wgrad_gemm(x, K, g, lo.r, lo.seg(lo.grads, module, 'lora_a'))
+        return dict(A2=g, lda2=lo.r, B2=A, ldb2=lo.r, K2=lo.r)
+
     def fwd_gemm(self, x, K, w, N, out, epi=L.EPI_STORE, out_dtype=None, acts=None, **kw):
         """out[T,N] = x[T,K] @ w[K,N]  (w stored (in, out) like hk.Linear: MN-major B operand); T from `acts` (default:
         the training set)"""
@@ -408,6 +437,10 @@ class Engine:
         if T != acts.B * n:
             raise L.ProgenError(f'forward: {T} token rows are not {acts.B} rows of length {n}')
         shift = cfg['shift_tokens']
+        lo = self.lora if acts is self.acts else None       # adapters run on the training set only
+        if lo is not None:
+            lo.activations(T)
+        tail = self.lora_fwd if lo is not None else (lambda *a: {})
         L.check(lib.progen_embed_fwd(acts.tok.data_ptr(), self.Pf(P + 'embed', 'embeddings').data_ptr(), acts.X[0].data_ptr(),
                                      T, d, self.V, st), 'embed_fwd')
         for i, kind in enumerate(self.kinds):
@@ -418,24 +451,24 @@ class Engine:
             # ---- LocalAttention (progen.py:73-103)
             self.ln_fwd(x0, d, self.Pf(a + 'layer_norm', 'scale'), s['y1'], d, s['mean1'], s['rstd1'], d, shift, acts=acts, seq_len=n)
             self.fwd_gemm(s['y1'], d, self.W(a + 'linear', 'w'), 3 * I, s['qkv'], epi=L.EPI_ROTARY, rot_sin=self.rot_sin,
-                          rot_cos=self.rot_cos, seq_len=n, dim_head=self.dh, acts=acts)
+                          rot_cos=self.rot_cos, seq_len=n, dim_head=self.dh, acts=acts, **tail(s['y1'], d, a + 'linear', 3 * I))
             if sink is not None:
                 sink(i, 'qkv', s['qkv'])
                 sink(i, 'y1', s['y1'])
             self.attn_fwd(s['qkv'], s['att'], s['lse'], acts=acts, seq_len=n)
             self.fwd_gemm(s['att'], I, self.W(a + 'linear_1', 'w'), d, x1, epi=L.EPI_RESIDUAL, bias=self.Pf(a + 'linear_1', 'b'),
-                          aux=None if acts.inplace else x0, ldaux=d, acts=acts)
+                          aux=None if acts.inplace else x0, ldaux=d, acts=acts, **tail(s['att'], I, a + 'linear_1', d))
             # ---- FeedForward (progen.py:131-149); s['u'] is None in the inference set: no pre-activation store
             self.ln_fwd(x1, d, self.Pf(f + 'layer_norm', 'scale'), s['y2'], d, s['mean2'], s['rstd2'], d, shift, acts=acts, seq_len=n)
             if sink is not None:
                 sink(i, 'y2', s['y2'])
             if kind == 'glu':
                 self.fwd_gemm(s['y2'], d, self.W(f + 'linear', 'w'), 2 * hid, s['hact'], epi=L.EPI_GLU, ldo=hid, out2=s['u'],
-                              ldo2=2 * hid, bias=self.Pf(f + 'linear', 'b'), acts=acts)
+                              ldo2=2 * hid, bias=self.Pf(f + 'linear', 'b'), acts=acts, **tail(s['y2'], d, f + 'linear', 2 * hid))
                 last, last_k = s['hact'], hid
             else:
                 self.fwd_gemm(s['y2'], d, self.W(f + 'linear', 'w'), hid, s['hact'], epi=L.EPI_GELU, out2=s['u'], ldo2=hid,
-                              bias=self.Pf(f + 'linear', 'b'), acts=acts)
+                              bias=self.Pf(f + 'linear', 'b'), acts=acts, **tail(s['y2'], d, f + 'linear', hid))
                 last, last_k = s['hact'], hid
             if kind == 'sgu':
                 half = hid // 2
@@ -455,7 +488,7 @@ class Engine:
                               acts=acts)
                 last, last_k = s['pj'], half
             self.fwd_gemm(last, last_k, self.W(f + 'linear_1', 'w'), d, x2, epi=L.EPI_RESIDUAL, bias=self.Pf(f + 'linear_1', 'b'),
-                          aux=None if acts.inplace else x1, ldaux=d, acts=acts)
+                          aux=None if acts.inplace else x1, ldaux=d, acts=acts, **tail(last, last_k, f + 'linear_1', d))
         if sink is not None:
             return
         # ---- to_logits (progen.py:219-222)
@@ -571,12 +604,23 @@ class Engine:
         self._forward_device()
         lib, st = self.lib, L.stream()
         self.loss.zero_()
+        self._check_zero_grads(zero_grads)
         if zero_grads:
-            self.grads.zero_()
+            self.train_grads().zero_()
         L.check(lib.progen_ce_fwd_bwd(self.logits.data_ptr(), L.F32, self.labels.data_ptr(), self.ce_w.data_ptr(),
                                       self.loss.data_ptr(), self.dlogits.data_ptr(), self.act_dt, self.B, self.n, self.V,
                                       1.0 / global_batch, st), 'ce_fwd_bwd')
         self._backward_device()
+
+    def _check_zero_grads(self, zero_grads):
+        if not zero_grads and self.lora is not None:
+            # the backward pass ends by scaling the whole B gradient by s (Adapters.scale_b_grads): an accumulated one
+            # would be scaled twice
+            raise L.ProgenError('adapters: gradients cannot accumulate across steps (zero_grads=False)')
+
+    def train_grads(self):
+        """the flat gradient buffer a training step writes: the adapters' with adapters (the base is frozen)"""
+        return self.base_grads() if self.lora is None else self.lora.grads
 
     def load_preference(self, rows, ref):
         """rows (2P, n+1): the chosen rows, then their rejected rows; ref [2P] float32: the reference log-likelihoods in
@@ -592,9 +636,10 @@ class Engine:
         (s(chosen), s(rejected), z, loss)."""
         if 2 * pairs != self.B:
             raise L.ProgenError(f'preference step: {pairs} pairs need {2 * pairs} resident rows, have {self.B}')
+        self._check_zero_grads(zero_grads)
         self._forward_device()
         if zero_grads:
-            self.grads.zero_()
+            self.train_grads().zero_()
         L.check(self.lib.progen_preference_head(self.logits.data_ptr(), L.F32, self.labels.data_ptr(), self.ref.data_ptr(),
                                                 self.logp.data_ptr(), self.seq_ll.data_ptr(), self.seq_count.data_ptr(),
                                                 self.ce_w.data_ptr(), self.stats.data_ptr(), self.loss.data_ptr(),
@@ -613,22 +658,29 @@ class Engine:
         the bias gradient of the block that is differentiated next (its output bias sees exactly this dres)."""
         L.check(self.lib.progen_ln_shift_bwd(dy.data_ptr(), self.d, self.act_dt, x.data_ptr(), self.d, L.F32, scale.data_ptr(),
                                              mean.data_ptr(), rstd.data_ptr(), self.dres.data_ptr(),
-                                             self.dres_lp.data_ptr() if self.mp else 0, self.d, dscale.data_ptr(),
+                                             self.dres_lp.data_ptr() if self.mp else 0, self.d, L.ptr(dscale),
                                              L.ptr(next_bias_grad), self.T, self.d, self.n, int(shift), 1, L.stream()), 'ln_bwd')
 
     def _backward_device(self):
+        """With adapters (self.lora) the base is frozen: no base weight, bias, LayerNorm-scale, SGU or embedding
+        gradient is computed, and every adapted projection's input gradient carries its adapter's tail (lora_bwd)."""
         lib, st = self.lib, L.stream()
         cfg, d, I, hid, T, n = self.cfg, self.d, self.I, self.hid, self.T, self.n
         shift = cfg['shift_tokens']
+        lo = self.lora
+        frozen = lo is not None
+        G = (lambda module, name: None) if frozen else self.G
+        tail = self.lora_bwd if frozen else (lambda *a: {})
         # ---- head
         hw, hl = P + 'linear', P + 'layer_norm'
-        self.colsum(self.dlogits, self.V, self.G(hw, 'b'))
-        self.wgrad_gemm(self.yf, d, self.dlogits, self.V, self.G(hw, 'w'))
+        if not frozen:
+            self.colsum(self.dlogits, self.V, self.G(hw, 'b'))
+            self.wgrad_gemm(self.yf, d, self.dlogits, self.V, self.G(hw, 'w'))
         self.dgrad_gemm(self.dlogits, self.V, self.W(hw, 'w'), d, self.dy)
         self.dres.zero_()
         nl = len(self.kinds)
-        self.ln_bwd_res(self.dy, self.X[-1], self.Pf(hl, 'scale'), self.meanf, self.rstdf, self.G(hl, 'scale'), False,
-                        next_bias_grad=self.G(P + f'ff{nl - 1}/~/linear_1', 'b'))
+        self.ln_bwd_res(self.dy, self.X[-1], self.Pf(hl, 'scale'), self.meanf, self.rstdf, G(hl, 'scale'), False,
+                        next_bias_grad=G(P + f'ff{nl - 1}/~/linear_1', 'b'))
         for i in reversed(range(len(self.kinds))):
             kind, s = self.kinds[i], self.lay[i]
             a, f = P + f'attn{i}/~/', P + f'ff{i}/~/'
@@ -638,20 +690,23 @@ class Engine:
             if kind == 'sgu':
                 half = hid // 2
                 g = f + 'sgu'
-                self.wgrad_gemm(s['pj'], half, dres_lp, d, self.G(f + 'linear_1', 'w'))
-                self.dgrad_gemm(dres_lp, d, self.W(f + 'linear_1', 'w'), half, self.dpj)
-                self.colsum(self.dpj, half, self.G(g + '/~/linear', 'b'))
-                self.wgrad_gemm(s['sg'], half, self.dpj, half, self.G(g + '/~/linear', 'w'))
+                if not frozen:
+                    self.wgrad_gemm(s['pj'], half, dres_lp, d, self.G(f + 'linear_1', 'w'))
+                self.dgrad_gemm(dres_lp, d, self.W(f + 'linear_1', 'w'), half, self.dpj, **tail(s['pj'], half, f + 'linear_1', dres_lp, d))
+                if not frozen:
+                    self.colsum(self.dpj, half, self.G(g + '/~/linear', 'b'))
+                    self.wgrad_gemm(s['sg'], half, self.dpj, half, self.G(g + '/~/linear', 'w'))
                 self.dgrad_gemm(self.dpj, half, self.W(g + '/~/linear', 'w'), half, self.dsg)
                 da = self.dh_                                            # gradient wrt gelu output a = [xs | gate], [T, hid]
                 L.check(lib.progen_sgu_gate_bwd(self.dsg.data_ptr(), half, s['hact'].data_ptr(), hid, s['gp'].data_ptr(), half,
                                                 self.Pf(g, 'spatial_biases').data_ptr(), da.data_ptr(), hid, self.dgp.data_ptr(),
-                                                half, self.G(g, 'spatial_biases').data_ptr(), self.act_dt, T, half, n, st),
+                                                half, L.ptr(G(g, 'spatial_biases')), self.act_dt, T, half, n, st),
                         'sgu_gate_bwd')
-                # d spatial_weights = tril(sum_b dGp_b @ gn_b^T)
-                self._mm(M=n, N=n, K=half, A=self.dgp, lda=half, B=s['gn'], ldb=half, out=self.G(g, 'spatial_weights'), ldo=n,
-                         epi=L.EPI_ACCUM, out_dtype=L.F32, batch=self.B, a_batch_rows=n, b_batch_rows=n, batch_reduce=True,
-                         atomic=True, tril=True, tril_rows=n)
+                if not frozen:
+                    # d spatial_weights = tril(sum_b dGp_b @ gn_b^T)
+                    self._mm(M=n, N=n, K=half, A=self.dgp, lda=half, B=s['gn'], ldb=half, out=self.G(g, 'spatial_weights'), ldo=n,
+                             epi=L.EPI_ACCUM, out_dtype=L.F32, batch=self.B, a_batch_rows=n, b_batch_rows=n, batch_reduce=True,
+                             atomic=True, tril=True, tril_rows=n)
                 # d gn_b = tril(W)^T @ dGp_b
                 self._mm(M=n, N=half, K=n, A=self.wm[i], lda=n, a_mn=True, B=self.dgp, ldb=half, b_mn=True, out=self.dgn,
                          ldo=half, out_dtype=self.act_dt, batch=self.B, b_batch_rows=n, d_batch_rows=n, causal=2)
@@ -659,39 +714,49 @@ class Engine:
                 L.check(lib.progen_ln_shift_bwd(self.dgn.data_ptr(), half, self.act_dt, gate.data_ptr(), hid, self.act_dt,
                                                 self.Pf(g + '/~/layer_norm', 'scale').data_ptr(), s['mean3'].data_ptr(),
                                                 s['rstd3'].data_ptr(), 0, da[:, half:].data_ptr(), hid,
-                                                self.G(g + '/~/layer_norm', 'scale').data_ptr(), 0, T, half, n, 0, 0, st), 'ln_bwd_sgu')
+                                                L.ptr(G(g + '/~/layer_norm', 'scale')), 0, T, half, n, 0, 0, st), 'ln_bwd_sgu')
                 L.check(lib.progen_gelu_bwd(da.data_ptr(), s['u'].data_ptr(), self.act_dt, T * hid, st), 'gelu_bwd')
                 du, n_in = da, hid
-                self.colsum(du, n_in, self.G(f + 'linear', 'b'))
+                if not frozen:
+                    self.colsum(du, n_in, self.G(f + 'linear', 'b'))
             elif kind == 'glu':
                 # the epilogue also adds the column sums of du into the proj_in bias gradient (interleaved like du)
-                self.wgrad_gemm(s['hact'], hid, dres_lp, d, self.G(f + 'linear_1', 'w'))
+                if not frozen:
+                    self.wgrad_gemm(s['hact'], hid, dres_lp, d, self.G(f + 'linear_1', 'w'))
                 self.dgrad_gemm(dres_lp, d, self.W(f + 'linear_1', 'w'), hid, self.du, epi=L.EPI_GLU_BWD, ldo=2 * hid,
-                                aux=s['u'], ldaux=2 * hid, colsum=self.G(f + 'linear', 'b'))
+                                aux=s['u'], ldaux=2 * hid, colsum=G(f + 'linear', 'b'),
+                                **tail(s['hact'], hid, f + 'linear_1', dres_lp, d))
                 du, n_in = self.du, 2 * hid
             else:
-                self.wgrad_gemm(s['hact'], hid, dres_lp, d, self.G(f + 'linear_1', 'w'))
+                if not frozen:
+                    self.wgrad_gemm(s['hact'], hid, dres_lp, d, self.G(f + 'linear_1', 'w'))
                 self.dgrad_gemm(dres_lp, d, self.W(f + 'linear_1', 'w'), hid, self.dh_, epi=L.EPI_GELU_BWD, aux=s['u'], ldaux=hid,
-                                colsum=self.G(f + 'linear', 'b'))
+                                colsum=G(f + 'linear', 'b'), **tail(s['hact'], hid, f + 'linear_1', dres_lp, d))
                 du, n_in = self.dh_, hid
-            self.wgrad_gemm(s['y2'], d, du, n_in, self.G(f + 'linear', 'w'))
-            self.dgrad_gemm(du, n_in, self.W(f + 'linear', 'w'), d, self.dy)
-            self.ln_bwd_res(self.dy, x1, self.Pf(f + 'layer_norm', 'scale'), s['mean2'], s['rstd2'], self.G(f + 'layer_norm', 'scale'), shift,
-                            next_bias_grad=self.G(a + 'linear_1', 'b'))
+            if not frozen:
+                self.wgrad_gemm(s['y2'], d, du, n_in, self.G(f + 'linear', 'w'))
+            self.dgrad_gemm(du, n_in, self.W(f + 'linear', 'w'), d, self.dy, **tail(s['y2'], d, f + 'linear', du, n_in))
+            self.ln_bwd_res(self.dy, x1, self.Pf(f + 'layer_norm', 'scale'), s['mean2'], s['rstd2'], G(f + 'layer_norm', 'scale'), shift,
+                            next_bias_grad=G(a + 'linear_1', 'b'))
             # ---- LocalAttention backward
-            self.wgrad_gemm(s['att'], I, dres_lp, d, self.G(a + 'linear_1', 'w'))
-            self.dgrad_gemm(dres_lp, d, self.W(a + 'linear_1', 'w'), I, self.datt)
+            if not frozen:
+                self.wgrad_gemm(s['att'], I, dres_lp, d, self.G(a + 'linear_1', 'w'))
+            self.dgrad_gemm(dres_lp, d, self.W(a + 'linear_1', 'w'), I, self.datt, **tail(s['att'], I, a + 'linear_1', dres_lp, d))
             self.attn_bwd(s['qkv'], s['att'], self.datt, s['lse'], self.dqkv)
             if not self.attn_tc:
                 L.check(lib.progen_rotary_bwd(self.dqkv.data_ptr(), 3 * I, self.act_dt, self.rot_sin.data_ptr(),
                                               self.rot_cos.data_ptr(), T, 3 * I, n, self.dh, st), 'rotary_bwd')
-            self.wgrad_gemm(s['y1'], d, self.dqkv, 3 * I, self.G(a + 'linear', 'w'))
-            self.dgrad_gemm(self.dqkv, 3 * I, self.W(a + 'linear', 'w'), d, self.dy)
-            self.ln_bwd_res(self.dy, x0, self.Pf(a + 'layer_norm', 'scale'), s['mean1'], s['rstd1'], self.G(a + 'layer_norm', 'scale'), shift,
-                            next_bias_grad=self.G(P + f'ff{i - 1}/~/linear_1', 'b') if i > 0 else None)
+            if not frozen:
+                self.wgrad_gemm(s['y1'], d, self.dqkv, 3 * I, self.G(a + 'linear', 'w'))
+            self.dgrad_gemm(self.dqkv, 3 * I, self.W(a + 'linear', 'w'), d, self.dy, **tail(s['y1'], d, a + 'linear', self.dqkv, 3 * I))
+            self.ln_bwd_res(self.dy, x0, self.Pf(a + 'layer_norm', 'scale'), s['mean1'], s['rstd1'], G(a + 'layer_norm', 'scale'), shift,
+                            next_bias_grad=G(P + f'ff{i - 1}/~/linear_1', 'b') if i > 0 else None)
             if self.on_layer_grads is not None:
                 # every weight-matrix gradient of layer i is final: the DDP trainer starts its all-reduce here so the
                 # transfer overlaps the backward pass of layers i-1 .. 0
                 self.on_layer_grads(i)
+        if frozen:
+            lo.scale_b_grads()
+            return
         L.check(lib.progen_embed_bwd(self.tok.data_ptr(), self.dres.data_ptr(), self.G(P + 'embed', 'embeddings').data_ptr(),
                                      T, d, self.V, st), 'embed_bwd')

@@ -33,6 +33,8 @@ class GemmDesc(C.Structure):
         ('A', C.c_void_p), ('B', C.c_void_p), ('out', C.c_void_p), ('out2', C.c_void_p),
         ('bias', C.c_void_p), ('aux', C.c_void_p), ('rot_sin', C.c_void_p), ('rot_cos', C.c_void_p),
         ('colsum', C.c_void_p),
+        ('lda2', C.c_int64), ('ldb2', C.c_int64), ('A2', C.c_void_p), ('B2', C.c_void_p),
+        ('K2', C.c_int32), ('a2_mn_major', C.c_int32), ('b2_mn_major', C.c_int32), ('_pad_tail', C.c_int32),
     ]
 
 
@@ -65,6 +67,7 @@ PROTOTYPES = {
     'progen_sgu_gate_bwd': [_P, _LL, _P, _LL, _P, _LL, _P, _P, _LL, _P, _LL, _P, _I, _LL, _I, _I, _P],
     'progen_gelu_bwd': [_P, _P, _I, _LL, _P],
     'progen_cast_f32': [_P, _P, _I, _LL, _P],
+    'progen_scale_cast_f32': [_P, _P, _I, _F, _LL, _P],
     'progen_tril_cast': [_P, _P, _I, _I, _P],
     'progen_decode_run': [_P, _P],
     'progen_gather_rows_f32': [_P, _LL, _I, _I, _LL, _P, _I, _I, _I, _I, _I, _I, _P, _LL, _LL, _LL, _P],
@@ -127,8 +130,9 @@ def stream():
 def gemm(*, M, N, K, A, lda, B, ldb, out, ldo, epi=EPI_STORE, backend, a_mn=False, b_mn=False, in_dtype, out_dtype=F32,
          batch=1, a_batch_rows=0, b_batch_rows=0, d_batch_rows=0, batch_reduce=False, causal=0, split_k=1,
          out2=None, ldo2=0, bias=None, aux=None, ldaux=0, rot_sin=None, rot_cos=None, seq_len=0, dim_head=0,
-         atomic=False, tril=False, tril_rows=0, colsum=None):
-    """Thin wrapper over progen_gemm; tensors are passed as torch tensors (or raw ints for sub-views)."""
+         atomic=False, tril=False, tril_rows=0, colsum=None, A2=None, lda2=0, a2_mn=None, B2=None, ldb2=0, b2_mn=None, K2=0):
+    """Thin wrapper over progen_gemm; tensors are passed as torch tensors (or raw ints for sub-views).  The tail pair
+    (A2, B2, K2 > 0) takes the major flags of (A, B) unless a2_mn / b2_mn say otherwise."""
     d = GemmDesc()
     d.M, d.N, d.K = M, N, K
     d.a_mn_major, d.b_mn_major = int(a_mn), int(b_mn)
@@ -143,4 +147,8 @@ def gemm(*, M, N, K, A, lda, B, ldb, out, ldo, epi=EPI_STORE, backend, a_mn=Fals
     d.A, d.B, d.out, d.out2 = as_ptr(A), as_ptr(B), as_ptr(out), as_ptr(out2)
     d.bias, d.aux, d.rot_sin, d.rot_cos = as_ptr(bias), as_ptr(aux), as_ptr(rot_sin), as_ptr(rot_cos)
     d.colsum = as_ptr(colsum)
+    if K2:
+        d.K2, d.lda2, d.ldb2, d.A2, d.B2 = K2, lda2, ldb2, as_ptr(A2), as_ptr(B2)
+        d.a2_mn_major = int(a_mn if a2_mn is None else a2_mn)
+        d.b2_mn_major = int(b_mn if b2_mn is None else b2_mn)
     check(load().progen_gemm(C.byref(d), stream()), 'progen_gemm')

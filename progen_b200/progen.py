@@ -269,6 +269,7 @@ class ProGen:
         return out
 
     def _ensure_loaded(self, params):
+        self.engine.lora = None                  # every path but the adapted training step runs the plain model
         if self._loaded is not params:
             self.engine.load_params(params)
             self._loaded = params
@@ -287,12 +288,49 @@ class ProGen:
 
     __call__ = apply
 
-    def loss_and_grad(self, params, data):
+    def loss_and_grad(self, params, data, *, adapters=None, lora_alpha=None):
         """Fused `loss, grads = value_and_grad(batched_loss_fn)(params, key, data)` (utils.py:61-76).
-        data: (B, n+1) integers.  Returns (python float loss, haiku-shaped dict of numpy fp32 gradients)."""
+        data: (B, n+1) integers.  Returns (python float loss, haiku-shaped dict of numpy fp32 gradients).
+        With `adapters` (a tree of `init_adapters`' shape; lora_alpha default: its rank) the loss is the adapted
+        model's, the base is frozen, and the gradients are the adapters' (a tree of the same shape)."""
         self._ensure_loaded(params)
+        if adapters is None:
+            loss = self.engine.loss_and_grad(data)
+            return float(loss.item()), self.engine.export_grads()
+        lo = self._attach_adapters(adapters, lora_alpha)
         loss = self.engine.loss_and_grad(data)
-        return float(loss.item()), self.engine.export_grads()
+        return float(loss.item()), lo.export_tree(lo.grads)
+
+    # ---- low-rank adapters (DESIGN.md §3.8)
+    def init_adapters(self, rng, rank, *, alpha=None):
+        """Initial low-rank adapters {module: {'lora_a': A [in, r], 'lora_b': B [r, out]}} on the QKV, attention output,
+        feed-forward in and feed-forward out projections of every layer (gMLP layers included): A ~
+        TruncatedNormal(1/sqrt(in)) from `rng` (an int seed or key-like array, as in `init`), B = 0, so the adapted model
+        starts as the base model.  rank: an integer multiple of 8 in [8, 64]; alpha (finite, > 0; default rank) is only
+        checked here: pass it as lora_alpha wherever the adapters are used, s = alpha / rank."""
+        from .lora import check_rank_alpha, init_adapters
+        rank, _ = check_rank_alpha(rank, alpha)
+        seed = int(np.asarray(rng).ravel()[-1]) if not isinstance(rng, (int, np.integer)) else int(rng)
+        return init_adapters(self.config, seed, rank)
+
+    def merge_adapters(self, params, adapters, *, lora_alpha=None):
+        """params with every adapted weight W replaced by W + s A B (s = lora_alpha / rank, default 1), computed on the
+        host in float64 and cast to float32.  `apply`, `score`, `generate` and the other inference paths run on it."""
+        from .lora import check_adapters, check_rank_alpha, merge_adapters
+        rank, alpha = check_rank_alpha(check_adapters(self.config, adapters), lora_alpha)
+        return merge_adapters(params, adapters, alpha / rank)
+
+    def _attach_adapters(self, adapters, lora_alpha):
+        """validate `adapters` and make them the engine's training-set adapters -> lora.Adapters"""
+        from .lora import Adapters, check_adapters, check_rank_alpha
+        rank, alpha = check_rank_alpha(check_adapters(self.config, adapters), lora_alpha)
+        eng = self.engine
+        lo = getattr(self, '_adapters', None)
+        if lo is None or lo.r != rank or lo.alpha != alpha:
+            lo = self._adapters = Adapters(eng, rank, alpha)
+        lo.load(adapters)
+        eng.lora = lo
+        return lo
 
     def preference_loss_and_grad(self, params, chosen, rejected, ref_chosen, ref_rejected, *, beta=0.1):
         """The preference (DPO, Rafailov et al. 2023) twin of `loss_and_grad`.  Pair i is (chosen[i], rejected[i]), each a
@@ -511,6 +549,8 @@ class ProGen:
             self._gen_decoder, self._gen_params = dec, params
         return dec
 
-    def trainer(self, params, **optim_kwargs):
+    def trainer(self, params, *, adapters=None, lora_alpha=None, **optim_kwargs):
+        """Device-resident training state over `params` (train.py's loop).  With `adapters` only the adapters train
+        (the base stays bitwise unchanged); lora_alpha as in `loss_and_grad`."""
         from .trainer import Trainer
-        return Trainer(self, params, **optim_kwargs)
+        return Trainer(self, params, adapters=adapters, lora_alpha=lora_alpha, **optim_kwargs)

@@ -1,6 +1,9 @@
 """Device-resident training state for the train.py loop: parameters, gradients, Adam moments and the apply_every
 accumulator live in flat fp32 buffers; one `step(data)` is one iteration of the reference's inner loop
-(train.py:186-190): loss+grads, optim.update, apply_updates."""
+(train.py:186-190): loss+grads, optim.update, apply_updates.
+
+With low-rank adapters (`adapters=`) the same state exists for the adapter buffer only: the base parameters are frozen
+and bitwise unchanged, and clip / AdamW / apply_every run over the adapters (weight decay on every A and B)."""
 import os
 
 import numpy as np
@@ -12,14 +15,29 @@ from . import parallel as PAR
 
 class Trainer:
     def __init__(self, model, params, learning_rate=2e-4, weight_decay=1e-3, max_grad_norm=0.5, grad_accum_every=4,
-                 b1=0.9, b2=0.999, eps=1e-8, optim_state=None, data_parallel=True, cuda_graph=False):
+                 b1=0.9, b2=0.999, eps=1e-8, optim_state=None, data_parallel=True, cuda_graph=False, adapters=None,
+                 lora_alpha=None):
         self.model = model
         self.eng = model.engine
         self.eng.load_params(params)
         model._loaded = None
+        self.lora = None
+        if adapters is not None:
+            from .lora import Adapters, check_adapters, check_rank_alpha
+            rank, alpha = check_rank_alpha(check_adapters(model.config, adapters), lora_alpha)
+            self.lora = Adapters(self.eng, rank, alpha)
+            self.lora.load(adapters)
+        # the flat buffers the optimizer owns: (parameters, size, ndim > 1 prefix, bf16 mirror or None); gradients: self.G
+        if self.lora is None:
+            e = self.eng
+            self.P, n, self.n_decay, self.P_lp = e.params, e.n_params_padded, e.n_decay, e.params_lp
+        else:
+            lo = self.lora
+            self.P, n, self.n_decay, self.P_lp = lo.params, lo.n_padded, lo.n_padded, None
+            self.eng.grads = None                  # nothing reads or writes the base gradient while adapters train
+        self.eng.lora = self.lora
         self.lr, self.wd, self.max_norm, self.every = learning_rate, weight_decay, max_grad_norm, grad_accum_every
         self.b1, self.b2, self.eps = b1, b2, eps
-        n = self.eng.n_params_padded
         z = lambda: torch.zeros(n, device=self.eng.dev, dtype=torch.float32)
         self.m, self.v, self.acc = z(), z(), z()
         self.count = 0
@@ -36,12 +54,20 @@ class Trainer:
         # NCCL kernels take SMs from the backward kernels and needs eager launches.  PROGEN_DDP_OVERLAP=1 selects that mode
         # (eager launches only) for models whose gradient is large enough to make the transfer itself matter.
         self.overlap = os.environ.get('PROGEN_DDP_OVERLAP', '0') == '1'
+        if self.overlap and self.lora is not None:
+            raise L.ProgenError('PROGEN_DDP_OVERLAP=1 does not support adapters: their gradient is one small buffer, '
+                                'all-reduced once per step')
         self.skip_allreduce = False                       # bench.py: "step without the exchange" for comm_exposed_ms
         if self.world > 1 and self.overlap:
             # overlap: a layer's weight gradients are all-reduced (async, NCCL's stream) as soon as its backward is done
             self.eng.on_layer_grads = self._reduce_layer
         if optim_state is not None:
             self.load_optim_state(optim_state)
+
+    @property
+    def G(self):
+        """the flat gradient the optimizer reads: the adapters', or every parameter's"""
+        return self.eng.base_grads() if self.lora is None else self.lora.grads
 
     # ---- one micro-step of train.py:186-190
     def step(self, data, sync_loss=False, global_batch=None):
@@ -51,9 +77,10 @@ class Trainer:
         (global mean when sync_loss)."""
         rows = data.shape[0]
         gb = int(global_batch) if global_batch is not None else (rows * self.world if self.world > 1 else rows)
+        self.eng.lora = self.lora
         if rows == 0:
             # a rank without rows (batch smaller than the world): zero contribution, but every collective is joined
-            self.eng.grads.zero_()
+            self.G.zero_()
             self.eng.loss.zero_()
             return self._update(sync_loss)
         self._drop_graph_unless(rows)
@@ -74,6 +101,7 @@ class Trainer:
     def step_resident(self, global_batch=None, sync_loss=False):
         """same, on tokens/labels already copied into engine.tok / engine.labels (bench: inputs resident in HBM)"""
         gb = global_batch or self.eng.B * self.world
+        self.eng.lora = self.lora
         self._drop_graph_unless(self.eng.B)
         if self._graph is not None and self._graph_key == (self.eng.B, gb):
             return self._replay(sync_loss)
@@ -97,6 +125,7 @@ class Trainer:
         if self.world > 1 and self.overlap:
             raise L.ProgenError('capture_graph: PROGEN_DDP_OVERLAP=1 launches its bucketed all-reduces eagerly')
         eng = self.eng
+        eng.lora = self.lora
         eng.ensure_batch(batch_rows)
         if self._adam_state is None:
             self._adam_state = torch.zeros(4, dtype=torch.int64, device=eng.dev)   # AdamDevState: count | bc1, bc2 | emit, pad
@@ -129,8 +158,9 @@ class Trainer:
                                           what='preference_step', allow_empty=True)
         P = rows.shape[0] // 2
         self._pref_pairs = P
+        self.eng.lora = self.lora
         if P == 0:
-            self.eng.grads.zero_()
+            self.G.zero_()
             self.eng.loss.zero_()
             return self._update(sync_loss)
         key = (2 * P, gp, 'preference', beta)
@@ -162,17 +192,24 @@ class Trainer:
         if self.overlap:
             self._finish_allreduce()
         else:
-            dist.all_reduce(self.eng.grads, op=dist.ReduceOp.SUM)
+            dist.all_reduce(self.G, op=dist.ReduceOp.SUM)
 
     def _update_captured(self):
         eng, lib, st = self.eng, L.load(), L.stream()
-        L.check(lib.progen_grad_sqnorm(eng.grads.data_ptr(), eng.n_params_padded, self.ws.data_ptr(), self.gnorm_sq.data_ptr(), st),
-                'grad_sqnorm')
-        L.check(lib.progen_adamw_step_dev(eng.params.data_ptr(), eng.params_lp.data_ptr() if eng.mp else 0, eng.grads.data_ptr(),
-                                          self.m.data_ptr(), self.v.data_ptr(), self.acc.data_ptr(), eng.n_params_padded,
-                                          eng.n_decay, self.gnorm_sq.data_ptr(), self.lr, self.b1, self.b2, self.eps, self.wd,
+        n = self.P.numel()
+        L.check(lib.progen_grad_sqnorm(self.G.data_ptr(), n, self.ws.data_ptr(), self.gnorm_sq.data_ptr(), st), 'grad_sqnorm')
+        L.check(lib.progen_adamw_step_dev(self.P.data_ptr(), L.ptr(self.P_lp), self.G.data_ptr(),
+                                          self.m.data_ptr(), self.v.data_ptr(), self.acc.data_ptr(), n,
+                                          self.n_decay, self.gnorm_sq.data_ptr(), self.lr, self.b1, self.b2, self.eps, self.wd,
                                           self.max_norm, self.every, self._adam_state.data_ptr(), st), 'adamw_step_dev')
-        eng.refresh_masked_copies()                        # every step (a no-op recompute between emits): keeps the graph static
+        self._refresh()                                    # every step (a no-op recompute between emits): keeps the graph static
+
+    def _refresh(self):
+        """the compute copies of what the optimizer changed"""
+        if self.lora is None:
+            self.eng.refresh_masked_copies()
+        else:
+            self.lora.refresh()
 
     def _drop_graph_unless(self, batch_rows):
         """a different batch size re-allocates the engine's activation buffers: the captured pointers would dangle"""
@@ -230,14 +267,14 @@ class Trainer:
         if self._adam_state is not None:
             self._adam_state[0] = self.count               # keep the device-side count in step with eager steps
         emit = int(self.count % self.every == 0)
-        L.check(lib.progen_grad_sqnorm(eng.grads.data_ptr(), eng.n_params_padded, self.ws.data_ptr(), self.gnorm_sq.data_ptr(), st),
-                'grad_sqnorm')
-        L.check(lib.progen_adamw_step(eng.params.data_ptr(), eng.params_lp.data_ptr() if eng.mp else 0, eng.grads.data_ptr(),
-                                      self.m.data_ptr(), self.v.data_ptr(), self.acc.data_ptr(), eng.n_params_padded, eng.n_decay,
+        n = self.P.numel()
+        L.check(lib.progen_grad_sqnorm(self.G.data_ptr(), n, self.ws.data_ptr(), self.gnorm_sq.data_ptr(), st), 'grad_sqnorm')
+        L.check(lib.progen_adamw_step(self.P.data_ptr(), L.ptr(self.P_lp), self.G.data_ptr(),
+                                      self.m.data_ptr(), self.v.data_ptr(), self.acc.data_ptr(), n, self.n_decay,
                                       self.gnorm_sq.data_ptr(), self.lr, self.b1, self.b2, self.eps, self.wd, self.max_norm,
                                       self.count, emit, st), 'adamw_step')
         if emit:
-            eng.refresh_masked_copies()
+            self._refresh()
         return eng.loss
 
     def evaluate(self, data):
@@ -245,6 +282,7 @@ class Trainer:
         eng = self.eng
         d = torch.as_tensor(np.asarray(data).astype(np.int32) if not isinstance(data, torch.Tensor) else data)
         self._drop_graph_unless(d.shape[0])
+        eng.lora = self.lora
         eng.ensure_batch(d.shape[0])
         dd = d.to(device=eng.dev, dtype=torch.int32)
         eng.tok.copy_(dd[:, :-1].reshape(-1))
@@ -257,15 +295,21 @@ class Trainer:
 
     # ---- checkpoint interchange (haiku-shaped trees, train.py:196-202)
     def params(self):
+        """the base parameters (with adapters: unchanged by training)"""
         return self.eng.export_params()
 
+    def adapters(self):
+        """the trained adapters, a tree of `ProGen.init_adapters`' shape (None without adapters)"""
+        return None if self.lora is None else self.lora.export_tree(self.lora.params)
+
     def optim_state(self):
-        e = self.eng
+        """{count, mu, nu, acc, every}: trees of the parameters (with adapters: of the adapters) the optimizer owns"""
+        e = self.eng if self.lora is None else self.lora
         return dict(count=self.count, mu=e.export_tree(self.m), nu=e.export_tree(self.v), acc=e.export_tree(self.acc),
                     every=self.every)
 
     def load_optim_state(self, st):
-        e = self.eng
+        e = self.eng if self.lora is None else self.lora
         if not (isinstance(st, dict) and {'count', 'mu', 'nu', 'acc'} <= set(st)):
             # e.g. an optax chain state from a reference checkpoint: only `params` interchange (checkpoint.py)
             import warnings
@@ -273,7 +317,7 @@ class Trainer:
             return
         self.count = int(st['count'])
         for buf, tree in ((self.m, st['mu']), (self.v, st['nu']), (self.acc, st['acc'])):
-            host = np.zeros(e.n_params_padded, np.float32)
+            host = np.zeros(self.P.numel(), np.float32)
             for s in e.specs:
                 a = np.asarray(tree[s.module][s.name], np.float32)
                 if s.interleave:

@@ -5,7 +5,7 @@ import click
 import numpy as np
 
 from progen_b200 import ProGen
-from progen_b200.checkpoint import get_checkpoint_fns
+from progen_b200.checkpoint import get_checkpoint_fns, package_params
 from progen_b200.data import decode_tokens, encode_tokens
 from progen_b200.utils import sample
 
@@ -22,7 +22,7 @@ def main(seed, checkpoint_path, prime, greedy, mixed_precision, no_kv_cache):
     last_checkpoint = get_last_checkpoint()
     if last_checkpoint is None:
         exit(f'no checkpoints found at {checkpoint_path}')
-    params = last_checkpoint['params']
+    params = package_params(last_checkpoint)             # plain params, or base + merged adapters
     num_seqs = max(last_checkpoint['next_seq_index'], 0)
     model_kwargs = last_checkpoint['model_config']
     model = ProGen(**{**model_kwargs, 'mixed_precision': mixed_precision})

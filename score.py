@@ -11,7 +11,7 @@ import click
 import numpy as np
 
 from progen_b200 import ProGen
-from progen_b200.checkpoint import get_checkpoint_fns
+from progen_b200.checkpoint import get_checkpoint_fns, package_params
 from progen_b200.data import collate
 
 
@@ -27,7 +27,7 @@ def main(checkpoint_path, input_path, output, embeddings, batch_size, mixed_prec
     last_checkpoint = get_last_checkpoint()
     if last_checkpoint is None:
         exit(f'no checkpoints found at {checkpoint_path}')
-    params = last_checkpoint['params']
+    params = package_params(last_checkpoint)             # plain params, or base + merged adapters
     model_kwargs = last_checkpoint['model_config']
     model = ProGen(**{**model_kwargs, 'mixed_precision': mixed_precision})
     seq_len = model_kwargs['seq_len']

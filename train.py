@@ -2,6 +2,12 @@
 H100 engine.  Additions: --synthetic (uniform-random tokens, the BASELINE workload), --num_steps, --text_file (one
 sequence per line, instead of TFRecords whose reader needs tensorflow).  Launch with torchrun for --data_parallel.
 
+Fine-tuning: --init_checkpoint DIR starts from the newest checkpoint there (its params and model_config).  With
+--lora_rank R (and --lora_alpha, default R) only low-rank adapters train on the frozen base; the checkpoints written
+are adapter packages that name the base checkpoint file instead of storing its parameters (checkpoint.py).  A resumed
+run keeps its mode and adapter settings: --lora_rank / --lora_alpha / --init_checkpoint that disagree with the
+checkpoint in --checkpoint_path are refused.
+
 The loop is the reference's (train.py:184-222): for each effective batch, grad_accum_every micro-steps of
 loss+grads -> optim.update -> apply_updates; checkpoint / validate / sample on the same cadence."""
 import os
@@ -15,7 +21,7 @@ import torch
 
 from progen_b200 import ProGen
 from progen_b200 import parallel as PAR
-from progen_b200.checkpoint import get_checkpoint_fns
+from progen_b200.checkpoint import count_params, get_checkpoint_fns, last_checkpoint_file, load_checkpoint_file
 from progen_b200.data import decode_tokens, iterator_from_sequences, iterator_from_tfrecords_folder, synthetic_iterator
 from progen_b200.utils import sample, confirm, exists
 
@@ -46,9 +52,13 @@ from progen_b200.utils import sample, confirm, exists
 @click.option('--text_file', default=None, help='one sequence per line (train); last 5%% of lines validate')
 @click.option('--num_steps', default=None, type=int, help='stop after this many effective batches')
 @click.option('--cuda_graph', default=False, is_flag=True, help='single GPU: capture the training step into a CUDA graph and replay it')
+@click.option('--init_checkpoint', default=None, help='fine-tune: start from the newest checkpoint in this directory')
+@click.option('--lora_rank', default=None, type=int, help='train low-rank adapters of this rank on the frozen --init_checkpoint')
+@click.option('--lora_alpha', default=None, type=float, help='adapter scale alpha (s = alpha / rank; default: the rank)')
 def main(seed, batch_size, grad_accum_every, learning_rate, weight_decay, data_parallel, max_grad_norm, validate_every,
          sample_every, checkpoint_every, checkpoint_path, checkpoint_keep_n, config_path, model_name, prime_length, seq_len,
-         mixed_precision, data_path, wandb_off, wandb_project_name, new, synthetic, text_file, num_steps, cuda_graph):
+         mixed_precision, data_path, wandb_off, wandb_project_name, new, synthetic, text_file, num_steps, cuda_graph,
+         init_checkpoint, lora_rank, lora_alpha):
     if data_parallel and 'RANK' in os.environ:
         import torch.distributed as dist
         torch.cuda.set_device(int(os.environ.get('LOCAL_RANK', '0')))
@@ -71,23 +81,64 @@ def main(seed, batch_size, grad_accum_every, learning_rate, weight_decay, data_p
         last_checkpoint = box[0]
     else:
         last_checkpoint = get_last_checkpoint()
-    if not exists(last_checkpoint):
+    lora = exists(last_checkpoint) and 'adapters' in last_checkpoint
+    base_file = None
+    # a resumed run keeps its own mode and adapter settings: flags that would change them are refused, not ignored
+    if lora:
+        base_file = last_checkpoint['base_checkpoint']          # resume an adapter run: its base, its adapters
+        got = last_checkpoint['lora']
+        if lora_rank is not None and lora_rank != got['rank']:
+            raise click.UsageError(f"--lora_rank {lora_rank}: {checkpoint_path} holds adapters of rank {got['rank']}")
+        if lora_alpha is not None and float(lora_alpha) != float(got['alpha']):
+            raise click.UsageError(f"--lora_alpha {lora_alpha}: {checkpoint_path} holds adapters with alpha {got['alpha']}")
+        if init_checkpoint is not None and last_checkpoint_file(init_checkpoint) != base_file:
+            raise click.UsageError(f'--init_checkpoint {init_checkpoint}: its newest checkpoint is not {base_file}, the base '
+                                   f'of the adapters in {checkpoint_path}')
+    elif exists(last_checkpoint):
+        if lora_rank is not None or lora_alpha is not None:
+            raise click.UsageError(f'--lora_rank / --lora_alpha: {checkpoint_path} holds a full-parameter checkpoint; '
+                                   f'train adapters into another --checkpoint_path')
+    elif lora_alpha is not None and lora_rank is None:
+        raise click.UsageError('--lora_alpha needs --lora_rank')
+    elif not exists(last_checkpoint) and lora_rank is not None and init_checkpoint is None:
+        raise click.UsageError('--lora_rank needs --init_checkpoint (the base the adapters are trained on)')
+    elif not exists(last_checkpoint) and init_checkpoint is not None:
+        base_file = last_checkpoint_file(init_checkpoint)
+        assert base_file is not None, f'no checkpoint found in --init_checkpoint {init_checkpoint}'
+        lora = lora_rank is not None
+    base = load_checkpoint_file(base_file) if base_file is not None else None
+    if exists(last_checkpoint):
+        model_kwargs = last_checkpoint['model_config']          # resume: config comes from the checkpoint (train.py:99-100)
+    elif base is not None:
+        model_kwargs = base['model_config']
+    else:
         cfg_file = Path(config_path) / f'{model_name}.toml'
         assert cfg_file.exists(), f'path to your model config {str(cfg_file)} does not exist'
         model_kwargs = toml.loads(cfg_file.read_text())
-    else:
-        model_kwargs = last_checkpoint['model_config']          # resume: config comes from the checkpoint (train.py:99-100)
 
     model = ProGen(**{**model_kwargs, 'mixed_precision': mixed_precision})
-    if exists(last_checkpoint):
+    adapters, lora_cfg = None, None
+    if lora and exists(last_checkpoint):
+        params = base['params']
+        assert count_params(params) == last_checkpoint['num_params'], f'base checkpoint {base_file} has changed'
+        adapters, lora_cfg = last_checkpoint['adapters'], last_checkpoint['lora']
+        optim_state, start_seq_index = last_checkpoint['optim_state'], last_checkpoint['next_seq_index']
+    elif exists(last_checkpoint):
         params, optim_state, start_seq_index = last_checkpoint['params'], last_checkpoint['optim_state'], last_checkpoint['next_seq_index']
+    elif base is not None:
+        params, optim_state, start_seq_index = base['params'], None, 0
+        if lora:
+            adapters = model.init_adapters(seed, lora_rank, alpha=lora_alpha)
+            lora_cfg = dict(rank=lora_rank, alpha=float(lora_rank if lora_alpha is None else lora_alpha))
     else:
         params, optim_state, start_seq_index = model.init(seed), None, 0
     trainer = model.trainer(params, learning_rate=learning_rate, weight_decay=weight_decay, max_grad_norm=max_grad_norm,
                             grad_accum_every=grad_accum_every, optim_state=optim_state, data_parallel=data_parallel,
-                            cuda_graph=cuda_graph)
+                            cuda_graph=cuda_graph, adapters=adapters, lora_alpha=None if lora_cfg is None else lora_cfg['alpha'])
     seq_len = model_kwargs['seq_len']                           # the --seq_len flag is dead in the reference too (train.py:137)
     num_params = model.engine.num_params
+    if rank == 0 and lora:
+        print(f"adapters: rank {lora_cfg['rank']}, alpha {lora_cfg['alpha']}, {trainer.lora.num_params} parameters on base {base_file}")
 
     if synthetic:
         total_train_seqs = 10 ** 9
@@ -130,8 +181,12 @@ def main(seed, batch_size, grad_accum_every, learning_rate, weight_decay, data_p
         if rank == 0:
             print(f'loss: {loss.item()}')
         if i % checkpoint_every == 0 and rank == 0:
-            package = {'next_seq_index': seq_index + effective_batch_size, 'params': trainer.params(),
-                       'optim_state': trainer.optim_state(), 'model_config': model_kwargs, 'run_id': run_id}
+            package = {'next_seq_index': seq_index + effective_batch_size, 'optim_state': trainer.optim_state(),
+                       'model_config': model_kwargs, 'run_id': run_id}
+            if lora:
+                package.update(adapters=trainer.adapters(), lora=lora_cfg, base_checkpoint=base_file, num_params=num_params)
+            else:
+                package['params'] = trainer.params()
             save_checkpoint(package, checkpoint_keep_n)
             print(f"checkpoint to start at sequence index of {package['next_seq_index']}")
         if i % validate_every == 0:
@@ -143,8 +198,10 @@ def main(seed, batch_size, grad_accum_every, learning_rate, weight_decay, data_p
             valid_data = next(valid_dataset)[0]
             prime = valid_data[:prime_length]
             prime_str = decode_tokens(prime)
-            cur = trainer.params()
+            cur = model.merge_adapters(params, trainer.adapters(), lora_alpha=lora_cfg['alpha']) if lora else trainer.params()
             sampled = sample(seed, model.apply, cur, prime, seq_len, top_k=25)
+            if lora:
+                trainer.eng.load_params(params)            # the engine's base again (apply loaded the merged weights)
             print(prime_str, '\n', '*' * 40, '\n', decode_tokens(sampled[prime_length:]))
     if rank == 0:
         print(f'tokens/sec (host clock, incl. logging syncs): {tokens / max(1e-9, time.time() - t0):.0f}')

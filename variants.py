@@ -17,7 +17,7 @@ import click
 import numpy as np
 
 from progen_b200 import ProGen
-from progen_b200.checkpoint import get_checkpoint_fns
+from progen_b200.checkpoint import get_checkpoint_fns, package_params
 from progen_b200.variants import AMINO_ACIDS, parse_positions
 
 
@@ -48,7 +48,7 @@ def main(checkpoint_path, wild_type, prefix, mutations_path, scan, positions, ou
     last_checkpoint = get_last_checkpoint()
     if last_checkpoint is None:
         exit(f'no checkpoints found at {checkpoint_path}')
-    params = last_checkpoint['params']
+    params = package_params(last_checkpoint)             # plain params, or base + merged adapters
     model_kwargs = last_checkpoint['model_config']
     model = ProGen(**{**model_kwargs, 'mixed_precision': mixed_precision})
     print(f'sequence length: {model_kwargs["seq_len"]}, wild type: {len(wild_type)} residues')
