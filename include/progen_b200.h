@@ -130,6 +130,24 @@ int progen_preference_head(const void* logits, int dtype, const int* labels, con
  * same mask as above: for a sequence of L residues, input positions 0..L (BOS and every residue). */
 int progen_masked_mean_pool(const void* x, long long ldx, int dtype, const int* labels, float* out, int B, int n, int d,
                             void* stream);
+/* backward of progen_masked_mean_pool: dy[b, t, :] = demb[b, :] / count_b at counted positions, 0 at every other position;
+ * dy [B*n, d] (stride ldy) in dtype, every row written (no memset needed).  d % 4 == 0, ldy % 4 == 0. */
+int progen_masked_mean_pool_bwd(const float* demb, const int* labels, void* dy, long long ldy, int dtype, int B, int n, int d,
+                                void* stream);
+
+/* property head on pooled embeddings (all fp32): pred [B, C] = emb [B, d] W [d, C] + bias [C].
+ *   regression (C >= 1, targets y [B, C]):        row_loss_b = sum_c (pred_bc - y_bc)^2 / C
+ *   classification (C >= 2, classes cls [B]):      row_loss_b = logsumexp(pred_b) - pred_b[cls_b]   (cls clamped to [0, C))
+ * *loss = inv_batch * sum_b row_loss_b (inv_batch = 1/global_batch, like progen_ce_fwd_bwd); dpred [B, C] = d loss / d pred;
+ * dw [d, C], db [C] and demb [B, d] the gradients of loss.  loss, dw and db are written, not accumulated, and every sum
+ * over rows runs in row order without atomics: every output is the same bits in every launch.  With y and cls both null
+ * only pred is written (inference) and the other pointers may be null.  C > PROGEN_PROPERTY_MAX_OUTPUTS is refused. */
+#define PROGEN_PROPERTY_MAX_OUTPUTS 64
+#define PROGEN_TASK_REGRESSION 0
+#define PROGEN_TASK_CLASSIFICATION 1
+int progen_property_head(const float* emb, const float* w, const float* bias, int B, int d, int C, int task, const float* y,
+                         const int* cls, float inv_batch, float* pred, float* row_loss, float* loss, float* dpred, float* dw,
+                         float* db, float* demb, void* stream);
 
 /* backward of apply_rotary_pos_emb (progen.py:36-41) on the [T, ncols] q|k|v gradient, in place */
 int progen_rotary_bwd(void* dqkv, long long ld, int dtype, const float* sin_t, const float* cos_t, long long T, int ncols,

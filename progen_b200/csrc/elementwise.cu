@@ -545,6 +545,131 @@ __global__ void masked_mean_pool_kernel(const TX* __restrict__ x, long long ldx,
   }
 }
 
+// Backward of the pool: dy[b, t, :] = demb[b, :] / count_b at the positions the mask counts, 0 at every other position of
+// row b.  Grid (ceil(n / POOL_BWD_ROWS), B), 256 threads: warp w writes positions w, w + 8, ... of the block's slice, lane
+// 4 columns at a time.  Every row is written, so dy needs no memset.
+constexpr int POOL_BWD_ROWS = 64;
+
+template <typename TO>
+__global__ void masked_mean_pool_bwd_kernel(const float* __restrict__ demb, const int* __restrict__ labels,
+                                            TO* __restrict__ dy, long long ldy, int n, int d) {
+  const int b = blockIdx.y;
+  const int* lb = labels + (long long)b * n;
+  int first, count;
+  seq_loss_mask(lb, n, first, count);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const float* g = demb + (long long)b * d;
+  const int t1 = min(n, (blockIdx.x + 1) * POOL_BWD_ROWS);
+  for (int t = blockIdx.x * POOL_BWD_ROWS + warp; t < t1; t += ROWS_PER_BLOCK) {
+    const bool on = lb[t] != 0 || t == first;
+    TO* row = dy + ((long long)b * n + t) * ldy;
+    for (int c = lane * 4; c < d; c += 128) {
+      float v[4] = {0.f, 0.f, 0.f, 0.f};
+      if (on) {
+        load4<float>(g + c, v);
+#pragma unroll
+        for (int i = 0; i < 4; ++i) v[i] = v[i] / (float)count;
+      }
+      store4(row + c, v);
+    }
+  }
+}
+
+// ------------------------------------------------------------------------------------------ property head
+// p[b, :] = emb[b, :] W + bias (W [d, C] row-major, C <= PROGEN_PROPERTY_MAX_OUTPUTS).  One 256-thread block per row: thread
+// t owns output c = t % 64 and the k-slice t / 64 (k = slice, slice + 4, ...), so a warp reads whole rows of W; the four
+// slice partials are added in slice order.  Then thread 0 computes the row's loss and d p (fixed order over c): regression
+// loss_b = sum_c (p - y)^2 / C, d p = 2 (p - y) / C * inv_batch; classification loss_b = lse(p) - p[y], d p = (softmax(p)
+// - onehot(y)) * inv_batch.  Finally demb[b, k] = sum_c dp_c W[k, c] in c order.  With y and cls null only p is written.
+constexpr int HEAD_THREADS = 256;
+constexpr int HEAD_COLS = 64;
+constexpr int HEAD_SLICES = HEAD_THREADS / HEAD_COLS;
+static_assert(HEAD_COLS == PROGEN_PROPERTY_MAX_OUTPUTS, "one thread column per head output");
+
+__global__ void property_head_rows_kernel(const float* __restrict__ emb, const float* __restrict__ w,
+                                          const float* __restrict__ bias, int d, int C, int task,
+                                          const float* __restrict__ y, const int* __restrict__ cls, float inv_batch,
+                                          float* __restrict__ pred, float* __restrict__ row_loss,
+                                          float* __restrict__ dpred, float* __restrict__ demb) {
+  __shared__ float part[HEAD_SLICES][HEAD_COLS];
+  __shared__ float p[HEAD_COLS], dp[HEAD_COLS];
+  const int b = blockIdx.x;
+  const int c = threadIdx.x % HEAD_COLS, slice = threadIdx.x / HEAD_COLS;
+  const float* e = emb + (long long)b * d;
+  float acc = 0.f;
+  if (c < C)
+    for (int k = slice; k < d; k += HEAD_SLICES) acc = fmaf(e[k], w[(long long)k * C + c], acc);
+  part[slice][c] = acc;
+  __syncthreads();
+  if (threadIdx.x < C) {
+    float s = 0.f;
+#pragma unroll
+    for (int i = 0; i < HEAD_SLICES; ++i) s += part[i][threadIdx.x];
+    s += bias[threadIdx.x];
+    p[threadIdx.x] = s;
+    pred[(long long)b * C + threadIdx.x] = s;
+  }
+  if (y == nullptr && cls == nullptr) return;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float l = 0.f;
+    if (task == PROGEN_TASK_REGRESSION) {
+      const float* yb = y + (long long)b * C;
+      for (int j = 0; j < C; ++j) {
+        const float r = p[j] - yb[j];
+        l += r * r;
+        dp[j] = 2.f * r / (float)C * inv_batch;
+      }
+      l /= (float)C;
+    } else {
+      const int t = min(max(cls[b], 0), C - 1);
+      float mx = -INFINITY;
+      for (int j = 0; j < C; ++j) mx = fmaxf(mx, p[j]);
+      float se = 0.f;
+      for (int j = 0; j < C; ++j) se += expf(p[j] - mx);
+      l = mx + logf(se) - p[t];
+      const float inv = 1.f / se;
+      for (int j = 0; j < C; ++j) dp[j] = (expf(p[j] - mx) * inv - (j == t ? 1.f : 0.f)) * inv_batch;
+    }
+    row_loss[b] = l;
+  }
+  __syncthreads();
+  if (threadIdx.x < C) dpred[(long long)b * C + threadIdx.x] = dp[threadIdx.x];
+  for (int k = threadIdx.x; k < d; k += HEAD_THREADS) {
+    const float* wk = w + (long long)k * C;
+    float s = 0.f;
+    for (int j = 0; j < C; ++j) s = fmaf(dp[j], wk[j], s);
+    demb[(long long)b * d + k] = s;
+  }
+}
+
+// dW[k, c] = sum_b emb[b, k] dp[b, c], one thread per (k, c), rows b in order; the last block writes db[c] = sum_b dp[b, c]
+// (threads c < C) and loss = inv_batch * sum_b loss_b (thread C, in double).  Written, not accumulated; no atomics.
+__global__ void property_head_params_kernel(const float* __restrict__ emb, const float* __restrict__ dpred,
+                                            const float* __restrict__ row_loss, int B, int d, int C, float inv_batch,
+                                            float* __restrict__ dw, float* __restrict__ db, float* __restrict__ loss) {
+  const long long dc = (long long)d * C;
+  if (blockIdx.x == gridDim.x - 1) {
+    const int c = threadIdx.x;
+    if (c < C) {
+      float s = 0.f;
+      for (int b = 0; b < B; ++b) s += dpred[(long long)b * C + c];
+      db[c] = s;
+    } else if (c == C) {
+      double s = 0.0;
+      for (int b = 0; b < B; ++b) s += (double)row_loss[b];
+      *loss = (float)(s * (double)inv_batch);
+    }
+    return;
+  }
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= dc) return;
+  const int k = (int)(i / C), c = (int)(i % C);
+  float s = 0.f;
+  for (int b = 0; b < B; ++b) s = fmaf(emb[(long long)b * d + k], dpred[(long long)b * C + c], s);
+  dw[i] = s;
+}
+
 // ------------------------------------------------------------------------------------------ rotary backward
 // forward (GEMM epilogue): o0 = x0 c - x1 s, o1 = x1 c + x0 s  =>  dx0 = d0 c + d1 s, dx1 = d1 c - d0 s.  In place.
 template <typename TO>
@@ -865,6 +990,49 @@ int progen_masked_mean_pool(const void* x, long long ldx, int dtype, const int* 
   if (dtype == PG_F32) masked_mean_pool_kernel<float><<<grid, 256, 0, s>>>((const float*)x, ldx, labels, out, n, d);
   else if (dtype == PG_BF16) masked_mean_pool_kernel<bf16><<<grid, 256, 0, s>>>((const bf16*)x, ldx, labels, out, n, d);
   else { progen_set_error("masked_mean_pool: unsupported dtype %d", dtype); return PROGEN_ERR_UNSUPPORTED; }
+  PG_LAUNCH_CHECK();
+  return PROGEN_OK;
+}
+
+int progen_masked_mean_pool_bwd(const float* demb, const int* labels, void* dy, long long ldy, int dtype, int B, int n, int d,
+                                void* stream) {
+  PG_CHECK_ARG(B > 0 && n > 0 && d > 0 && d % 4 == 0 && ldy >= d && ldy % 4 == 0 && demb && labels && dy);
+  cudaStream_t s = (cudaStream_t)stream;
+  dim3 grid((n + POOL_BWD_ROWS - 1) / POOL_BWD_ROWS, B);
+  if (dtype == PG_F32) masked_mean_pool_bwd_kernel<float><<<grid, 256, 0, s>>>(demb, labels, (float*)dy, ldy, n, d);
+  else if (dtype == PG_BF16) masked_mean_pool_bwd_kernel<bf16><<<grid, 256, 0, s>>>(demb, labels, (bf16*)dy, ldy, n, d);
+  else { progen_set_error("masked_mean_pool_bwd: unsupported dtype %d", dtype); return PROGEN_ERR_UNSUPPORTED; }
+  PG_LAUNCH_CHECK();
+  return PROGEN_OK;
+}
+
+int progen_property_head(const float* emb, const float* w, const float* bias, int B, int d, int C, int task, const float* y,
+                         const int* cls, float inv_batch, float* pred, float* row_loss, float* loss, float* dpred, float* dw,
+                         float* db, float* demb, void* stream) {
+  if (C < 1 || C > PROGEN_PROPERTY_MAX_OUTPUTS) {
+    progen_set_error("property_head: %d outputs, the head supports 1..%d (PROGEN_PROPERTY_MAX_OUTPUTS)", C,
+                     PROGEN_PROPERTY_MAX_OUTPUTS);
+    return PROGEN_ERR_ARG;
+  }
+  PG_CHECK_ARG(B > 0 && d > 0 && emb && w && bias && pred);
+  PG_CHECK_ARG(task == PROGEN_TASK_REGRESSION || task == PROGEN_TASK_CLASSIFICATION);
+  if (task == PROGEN_TASK_CLASSIFICATION && C < 2) {
+    progen_set_error("property_head: classification needs at least 2 classes, got %d", C);
+    return PROGEN_ERR_ARG;
+  }
+  const bool train = y != nullptr || cls != nullptr;
+  if (train) {
+    PG_CHECK_ARG((task == PROGEN_TASK_REGRESSION ? y != nullptr && cls == nullptr : cls != nullptr && y == nullptr));
+    PG_CHECK_ARG(row_loss && loss && dpred && dw && db && demb && std::isfinite(inv_batch) && inv_batch > 0.f);
+  }
+  cudaStream_t s = (cudaStream_t)stream;
+  property_head_rows_kernel<<<B, HEAD_THREADS, 0, s>>>(emb, w, bias, d, C, task, y, cls, inv_batch, pred, row_loss, dpred,
+                                                       demb);
+  PG_LAUNCH_CHECK();
+  if (!train) return PROGEN_OK;
+  const long long dc = (long long)d * C;
+  property_head_params_kernel<<<(unsigned)((dc + 255) / 256 + 1), 256, 0, s>>>(emb, dpred, row_loss, B, d, C, inv_batch, dw,
+                                                                               db, loss);
   PG_LAUNCH_CHECK();
   return PROGEN_OK;
 }

@@ -302,6 +302,11 @@ class Engine:
         # stay valid
         self.logp, self.seq_ll, self.seq_count, self.ref = F(T), F(B), F(B), F(B)
         self.stats, self.ce_scratch = F(max(1, B // 2), 4), F(1)
+        # property head (property_step_device): pooled embedding and its gradient, predictions, targets, per-row losses
+        C = L.PROPERTY_MAX_OUTPUTS
+        self.emb, self.demb = F(B, d), F(B, d)
+        self.pred, self.dpred, self.ptarget, self.prow_loss = F(B * C), F(B * C), F(B * C), F(B)
+        self.pclass = torch.empty(B, device=dev, dtype=torch.int32)
         # backward temporaries (shared by all layers)
         self.dres = F(T, d)
         self.dres_lp = A(T, d) if self.mp else self.dres
@@ -425,9 +430,10 @@ class Engine:
         acts.tok.copy_(torch.as_tensor(ids).reshape(-1).to(device=self.dev, dtype=torch.int32))
         self._forward_device(acts, sink=lambda i, name, buf: sink(i, name, buf, P))
 
-    def _forward_device(self, acts=None, sink=None, length=None):
+    def _forward_device(self, acts=None, sink=None, length=None, logits=True):
         """forward pass on activation set `acts` (default: the training set, which keeps what the backward pass reads);
-        with a `sink` (Engine.prefill) the layers' state goes to it and the logits head is skipped.
+        with a `sink` (Engine.prefill) the layers' state goes to it and the logits head is skipped; `logits=False` stops
+        after the final LayerNorm (acts.yf), for the property head.
         `length` (default seq_len): the positions per row, acts.T = acts.B * length.  Every mixing op is causal, so a
         forward cut to the first `length` positions computes exactly those positions of the full one (DESIGN.md §3.6)."""
         acts = self.acts if acts is None else acts
@@ -494,6 +500,8 @@ class Engine:
         # ---- to_logits (progen.py:219-222)
         xl = acts.X[-1]
         self.ln_fwd(xl, d, self.Pf(P + 'layer_norm', 'scale'), acts.yf, d, acts.meanf, acts.rstdf, d, False, acts=acts, seq_len=n)
+        if not logits:
+            return
         self.fwd_gemm(acts.yf, d, self.W(P + 'linear', 'w'), self.V, acts.logits, bias=self.Pf(P + 'linear', 'b'), out_dtype=L.F32,
                       acts=acts)
 
@@ -661,9 +669,103 @@ class Engine:
                                              self.dres_lp.data_ptr() if self.mp else 0, self.d, L.ptr(dscale),
                                              L.ptr(next_bias_grad), self.T, self.d, self.n, int(shift), 1, L.stream()), 'ln_bwd')
 
+    # ------------------------------------------------------------------------------------------ property head
+    def load_property(self, rows, task, targets):
+        """rows (B, n+1) and checked targets (regression: float32 [B, C]; classification: int32 [B]) -> self.tok /
+        self.labels / self.ptarget or self.pclass; returns B"""
+        B = self.load_batch(rows)
+        t = torch.as_tensor(targets)
+        if task == L.TASK_REGRESSION:
+            self.ptarget[:t.numel()].copy_(t.reshape(-1), non_blocking=True)
+        else:
+            self.pclass.copy_(t, non_blocking=True)
+        return B
+
+    def property_step_device(self, task, global_batch, zero_grads=True):
+        """forward (without the logits GEMM) + final LayerNorm + masked mean pool + property head + pool backward + the
+        frozen-base backward from the final LayerNorm down, on rows resident in self.tok / self.labels and their targets in
+        self.ptarget / self.pclass (load_property).  The head's parameters and gradients are the last segments of the
+        adapter buffer (lora.Adapters with head_outputs); its loss is scaled by 1/global_batch (DESIGN.md §3.9)."""
+        lo = self.lora
+        if lo is None or not lo.head_outputs:
+            raise L.ProgenError('property step: needs adapters with a property head (the base stays frozen)')
+        self._check_zero_grads(zero_grads)
+        lib, st, B, d, C = self.lib, L.stream(), self.B, self.d, lo.head_outputs
+        self._forward_device(logits=False)
+        if zero_grads:
+            self.train_grads().zero_()
+        L.check(lib.progen_masked_mean_pool(self.yf.data_ptr(), d, self.act_dt, self.labels.data_ptr(), self.emb.data_ptr(),
+                                            B, self.n, d, st), 'masked_mean_pool')
+        reg = task == L.TASK_REGRESSION
+        L.check(lib.progen_property_head(self.emb.data_ptr(), lo.head(lo.params, 'w').data_ptr(),
+                                         lo.head(lo.params, 'b').data_ptr(), B, d, C, task,
+                                         self.ptarget.data_ptr() if reg else 0, 0 if reg else self.pclass.data_ptr(),
+                                         1.0 / global_batch, self.pred.data_ptr(), self.prow_loss.data_ptr(),
+                                         self.loss.data_ptr(), self.dpred.data_ptr(), lo.head(lo.grads, 'w').data_ptr(),
+                                         lo.head(lo.grads, 'b').data_ptr(), self.demb.data_ptr(), st), 'property_head')
+        L.check(lib.progen_masked_mean_pool_bwd(self.demb.data_ptr(), self.labels.data_ptr(), self.dy.data_ptr(), d,
+                                                self.act_dt, B, self.n, d, st), 'masked_mean_pool_bwd')
+        self._backward_body()
+
+    def property_stats(self, rows):
+        """the last property step's predictions [rows, C] and per-row losses [rows] as numpy float32"""
+        C = self.lora.head_outputs if self.lora is not None else 0
+        if not rows or not C:
+            return dict(prediction=np.zeros((0, C), np.float32), loss=np.zeros(0, np.float32))
+        return dict(prediction=self.pred[:rows * C].view(rows, C).cpu().numpy(), loss=self.prow_loss[:rows].cpu().numpy())
+
+    def predict(self, data, w, b, batch_size=64):
+        """data: (N, n+1) integer rows; w [d, C], b [C] float32 head parameters -> (prediction [N, C], embedding [N, d])
+        numpy float32.  Runs the inference forward cut to the rows' cut_length (the pooled embedding reads counted
+        positions only, so it is bitwise the full-length one), without the logits GEMM, then progen_masked_mean_pool and
+        progen_property_head without targets, batch_size rows at a time, one D2H copy per chunk."""
+        rows = torch.as_tensor(np.asarray(data).astype(np.int32))
+        N, n, d = rows.shape[0], self.n, self.d
+        C = int(np.asarray(w).shape[1])
+        out_p, out_e = np.zeros((N, C), np.float32), np.zeros((N, d), np.float32)
+        if N == 0:
+            return out_p, out_e
+        cut = cut_length(rows[:, 1:].numpy())
+        hw = torch.tensor(np.asarray(w, np.float32), device=self.dev)
+        hb = torch.tensor(np.asarray(b, np.float32), device=self.dev)
+        full = self.inference_acts(min(batch_size, N))
+        res = torch.empty(full.B * (d + C), device=self.dev, dtype=torch.float32)
+        lib, st = self.lib, L.stream()
+        for r0 in range(0, N, batch_size):
+            chunk = rows[r0:r0 + batch_size]
+            B = chunk.shape[0]
+            acts = full if B == full.B and cut == n else full.view(B, cut)
+            staged = acts.rows if cut == n else full.rows.view(-1)[:B * (cut + 1)].view(B, cut + 1)
+            staged.copy_(chunk if cut == n else chunk[:, :cut + 1])
+            acts.tok.view(B, cut).copy_(staged[:, :-1])
+            acts.labels.view(B, cut).copy_(staged[:, 1:])
+            self._forward_device(acts, length=cut, logits=False)
+            emb, pred = res[:B * d], res[B * d:B * (d + C)]
+            L.check(lib.progen_masked_mean_pool(acts.yf.data_ptr(), d, self.act_dt, acts.labels.data_ptr(), emb.data_ptr(),
+                                                B, cut, d, st), 'masked_mean_pool')
+            L.check(lib.progen_property_head(emb.data_ptr(), hw.data_ptr(), hb.data_ptr(), B, d, C, L.TASK_REGRESSION, 0, 0,
+                                             1.0, pred.data_ptr(), 0, 0, 0, 0, 0, 0, st), 'property_head')
+            host = res[:B * (d + C)].cpu().numpy()
+            out_e[r0:r0 + B] = host[:B * d].reshape(B, d)
+            out_p[r0:r0 + B] = host[B * d:].reshape(B, C)
+        return out_p, out_e
+
     def _backward_device(self):
         """With adapters (self.lora) the base is frozen: no base weight, bias, LayerNorm-scale, SGU or embedding
         gradient is computed, and every adapted projection's input gradient carries its adapter's tail (lora_bwd)."""
+        d = self.d
+        frozen = self.lora is not None
+        # ---- head
+        hw = P + 'linear'
+        if not frozen:
+            self.colsum(self.dlogits, self.V, self.G(hw, 'b'))
+            self.wgrad_gemm(self.yf, d, self.dlogits, self.V, self.G(hw, 'w'))
+        self.dgrad_gemm(self.dlogits, self.V, self.W(hw, 'w'), d, self.dy)
+        self._backward_body()
+
+    def _backward_body(self):
+        """the backward pass below the logits head, from self.dy = d loss / d (final LayerNorm output): the LM head
+        (_backward_device) and the property head (property_step_device) both enter here"""
         lib, st = self.lib, L.stream()
         cfg, d, I, hid, T, n = self.cfg, self.d, self.I, self.hid, self.T, self.n
         shift = cfg['shift_tokens']
@@ -671,12 +773,7 @@ class Engine:
         frozen = lo is not None
         G = (lambda module, name: None) if frozen else self.G
         tail = self.lora_bwd if frozen else (lambda *a: {})
-        # ---- head
-        hw, hl = P + 'linear', P + 'layer_norm'
-        if not frozen:
-            self.colsum(self.dlogits, self.V, self.G(hw, 'b'))
-            self.wgrad_gemm(self.yf, d, self.dlogits, self.V, self.G(hw, 'w'))
-        self.dgrad_gemm(self.dlogits, self.V, self.W(hw, 'w'), d, self.dy)
+        hl = P + 'layer_norm'
         self.dres.zero_()
         nl = len(self.kinds)
         self.ln_bwd_res(self.dy, self.X[-1], self.Pf(hl, 'scale'), self.meanf, self.rstdf, G(hl, 'scale'), False,

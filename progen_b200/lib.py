@@ -10,6 +10,8 @@ import torch
 F32, BF16 = 0, 1
 BACKEND_SIMT, BACKEND_TC = 0, 1
 EPI_STORE, EPI_ROTARY, EPI_RESIDUAL, EPI_GLU, EPI_GELU, EPI_GLU_BWD, EPI_GELU_BWD, EPI_ACCUM = range(8)
+TASK_REGRESSION, TASK_CLASSIFICATION = 0, 1
+PROPERTY_MAX_OUTPUTS = 64          # PROGEN_PROPERTY_MAX_OUTPUTS: outputs (or classes) of a property head
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'libprogen_b200.so')
@@ -58,6 +60,8 @@ PROTOTYPES = {
     'progen_token_logprob': [_P, _I, _P, _P, _P, _P, _I, _I, _I, _P],
     'progen_preference_head': [_P, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _F, _F, _P],
     'progen_masked_mean_pool': [_P, _LL, _I, _P, _P, _I, _I, _I, _P],
+    'progen_masked_mean_pool_bwd': [_P, _P, _P, _LL, _I, _I, _I, _I, _P],
+    'progen_property_head': [_P, _P, _P, _I, _I, _I, _I, _P, _P, _F, _P, _P, _P, _P, _P, _P, _P, _P],
     'progen_rotary_bwd': [_P, _LL, _I, _P, _P, _LL, _I, _I, _I, _P],
     'progen_local_attn_fwd_simt': [_P, _P, _P, _I, _I, _I, _I, _I, _I, _P],
     'progen_local_attn_bwd_simt': [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P],

@@ -36,11 +36,18 @@ def adapter_shapes(cfg, rank):
     return {m: {'lora_a': (i, rank), 'lora_b': (rank, o)} for m, i, o, _ in adapter_modules(cfg)}
 
 
-def build_adapter_specs(cfg, rank):
-    """engine layout of the adapter buffer: (specs, padded size, offset of the first B segment)"""
+HEAD = 'property_head'              # module of a property head's {'w': [d, C], 'b': [C]} (DESIGN.md §3.9)
+
+
+def build_adapter_specs(cfg, rank, head_outputs=0):
+    """engine layout of the adapter buffer: (specs, padded size, offset of the first B segment).  A property head of
+    head_outputs > 0 outputs takes the last segments: the trained flat state is then adapters plus head, and the
+    compute copy (A | s B) stops before it."""
     mods = adapter_modules(cfg)
     specs = ([ParamSpec(m, 'lora_a', (i, rank)) for m, i, o, _ in mods] +
              [ParamSpec(m, 'lora_b', (rank, o), interleave=glu) for m, i, o, glu in mods])
+    if head_outputs:
+        specs += [ParamSpec(HEAD, 'w', (cfg['dim'], head_outputs)), ParamSpec(HEAD, 'b', (head_outputs,))]
     off, n_a = 0, None
     for s in specs:
         if s.name == 'lora_b' and n_a is None:
@@ -125,12 +132,14 @@ class Adapters:
     """The device state of one adapter tree for an Engine: flat fp32 parameters and gradients in engine layout, the
     act-dtype compute copy (A | s B), and per-projection u = x A activations of the training set."""
 
-    def __init__(self, eng, rank, alpha):
+    def __init__(self, eng, rank, alpha, head_outputs=0):
         self.eng = eng
         self.r, self.alpha = rank, float(alpha)
         self.scale = self.alpha / rank
-        self.specs, self.n_padded, self.n_a = build_adapter_specs(eng.cfg, rank)
+        self.head_outputs = int(head_outputs)
+        self.specs, self.n_padded, self.n_a = build_adapter_specs(eng.cfg, rank, self.head_outputs)
         self.by_key = {(s.module, s.name): s for s in self.specs}
+        self.n_head = self.by_key[(HEAD, 'w')].offset if self.head_outputs else self.n_padded   # end of the A | B segments
         self.num_params = sum(s.size for s in self.specs)
         f32 = dict(device=eng.dev, dtype=torch.float32)
         self.params = torch.zeros(self.n_padded, **f32)
@@ -142,6 +151,10 @@ class Adapters:
         s = self.by_key[(module, name)]
         return buf[s.offset:s.offset + s.size]
 
+    def head(self, buf, name):
+        """the property head's fp32 segment `name` ('w' [d, C] or 'b' [C]) of buffer `buf`"""
+        return self.seg(buf, HEAD, name)
+
     def flat(self, tree):
         host = np.zeros(self.n_padded, np.float32)
         for s in self.specs:
@@ -150,8 +163,9 @@ class Adapters:
             host[s.offset:s.offset + s.size] = (_interleave(a) if s.interleave else a).ravel()
         return torch.from_numpy(host)
 
-    def load(self, tree):
-        self.params.copy_(self.flat(tree))
+    def load(self, tree, head=None):
+        """adapter tree (and, with head_outputs, the head tree {'property_head': {'w', 'b'}}) -> the device buffer"""
+        self.params.copy_(self.flat(tree if head is None else {**tree, **head}))
         self.refresh()
 
     def export_tree(self, buf):
@@ -162,18 +176,25 @@ class Adapters:
             out.setdefault(s.module, {})[s.name] = _deinterleave(a) if s.interleave else a
         return out
 
+    def split(self, tree):
+        """a tree exported from this buffer -> (adapter tree, head tree or None)"""
+        head = tree.pop(HEAD, None)
+        return tree, None if head is None else {HEAD: head}
+
     def refresh(self):
-        """compute copy: A as is, B times s, in the act dtype; call after every parameter change"""
+        """compute copy: A as is, B times s, in the act dtype; call after every parameter change.  A property head
+        (fp32, read by progen_property_head from the parameters) has no compute copy."""
         lib, st, n_a = self.eng.lib, L.stream(), self.n_a
         L.check(lib.progen_scale_cast_f32(self.params.data_ptr(), self.lp.data_ptr(), self.eng.act_dt, 1.0, n_a, st),
                 'adapter copy A')
         L.check(lib.progen_scale_cast_f32(self.params[n_a:].data_ptr(), self.lp[n_a:].data_ptr(), self.eng.act_dt,
-                                          self.scale, self.n_padded - n_a, st), 'adapter copy s B')
+                                          self.scale, self.n_head - n_a, st), 'adapter copy s B')
 
     def scale_b_grads(self):
-        """dB = s u^T dy: the wgrad GEMMs accumulate u^T dy, the scale follows in one pass over the B gradients"""
+        """dB = s u^T dy: the wgrad GEMMs accumulate u^T dy, the scale follows in one pass over the B gradients (not
+        the property head's)"""
         if self.scale != 1.0:
-            g = self.grads[self.n_a:]
+            g = self.grads[self.n_a:self.n_head]
             L.check(self.eng.lib.progen_scale_cast_f32(g.data_ptr(), g.data_ptr(), L.F32, self.scale, g.numel(), L.stream()),
                     'adapter grad s')
 

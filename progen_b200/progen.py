@@ -320,15 +320,17 @@ class ProGen:
         rank, alpha = check_rank_alpha(check_adapters(self.config, adapters), lora_alpha)
         return merge_adapters(params, adapters, alpha / rank)
 
-    def _attach_adapters(self, adapters, lora_alpha):
-        """validate `adapters` and make them the engine's training-set adapters -> lora.Adapters"""
-        from .lora import Adapters, check_adapters, check_rank_alpha
+    def _attach_adapters(self, adapters, lora_alpha, head=None):
+        """validate `adapters` and make them (with a checked property `head`: and it) the engine's training-set adapters
+        -> lora.Adapters"""
+        from .lora import HEAD, Adapters, check_adapters, check_rank_alpha
         rank, alpha = check_rank_alpha(check_adapters(self.config, adapters), lora_alpha)
+        C = 0 if head is None else int(np.asarray(head[HEAD]['b']).shape[0])
         eng = self.engine
         lo = getattr(self, '_adapters', None)
-        if lo is None or lo.r != rank or lo.alpha != alpha:
-            lo = self._adapters = Adapters(eng, rank, alpha)
-        lo.load(adapters)
+        if lo is None or lo.r != rank or lo.alpha != alpha or lo.head_outputs != C:
+            lo = self._adapters = Adapters(eng, rank, alpha, head_outputs=C)
+        lo.load(adapters, head)
         eng.lora = lo
         return lo
 
@@ -549,8 +551,61 @@ class ProGen:
             self._gen_decoder, self._gen_params = dec, params
         return dec
 
-    def trainer(self, params, *, adapters=None, lora_alpha=None, **optim_kwargs):
+    def trainer(self, params, *, adapters=None, lora_alpha=None, head=None, task=None, **optim_kwargs):
         """Device-resident training state over `params` (train.py's loop).  With `adapters` only the adapters train
-        (the base stays bitwise unchanged); lora_alpha as in `loss_and_grad`."""
+        (the base stays bitwise unchanged); lora_alpha as in `loss_and_grad`.  With a property `head` (`init_head`) and
+        its `task` ('regression' | 'classification') the adapters and the head train together through
+        `Trainer.property_step`."""
         from .trainer import Trainer
-        return Trainer(self, params, adapters=adapters, lora_alpha=lora_alpha, **optim_kwargs)
+        return Trainer(self, params, adapters=adapters, lora_alpha=lora_alpha, head=head, task=task, **optim_kwargs)
+
+    # ---- property fine-tuning (DESIGN.md §3.9)
+    def init_head(self, rng, num_outputs):
+        """An initial property head {'property_head': {'w': [dim, C], 'b': [C]}} on the pooled embedding: w ~
+        TruncatedNormal(1/sqrt(dim)) from `rng` (an int seed or key-like array, as in `init`), b = 0.  num_outputs C in
+        [1, 64]: the regression outputs, or the classes (>= 2) of a classification head."""
+        from .property import init_head
+        seed = int(np.asarray(rng).ravel()[-1]) if not isinstance(rng, (int, np.integer)) else int(rng)
+        return init_head(self.config['dim'], seed, num_outputs)
+
+    def property_loss_and_grad(self, params, rows, targets, *, adapters, head, task, lora_alpha=None):
+        """Loss and gradients of property fine-tuning: the head on the pooled embedding of the adapted model (the
+        embedding `score(..., return_embeddings=True)` returns: the mean of the final LayerNorm output over the counted
+        positions).  rows: (B, n+1) integer rows of the `collate` contract; task 'regression' (targets float [B, C]; loss
+        = sum_b sum_c (p - y)^2 / (C B)) or 'classification' (targets class indices [B]; loss = mean cross entropy).
+        The base is frozen.  Inputs are checked before any device work (ProgenError).
+        Returns (python float loss, adapter gradients, head gradients, predictions [B, C] numpy float32: the regression
+        values or the class logits)."""
+        from .lora import check_adapters, check_rank_alpha
+        from .property import check_head, check_rows, check_targets, check_task
+        code = check_task(task)
+        C = check_head(self.config, head, task)
+        check_rank_alpha(check_adapters(self.config, adapters), lora_alpha)
+        r = check_rows(rows, self.config['seq_len'], 'property_loss_and_grad')
+        if r.shape[0] < 1:
+            raise L.ProgenError('property_loss_and_grad: needs at least one row')
+        y = check_targets(targets, task, C, r.shape[0], 'property_loss_and_grad')
+        self._ensure_loaded(params)
+        lo = self._attach_adapters(adapters, lora_alpha, head)
+        eng = self.engine
+        B = eng.load_property(r, code, y)
+        eng.property_step_device(code, B)
+        grads, hgrads = lo.split(lo.export_tree(lo.grads))
+        return float(eng.loss.item()), grads, hgrads, eng.property_stats(B)['prediction']
+
+    def predict(self, params, head, data, *, batch_size=64):
+        """Property predictions of sequences: the head on the pooled embedding, on the inference forward (like `score`;
+        pass merged parameters for a fine-tuned model: `merge_adapters`, `checkpoint.package_params`).  data: (N, n+1)
+        integer rows of the `collate` contract.  The forward is cut to the rows' counted length rounded up to 128
+        (`engine.cut_length`): the embedding reads counted positions only, so it is bitwise the full-length one.
+        Returns a dict of numpy float32 arrays: prediction [N, C] (regression values, or class logits) and embedding
+        [N, d] (bitwise `score(..., return_embeddings=True)['embedding']`).  Results do not depend on batch_size."""
+        from .lora import HEAD
+        from .property import check_head, check_rows
+        check_head(self.config, head)
+        if isinstance(batch_size, (bool, np.bool_)) or not isinstance(batch_size, (int, np.integer)) or batch_size < 1:
+            raise L.ProgenError(f'predict: batch_size must be an integer >= 1, got {batch_size!r}')
+        r = check_rows(data, self.config['seq_len'], 'predict')
+        self._ensure_loaded(params)
+        pred, emb = self.engine.predict(r, head[HEAD]['w'], head[HEAD]['b'], batch_size=int(batch_size))
+        return dict(prediction=pred, embedding=emb)

@@ -3,7 +3,8 @@ accumulator live in flat fp32 buffers; one `step(data)` is one iteration of the 
 (train.py:186-190): loss+grads, optim.update, apply_updates.
 
 With low-rank adapters (`adapters=`) the same state exists for the adapter buffer only: the base parameters are frozen
-and bitwise unchanged, and clip / AdamW / apply_every run over the adapters (weight decay on every A and B)."""
+and bitwise unchanged, and clip / AdamW / apply_every run over the adapters (weight decay on every A and B).  A property
+head (`head=`, `task=`) joins that buffer: `property_step` trains adapters and head together (DESIGN.md §3.9)."""
 import os
 
 import numpy as np
@@ -16,8 +17,18 @@ from . import parallel as PAR
 class Trainer:
     def __init__(self, model, params, learning_rate=2e-4, weight_decay=1e-3, max_grad_norm=0.5, grad_accum_every=4,
                  b1=0.9, b2=0.999, eps=1e-8, optim_state=None, data_parallel=True, cuda_graph=False, adapters=None,
-                 lora_alpha=None):
+                 lora_alpha=None, head=None, task=None):
         self.model = model
+        self.task = None
+        if head is not None or task is not None:
+            from .property import check_head, check_task
+            if adapters is None:
+                raise L.ProgenError('a property head trains with adapters on the frozen base: pass adapters= '
+                                    '(full-parameter property fine-tuning is not supported)')
+            if head is None or task is None:
+                raise L.ProgenError('property fine-tuning needs both head= and task=')
+            self.task = check_task(task)
+            C = check_head(model.config, head, task)
         self.eng = model.engine
         self.eng.load_params(params)
         model._loaded = None
@@ -25,8 +36,8 @@ class Trainer:
         if adapters is not None:
             from .lora import Adapters, check_adapters, check_rank_alpha
             rank, alpha = check_rank_alpha(check_adapters(model.config, adapters), lora_alpha)
-            self.lora = Adapters(self.eng, rank, alpha)
-            self.lora.load(adapters)
+            self.lora = Adapters(self.eng, rank, alpha, head_outputs=C if head is not None else 0)
+            self.lora.load(adapters, head)
         # the flat buffers the optimizer owns: (parameters, size, ndim > 1 prefix, bf16 mirror or None); gradients: self.G
         if self.lora is None:
             e = self.eng
@@ -179,6 +190,54 @@ class Trainer:
                 self._eager_run = 0
         return loss
 
+    # ---- property fine-tuning (a head on the pooled embedding, adapters on the frozen base)
+    def property_step(self, rows, targets, sync_loss=False):
+        """One micro-step of property fine-tuning: the loss and gradients of `ProGen.property_loss_and_grad` over the
+        adapters and the head, then one clip / AdamW / apply_every update of both (weight decay on every trained
+        parameter).  rows: (B, n+1) integer rows; targets: regression float [B, C], classification class indices [B].
+        With cuda_graph=True the step is captured after two eager steps of one batch size and replayed from then on.
+        Single process only.  Returns the device scalar loss; `property_stats()` has the predictions and per-row losses."""
+        from .property import check_rows, check_targets
+        if self.task is None:
+            raise L.ProgenError('property_step: this trainer has no property head (model.trainer(..., head=, task=))')
+        if self.world > 1:
+            raise L.ProgenError('property_step: data-parallel property fine-tuning is not supported; run one process '
+                                '(data_parallel=False or without torchrun)')
+        task = 'regression' if self.task == L.TASK_REGRESSION else 'classification'
+        r = check_rows(rows, self.eng.n, 'property_step')
+        B = r.shape[0]
+        if B < 1:
+            raise L.ProgenError('property_step: needs at least one row')
+        y = check_targets(targets, task, self.lora.head_outputs, B, 'property_step')
+        self._prop_rows = B
+        self.eng.lora = self.lora
+        key = (B, B, 'property', self.task)
+        self._drop_graph_unless(B)
+        if self._graph is not None and self._graph_key == key:
+            self.eng.load_property(r, self.task, y)        # H2D copies stay outside the graph
+            return self._replay(sync_loss)
+        self.eng.load_property(r, self.task, y)
+        self.eng.property_step_device(self.task, B)
+        loss = self._update(sync_loss)
+        if self._auto_graph:
+            self._eager_run = self._eager_run + 1 if key == self._eager_key else 1
+            self._eager_key = key
+            if self._eager_run >= 2:
+                self._capture(B, key, lambda: self.eng.property_step_device(self.task, B))
+                self._eager_run = 0
+        return loss
+
+    def property_stats(self):
+        """the last `property_step`'s predictions [B, C] (regression values, or class logits) and per-row losses [B] as
+        numpy float32"""
+        return self.eng.property_stats(getattr(self, '_prop_rows', 0))
+
+    def head(self):
+        """the trained property head {'property_head': {'w', 'b'}} (None without one)"""
+        if self.lora is None or not self.lora.head_outputs:
+            return None
+        return self.lora.split(self.lora.export_tree(self.lora.params))[1]
+
     def preference_stats(self):
         """this rank's statistics of its last `preference_step` as numpy float32 [P] arrays: policy_chosen and
         policy_rejected (the policy's log-likelihoods s), margin (z) and loss (each pair's softplus(-z))"""
@@ -300,7 +359,7 @@ class Trainer:
 
     def adapters(self):
         """the trained adapters, a tree of `ProGen.init_adapters`' shape (None without adapters)"""
-        return None if self.lora is None else self.lora.export_tree(self.lora.params)
+        return None if self.lora is None else self.lora.split(self.lora.export_tree(self.lora.params))[0]
 
     def optim_state(self):
         """{count, mu, nu, acc, every}: trees of the parameters (with adapters: of the adapters) the optimizer owns"""
