@@ -298,11 +298,11 @@ class Engine:
         self.logits = F(T, self.V)
         self.dlogits = A(T, self.V)
         self.ce_w = F(T)
-        # preference (DPO) head (preference_step_device): B = 2 * pairs rows; allocated here so a captured step's pointers
+        # preference (DPO) head (train_step): B = 2 * pairs rows; allocated here so a captured step's pointers
         # stay valid
         self.logp, self.seq_ll, self.seq_count, self.ref = F(T), F(B), F(B), F(B)
         self.stats, self.ce_scratch = F(max(1, B // 2), 4), F(1)
-        # property head (property_step_device): pooled embedding and its gradient, predictions, targets, per-row losses
+        # property head (train_step): pooled embedding and its gradient, predictions, targets, per-row losses
         C = L.PROPERTY_MAX_OUTPUTS
         self.emb, self.demb = F(B, d), F(B, d)
         self.pred, self.dpred, self.ptarget, self.prow_loss = F(B * C), F(B * C), F(B * C), F(B)
@@ -594,7 +594,7 @@ class Engine:
         Mirrors utils.py:61-76: ids = data[:, :-1], labels = data[:, 1:], mean over rows of the masked CE.
         `global_batch` (DDP): scale by 1/global_batch so that a SUM all-reduce yields the global-mean gradient."""
         B = self.load_batch(data)
-        self.step_device(global_batch or B, zero_grads)
+        self.train_step((), global_batch or B, zero_grads)
         return self.loss
 
     def load_batch(self, data):
@@ -607,24 +607,69 @@ class Engine:
         self.labels.copy_(dd[:, 1:].reshape(-1))
         return B
 
-    def step_device(self, global_batch, zero_grads=True):
-        """forward + loss + backward on tokens/labels already resident in self.tok / self.labels"""
-        self._forward_device()
-        lib, st = self.lib, L.stream()
-        self.loss.zero_()
-        self._check_zero_grads(zero_grads)
-        if zero_grads:
-            self.train_grads().zero_()
-        L.check(lib.progen_ce_fwd_bwd(self.logits.data_ptr(), L.F32, self.labels.data_ptr(), self.ce_w.data_ptr(),
-                                      self.loss.data_ptr(), self.dlogits.data_ptr(), self.act_dt, self.B, self.n, self.V,
-                                      1.0 / global_batch, st), 'ce_fwd_bwd')
-        self._backward_device()
-
-    def _check_zero_grads(self, zero_grads):
-        if not zero_grads and self.lora is not None:
+    def train_step(self, objective, global_rows, zero_grads=True, backward=True):
+        """forward + loss head + backward of one training objective on rows resident in self.tok / self.labels.
+        `objective` (also the tail of Trainer's graph key) selects the loss head:
+          ()                    the language-model loss: the masked cross entropy, mean over rows (utils.py:45-59);
+          ('preference', beta)  the preference (DPO) loss (DESIGN.md §3.7) over the resident rows as pairs, rows 0..P-1
+                                chosen and row i + P the rejected row of pair i, with their reference log-likelihoods in
+                                self.ref (load_preference); self.stats [P, 4] holds each pair's (s(chosen), s(rejected),
+                                z, loss);
+          ('property', task)    the property head on the pooled embedding (DESIGN.md §3.9), task L.TASK_REGRESSION or
+                                L.TASK_CLASSIFICATION, targets in self.ptarget / self.pclass (load_property); the
+                                forward stops after the final LayerNorm.  Needs
+                                adapters with a head (lora.Adapters with head_outputs): the base stays frozen.
+        The loss is scaled by 1/global_rows (the preference loss: 1/global pairs), so that a SUM all-reduce of the
+        per-rank gradients is the global mean.  With adapters (self.lora) no base gradient is computed.
+        `backward=False`: the forward and the loss only (a validation loss), no gradient."""
+        lib, st, lo, d = self.lib, L.stream(), self.lora, self.d
+        kind = objective[0] if objective else None
+        pairs = self.B // 2
+        if kind == 'preference' and 2 * pairs != self.B:
+            raise L.ProgenError(f'preference step: {pairs} pairs need {2 * pairs} resident rows, have {self.B}')
+        if kind == 'property' and (lo is None or not lo.head_outputs):
+            raise L.ProgenError('property step: needs adapters with a property head (the base stays frozen)')
+        if not zero_grads and lo is not None:
             # the backward pass ends by scaling the whole B gradient by s (Adapters.scale_b_grads): an accumulated one
             # would be scaled twice
             raise L.ProgenError('adapters: gradients cannot accumulate across steps (zero_grads=False)')
+        self._forward_device(logits=kind != 'property')
+        if kind is None:
+            self.loss.zero_()
+        if zero_grads and backward:
+            self.train_grads().zero_()
+        if kind is None:
+            L.check(lib.progen_ce_fwd_bwd(self.logits.data_ptr(), L.F32, self.labels.data_ptr(), self.ce_w.data_ptr(),
+                                          self.loss.data_ptr(), self.dlogits.data_ptr() if backward else 0, self.act_dt,
+                                          self.B, self.n, self.V, 1.0 / global_rows, st), 'ce_fwd_bwd')
+        elif kind == 'preference':
+            L.check(lib.progen_preference_head(self.logits.data_ptr(), L.F32, self.labels.data_ptr(), self.ref.data_ptr(),
+                                               self.logp.data_ptr(), self.seq_ll.data_ptr(), self.seq_count.data_ptr(),
+                                               self.ce_w.data_ptr(), self.stats.data_ptr(), self.loss.data_ptr(),
+                                               self.ce_scratch.data_ptr(), self.dlogits.data_ptr(), self.act_dt, pairs,
+                                               self.n, self.V, objective[1], 1.0 / global_rows, st), 'preference_head')
+        else:
+            B, C, reg = self.B, lo.head_outputs, objective[1] == L.TASK_REGRESSION
+            L.check(lib.progen_masked_mean_pool(self.yf.data_ptr(), d, self.act_dt, self.labels.data_ptr(),
+                                                self.emb.data_ptr(), B, self.n, d, st), 'masked_mean_pool')
+            L.check(lib.progen_property_head(self.emb.data_ptr(), lo.head(lo.params, 'w').data_ptr(),
+                                             lo.head(lo.params, 'b').data_ptr(), B, d, C, objective[1],
+                                             self.ptarget.data_ptr() if reg else 0, 0 if reg else self.pclass.data_ptr(),
+                                             1.0 / global_rows, self.pred.data_ptr(), self.prow_loss.data_ptr(),
+                                             self.loss.data_ptr(), self.dpred.data_ptr(), lo.head(lo.grads, 'w').data_ptr(),
+                                             lo.head(lo.grads, 'b').data_ptr(), self.demb.data_ptr(), st), 'property_head')
+        if not backward:
+            return
+        if kind == 'property':
+            L.check(lib.progen_masked_mean_pool_bwd(self.demb.data_ptr(), self.labels.data_ptr(), self.dy.data_ptr(), d,
+                                                    self.act_dt, self.B, self.n, d, st), 'masked_mean_pool_bwd')
+        else:
+            hw = P + 'linear'
+            if lo is None:
+                self.colsum(self.dlogits, self.V, self.G(hw, 'b'))
+                self.wgrad_gemm(self.yf, d, self.dlogits, self.V, self.G(hw, 'w'))
+            self.dgrad_gemm(self.dlogits, self.V, self.W(hw, 'w'), d, self.dy)
+        self._backward_body()
 
     def train_grads(self):
         """the flat gradient buffer a training step writes: the adapters' with adapters (the base is frozen)"""
@@ -636,24 +681,6 @@ class Engine:
         B = self.load_batch(rows)
         self.ref.copy_(torch.as_tensor(np.asarray(ref, np.float32)), non_blocking=True)
         return B // 2
-
-    def preference_step_device(self, pairs, beta, global_pairs, zero_grads=True):
-        """forward + preference (DPO) head + backward on 2 * pairs rows already resident in self.tok / self.labels (rows
-        0..P-1 chosen, row i + P the rejected row of pair i) and their reference log-likelihoods in self.ref.  The loss is
-        the sum of the pair losses softplus(-z) over 1/global_pairs (DESIGN.md §3.7); self.stats [P, 4] holds each pair's
-        (s(chosen), s(rejected), z, loss)."""
-        if 2 * pairs != self.B:
-            raise L.ProgenError(f'preference step: {pairs} pairs need {2 * pairs} resident rows, have {self.B}')
-        self._check_zero_grads(zero_grads)
-        self._forward_device()
-        if zero_grads:
-            self.train_grads().zero_()
-        L.check(self.lib.progen_preference_head(self.logits.data_ptr(), L.F32, self.labels.data_ptr(), self.ref.data_ptr(),
-                                                self.logp.data_ptr(), self.seq_ll.data_ptr(), self.seq_count.data_ptr(),
-                                                self.ce_w.data_ptr(), self.stats.data_ptr(), self.loss.data_ptr(),
-                                                self.ce_scratch.data_ptr(), self.dlogits.data_ptr(), self.act_dt, pairs, self.n,
-                                                self.V, beta, 1.0 / global_pairs, L.stream()), 'preference_head')
-        self._backward_device()
 
     def preference_stats(self, pairs):
         """the last preference step's per-pair statistics as numpy float32 [pairs]"""
@@ -680,32 +707,6 @@ class Engine:
         else:
             self.pclass.copy_(t, non_blocking=True)
         return B
-
-    def property_step_device(self, task, global_batch, zero_grads=True):
-        """forward (without the logits GEMM) + final LayerNorm + masked mean pool + property head + pool backward + the
-        frozen-base backward from the final LayerNorm down, on rows resident in self.tok / self.labels and their targets in
-        self.ptarget / self.pclass (load_property).  The head's parameters and gradients are the last segments of the
-        adapter buffer (lora.Adapters with head_outputs); its loss is scaled by 1/global_batch (DESIGN.md §3.9)."""
-        lo = self.lora
-        if lo is None or not lo.head_outputs:
-            raise L.ProgenError('property step: needs adapters with a property head (the base stays frozen)')
-        self._check_zero_grads(zero_grads)
-        lib, st, B, d, C = self.lib, L.stream(), self.B, self.d, lo.head_outputs
-        self._forward_device(logits=False)
-        if zero_grads:
-            self.train_grads().zero_()
-        L.check(lib.progen_masked_mean_pool(self.yf.data_ptr(), d, self.act_dt, self.labels.data_ptr(), self.emb.data_ptr(),
-                                            B, self.n, d, st), 'masked_mean_pool')
-        reg = task == L.TASK_REGRESSION
-        L.check(lib.progen_property_head(self.emb.data_ptr(), lo.head(lo.params, 'w').data_ptr(),
-                                         lo.head(lo.params, 'b').data_ptr(), B, d, C, task,
-                                         self.ptarget.data_ptr() if reg else 0, 0 if reg else self.pclass.data_ptr(),
-                                         1.0 / global_batch, self.pred.data_ptr(), self.prow_loss.data_ptr(),
-                                         self.loss.data_ptr(), self.dpred.data_ptr(), lo.head(lo.grads, 'w').data_ptr(),
-                                         lo.head(lo.grads, 'b').data_ptr(), self.demb.data_ptr(), st), 'property_head')
-        L.check(lib.progen_masked_mean_pool_bwd(self.demb.data_ptr(), self.labels.data_ptr(), self.dy.data_ptr(), d,
-                                                self.act_dt, B, self.n, d, st), 'masked_mean_pool_bwd')
-        self._backward_body()
 
     def property_stats(self, rows):
         """the last property step's predictions [rows, C] and per-row losses [rows] as numpy float32"""
@@ -750,22 +751,10 @@ class Engine:
             out_p[r0:r0 + B] = host[B * d:].reshape(B, C)
         return out_p, out_e
 
-    def _backward_device(self):
-        """With adapters (self.lora) the base is frozen: no base weight, bias, LayerNorm-scale, SGU or embedding
-        gradient is computed, and every adapted projection's input gradient carries its adapter's tail (lora_bwd)."""
-        d = self.d
-        frozen = self.lora is not None
-        # ---- head
-        hw = P + 'linear'
-        if not frozen:
-            self.colsum(self.dlogits, self.V, self.G(hw, 'b'))
-            self.wgrad_gemm(self.yf, d, self.dlogits, self.V, self.G(hw, 'w'))
-        self.dgrad_gemm(self.dlogits, self.V, self.W(hw, 'w'), d, self.dy)
-        self._backward_body()
-
     def _backward_body(self):
-        """the backward pass below the logits head, from self.dy = d loss / d (final LayerNorm output): the LM head
-        (_backward_device) and the property head (property_step_device) both enter here"""
+        """the backward pass below the loss head (train_step), from self.dy = d loss / d (final LayerNorm output).
+        With adapters (self.lora) the base is frozen: no base weight, bias, LayerNorm-scale, SGU or embedding
+        gradient is computed, and every adapted projection's input gradient carries its adapter's tail (lora_bwd)."""
         lib, st = self.lib, L.stream()
         cfg, d, I, hid, T, n = self.cfg, self.d, self.I, self.hid, self.T, self.n
         shift = cfg['shift_tokens']

@@ -294,12 +294,9 @@ class ProGen:
         With `adapters` (a tree of `init_adapters`' shape; lora_alpha default: its rank) the loss is the adapted
         model's, the base is frozen, and the gradients are the adapters' (a tree of the same shape)."""
         self._ensure_loaded(params)
-        if adapters is None:
-            loss = self.engine.loss_and_grad(data)
-            return float(loss.item()), self.engine.export_grads()
-        lo = self._attach_adapters(adapters, lora_alpha)
+        lo = None if adapters is None else self._attach_adapters(adapters, lora_alpha)
         loss = self.engine.loss_and_grad(data)
-        return float(loss.item()), lo.export_tree(lo.grads)
+        return float(loss.item()), self.engine.export_grads() if lo is None else lo.export_tree(lo.grads)
 
     # ---- low-rank adapters (DESIGN.md §3.8)
     def init_adapters(self, rng, rank, *, alpha=None):
@@ -347,7 +344,7 @@ class ProGen:
         self._ensure_loaded(params)
         eng = self.engine
         P = eng.load_preference(rows, ref)
-        eng.preference_step_device(P, beta, P)
+        eng.train_step(('preference', beta), P)
         return float(eng.loss.item()), eng.export_grads(), eng.preference_stats(P)
 
     def score(self, params, data, *, batch_size=64, return_tokens=False, return_embeddings=False):
@@ -589,7 +586,7 @@ class ProGen:
         lo = self._attach_adapters(adapters, lora_alpha, head)
         eng = self.engine
         B = eng.load_property(r, code, y)
-        eng.property_step_device(code, B)
+        eng.train_step(('property', code), B)
         grads, hgrads = lo.split(lo.export_tree(lo.grads))
         return float(eng.loss.item()), grads, hgrads, eng.property_stats(B)['prediction']
 

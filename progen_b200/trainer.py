@@ -46,7 +46,6 @@ class Trainer:
             lo = self.lora
             self.P, n, self.n_decay, self.P_lp = lo.params, lo.n_padded, lo.n_padded, None
             self.eng.grads = None                  # nothing reads or writes the base gradient while adapters train
-        self.eng.lora = self.lora
         self.lr, self.wd, self.max_norm, self.every = learning_rate, weight_decay, max_grad_norm, grad_accum_every
         self.b1, self.b2, self.eps = b1, b2, eps
         z = lambda: torch.zeros(n, device=self.eng.dev, dtype=torch.float32)
@@ -58,7 +57,7 @@ class Trainer:
         self._works, self._done = [], []
         self._graph, self._graph_key, self._graph_epoch, self._adam_state = None, None, 0, None
         # cuda_graph=True: after two eager steps of one batch shape the step is captured and replayed from then on
-        self._auto_graph, self._eager_key, self._eager_run = bool(cuda_graph), None, 0
+        self._auto_graph, self._eager_key = bool(cuda_graph), None
         self._bucket, self._bucket_layers = None, max(1, int(os.environ.get('PROGEN_DDP_BUCKET_LAYERS', '3')))
         # Gradient exchange (world > 1).  Default: ONE SUM all-reduce of the whole flat buffer after the backward pass, on
         # the compute stream, inside the captured CUDA graph.  Overlapping per-layer buckets with the backward pass lets the
@@ -87,54 +86,55 @@ class Trainer:
         at all — must all scale by 1/5).  Without it the shards are assumed equal.  Returns the device scalar loss
         (global mean when sync_loss)."""
         rows = data.shape[0]
-        gb = int(global_batch) if global_batch is not None else (rows * self.world if self.world > 1 else rows)
-        self.eng.lora = self.lora
-        if rows == 0:
-            # a rank without rows (batch smaller than the world): zero contribution, but every collective is joined
-            self.G.zero_()
-            self.eng.loss.zero_()
-            return self._update(sync_loss)
-        self._drop_graph_unless(rows)
-        if self._graph is not None and self._graph_key == (rows, gb):
-            self.eng.load_batch(data)                      # H2D copies stay outside the graph
-            return self._replay(sync_loss)
-        self.eng.loss_and_grad(data, global_batch=gb)
-        loss = self._update(sync_loss)
-        if self._auto_graph and not self.overlap:
-            key = (data.shape[0], gb)
-            self._eager_run = self._eager_run + 1 if key == self._eager_key else 1
-            self._eager_key = key
-            if self._eager_run >= 2:
-                self.capture_graph(data.shape[0], gb)      # capture does not execute: eng.loss still holds this step's value
-                self._eager_run = 0
-        return loss
+        gb = int(global_batch) if global_batch is not None else rows * self.world
+        return self._step(rows, gb, (), lambda: self.eng.load_batch(data), sync_loss)
 
     def step_resident(self, global_batch=None, sync_loss=False):
         """same, on tokens/labels already copied into engine.tok / engine.labels (bench: inputs resident in HBM)"""
-        gb = global_batch or self.eng.B * self.world
-        self.eng.lora = self.lora
-        self._drop_graph_unless(self.eng.B)
-        if self._graph is not None and self._graph_key == (self.eng.B, gb):
+        return self._step(self.eng.B, global_batch or self.eng.B * self.world, (), None, sync_loss)
+
+    def _step(self, rows, global_rows, objective, load, sync_loss):
+        """One micro-step of `objective` (Engine.train_step) on `rows` rows, then the optimizer update.  `load()` makes
+        the rows resident (None: they are); its H2D copies stay outside the graph.  A captured graph whose key is
+        (rows, global_rows) + objective replays; otherwise the step runs eagerly, and with cuda_graph=True the second
+        eager step in a row of one key is captured for the next one to replay."""
+        eng = self.eng
+        eng.lora = self.lora
+        if rows == 0:
+            # a rank without rows (batch smaller than the world): zero contribution, but every collective is joined
+            self.G.zero_()
+            eng.loss.zero_()
+            return self._update(sync_loss)
+        key = (rows, global_rows) + objective
+        self._drop_graph_unless(rows)
+        if load is not None:
+            load()
+        if self._graph is not None and self._graph_key == key:
             return self._replay(sync_loss)
-        self.eng.step_device(gb)
-        return self._update(sync_loss)
+        eng.train_step(objective, global_rows)
+        loss = self._update(sync_loss)
+        if self._auto_graph and not (self.world > 1 and self.overlap):
+            # _eager_key starts as None, so _eager_run is set here before it is read
+            self._eager_run = self._eager_run + 1 if key == self._eager_key else 1
+            self._eager_key = key
+            if self._eager_run >= 2:
+                self.capture_graph(rows, global_rows, objective=objective)   # capture does not execute: eng.loss
+                self._eager_run = 0                                         # still holds this step's value
+        return loss
 
     # ---- CUDA graph of the whole step: forward, loss, backward, (gradient all-reduce), norm, AdamW, masked copies
-    def capture_graph(self, batch_rows, global_batch=None, install=True):
+    def capture_graph(self, batch_rows, global_batch=None, install=True, objective=()):
         """Capture one training step for batches of `batch_rows` rows into a CUDA graph; later `step` / `step_resident`
         calls with that shape replay it.  The step-dependent optimizer scalars live on the device
         (`progen_adamw_step_dev`), so the graph is identical for every step.  Under data parallelism the NCCL all-reduce
         of the gradient buffer is part of the graph (issued on the capture stream between backward and the norm).  Call
         after at least one eager step of the same shape (kernel attributes, tensor maps, buffers and the NCCL communicator
-        must exist before capture).  `install=False` returns the graph without making it the one `step` replays."""
-        gb = global_batch or batch_rows * self.world
-        return self._capture(batch_rows, (batch_rows, gb), lambda: self.eng.step_device(gb), install)
-
-    def _capture(self, batch_rows, key, step_device, install=True):
-        """capture step_device() + gradient exchange + optimizer for batches of `batch_rows` rows; `key` is what a later
-        step must match to replay it"""
+        must exist before capture).  `install=False` returns the graph without making it the one `step` replays.
+        `objective` (Engine.train_step) selects the loss: ('preference', beta) captures the step `preference_step`
+        replays, with batch_rows = 2 * pairs and global_batch = the global pair count."""
         if self.world > 1 and self.overlap:
             raise L.ProgenError('capture_graph: PROGEN_DDP_OVERLAP=1 launches its bucketed all-reduces eagerly')
+        gb = global_batch or batch_rows * self.world
         eng = self.eng
         eng.lora = self.lora
         eng.ensure_batch(batch_rows)
@@ -144,11 +144,11 @@ class Trainer:
         torch.cuda.synchronize()
         g = torch.cuda.CUDAGraph()
         with torch.cuda.graph(g):
-            step_device()
+            eng.train_step(objective, gb)
             self._allreduce_grads()
             self._update_captured()
         if install:
-            self._graph, self._graph_key, self._graph_epoch = g, key, getattr(eng, 'alloc_epoch', 0)
+            self._graph, self._graph_key, self._graph_epoch = g, (batch_rows, gb) + objective, getattr(eng, 'alloc_epoch', 0)
         return g
 
     # ---- preference (DPO) fine-tuning
@@ -169,26 +169,7 @@ class Trainer:
                                           what='preference_step', allow_empty=True)
         P = rows.shape[0] // 2
         self._pref_pairs = P
-        self.eng.lora = self.lora
-        if P == 0:
-            self.G.zero_()
-            self.eng.loss.zero_()
-            return self._update(sync_loss)
-        key = (2 * P, gp, 'preference', beta)
-        self._drop_graph_unless(2 * P)
-        if self._graph is not None and self._graph_key == key:
-            self.eng.load_preference(rows, ref)            # H2D copies stay outside the graph
-            return self._replay(sync_loss)
-        self.eng.load_preference(rows, ref)
-        self.eng.preference_step_device(P, beta, gp)
-        loss = self._update(sync_loss)
-        if self._auto_graph and not self.overlap:
-            self._eager_run = self._eager_run + 1 if key == self._eager_key else 1
-            self._eager_key = key
-            if self._eager_run >= 2:
-                self._capture(2 * P, key, lambda: self.eng.preference_step_device(P, beta, gp))
-                self._eager_run = 0
-        return loss
+        return self._step(2 * P, gp, ('preference', beta), lambda: self.eng.load_preference(rows, ref), sync_loss)
 
     # ---- property fine-tuning (a head on the pooled embedding, adapters on the frozen base)
     def property_step(self, rows, targets, sync_loss=False):
@@ -210,22 +191,7 @@ class Trainer:
             raise L.ProgenError('property_step: needs at least one row')
         y = check_targets(targets, task, self.lora.head_outputs, B, 'property_step')
         self._prop_rows = B
-        self.eng.lora = self.lora
-        key = (B, B, 'property', self.task)
-        self._drop_graph_unless(B)
-        if self._graph is not None and self._graph_key == key:
-            self.eng.load_property(r, self.task, y)        # H2D copies stay outside the graph
-            return self._replay(sync_loss)
-        self.eng.load_property(r, self.task, y)
-        self.eng.property_step_device(self.task, B)
-        loss = self._update(sync_loss)
-        if self._auto_graph:
-            self._eager_run = self._eager_run + 1 if key == self._eager_key else 1
-            self._eager_key = key
-            if self._eager_run >= 2:
-                self._capture(B, key, lambda: self.eng.property_step_device(self.task, B))
-                self._eager_run = 0
-        return loss
+        return self._step(B, B, ('property', self.task), lambda: self.eng.load_property(r, self.task, y), sync_loss)
 
     def property_stats(self):
         """the last `property_step`'s predictions [B, C] (regression values, or class logits) and per-row losses [B] as
@@ -339,17 +305,10 @@ class Trainer:
     def evaluate(self, data):
         """validation loss (train.py:207-211): forward + loss only"""
         eng = self.eng
-        d = torch.as_tensor(np.asarray(data).astype(np.int32) if not isinstance(data, torch.Tensor) else data)
-        self._drop_graph_unless(d.shape[0])
         eng.lora = self.lora
-        eng.ensure_batch(d.shape[0])
-        dd = d.to(device=eng.dev, dtype=torch.int32)
-        eng.tok.copy_(dd[:, :-1].reshape(-1))
-        eng.labels.copy_(dd[:, 1:].reshape(-1))
-        eng._forward_device()
-        eng.loss.zero_()
-        L.check(L.load().progen_ce_fwd_bwd(eng.logits.data_ptr(), L.F32, eng.labels.data_ptr(), eng.ce_w.data_ptr(), eng.loss.data_ptr(),
-                                           0, eng.act_dt, eng.B, eng.n, eng.V, 1.0 / d.shape[0], L.stream()), 'ce_fwd')
+        B = eng.load_batch(data)
+        self._drop_graph_unless(B)
+        eng.train_step((), B, backward=False)
         return eng.loss
 
     # ---- checkpoint interchange (haiku-shaped trees, train.py:196-202)

@@ -62,7 +62,7 @@ def main():
         tr.preference_step(c, r, rc, rr, beta=beta)
     torch.cuda.synchronize()
     g_plain = tr.capture_graph(B, B, install=False)
-    g_pref = tr._capture(B, None, lambda: eng.preference_step_device(P, beta, P), install=False)
+    g_pref = tr.capture_graph(B, P, install=False, objective=('preference', beta))
     eng.load_preference(*(np.concatenate(x) for x in ((c, r), (rc, rr))))
     for g in (g_plain, g_pref):
         timed(g.replay, 2)

@@ -147,7 +147,7 @@ def test_ln_residual_shift_wide(d, B, n):
 # ------------------------------------------------------------------------------------------------ GEMM
 def _gemm_shapes(name):
     """{id: (M, N, K, a_mn, b_mn, epi, wgrad (K_in, N_out) or None)} of every GEMM of one GLU and one gMLP layer of config
-    `name` (the spatial GEMMs apart: test_sgu_spatial_gemms), as Engine._forward_device / _backward_device issue them at
+    `name` (the spatial GEMMs apart: test_sgu_spatial_gemms), as Engine._forward_device / _backward_body issue them at
     the benchmarked batch"""
     from progen_b200 import lib as L
     c = CONFIGS[name]

@@ -319,7 +319,7 @@ def test_refusals():
         tr.property_step(rows, y)
     model.property_loss_and_grad(params, rows, y, adapters=ad, head=head, task='regression')
     with pytest.raises(L.ProgenError, match='zero_grads'):
-        model.engine.property_step_device(L.TASK_REGRESSION, 3, zero_grads=False)
+        model.engine.train_step(('property', L.TASK_REGRESSION), 3, zero_grads=False)
     big = {HEAD: {'w': np.zeros((128, 65), np.float32), 'b': np.zeros(65, np.float32)}}
     with pytest.raises(L.ProgenError, match='1 to 64'):
         model.trainer(params, adapters=ad, head=big, task='regression')
