@@ -55,17 +55,71 @@ def layer_kinds(depth, global_mlp_depth, ff_glu):
 
 
 class ParamSpec:
-    __slots__ = ('module', 'name', 'shape', 'decay', 'interleave', 'offset', 'size')
+    __slots__ = ('module', 'name', 'shape', 'decay', 'interleave', 'offset', 'stop', 'size')
 
     def __init__(self, module, name, shape, interleave=False):
         self.module, self.name, self.shape = module, name, tuple(shape)
         self.decay = len(shape) > 1                    # optax mask: tree_map(lambda x: x.ndim > 1) — train.py:113
         self.interleave = interleave
         self.size = int(np.prod(shape))
-        self.offset = -1
+        self.offset = self.stop = -1                   # [offset, stop): the padded segment (set by Layout)
+
+
+class Layout:
+    """The engine layout of a flat fp32 buffer of haiku-shaped leaves: the ndim > 1 leaves first (the weight-decay mask
+    is then one prefix), then the rest, each group in the order of `specs`; every segment starts on an ALIGN boundary;
+    a GLU feed-forward input's columns (value | gate) are interleaved (value_j, gate_j), so both halves of a pair land
+    in one GEMM tile.  Trees keep the order of `specs`.  Needs no device."""
+
+    def __init__(self, specs):
+        self.specs = list(specs)
+        self.by_key = {(s.module, s.name): s for s in self.specs}
+        off = 0
+        for s in [s for s in self.specs if s.decay] + [s for s in self.specs if not s.decay]:
+            s.offset = off
+            off += (s.size + ALIGN - 1) // ALIGN * ALIGN
+            s.stop = off
+        self.size = off                                 # padded size of the buffer
+        self.num_params = sum(s.size for s in self.specs)
+
+    def span(self, specs):
+        """[start, stop) of the padded segments of `specs` (contiguous when they are adjacent in the layout)"""
+        return min(s.offset for s in specs), max(s.stop for s in specs)
+
+    def seg(self, buf, module, name):
+        s = self.by_key[(module, name)]
+        return buf[s.offset:s.offset + s.size]
+
+    def pack(self, tree):
+        """haiku-shaped tree {module: {name: array}} (numpy or torch leaves) -> host float32 [size] in this layout"""
+        host = np.zeros(self.size, np.float32)
+        for s in self.specs:
+            a = tree[s.module][s.name]
+            a = (a.detach().cpu().numpy() if isinstance(a, torch.Tensor) else np.asarray(a)).astype(np.float32)
+            if a.shape != s.shape:
+                raise L.ProgenError(f'{s.module}/{s.name}: expected shape {s.shape}, got {a.shape}')
+            host[s.offset:s.offset + s.size] = (_interleave(a) if s.interleave else a).ravel()
+        return host
+
+    def unpack(self, buf):
+        """a tensor in this layout -> haiku-shaped tree of float32 numpy arrays"""
+        host = buf.detach().float().cpu().numpy()
+        out = {}
+        for s in self.specs:
+            a = host[s.offset:s.offset + s.size].reshape(s.shape).copy()
+            out.setdefault(s.module, {})[s.name] = _deinterleave(a) if s.interleave else a
+        return out
+
+    def shapes(self):
+        """the shape tree {module: {name: shape}}"""
+        out = {}
+        for s in self.specs:
+            out.setdefault(s.module, {})[s.name] = s.shape
+        return out
 
 
 def build_param_specs(cfg):
+    """the Layout of the model's parameters"""
     d, V, n = cfg['dim'], cfg['num_tokens'], cfg['seq_len']
     inner = cfg['heads'] * cfg['dim_head']
     hid = d * cfg['ff_mult']
@@ -89,12 +143,7 @@ def build_param_specs(cfg):
         specs += [ParamSpec(f + 'linear_1', 'w', (h_out, d)), ParamSpec(f + 'linear_1', 'b', (d,))]
     specs += [ParamSpec(P + 'layer_norm', 'scale', (d,)),
               ParamSpec(P + 'linear', 'w', (d, V)), ParamSpec(P + 'linear', 'b', (V,))]
-    off = 0
-    for s in [s for s in specs if s.decay] + [s for s in specs if not s.decay]:
-        s.offset = off
-        off += (s.size + ALIGN - 1) // ALIGN * ALIGN
-    n_decay = sum((s.size + ALIGN - 1) // ALIGN * ALIGN for s in specs if s.decay)
-    return specs, off, n_decay
+    return Layout(specs)
 
 
 def _interleave(a):
@@ -108,25 +157,30 @@ def _deinterleave(a):
 
 
 class Acts:
-    """One activation set: the buffers one forward pass runs on (B sequences, T = B * seq_len token rows).
+    """One activation set: the buffers one forward pass runs on (B sequences of n positions, T = B * n token rows).
     `X` lists the residual stream at every LayerNorm input and `lay` one scratch dict per layer.  The training set keeps
     all of them (the backward pass reads them); the inference set (`inplace`) repeats one residual buffer, updated in
     place, and one layer's scratch, and stores no GLU / GELU pre-activation (`u` is None)."""
 
-    def __init__(self, B, T, tok, labels, X, lay, meanf, rstdf, yf, logits, inplace=False, rows=None, res=None):
-        self.B, self.T, self.tok, self.labels, self.X, self.lay = B, T, tok, labels, X, lay
+    def __init__(self, B, n, tok, labels, X, lay, meanf, rstdf, yf, logits, inplace=False, rows=None, res=None):
+        self.B, self.n, self.T = B, n, B * n
+        self.tok, self.labels, self.X, self.lay = tok, labels, X, lay
         self.meanf, self.rstdf, self.yf, self.logits = meanf, rstdf, yf, logits
         self.inplace = inplace
         self.rows = rows        # inference: [B, n+1] int32 staging of the input rows (one H2D copy per chunk)
         self.res = res          # inference: flat fp32 per-chunk results (see Engine.score)
 
     def view(self, B, n):
-        """the first B sequences of this set (same memory): a ragged last chunk runs on the cached buffers"""
+        """the first B sequences of this set, cut to their first n positions (same memory): a ragged last chunk or a
+        cut forward runs on the cached buffers.  `rows` is the contiguous (B, n+1) prefix of the staging buffer."""
+        if (B, n) == (self.B, self.n):
+            return self
         T = B * n
         cut = lambda t: None if t is None else t[:T]
-        return Acts(B, T, cut(self.tok), cut(self.labels), [cut(x) for x in self.X],
+        rows = None if self.rows is None else self.rows.view(-1)[:B * (n + 1)].view(B, n + 1)
+        return Acts(B, n, cut(self.tok), cut(self.labels), [cut(x) for x in self.X],
                     [{k: cut(v) for k, v in s.items()} for s in self.lay], cut(self.meanf), cut(self.rstdf), cut(self.yf),
-                    cut(self.logits), self.inplace, None if self.rows is None else self.rows[:B], self.res)
+                    cut(self.logits), self.inplace, rows, self.res)
 
 
 class Engine:
@@ -166,9 +220,9 @@ class Engine:
             bad = [k for k, v in dict(dim=d, inner=self.I, seq_len=n, num_tokens=self.V).items() if v % 64]
             if bad:
                 raise L.ProgenError(f'mixed_precision (tensor-core path) needs {bad} to be multiples of 64')
-        self.specs, self.n_params_padded, self.n_decay = build_param_specs(cfg)
-        self.by_key = {(s.module, s.name): s for s in self.specs}
-        self.num_params = sum(s.size for s in self.specs)
+        self.layout = build_param_specs(cfg)
+        self.n_params_padded, self.num_params = self.layout.size, self.layout.num_params
+        self.n_decay = self.layout.span([s for s in self.layout.specs if s.decay])[1]
         f32 = dict(device=self.dev, dtype=torch.float32)
         self.params = torch.zeros(self.n_params_padded, **f32)
         self.grads = torch.zeros(self.n_params_padded, **f32)
@@ -195,44 +249,19 @@ class Engine:
     def layer_grad_range(self, i):
         """[start, stop) of layer i's ndim>1 parameters inside the flat buffers (contiguous by construction)."""
         pre = (P + f'attn{i}/~/', P + f'ff{i}/~/')
-        segs = [s for s in self.specs if s.decay and s.module.startswith(pre)]
-        return min(s.offset for s in segs), max(s.offset + (s.size + ALIGN - 1) // ALIGN * ALIGN for s in segs)
+        return self.layout.span([s for s in self.layout.specs if s.decay and s.module.startswith(pre)])
 
     # ------------------------------------------------------------------------------------------ parameters
-    def seg(self, buf, module, name):
-        s = self.by_key[(module, name)]
-        return buf[s.offset:s.offset + s.size]
-
     def load_params(self, params):
         """haiku-shaped nested dict {module: {name: array}} (numpy or torch) -> flat engine layout on the device."""
-        host = np.zeros(self.n_params_padded, np.float32)
-        for s in self.specs:
-            a = params[s.module][s.name]
-            a = a.detach().cpu().numpy() if isinstance(a, torch.Tensor) else np.asarray(a)
-            a = a.astype(np.float32)
-            if a.shape != s.shape:
-                raise L.ProgenError(f'{s.module}/{s.name}: expected shape {s.shape}, got {a.shape}')
-            if s.interleave:
-                a = _interleave(a)
-            host[s.offset:s.offset + s.size] = a.ravel()
-        self.params.copy_(torch.from_numpy(host))
+        self.params.copy_(torch.from_numpy(self.layout.pack(params)))
         self.refresh_compute_copies()
 
-    def export_tree(self, buf):
-        host = buf.detach().float().cpu().numpy()
-        out = {}
-        for s in self.specs:
-            a = host[s.offset:s.offset + s.size].reshape(s.shape).copy()
-            if s.interleave:
-                a = _deinterleave(a)
-            out.setdefault(s.module, {})[s.name] = a
-        return out
-
     def export_params(self):
-        return self.export_tree(self.params)
+        return self.layout.unpack(self.params)
 
     def export_grads(self):
-        return self.export_tree(self.base_grads())
+        return self.layout.unpack(self.base_grads())
 
     def base_grads(self):
         """the flat fp32 gradient of every parameter; released while adapters train (a LoRA Trainer) and allocated
@@ -252,18 +281,18 @@ class Engine:
     def refresh_masked_copies(self):
         st = L.stream()
         for i, wm in self.wm.items():
-            src = self.seg(self.params, P + f'ff{i}/~/sgu', 'spatial_weights')
+            src = self.Pf(P + f'ff{i}/~/sgu', 'spatial_weights')
             L.check(self.lib.progen_tril_cast(src.data_ptr(), wm.data_ptr(), self.act_dt, self.n, st), 'tril_cast')
 
     def W(self, module, name):
         """GEMM operand view of a parameter: bf16 mirror under mixed precision, fp32 master otherwise."""
-        return self.seg(self.params_lp if self.mp else self.params, module, name)
+        return self.layout.seg(self.params_lp if self.mp else self.params, module, name)
 
     def Pf(self, module, name):
-        return self.seg(self.params, module, name)
+        return self.layout.seg(self.params, module, name)
 
     def G(self, module, name):
-        return self.seg(self.base_grads(), module, name)
+        return self.layout.seg(self.base_grads(), module, name)
 
     # ------------------------------------------------------------------------------------------ workspaces
     def ensure_batch(self, B):
@@ -319,7 +348,7 @@ class Engine:
         half = hid // 2
         if 'sgu' in self.kinds:
             self.dpj, self.dsg, self.dgp, self.dgn = A(T, half), A(T, half), A(T, half), A(T, half)
-        self.acts = Acts(B, T, self.tok, self.labels, self.X, self.lay, self.meanf, self.rstdf, self.yf, self.logits)
+        self.acts = Acts(B, self.n, self.tok, self.labels, self.X, self.lay, self.meanf, self.rstdf, self.yf, self.logits)
 
     def inference_acts(self, B):
         """Activation set of a forward pass that keeps no training state, for up to B sequences: one fp32 residual buffer
@@ -327,7 +356,7 @@ class Engine:
         the fp32 logits and the scoring outputs.  Allocated on first use and kept for later calls of the same or smaller
         row count, apart from the training set: `ensure_batch`, `alloc_epoch` and captured training graphs are untouched."""
         if self.infer is not None and self.infer.B >= B:
-            return self.infer if self.infer.B == B else self.infer.view(B, self.n)
+            return self.infer.view(B, self.n)
         self.infer = None                                       # release the smaller set before allocating the larger one
         n, d, I, hid, V = self.n, self.d, self.I, self.hid, self.V
         T = B * n
@@ -345,7 +374,7 @@ class Engine:
             # overwrites the spatial GEMM output (dead once the gate has read it)
             s.update(mean3=F(T), rstd3=F(T), gn=gn, gp=gp, sg=gn, pj=gp)
         nl = len(self.kinds)
-        self.infer = Acts(B, T, torch.empty(T, device=dev, dtype=torch.int32), torch.empty(T, device=dev, dtype=torch.int32),
+        self.infer = Acts(B, n, torch.empty(T, device=dev, dtype=torch.int32), torch.empty(T, device=dev, dtype=torch.int32),
                           [x] * (2 * nl + 1), [s] * nl, F(T), F(T), A(T, d), F(T, V), inplace=True,
                           rows=torch.empty(B, n + 1, device=dev, dtype=torch.int32), res=F(B * (2 + n + d)))
         return self.infer
@@ -359,9 +388,9 @@ class Engine:
         lo = self.lora
         if lo is None:
             return {}
-        u = lo.u[module]
-        self.fwd_gemm(x, K, lo.seg(lo.lp, module, 'lora_a'), lo.r, u)
-        return dict(A2=u, lda2=lo.r, B2=lo.seg(lo.lp, module, 'lora_b'), ldb2=N, K2=lo.r)
+        u, seg = lo.u[module], lo.layout.seg
+        self.fwd_gemm(x, K, seg(lo.lp, module, 'lora_a'), lo.r, u)
+        return dict(A2=u, lda2=lo.r, B2=seg(lo.lp, module, 'lora_b'), ldb2=N, K2=lo.r)
 
     def lora_bwd(self, x, K, module, dy, N):
         """adapters: from the projection's output gradient dy [T, N], g' = s g = dy (s B)^T, dB += u^T dy (scaled by s
@@ -369,10 +398,11 @@ class Engine:
         lo = self.lora
         if lo is None:
             return {}
-        g, A = lo.g, lo.seg(lo.lp, module, 'lora_a')
-        self.dgrad_gemm(dy, N, lo.seg(lo.lp, module, 'lora_b'), lo.r, g)
-        self.wgrad_gemm(lo.u[module], lo.r, dy, N, lo.seg(lo.grads, module, 'lora_b'))
-        self.wgrad_gemm(x, K, g, lo.r, lo.seg(lo.grads, module, 'lora_a'))
+        seg = lo.layout.seg
+        g, A = lo.g, seg(lo.lp, module, 'lora_a')
+        self.dgrad_gemm(dy, N, seg(lo.lp, module, 'lora_b'), lo.r, g)
+        self.wgrad_gemm(lo.u[module], lo.r, dy, N, seg(lo.grads, module, 'lora_b'))
+        self.wgrad_gemm(x, K, g, lo.r, seg(lo.grads, module, 'lora_a'))
         return dict(A2=g, lda2=lo.r, B2=A, ldb2=lo.r, K2=lo.r)
 
     def fwd_gemm(self, x, K, w, N, out, epi=L.EPI_STORE, out_dtype=None, acts=None, **kw):
@@ -402,10 +432,11 @@ class Engine:
     def colsum(self, t, N, out, ld=None):
         L.check(self.lib.progen_colsum(t.data_ptr(), N if ld is None else ld, L.dt(t), out.data_ptr(), self.T, N, L.stream()), 'colsum')
 
-    def ln_fwd(self, x, ldx, scale, y, ldy, mean, rstd, dcols, shift, acts=None, seq_len=None):
+    def ln_fwd(self, x, ldx, scale, y, ldy, mean, rstd, dcols, shift, acts=None):
+        a = acts or self.acts
         L.check(self.lib.progen_ln_shift_fwd(x.data_ptr(), ldx, L.dt(x), scale.data_ptr(), y.data_ptr(), ldy, L.dt(y),
-                                             mean.data_ptr(), rstd.data_ptr(), (acts or self.acts).T, dcols,
-                                             self.n if seq_len is None else seq_len, int(shift), L.stream()), 'ln_fwd')
+                                             mean.data_ptr(), rstd.data_ptr(), a.T, dcols, a.n, int(shift), L.stream()),
+                'ln_fwd')
 
     # ------------------------------------------------------------------------------------------ forward
     def forward(self, ids):
@@ -430,18 +461,15 @@ class Engine:
         acts.tok.copy_(torch.as_tensor(ids).reshape(-1).to(device=self.dev, dtype=torch.int32))
         self._forward_device(acts, sink=lambda i, name, buf: sink(i, name, buf, P))
 
-    def _forward_device(self, acts=None, sink=None, length=None, logits=True):
-        """forward pass on activation set `acts` (default: the training set, which keeps what the backward pass reads);
-        with a `sink` (Engine.prefill) the layers' state goes to it and the logits head is skipped; `logits=False` stops
-        after the final LayerNorm (acts.yf), for the property head.
-        `length` (default seq_len): the positions per row, acts.T = acts.B * length.  Every mixing op is causal, so a
-        forward cut to the first `length` positions computes exactly those positions of the full one (DESIGN.md §3.6)."""
+    def _forward_device(self, acts=None, sink=None, logits=True):
+        """forward pass on activation set `acts` (default: the training set, which keeps what the backward pass reads)
+        over its acts.n positions per row; with a `sink` (Engine.prefill) the layers' state goes to it and the logits
+        head is skipped; `logits=False` stops after the final LayerNorm (acts.yf), for the property head.  Every mixing
+        op is causal, so a forward on a view cut to the first n positions computes exactly those positions of the full
+        one (DESIGN.md §3.6)."""
         acts = self.acts if acts is None else acts
         lib, st = self.lib, L.stream()
-        cfg, d, I, hid, T = self.cfg, self.d, self.I, self.hid, acts.T
-        n = self.n if length is None else length
-        if T != acts.B * n:
-            raise L.ProgenError(f'forward: {T} token rows are not {acts.B} rows of length {n}')
+        cfg, d, I, hid, T, n = self.cfg, self.d, self.I, self.hid, acts.T, acts.n
         shift = cfg['shift_tokens']
         lo = self.lora if acts is self.acts else None       # adapters run on the training set only
         if lo is not None:
@@ -455,17 +483,17 @@ class Engine:
             # in place (inference): x0 = x1 = x2 is one buffer, and the residual epilogue without aux reads its output
             x0, x1, x2 = acts.X[2 * i], acts.X[2 * i + 1], acts.X[2 * i + 2]
             # ---- LocalAttention (progen.py:73-103)
-            self.ln_fwd(x0, d, self.Pf(a + 'layer_norm', 'scale'), s['y1'], d, s['mean1'], s['rstd1'], d, shift, acts=acts, seq_len=n)
+            self.ln_fwd(x0, d, self.Pf(a + 'layer_norm', 'scale'), s['y1'], d, s['mean1'], s['rstd1'], d, shift, acts=acts)
             self.fwd_gemm(s['y1'], d, self.W(a + 'linear', 'w'), 3 * I, s['qkv'], epi=L.EPI_ROTARY, rot_sin=self.rot_sin,
                           rot_cos=self.rot_cos, seq_len=n, dim_head=self.dh, acts=acts, **tail(s['y1'], d, a + 'linear', 3 * I))
             if sink is not None:
                 sink(i, 'qkv', s['qkv'])
                 sink(i, 'y1', s['y1'])
-            self.attn_fwd(s['qkv'], s['att'], s['lse'], acts=acts, seq_len=n)
+            self.attn_fwd(s['qkv'], s['att'], s['lse'], acts=acts)
             self.fwd_gemm(s['att'], I, self.W(a + 'linear_1', 'w'), d, x1, epi=L.EPI_RESIDUAL, bias=self.Pf(a + 'linear_1', 'b'),
                           aux=None if acts.inplace else x0, ldaux=d, acts=acts, **tail(s['att'], I, a + 'linear_1', d))
             # ---- FeedForward (progen.py:131-149); s['u'] is None in the inference set: no pre-activation store
-            self.ln_fwd(x1, d, self.Pf(f + 'layer_norm', 'scale'), s['y2'], d, s['mean2'], s['rstd2'], d, shift, acts=acts, seq_len=n)
+            self.ln_fwd(x1, d, self.Pf(f + 'layer_norm', 'scale'), s['y2'], d, s['mean2'], s['rstd2'], d, shift, acts=acts)
             if sink is not None:
                 sink(i, 'y2', s['y2'])
             if kind == 'glu':
@@ -481,7 +509,7 @@ class Engine:
                 g = f + 'sgu'
                 gate = s['hact'][:, half:]
                 self.ln_fwd(gate, hid, self.Pf(g + '/~/layer_norm', 'scale'), s['gn'], half, s['mean3'], s['rstd3'], half, False,
-                            acts=acts, seq_len=n)
+                            acts=acts)
                 # gate_b = tril(W) @ gn_b for every sequence b; masked K tiles are skipped (causal=1)
                 self._mm(M=n, N=half, K=n, A=self.wm[i], lda=self.n, B=s['gn'], ldb=half, b_mn=True, out=s['gp'], ldo=half,
                          out_dtype=self.act_dt, batch=acts.B, b_batch_rows=n, d_batch_rows=n, causal=1)
@@ -499,15 +527,15 @@ class Engine:
             return
         # ---- to_logits (progen.py:219-222)
         xl = acts.X[-1]
-        self.ln_fwd(xl, d, self.Pf(P + 'layer_norm', 'scale'), acts.yf, d, acts.meanf, acts.rstdf, d, False, acts=acts, seq_len=n)
+        self.ln_fwd(xl, d, self.Pf(P + 'layer_norm', 'scale'), acts.yf, d, acts.meanf, acts.rstdf, d, False, acts=acts)
         if not logits:
             return
         self.fwd_gemm(acts.yf, d, self.W(P + 'linear', 'w'), self.V, acts.logits, bias=self.Pf(P + 'linear', 'b'), out_dtype=L.F32,
                       acts=acts)
 
-    def attn_fwd(self, qkv, out, lse, acts=None, seq_len=None):
-        B = (acts or self.acts).B
-        n = self.n if seq_len is None else seq_len
+    def attn_fwd(self, qkv, out, lse, acts=None):
+        a = acts or self.acts
+        B, n = a.B, a.n
         if self.attn_tc:
             L.check(self.lib.progen_local_attn_fwd_tc(qkv.data_ptr(), out.data_ptr(), lse.data_ptr(), B, n, self.w, self.h,
                                                       self.dh, L.stream()), 'local_attn_fwd')
@@ -526,6 +554,20 @@ class Engine:
                                                     L.stream()), 'local_attn_bwd')
 
     # ------------------------------------------------------------------------------------------ scoring (inference)
+    def _chunks(self, rows, batch_size, n):
+        """The inference forward's chunks of rows (N >= 1, seq_len + 1), a host int32 tensor, batch_size rows at a time,
+        each cut to its first n positions: yields (r0, acts), acts the (B, n) view of the inference set with the chunk's
+        ids and labels in acts.tok / acts.labels, staged by one H2D copy of the contiguous (B, n + 1) block acts.rows."""
+        full = self.inference_acts(min(batch_size, rows.shape[0]))
+        for r0 in range(0, rows.shape[0], batch_size):
+            chunk = rows[r0:r0 + batch_size, :n + 1]
+            B = chunk.shape[0]
+            acts = full.view(B, n)
+            acts.rows.copy_(chunk)
+            acts.tok.view(B, n).copy_(acts.rows[:, :-1])
+            acts.labels.view(B, n).copy_(acts.rows[:, 1:])
+            yield r0, acts
+
     def score(self, data, batch_size=64, tokens=False, embeddings=False, length=None):
         """data: (N, n+1) integer rows (ids = data[:, :-1], labels = data[:, 1:], as in loss_and_grad) -> dict of numpy
         arrays: log_likelihood [N] (sum of the label log-probabilities under the loss mask), num_tokens [N] (mask size);
@@ -543,14 +585,13 @@ class Engine:
         if batch_size < 1:
             raise L.ProgenError(f'score: batch_size must be >= 1, got {batch_size}')
         N, n, d = rows.shape[0], self.n, self.d
-        cut = n if length is None else length
         if length is not None:
             if not isinstance(length, (int, np.integer)) or not (length == n or (0 < length < n and length % CUT_ALIGN == 0)):
                 raise L.ProgenError(f'score: length must be seq_len ({n}) or a multiple of {CUT_ALIGN} below it, got {length!r}')
             if N and int(counted_length(rows[:, 1:].numpy()).max()) > length:
                 raise L.ProgenError(f'score: length {length} cuts off counted positions (cut_length of these rows: '
                                     f'{cut_length(rows[:, 1:].numpy())})')
-            cut = int(length)
+        cut = n if length is None else int(length)
         out = dict(log_likelihood=np.zeros(N, np.float32), num_tokens=np.zeros(N, np.int64))
         if tokens:
             out['token_logp'] = np.zeros((N, n), np.float32)
@@ -558,28 +599,19 @@ class Engine:
             out['embedding'] = np.zeros((N, d), np.float32)
         if N == 0:
             return out
-        full = self.inference_acts(min(batch_size, N))
         lib, st = self.lib, L.stream()
-        for r0 in range(0, N, batch_size):
-            chunk = rows[r0:r0 + batch_size]
-            B = chunk.shape[0]
-            acts = full if B == full.B and cut == n else full.view(B, cut)
-            T = acts.T
-            # the rows staged as one contiguous (B, cut + 1) block: one H2D copy of what the cut forward reads
-            staged = acts.rows if cut == n else full.rows.view(-1)[:B * (cut + 1)].view(B, cut + 1)
-            staged.copy_(chunk if cut == n else chunk[:, :cut + 1])
-            acts.tok.view(B, cut).copy_(staged[:, :-1])
-            acts.labels.view(B, cut).copy_(staged[:, 1:])
-            self._forward_device(acts, length=length)
+        for r0, acts in self._chunks(rows, batch_size, cut):
+            B, T, res = acts.B, acts.T, acts.res
+            self._forward_device(acts)
             # results, packed for one D2H copy: seq_ll [B] | seq_count [B] | logp [T] | embedding [B, d]
-            ll, cnt, lp, emb = full.res[:B], full.res[B:2 * B], full.res[2 * B:2 * B + T], full.res[2 * B + T:2 * B + T + B * d]
+            ll, cnt, lp, emb = res[:B], res[B:2 * B], res[2 * B:2 * B + T], res[2 * B + T:2 * B + T + B * d]
             L.check(lib.progen_token_logprob(acts.logits.data_ptr(), L.F32, acts.labels.data_ptr(), lp.data_ptr(), ll.data_ptr(),
                                              cnt.data_ptr(), B, cut, self.V, st), 'token_logprob')
             if embeddings:
                 L.check(lib.progen_masked_mean_pool(acts.yf.data_ptr(), d, self.act_dt, acts.labels.data_ptr(), emb.data_ptr(),
                                                     B, cut, d, st), 'masked_mean_pool')
             used = 2 * B + (T + B * d if embeddings else T if tokens else 0)
-            host = full.res[:used].cpu().numpy()
+            host = res[:used].cpu().numpy()
             out['log_likelihood'][r0:r0 + B] = host[:B]
             out['num_tokens'][r0:r0 + B] = host[B:2 * B].astype(np.int64)
             if tokens:
@@ -721,29 +753,21 @@ class Engine:
         positions only, so it is bitwise the full-length one), without the logits GEMM, then progen_masked_mean_pool and
         progen_property_head without targets, batch_size rows at a time, one D2H copy per chunk."""
         rows = torch.as_tensor(np.asarray(data).astype(np.int32))
-        N, n, d = rows.shape[0], self.n, self.d
+        N, d = rows.shape[0], self.d
         C = int(np.asarray(w).shape[1])
         out_p, out_e = np.zeros((N, C), np.float32), np.zeros((N, d), np.float32)
         if N == 0:
             return out_p, out_e
-        cut = cut_length(rows[:, 1:].numpy())
         hw = torch.tensor(np.asarray(w, np.float32), device=self.dev)
         hb = torch.tensor(np.asarray(b, np.float32), device=self.dev)
-        full = self.inference_acts(min(batch_size, N))
-        res = torch.empty(full.B * (d + C), device=self.dev, dtype=torch.float32)
+        res = torch.empty(min(batch_size, N) * (d + C), device=self.dev, dtype=torch.float32)
         lib, st = self.lib, L.stream()
-        for r0 in range(0, N, batch_size):
-            chunk = rows[r0:r0 + batch_size]
-            B = chunk.shape[0]
-            acts = full if B == full.B and cut == n else full.view(B, cut)
-            staged = acts.rows if cut == n else full.rows.view(-1)[:B * (cut + 1)].view(B, cut + 1)
-            staged.copy_(chunk if cut == n else chunk[:, :cut + 1])
-            acts.tok.view(B, cut).copy_(staged[:, :-1])
-            acts.labels.view(B, cut).copy_(staged[:, 1:])
-            self._forward_device(acts, length=cut, logits=False)
+        for r0, acts in self._chunks(rows, batch_size, cut_length(rows[:, 1:].numpy())):
+            B = acts.B
+            self._forward_device(acts, logits=False)
             emb, pred = res[:B * d], res[B * d:B * (d + C)]
             L.check(lib.progen_masked_mean_pool(acts.yf.data_ptr(), d, self.act_dt, acts.labels.data_ptr(), emb.data_ptr(),
-                                                B, cut, d, st), 'masked_mean_pool')
+                                                B, acts.n, d, st), 'masked_mean_pool')
             L.check(lib.progen_property_head(emb.data_ptr(), hw.data_ptr(), hb.data_ptr(), B, d, C, L.TASK_REGRESSION, 0, 0,
                                              1.0, pred.data_ptr(), 0, 0, 0, 0, 0, 0, st), 'property_head')
             host = res[:B * (d + C)].cpu().numpy()

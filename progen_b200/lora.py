@@ -5,15 +5,15 @@ adapter tree is haiku-shaped, {module: {'lora_a': A, 'lora_b': B}}, over the mod
 of a GLU feed-forward input's B are in haiku order (value | gate) there and interleaved in the engine, like the base
 weight.  Everything else of the model stays frozen.
 
-On the device the adapters live in one flat fp32 buffer in engine layout (every A segment, then every B segment, each
-on an ALIGN boundary) with a compute copy in the act dtype that holds A and s B: the forward folds u B into the
-projection's GEMM as a tail operand pair (progen_gemm's A2 / B2), the backward folds s g A^T into the input-gradient
-GEMM the same way (DESIGN.md §3.8)."""
+On the device the adapters live in one flat fp32 buffer in engine layout (`engine.Layout`: every A segment, then every
+B segment, each on an ALIGN boundary) with a compute copy in the act dtype that holds A and s B: the forward folds u B
+into the projection's GEMM as a tail operand pair (progen_gemm's A2 / B2), the backward folds s g A^T into the
+input-gradient GEMM the same way (DESIGN.md §3.8)."""
 import numpy as np
 import torch
 
 from . import lib as L
-from .engine import ALIGN, P, ParamSpec, _deinterleave, _interleave, layer_kinds
+from .engine import P, Layout, ParamSpec, layer_kinds
 
 RANKS = tuple(range(8, 65, 8))      # multiples of 8: 16-byte TMA row strides, and one tail k-block of 64
 
@@ -40,21 +40,15 @@ HEAD = 'property_head'              # module of a property head's {'w': [d, C], 
 
 
 def build_adapter_specs(cfg, rank, head_outputs=0):
-    """engine layout of the adapter buffer: (specs, padded size, offset of the first B segment).  A property head of
-    head_outputs > 0 outputs takes the last segments: the trained flat state is then adapters plus head, and the
-    compute copy (A | s B) stops before it."""
+    """the Layout of the adapter buffer: every A segment, then every B segment.  A property head of head_outputs > 0
+    outputs takes the last segments: the trained flat state is then adapters plus head, and the compute copy (A | s B)
+    stops before it."""
     mods = adapter_modules(cfg)
     specs = ([ParamSpec(m, 'lora_a', (i, rank)) for m, i, o, _ in mods] +
              [ParamSpec(m, 'lora_b', (rank, o), interleave=glu) for m, i, o, glu in mods])
     if head_outputs:
         specs += [ParamSpec(HEAD, 'w', (cfg['dim'], head_outputs)), ParamSpec(HEAD, 'b', (head_outputs,))]
-    off, n_a = 0, None
-    for s in specs:
-        if s.name == 'lora_b' and n_a is None:
-            n_a = off
-        s.offset = off
-        off += (s.size + ALIGN - 1) // ALIGN * ALIGN
-    return specs, off, n_a
+    return Layout(specs)
 
 
 def check_rank_alpha(rank, alpha):
@@ -137,44 +131,24 @@ class Adapters:
         self.r, self.alpha = rank, float(alpha)
         self.scale = self.alpha / rank
         self.head_outputs = int(head_outputs)
-        self.specs, self.n_padded, self.n_a = build_adapter_specs(eng.cfg, rank, self.head_outputs)
-        self.by_key = {(s.module, s.name): s for s in self.specs}
-        self.n_head = self.by_key[(HEAD, 'w')].offset if self.head_outputs else self.n_padded   # end of the A | B segments
-        self.num_params = sum(s.size for s in self.specs)
+        self.layout = lay = build_adapter_specs(eng.cfg, rank, self.head_outputs)
+        self.n_a = lay.span([s for s in lay.specs if s.name == 'lora_a'])[1]
+        self.n_head = lay.span([s for s in lay.specs if s.module != HEAD])[1]          # end of the A | B segments
+        self.num_params = lay.num_params
         f32 = dict(device=eng.dev, dtype=torch.float32)
-        self.params = torch.zeros(self.n_padded, **f32)
-        self.grads = torch.zeros(self.n_padded, **f32)
-        self.lp = torch.zeros(self.n_padded, device=eng.dev, dtype=eng.act)
+        self.params = torch.zeros(lay.size, **f32)
+        self.grads = torch.zeros(lay.size, **f32)
+        self.lp = torch.zeros(lay.size, device=eng.dev, dtype=eng.act)
         self.u, self.g, self.T = None, None, 0
-
-    def seg(self, buf, module, name):
-        s = self.by_key[(module, name)]
-        return buf[s.offset:s.offset + s.size]
 
     def head(self, buf, name):
         """the property head's fp32 segment `name` ('w' [d, C] or 'b' [C]) of buffer `buf`"""
-        return self.seg(buf, HEAD, name)
-
-    def flat(self, tree):
-        host = np.zeros(self.n_padded, np.float32)
-        for s in self.specs:
-            a = tree[s.module][s.name]
-            a = (a.detach().cpu().numpy() if isinstance(a, torch.Tensor) else np.asarray(a)).astype(np.float32)
-            host[s.offset:s.offset + s.size] = (_interleave(a) if s.interleave else a).ravel()
-        return torch.from_numpy(host)
+        return self.layout.seg(buf, HEAD, name)
 
     def load(self, tree, head=None):
         """adapter tree (and, with head_outputs, the head tree {'property_head': {'w', 'b'}}) -> the device buffer"""
-        self.params.copy_(self.flat(tree if head is None else {**tree, **head}))
+        self.params.copy_(torch.from_numpy(self.layout.pack(tree if head is None else {**tree, **head})))
         self.refresh()
-
-    def export_tree(self, buf):
-        host = buf.detach().float().cpu().numpy()
-        out = {}
-        for s in self.specs:
-            a = host[s.offset:s.offset + s.size].reshape(s.shape).copy()
-            out.setdefault(s.module, {})[s.name] = _deinterleave(a) if s.interleave else a
-        return out
 
     def split(self, tree):
         """a tree exported from this buffer -> (adapter tree, head tree or None)"""

@@ -29,6 +29,18 @@ def _trunc_normal(rng, shape, std):
     return (r.reshape(shape) * std).astype(np.float32)
 
 
+def _seed(rng):
+    """an int seed, or the last element of a key-like array (a jax PRNGKey) -> int"""
+    return int(rng) if isinstance(rng, (int, np.integer)) else int(np.asarray(rng).ravel()[-1])
+
+
+def _batch_size(batch_size, what):
+    """batch_size checked as an integer >= 1 -> int"""
+    if isinstance(batch_size, (bool, np.bool_)) or not isinstance(batch_size, (int, np.integer)) or batch_size < 1:
+        raise L.ProgenError(f'{what}: batch_size must be an integer >= 1, got {batch_size!r}')
+    return int(batch_size)
+
+
 def plan_launches(lengths, batch_size, by_length=False):
     """The decoder launches of `ProGen.generate` for N = len(lengths) rows (lengths[r]: row r's prompt length).
     Returns a list of (rows, real): rows is an int64 array of row indices, whose first `real` entries are the launch's rows
@@ -237,19 +249,14 @@ class ProGen:
         return self._engine
 
     def param_shapes(self):
-        specs, _, _ = build_param_specs(self.config)
-        out = {}
-        for s in specs:
-            out.setdefault(s.module, {})[s.name] = s.shape
-        return out
+        return build_param_specs(self.config).shapes()
 
     # ---- reference surface
     def init(self, rng, seq=None):
         """`model.init(rng, seq)` (train.py:130-131).  `rng` may be an int seed or a key-like array.  Distributions are the
         haiku defaults the reference relies on: Linear w ~ TruncatedNormal(1/sqrt(fan_in)), b = 0; Embed ~
         TruncatedNormal(1); LayerNorm scale = 1; SGU spatial_weights ~ U(+-1e-3/n), spatial_biases = 1 (progen.py:172-176)."""
-        seed = int(np.asarray(rng).ravel()[-1]) if not isinstance(rng, (int, np.integer)) else int(rng)
-        g = np.random.default_rng(seed)
+        g = np.random.default_rng(_seed(rng))
         n = self.config['seq_len']
         out = {}
         for module, names in self.param_shapes().items():
@@ -296,7 +303,7 @@ class ProGen:
         self._ensure_loaded(params)
         lo = None if adapters is None else self._attach_adapters(adapters, lora_alpha)
         loss = self.engine.loss_and_grad(data)
-        return float(loss.item()), self.engine.export_grads() if lo is None else lo.export_tree(lo.grads)
+        return float(loss.item()), self.engine.export_grads() if lo is None else lo.layout.unpack(lo.grads)
 
     # ---- low-rank adapters (DESIGN.md §3.8)
     def init_adapters(self, rng, rank, *, alpha=None):
@@ -307,8 +314,7 @@ class ProGen:
         checked here: pass it as lora_alpha wherever the adapters are used, s = alpha / rank."""
         from .lora import check_rank_alpha, init_adapters
         rank, _ = check_rank_alpha(rank, alpha)
-        seed = int(np.asarray(rng).ravel()[-1]) if not isinstance(rng, (int, np.integer)) else int(rng)
-        return init_adapters(self.config, seed, rank)
+        return init_adapters(self.config, _seed(rng), rank)
 
     def merge_adapters(self, params, adapters, *, lora_alpha=None):
         """params with every adapted weight W replaced by W + s A B (s = lora_alpha / rank, default 1), computed on the
@@ -399,8 +405,7 @@ class ProGen:
         from .variants import parse_mutations, variant_rows
         n = self.config['seq_len']
         subs = parse_mutations(wild_type, mutations, n, prefix)
-        if isinstance(batch_size, (bool, np.bool_)) or not isinstance(batch_size, (int, np.integer)) or batch_size < 1:
-            raise L.ProgenError(f'score_variants: batch_size must be an integer >= 1, got {batch_size!r}')
+        batch_size = _batch_size(batch_size, 'score_variants')
         rows = variant_rows(wild_type, subs, n, prefix)
         length = cut_length(rows[:, 1:])
         self._ensure_loaded(params)
@@ -562,8 +567,7 @@ class ProGen:
         TruncatedNormal(1/sqrt(dim)) from `rng` (an int seed or key-like array, as in `init`), b = 0.  num_outputs C in
         [1, 64]: the regression outputs, or the classes (>= 2) of a classification head."""
         from .property import init_head
-        seed = int(np.asarray(rng).ravel()[-1]) if not isinstance(rng, (int, np.integer)) else int(rng)
-        return init_head(self.config['dim'], seed, num_outputs)
+        return init_head(self.config['dim'], _seed(rng), num_outputs)
 
     def property_loss_and_grad(self, params, rows, targets, *, adapters, head, task, lora_alpha=None):
         """Loss and gradients of property fine-tuning: the head on the pooled embedding of the adapted model (the
@@ -587,7 +591,7 @@ class ProGen:
         eng = self.engine
         B = eng.load_property(r, code, y)
         eng.train_step(('property', code), B)
-        grads, hgrads = lo.split(lo.export_tree(lo.grads))
+        grads, hgrads = lo.split(lo.layout.unpack(lo.grads))
         return float(eng.loss.item()), grads, hgrads, eng.property_stats(B)['prediction']
 
     def predict(self, params, head, data, *, batch_size=64):
@@ -600,9 +604,8 @@ class ProGen:
         from .lora import HEAD
         from .property import check_head, check_rows
         check_head(self.config, head)
-        if isinstance(batch_size, (bool, np.bool_)) or not isinstance(batch_size, (int, np.integer)) or batch_size < 1:
-            raise L.ProgenError(f'predict: batch_size must be an integer >= 1, got {batch_size!r}')
+        batch_size = _batch_size(batch_size, 'predict')
         r = check_rows(data, self.config['seq_len'], 'predict')
         self._ensure_loaded(params)
-        pred, emb = self.engine.predict(r, head[HEAD]['w'], head[HEAD]['b'], batch_size=int(batch_size))
+        pred, emb = self.engine.predict(r, head[HEAD]['w'], head[HEAD]['b'], batch_size=batch_size)
         return dict(prediction=pred, embedding=emb)

@@ -7,7 +7,6 @@ and bitwise unchanged, and clip / AdamW / apply_every run over the adapters (wei
 head (`head=`, `task=`) joins that buffer: `property_step` trains adapters and head together (DESIGN.md §3.9)."""
 import os
 
-import numpy as np
 import torch
 
 from . import lib as L
@@ -38,14 +37,16 @@ class Trainer:
             rank, alpha = check_rank_alpha(check_adapters(model.config, adapters), lora_alpha)
             self.lora = Adapters(self.eng, rank, alpha, head_outputs=C if head is not None else 0)
             self.lora.load(adapters, head)
-        # the flat buffers the optimizer owns: (parameters, size, ndim > 1 prefix, bf16 mirror or None); gradients: self.G
+        # the flat buffers the optimizer owns: (their layout, parameters, ndim > 1 prefix, bf16 mirror or None);
+        # gradients: self.G
         if self.lora is None:
             e = self.eng
-            self.P, n, self.n_decay, self.P_lp = e.params, e.n_params_padded, e.n_decay, e.params_lp
+            self.layout, self.P, self.n_decay, self.P_lp = e.layout, e.params, e.n_decay, e.params_lp
         else:
             lo = self.lora
-            self.P, n, self.n_decay, self.P_lp = lo.params, lo.n_padded, lo.n_padded, None
+            self.layout, self.P, self.n_decay, self.P_lp = lo.layout, lo.params, lo.layout.size, None
             self.eng.grads = None                  # nothing reads or writes the base gradient while adapters train
+        n = self.layout.size
         self.lr, self.wd, self.max_norm, self.every = learning_rate, weight_decay, max_grad_norm, grad_accum_every
         self.b1, self.b2, self.eps = b1, b2, eps
         z = lambda: torch.zeros(n, device=self.eng.dev, dtype=torch.float32)
@@ -202,7 +203,7 @@ class Trainer:
         """the trained property head {'property_head': {'w', 'b'}} (None without one)"""
         if self.lora is None or not self.lora.head_outputs:
             return None
-        return self.lora.split(self.lora.export_tree(self.lora.params))[1]
+        return self.lora.split(self.layout.unpack(self.lora.params))[1]
 
     def preference_stats(self):
         """this rank's statistics of its last `preference_step` as numpy float32 [P] arrays: policy_chosen and
@@ -318,28 +319,21 @@ class Trainer:
 
     def adapters(self):
         """the trained adapters, a tree of `ProGen.init_adapters`' shape (None without adapters)"""
-        return None if self.lora is None else self.lora.split(self.lora.export_tree(self.lora.params))[0]
+        return None if self.lora is None else self.lora.split(self.layout.unpack(self.lora.params))[0]
 
     def optim_state(self):
         """{count, mu, nu, acc, every}: trees of the parameters (with adapters: of the adapters) the optimizer owns"""
-        e = self.eng if self.lora is None else self.lora
-        return dict(count=self.count, mu=e.export_tree(self.m), nu=e.export_tree(self.v), acc=e.export_tree(self.acc),
-                    every=self.every)
+        u = self.layout.unpack
+        return dict(count=self.count, mu=u(self.m), nu=u(self.v), acc=u(self.acc), every=self.every)
 
     def load_optim_state(self, st):
-        e = self.eng if self.lora is None else self.lora
+        """a state of `optim_state`'s form -> the optimizer; ProgenError names a leaf of the wrong shape"""
         if not (isinstance(st, dict) and {'count', 'mu', 'nu', 'acc'} <= set(st)):
             # e.g. an optax chain state from a reference checkpoint: only `params` interchange (checkpoint.py)
             import warnings
             warnings.warn('optim_state is not a progen_b200 Trainer state (reference / optax checkpoint?): optimizer state re-initialised')
             return
+        host = [self.layout.pack(st[k]) for k in ('mu', 'nu', 'acc')]
         self.count = int(st['count'])
-        for buf, tree in ((self.m, st['mu']), (self.v, st['nu']), (self.acc, st['acc'])):
-            host = np.zeros(self.P.numel(), np.float32)
-            for s in e.specs:
-                a = np.asarray(tree[s.module][s.name], np.float32)
-                if s.interleave:
-                    from .engine import _interleave
-                    a = _interleave(a)
-                host[s.offset:s.offset + s.size] = a.ravel()
-            buf.copy_(torch.from_numpy(host))
+        for buf, h in zip((self.m, self.v, self.acc), host):
+            buf.copy_(torch.from_numpy(h))

@@ -290,7 +290,7 @@ def test_preference_step_with_adapters_matches_float64():
     tr = model.trainer(params, adapters=ad, lora_alpha=32.0, grad_accum_every=1, learning_rate=1e-3)
     base = tr.eng.params.clone()
     loss = float(tr.preference_step(c, r, sc[:2], sc[2:], beta=0.1).item())
-    grads = tr.lora.export_tree(tr.lora.grads)             # the optimizer reads the gradient and leaves it in place
+    grads = tr.lora.layout.unpack(tr.lora.grads)             # the optimizer reads the gradient and leaves it in place
     s = 2.0
     merged = {m: dict(v) for m, v in params.items()}
     for m, v in ad.items():

@@ -110,7 +110,8 @@ def test_glu_interleave_round_trip():
     B is interleaved (value_j, gate_j) like the base weight, and the export gives the haiku order back."""
     from progen_b200.engine import _deinterleave, _interleave
     cfg = ProGen(**CFG).config
-    specs, n, n_a = build_adapter_specs(cfg, 8)
+    lay = build_adapter_specs(cfg, 8)
+    specs, n, n_a = lay.specs, lay.size, lay.span([s for s in lay.specs if s.name == 'lora_a'])[1]
     assert [s.name for s in specs] == ['lora_a'] * (len(specs) // 2) + ['lora_b'] * (len(specs) // 2)
     assert all(s.offset % 64 == 0 for s in specs) and n % 64 == 0 and n_a == specs[len(specs) // 2].offset
     assert all(s.decay for s in specs)

@@ -166,8 +166,9 @@ def test_head_segments_follow_the_adapters():
     """the head is the last segment of the adapter buffer: the compute copy and the B-gradient scale stop before it"""
     from progen_b200.lora import build_adapter_specs
     cfg = _model().config
-    specs, n, n_a = build_adapter_specs(cfg, 8, 3)
-    plain, n0, n_a0 = build_adapter_specs(cfg, 8)
+    lay, lay0 = build_adapter_specs(cfg, 8, 3), build_adapter_specs(cfg, 8)
+    specs, n, n_a = lay.specs, lay.size, lay.span([s for s in lay.specs if s.name == 'lora_a'])[1]
+    plain, n0, n_a0 = lay0.specs, lay0.size, lay0.span([s for s in lay0.specs if s.name == 'lora_a'])[1]
     assert n_a == n_a0 and [(s.module, s.name, s.offset) for s in specs[:len(plain)]] == \
         [(s.module, s.name, s.offset) for s in plain]
     hw, hb = specs[-2:]
