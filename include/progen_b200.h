@@ -190,15 +190,13 @@ int progen_tril_cast(const float* w, void* out, int out_dtype, int n, void* stre
 /* optimizer: optax.chain(clip_by_global_norm, adamw(mask = ndim > 1), apply_every(k)) — train.py:115-121,189-190 */
 int progen_optim_workspace_floats(void);
 int progen_grad_sqnorm(const float* g, long long n, float* workspace, float* out_sqnorm, void* stream);
+/* one optimizer call.  The step-dependent scalars (Adam count, bias corrections, emit = count % apply_every == 0) live in
+ * a 32-byte device `state` ({int64 count; float bc1, bc2; int32 emit; pad}, zeroed before the first call) that a 1-thread
+ * kernel advances: every launch argument is step-invariant, so a captured CUDA graph of the whole training step
+ * (train.py:186-190) can be replayed.  p_lp (may be null) receives the bf16 mirror of the parameters whenever they change */
 int progen_adamw_step(float* p, void* p_lp, const float* g, float* m, float* v, float* acc, long long n, long long n_decay,
                       const float* gnorm_sq, float lr, float b1, float b2, float eps, float wd, float max_norm,
-                      long long step, int emit, void* stream);
-/* same call with the step-dependent scalars (Adam count, bias corrections, emit = count % apply_every == 0) kept in a
- * 32-byte device `state` ({int64 count; float bc1, bc2; int32 emit; pad}) that a 1-thread kernel advances: every launch
- * argument is step-invariant, so a captured CUDA graph of the whole training step (train.py:186-190) can be replayed */
-int progen_adamw_step_dev(float* p, void* p_lp, const float* g, float* m, float* v, float* acc, long long n, long long n_decay,
-                          const float* gnorm_sq, float lr, float b1, float b2, float eps, float wd, float max_norm,
-                          int apply_every, void* state, void* stream);
+                      int apply_every, void* state, void* stream);
 
 /* ---- KV-cached decode (BASELINE config 5; replaces the full re-forward per token of utils.py:115-117) ----
  * Weights are TRANSPOSED copies ([out, in], fp32 or bf16 per `wdtype`); caches and scratch are fp32 device buffers owned

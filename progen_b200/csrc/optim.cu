@@ -45,9 +45,7 @@ __global__ void sqnorm_final_kernel(const float* __restrict__ partial, int nbloc
 }
 
 struct AdamArgs {
-  float lr, b1, b2, eps, wd, max_norm, bc1, bc2;
-  int emit;
-  const struct AdamDevState* dev;      // non-null: bias corrections and the emit flag come from device memory (CUDA-graph replay)
+  float lr, b1, b2, eps, wd, max_norm;
 };
 
 // Step-dependent scalars of the optimizer kept on the device, so that a captured CUDA graph of the whole training step
@@ -69,11 +67,12 @@ __global__ void adam_tick_kernel(AdamDevState* st, double b1, double b2, int eve
 template <bool WRITE_LP>
 __global__ void adamw_kernel(float* __restrict__ p, bf16* __restrict__ p_lp, const float* __restrict__ g,
                              float* __restrict__ m, float* __restrict__ v, float* __restrict__ acc, long long n,
-                             long long n_decay, const float* __restrict__ gnorm_sq, const AdamArgs a) {
+                             long long n_decay, const float* __restrict__ gnorm_sq, const AdamDevState* __restrict__ st,
+                             const AdamArgs a) {
   const float gn = sqrtf(gnorm_sq[0]);
   const float clip = a.max_norm / fmaxf(gn, a.max_norm);            // optax.clip_by_global_norm
-  const float bc1 = a.dev ? a.dev->bc1 : a.bc1, bc2 = a.dev ? a.dev->bc2 : a.bc2;
-  const bool emit = a.dev ? a.dev->emit != 0 : a.emit != 0;
+  const float bc1 = st->bc1, bc2 = st->bc2;
+  const bool emit = st->emit != 0;
   const long long n4 = n / 4;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
     float4 pv = reinterpret_cast<float4*>(p)[i];
@@ -129,48 +128,26 @@ int progen_grad_sqnorm(const float* g, long long n, float* workspace, float* out
   return PROGEN_OK;
 }
 
-// One optimizer call (train.py:189-190).  step = 1-based Adam count; emit = (step % apply_every == 0).
-// p_lp (may be null) receives the bf16 mirror of the parameters whenever they change.
+// One optimizer call (train.py:189-190) with the step-dependent scalars in device memory (`state`: 32 bytes, see
+// AdamDevState; its `step` field holds the number of calls made so far).  Two launches with launch-invariant arguments, so
+// a captured CUDA graph of a training step stays valid: tick (count, bias corrections, emit = count % apply_every == 0),
+// then the update.  p_lp (may be null) receives the bf16 mirror of the parameters whenever they change.
 int progen_adamw_step(float* p, void* p_lp, const float* g, float* m, float* v, float* acc, long long n, long long n_decay,
                       const float* gnorm_sq, float lr, float b1, float b2, float eps, float wd, float max_norm,
-                      long long step, int emit, void* stream) {
-  PG_CHECK_ARG(n > 0 && n % 4 == 0 && n_decay >= 0 && n_decay <= n && step >= 1);
-  AdamArgs a;
-  a.lr = lr; a.b1 = b1; a.b2 = b2; a.eps = eps; a.wd = wd; a.max_norm = max_norm;
-  a.bc1 = (float)(1.0 - pow((double)b1, (double)step));
-  a.bc2 = (float)(1.0 - pow((double)b2, (double)step));
-  a.emit = emit;
-  a.dev = nullptr;
-  cudaStream_t s = (cudaStream_t)stream;
-  long long b = (n / 4 + 255) / 256;
-  const long long cap = (long long)pg_num_sms() * 8;
-  const int blocks = (int)(b > cap ? cap : b);
-  if (p_lp) adamw_kernel<true><<<blocks, 256, 0, s>>>(p, (bf16*)p_lp, g, m, v, acc, n, n_decay, gnorm_sq, a);
-  else adamw_kernel<false><<<blocks, 256, 0, s>>>(p, nullptr, g, m, v, acc, n, n_decay, gnorm_sq, a);
-  PG_LAUNCH_CHECK();
-  return PROGEN_OK;
-}
-
-// Same optimizer call with the step-dependent scalars in device memory (`state`: 32 bytes, see AdamDevState; its `step`
-// field holds the number of calls made so far).  Two launches with launch-invariant arguments, so a captured CUDA graph of
-// a training step stays valid: tick (count, bias corrections, emit = count % apply_every == 0), then the update.
-int progen_adamw_step_dev(float* p, void* p_lp, const float* g, float* m, float* v, float* acc, long long n, long long n_decay,
-                          const float* gnorm_sq, float lr, float b1, float b2, float eps, float wd, float max_norm,
-                          int apply_every, void* state, void* stream) {
+                      int apply_every, void* state, void* stream) {
   PG_CHECK_ARG(n > 0 && n % 4 == 0 && n_decay >= 0 && n_decay <= n && apply_every >= 1 && state != nullptr);
   PG_CHECK_ARG((reinterpret_cast<uintptr_t>(state) & 7) == 0);
   AdamArgs a;
   a.lr = lr; a.b1 = b1; a.b2 = b2; a.eps = eps; a.wd = wd; a.max_norm = max_norm;
-  a.bc1 = a.bc2 = 1.f; a.emit = 0;
-  a.dev = reinterpret_cast<const AdamDevState*>(state);
+  AdamDevState* st = reinterpret_cast<AdamDevState*>(state);
   cudaStream_t s = (cudaStream_t)stream;
-  adam_tick_kernel<<<1, 1, 0, s>>>(reinterpret_cast<AdamDevState*>(state), (double)b1, (double)b2, apply_every);
+  adam_tick_kernel<<<1, 1, 0, s>>>(st, (double)b1, (double)b2, apply_every);
   PG_LAUNCH_CHECK();
   long long b = (n / 4 + 255) / 256;
   const long long cap = (long long)pg_num_sms() * 8;
   const int blocks = (int)(b > cap ? cap : b);
-  if (p_lp) adamw_kernel<true><<<blocks, 256, 0, s>>>(p, (bf16*)p_lp, g, m, v, acc, n, n_decay, gnorm_sq, a);
-  else adamw_kernel<false><<<blocks, 256, 0, s>>>(p, nullptr, g, m, v, acc, n, n_decay, gnorm_sq, a);
+  if (p_lp) adamw_kernel<true><<<blocks, 256, 0, s>>>(p, (bf16*)p_lp, g, m, v, acc, n, n_decay, gnorm_sq, st, a);
+  else adamw_kernel<false><<<blocks, 256, 0, s>>>(p, nullptr, g, m, v, acc, n, n_decay, gnorm_sq, st, a);
   PG_LAUNCH_CHECK();
   return PROGEN_OK;
 }

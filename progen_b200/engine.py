@@ -237,19 +237,14 @@ class Engine:
         self.rot_sin = torch.tensor(np.sin(ang), **f32).contiguous()
         self.rot_cos = torch.tensor(np.cos(ang), **f32).contiguous()
         self.B = 0
+        self.alloc_epoch = 0      # counts re-allocations of the training activations: a captured step holds for one epoch
         self.acts = None          # training activation set (ensure_batch)
         self.infer = None         # inference activation set (inference_acts), cached by row count
         self.loss = torch.zeros(1, device=self.dev)       # exists before the first batch: a rank without rows still reports 0
         self.loaded_token = None
-        self.on_layer_grads = None        # optional callback(layer_index) fired when a layer's weight gradients are final
         self.lora = None                  # lora.Adapters: the training set runs the adapted model with a frozen base
         self.lib = L.load()
         self.num_sms = torch.cuda.get_device_properties(self.dev).multi_processor_count
-
-    def layer_grad_range(self, i):
-        """[start, stop) of layer i's ndim>1 parameters inside the flat buffers (contiguous by construction)."""
-        pre = (P + f'attn{i}/~/', P + f'ff{i}/~/')
-        return self.layout.span([s for s in self.layout.specs if s.decay and s.module.startswith(pre)])
 
     # ------------------------------------------------------------------------------------------ parameters
     def load_params(self, params):
@@ -299,7 +294,7 @@ class Engine:
         if B == self.B:
             return
         self.B = B
-        self.alloc_epoch = getattr(self, 'alloc_epoch', 0) + 1      # activation buffers are re-allocated below: captured
+        self.alloc_epoch += 1                                       # activation buffers are re-allocated below: captured
                                                                     # CUDA graphs (Trainer.capture_graph) become invalid
         T = B * self.n
         self.T = T
@@ -861,10 +856,6 @@ class Engine:
             self.dgrad_gemm(self.dqkv, 3 * I, self.W(a + 'linear', 'w'), d, self.dy, **tail(s['y1'], d, a + 'linear', self.dqkv, 3 * I))
             self.ln_bwd_res(self.dy, x0, self.Pf(a + 'layer_norm', 'scale'), s['mean1'], s['rstd1'], G(a + 'layer_norm', 'scale'), shift,
                             next_bias_grad=G(P + f'ff{i - 1}/~/linear_1', 'b') if i > 0 else None)
-            if self.on_layer_grads is not None:
-                # every weight-matrix gradient of layer i is final: the DDP trainer starts its all-reduce here so the
-                # transfer overlaps the backward pass of layers i-1 .. 0
-                self.on_layer_grads(i)
         if frozen:
             lo.scale_b_grads()
             return

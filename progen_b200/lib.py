@@ -77,8 +77,7 @@ PROTOTYPES = {
     'progen_gather_rows_f32': [_P, _LL, _I, _I, _LL, _P, _I, _I, _I, _I, _I, _I, _P, _LL, _LL, _LL, _P],
     'progen_optim_workspace_floats': [],
     'progen_grad_sqnorm': [_P, _LL, _P, _P, _P],
-    'progen_adamw_step': [_P, _P, _P, _P, _P, _P, _LL, _LL, _P, _F, _F, _F, _F, _F, _F, _LL, _I, _P],
-    'progen_adamw_step_dev': [_P, _P, _P, _P, _P, _P, _LL, _LL, _P, _F, _F, _F, _F, _F, _F, _I, _P, _P],
+    'progen_adamw_step': [_P, _P, _P, _P, _P, _P, _LL, _LL, _P, _F, _F, _F, _F, _F, _F, _I, _P, _P],
 }
 _RESTYPES = {'progen_version': C.c_char_p, 'progen_last_error': C.c_char_p, 'progen_launch_count': C.c_longlong}
 

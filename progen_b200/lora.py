@@ -180,5 +180,5 @@ class Adapters:
             self.u = {m: A() for m, _, _, _ in adapter_modules(self.eng.cfg)}
             self.g = A()
             self.T = T
-            self.eng.alloc_epoch = getattr(self.eng, 'alloc_epoch', 0) + 1
+            self.eng.alloc_epoch += 1
         return self.u

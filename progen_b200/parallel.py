@@ -33,19 +33,6 @@ def shard_batch(data, rank=None, world_size=None):
     return data[a:b]
 
 
-def allreduce_sum_(flat, group=None, bucket_elems=64 * 1024 * 1024):
-    """In-place SUM all-reduce of a flat buffer in large buckets (NVSwitch: latency- not link-bound, so few big
-    messages).  Returns the list of async work handles (already waited when `wait` is True)."""
-    if not (dist.is_available() and dist.is_initialized()) or dist.get_world_size(group) == 1:
-        return
-    works = []
-    n = flat.numel()
-    for s in range(0, n, bucket_elems):
-        works.append(dist.all_reduce(flat[s:min(n, s + bucket_elems)], op=dist.ReduceOp.SUM, group=group, async_op=True))
-    for w_ in works:
-        w_.wait()
-
-
 def allreduce_scalar_(t, group=None):
     if dist.is_available() and dist.is_initialized() and dist.get_world_size(group) > 1:
         dist.all_reduce(t, op=dist.ReduceOp.SUM, group=group)

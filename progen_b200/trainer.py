@@ -5,8 +5,6 @@ accumulator live in flat fp32 buffers; one `step(data)` is one iteration of the 
 With low-rank adapters (`adapters=`) the same state exists for the adapter buffer only: the base parameters are frozen
 and bitwise unchanged, and clip / AdamW / apply_every run over the adapters (weight decay on every A and B).  A property
 head (`head=`, `task=`) joins that buffer: `property_step` trains adapters and head together (DESIGN.md §3.9)."""
-import os
-
 import torch
 
 from . import lib as L
@@ -14,6 +12,8 @@ from . import parallel as PAR
 
 
 class Trainer:
+    overlap = False         # exists only because bench.py reads it: the gradient exchange is never overlapped
+
     def __init__(self, model, params, learning_rate=2e-4, weight_decay=1e-3, max_grad_norm=0.5, grad_accum_every=4,
                  b1=0.9, b2=0.999, eps=1e-8, optim_state=None, data_parallel=True, cuda_graph=False, adapters=None,
                  lora_alpha=None, head=None, task=None):
@@ -51,27 +51,16 @@ class Trainer:
         self.b1, self.b2, self.eps = b1, b2, eps
         z = lambda: torch.zeros(n, device=self.eng.dev, dtype=torch.float32)
         self.m, self.v, self.acc = z(), z(), z()
-        self.count = 0
+        self.count = 0                                     # host copy of the Adam count, for optim_state()
+        # AdamDevState (count | bc1, bc2 | emit, pad): progen_adamw_step advances it on the device, eager or replayed
+        self._adam_state = torch.zeros(4, dtype=torch.int64, device=self.eng.dev)
         self.ws = torch.empty(L.load().progen_optim_workspace_floats(), device=self.eng.dev)
         self.gnorm_sq = torch.zeros(1, device=self.eng.dev)
         self.rank, self.world = PAR.world() if data_parallel else (0, 1)
-        self._works, self._done = [], []
-        self._graph, self._graph_key, self._graph_epoch, self._adam_state = None, None, 0, None
+        self._graph, self._graph_key, self._graph_epoch = None, None, 0
         # cuda_graph=True: after two eager steps of one batch shape the step is captured and replayed from then on
         self._auto_graph, self._eager_key = bool(cuda_graph), None
-        self._bucket, self._bucket_layers = None, max(1, int(os.environ.get('PROGEN_DDP_BUCKET_LAYERS', '3')))
-        # Gradient exchange (world > 1).  Default: ONE SUM all-reduce of the whole flat buffer after the backward pass, on
-        # the compute stream, inside the captured CUDA graph.  Overlapping per-layer buckets with the backward pass lets the
-        # NCCL kernels take SMs from the backward kernels and needs eager launches.  PROGEN_DDP_OVERLAP=1 selects that mode
-        # (eager launches only) for models whose gradient is large enough to make the transfer itself matter.
-        self.overlap = os.environ.get('PROGEN_DDP_OVERLAP', '0') == '1'
-        if self.overlap and self.lora is not None:
-            raise L.ProgenError('PROGEN_DDP_OVERLAP=1 does not support adapters: their gradient is one small buffer, '
-                                'all-reduced once per step')
         self.skip_allreduce = False                       # bench.py: "step without the exchange" for comm_exposed_ms
-        if self.world > 1 and self.overlap:
-            # overlap: a layer's weight gradients are all-reduced (async, NCCL's stream) as soon as its backward is done
-            self.eng.on_layer_grads = self._reduce_layer
         if optim_state is not None:
             self.load_optim_state(optim_state)
 
@@ -105,7 +94,7 @@ class Trainer:
             # a rank without rows (batch smaller than the world): zero contribution, but every collective is joined
             self.G.zero_()
             eng.loss.zero_()
-            return self._update(sync_loss)
+            return self._eager_update(sync_loss)
         key = (rows, global_rows) + objective
         self._drop_graph_unless(rows)
         if load is not None:
@@ -113,8 +102,8 @@ class Trainer:
         if self._graph is not None and self._graph_key == key:
             return self._replay(sync_loss)
         eng.train_step(objective, global_rows)
-        loss = self._update(sync_loss)
-        if self._auto_graph and not (self.world > 1 and self.overlap):
+        loss = self._eager_update(sync_loss)
+        if self._auto_graph:
             # _eager_key starts as None, so _eager_run is set here before it is read
             self._eager_run = self._eager_run + 1 if key == self._eager_key else 1
             self._eager_key = key
@@ -127,29 +116,24 @@ class Trainer:
     def capture_graph(self, batch_rows, global_batch=None, install=True, objective=()):
         """Capture one training step for batches of `batch_rows` rows into a CUDA graph; later `step` / `step_resident`
         calls with that shape replay it.  The step-dependent optimizer scalars live on the device
-        (`progen_adamw_step_dev`), so the graph is identical for every step.  Under data parallelism the NCCL all-reduce
+        (`progen_adamw_step`), so the graph is identical for every step.  Under data parallelism the NCCL all-reduce
         of the gradient buffer is part of the graph (issued on the capture stream between backward and the norm).  Call
         after at least one eager step of the same shape (kernel attributes, tensor maps, buffers and the NCCL communicator
         must exist before capture).  `install=False` returns the graph without making it the one `step` replays.
         `objective` (Engine.train_step) selects the loss: ('preference', beta) captures the step `preference_step`
         replays, with batch_rows = 2 * pairs and global_batch = the global pair count."""
-        if self.world > 1 and self.overlap:
-            raise L.ProgenError('capture_graph: PROGEN_DDP_OVERLAP=1 launches its bucketed all-reduces eagerly')
         gb = global_batch or batch_rows * self.world
         eng = self.eng
         eng.lora = self.lora
         eng.ensure_batch(batch_rows)
-        if self._adam_state is None:
-            self._adam_state = torch.zeros(4, dtype=torch.int64, device=eng.dev)   # AdamDevState: count | bc1, bc2 | emit, pad
-        self._adam_state[0] = self.count
         torch.cuda.synchronize()
         g = torch.cuda.CUDAGraph()
         with torch.cuda.graph(g):
             eng.train_step(objective, gb)
             self._allreduce_grads()
-            self._update_captured()
+            self._update()
         if install:
-            self._graph, self._graph_key, self._graph_epoch = g, (batch_rows, gb) + objective, getattr(eng, 'alloc_epoch', 0)
+            self._graph, self._graph_key, self._graph_epoch = g, (batch_rows, gb) + objective, eng.alloc_epoch
         return g
 
     # ---- preference (DPO) fine-tuning
@@ -215,19 +199,26 @@ class Trainer:
         if self.world <= 1 or self.skip_allreduce:
             return
         import torch.distributed as dist
-        if self.overlap:
-            self._finish_allreduce()
-        else:
-            dist.all_reduce(self.G, op=dist.ReduceOp.SUM)
+        dist.all_reduce(self.G, op=dist.ReduceOp.SUM)
 
-    def _update_captured(self):
-        eng, lib, st = self.eng, L.load(), L.stream()
+    def _eager_update(self, sync_loss):
+        """the rest of an eager step after the backward pass: the gradient exchange, the logged loss, the optimizer"""
+        self._allreduce_grads()
+        if sync_loss and self.world > 1:
+            PAR.allreduce_scalar_(self.eng.loss)
+        self.count += 1
+        self._update()
+        return self.eng.loss
+
+    def _update(self):
+        """norm, AdamW with the device-side count, masked copies: the same launches eagerly and in a captured graph"""
+        lib, st = L.load(), L.stream()
         n = self.P.numel()
         L.check(lib.progen_grad_sqnorm(self.G.data_ptr(), n, self.ws.data_ptr(), self.gnorm_sq.data_ptr(), st), 'grad_sqnorm')
-        L.check(lib.progen_adamw_step_dev(self.P.data_ptr(), L.ptr(self.P_lp), self.G.data_ptr(),
-                                          self.m.data_ptr(), self.v.data_ptr(), self.acc.data_ptr(), n,
-                                          self.n_decay, self.gnorm_sq.data_ptr(), self.lr, self.b1, self.b2, self.eps, self.wd,
-                                          self.max_norm, self.every, self._adam_state.data_ptr(), st), 'adamw_step_dev')
+        L.check(lib.progen_adamw_step(self.P.data_ptr(), L.ptr(self.P_lp), self.G.data_ptr(),
+                                      self.m.data_ptr(), self.v.data_ptr(), self.acc.data_ptr(), n,
+                                      self.n_decay, self.gnorm_sq.data_ptr(), self.lr, self.b1, self.b2, self.eps, self.wd,
+                                      self.max_norm, self.every, self._adam_state.data_ptr(), st), 'adamw_step')
         self._refresh()                                    # every step (a no-op recompute between emits): keeps the graph static
 
     def _refresh(self):
@@ -240,7 +231,7 @@ class Trainer:
     def _drop_graph_unless(self, batch_rows):
         """a different batch size re-allocates the engine's activation buffers: the captured pointers would dangle"""
         if self._graph is not None and (batch_rows != self._graph_key[0] or
-                                        getattr(self.eng, 'alloc_epoch', 0) != self._graph_epoch):
+                                        self.eng.alloc_epoch != self._graph_epoch):
             self._graph, self._graph_key = None, None      # (model.apply / sampling with another batch size re-allocates too)
 
     def _replay(self, sync_loss=False):
@@ -249,59 +240,6 @@ class Trainer:
         if sync_loss and self.world > 1:
             PAR.allreduce_scalar_(self.eng.loss)           # logged loss only; the next replay zeroes it again
         return self.eng.loss
-
-    def _reduce_layer(self, i):
-        """Layer i's backward is done (layers arrive in descending order).  Consecutive layers are merged into one
-        bucket of `PROGEN_DDP_BUCKET_LAYERS` layers (default 3): every NCCL kernel holds SMs while it waits for the slowest
-        rank, and the statically partitioned persistent kernels running beside it end late by that long, so fewer, larger
-        all-reduces cost less than one per layer."""
-        import torch.distributed as dist
-        a, b = self.eng.layer_grad_range(i)
-        if self._bucket is None:
-            self._bucket = [a, b, 0]
-        assert b == self._bucket[0] or (a, b) == tuple(self._bucket[:2]), 'layer gradient ranges must be adjacent'
-        self._bucket[0] = min(self._bucket[0], a)
-        self._bucket[2] += 1
-        if self._bucket[2] >= self._bucket_layers or i == 0:
-            lo, hi, _ = self._bucket
-            self._works.append(dist.all_reduce(self.eng.grads[lo:hi], op=dist.ReduceOp.SUM, async_op=True))
-            self._done.append((lo, hi))
-            self._bucket = None
-
-    def _finish_allreduce(self):
-        """everything the per-layer reductions did not cover: embedding (final only at the very end of backward), head,
-        and the small ndim<=1 section; then wait for the overlapped ones"""
-        eng = self.eng
-        lo = min((a for a, _ in self._done), default=eng.n_params_padded)
-        hi = max((b for _, b in self._done), default=eng.n_params_padded)
-        if self._done:
-            PAR.allreduce_sum_(eng.grads[:lo])
-            PAR.allreduce_sum_(eng.grads[hi:])
-        else:
-            PAR.allreduce_sum_(eng.grads)
-        for w in self._works:
-            w.wait()
-        self._works, self._done = [], []
-
-    def _update(self, sync_loss):
-        eng, lib, st = self.eng, L.load(), L.stream()
-        if self.world > 1:
-            self._allreduce_grads()
-            if sync_loss:
-                PAR.allreduce_scalar_(eng.loss)
-        self.count += 1
-        if self._adam_state is not None:
-            self._adam_state[0] = self.count               # keep the device-side count in step with eager steps
-        emit = int(self.count % self.every == 0)
-        n = self.P.numel()
-        L.check(lib.progen_grad_sqnorm(self.G.data_ptr(), n, self.ws.data_ptr(), self.gnorm_sq.data_ptr(), st), 'grad_sqnorm')
-        L.check(lib.progen_adamw_step(self.P.data_ptr(), L.ptr(self.P_lp), self.G.data_ptr(),
-                                      self.m.data_ptr(), self.v.data_ptr(), self.acc.data_ptr(), n, self.n_decay,
-                                      self.gnorm_sq.data_ptr(), self.lr, self.b1, self.b2, self.eps, self.wd, self.max_norm,
-                                      self.count, emit, st), 'adamw_step')
-        if emit:
-            self._refresh()
-        return eng.loss
 
     def evaluate(self, data):
         """validation loss (train.py:207-211): forward + loss only"""
@@ -335,5 +273,6 @@ class Trainer:
             return
         host = [self.layout.pack(st[k]) for k in ('mu', 'nu', 'acc')]
         self.count = int(st['count'])
+        self._adam_state[0] = self.count
         for buf, h in zip((self.m, self.v, self.acc), host):
             buf.copy_(torch.from_numpy(h))

@@ -326,6 +326,7 @@ def test_optimizer_chain_matches_oracle():
     m, v, acc = (torch.zeros(n, device=dev) for _ in range(3))
     ws = torch.empty(L.load().progen_optim_workspace_floats(), device=dev)
     gn = torch.empty(1, device=dev)
+    state = torch.zeros(4, dtype=torch.int64, device=dev)     # AdamDevState: the kernel counts the steps
     st = O.optim_init(params, every=4)
     cur = params
     for step in range(1, 10):
@@ -334,7 +335,7 @@ def test_optimizer_chain_matches_oracle():
         gflat = torch.tensor(np.concatenate([grads['a']['w'].ravel(), grads['b']['b']]).astype(np.float32), device=dev)
         L.check(L.load().progen_grad_sqnorm(gflat.data_ptr(), n, ws.data_ptr(), gn.data_ptr(), L.stream()))
         L.check(L.load().progen_adamw_step(p.data_ptr(), p_lp.data_ptr(), gflat.data_ptr(), m.data_ptr(), v.data_ptr(), acc.data_ptr(),
-                                           n, n_decay, gn.data_ptr(), 2e-4, 0.9, 0.999, 1e-8, 1e-3, 0.5, step, int(step % 4 == 0),
+                                           n, n_decay, gn.data_ptr(), 2e-4, 0.9, 0.999, 1e-8, 1e-3, 0.5, 4, state.data_ptr(),
                                            L.stream()))
         g32 = {k: {kk: vv.astype(np.float32) for kk, vv in d.items()} for k, d in grads.items()}
         cur, gnorm = O.optim_step(cur, g32, st)

@@ -354,14 +354,6 @@ def test_two_rank_lora_trainer_equals_single_process(mp):
     assert res['even_4_rows_graph']['graph'], 'the data-parallel LoRA step was not captured into a CUDA graph'
 
 
-def test_ddp_overlap_with_adapters_is_refused(monkeypatch):
-    from progen_b200 import lib as L
-    model, _, params, ad, _ = _setup('glu', False)
-    monkeypatch.setenv('PROGEN_DDP_OVERLAP', '1')
-    with pytest.raises(L.ProgenError, match='PROGEN_DDP_OVERLAP'):
-        model.trainer(params, adapters=ad)
-
-
 def test_cli_lora_train_resume_generate_score(tmp_path):
     """train a base for one step, then adapters on it for 3 steps and 2 more after a resume; generate.py and score.py
     load the adapter package"""

@@ -75,19 +75,20 @@ def test_optim_state_rejects_a_wrong_shape():
     tr = Trainer.__new__(Trainer)
     tr.layout, tr.count = lay, 5
     tr.m, tr.v, tr.acc = (torch.zeros(lay.size) for _ in range(3))
+    tr._adam_state = torch.zeros(4, dtype=torch.int64)
     st = {k: _random_tree(lay.shapes(), i) for i, k in enumerate(('mu', 'nu', 'acc'))}
     tr.load_optim_state(dict(count=7, every=4, **st))
     assert tr.count == 7 and torch.equal(tr.v, torch.from_numpy(lay.pack(st['nu'])))
+    assert int(tr._adam_state[0]) == 7                   # the optimizer kernel's count follows the loaded one
     st['acc'][HEAD]['w'] = st['acc'][HEAD]['w'].T.copy()
     with pytest.raises(L.ProgenError, match=f'{HEAD}/w: expected shape'):
         tr.load_optim_state(dict(count=9, every=4, **st))
-    assert tr.count == 7
+    assert tr.count == 7 and int(tr._adam_state[0]) == 7
 
 
 @pytest.mark.parametrize('name', list(MODELS))
 def test_engine_segments(name):
-    """64-aligned, ndim > 1 leaves first, each group in tree order, and each layer's ndim > 1 leaves one contiguous range
-    (Engine.layer_grad_range)"""
+    """64-aligned, ndim > 1 leaves first, each group in tree order, and each layer's ndim > 1 leaves one contiguous range"""
     kw = MODELS[name]
     cfg = ProGen(**kw).config
     lay = build_param_specs(cfg)

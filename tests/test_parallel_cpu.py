@@ -45,7 +45,7 @@ def _worker(rank, world, port, ret):
     loss.backward()
     keys = sorted((m, k) for m, d in prm.items() for k in d)
     flat = torch.cat([prm[m][k].grad.reshape(-1) for m, k in keys])
-    PAR.allreduce_sum_(flat, bucket_elems=1000)          # several buckets
+    dist.all_reduce(flat, op=dist.ReduceOp.SUM)          # the exchange Trainer makes
     lt = PAR.allreduce_scalar_(loss.detach().clone())
     if rank == 0:
         ref_loss, ref = T.loss_and_grads(params, data, cfg)
@@ -63,44 +63,3 @@ def test_two_rank_gloo_allreduce_equals_single_process_gradient():
     mp.spawn(_worker, args=(2, port, ret), nprocs=2, join=True)
     assert ret['loss_err'] < 1e-12 and ret['grad_err'] < 1e-12, dict(ret)
 
-
-def _bucket_worker(rank, world, port, ret):
-    """The Trainer's overlapped, bucketed gradient all-reduce on a stand-in engine (flat CPU buffer, gloo): every element of
-    the flat buffer is reduced exactly once, whatever the bucket size, and the result is the sum over ranks."""
-    sys.path.insert(0, ROOT)
-    os.environ.update(MASTER_ADDR='127.0.0.1', MASTER_PORT=str(port))
-    dist.init_process_group('gloo', rank=rank, world_size=world)
-    from progen_b200.trainer import Trainer
-
-    class FakeEngine:
-        # layout like the real one: [embedding/head | layer 0 | layer 1 | ... | layer L-1 | small ndim<=1 section]
-        def __init__(self, layers=5, per_layer=24, head=16, tail=8):
-            self.layers, self.per_layer, self.head = layers, per_layer, head
-            self.n_params_padded = head + layers * per_layer + tail
-            self.grads = torch.arange(self.n_params_padded, dtype=torch.float32) * (rank + 1)
-
-        def layer_grad_range(self, i):
-            a = self.head + i * self.per_layer
-            return a, a + self.per_layer
-
-    ok = True
-    for bucket_layers in (1, 2, 3, 7):
-        tr = Trainer.__new__(Trainer)
-        tr.eng = FakeEngine()
-        tr.world, tr.rank = world, rank
-        tr._works, tr._done, tr._bucket, tr._bucket_layers = [], [], None, bucket_layers
-        for i in reversed(range(tr.eng.layers)):            # backward visits the layers from last to first
-            tr._reduce_layer(i)
-        tr._finish_allreduce()
-        expect = torch.arange(tr.eng.n_params_padded, dtype=torch.float32) * sum(r + 1 for r in range(world))
-        ok = ok and bool(torch.equal(tr.eng.grads, expect)) and tr._bucket is None and not tr._works
-    ret[rank] = ok
-    dist.destroy_process_group()
-
-
-def test_trainer_bucketed_allreduce_covers_every_gradient_once():
-    world = 2
-    mgr = mp.Manager()
-    ret = mgr.dict()
-    mp.spawn(_bucket_worker, args=(world, 29641, ret), nprocs=world, join=True)
-    assert all(ret[r] for r in range(world)), dict(ret)
