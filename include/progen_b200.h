@@ -162,6 +162,13 @@ int progen_local_attn_fwd_simt(const void* qkv, void* out, float* lse, int dtype
 int progen_local_attn_bwd_simt(const void* qkv, const void* out, const void* dout, const float* lse, void* dqkv,
                                float* delta, int dtype, int B, int seq_len, int window, int heads, int dim_head,
                                void* stream);
+/* the backward over a partial last window (any seq_len > 0), for a training step cut to its rows' counted length: a key
+ * streams its own window's queries up to min(window end, seq_len) and the next window's below seq_len.  The rows of a
+ * cut call are bitwise the first seq_len rows of the backward at a longer length whose dout is zero from seq_len on.  At
+ * whole windows it makes the same launches, with the same bounds, as progen_local_attn_bwd_simt. */
+int progen_local_attn_bwd_cut_simt(const void* qkv, const void* out, const void* dout, const float* lse, void* dqkv,
+                                   float* delta, int dtype, int B, int seq_len, int window, int heads, int dim_head,
+                                   void* stream);
 
 /* tensor-core version (bf16, dim_head 64, window % 64 == 0): flash-style with TMA-fed K/V (or Q/dO) tiles and wgmma,
  * scores stay on chip; same buffers as above.  With rot_sin/rot_cos set, the backward applies the rotary backward to
@@ -171,6 +178,11 @@ int progen_local_attn_fwd_tc(const void* qkv, void* out, float* lse, int B, int 
 int progen_local_attn_bwd_tc(const void* qkv, const void* out, const void* dout, const float* lse, void* dqkv, float* delta,
                              const float* rot_sin, const float* rot_cos, int B, int seq_len, int window, int heads, int dim_head,
                              void* stream);
+/* the tensor-core backward over a partial last window (seq_len % 64 == 0, the forward's rule); same contract as
+ * progen_local_attn_bwd_cut_simt, same launcher and launches as progen_local_attn_bwd_tc. */
+int progen_local_attn_bwd_cut_tc(const void* qkv, const void* out, const void* dout, const float* lse, void* dqkv,
+                                 float* delta, const float* rot_sin, const float* rot_cos, int B, int seq_len, int window,
+                                 int heads, int dim_head, void* stream);
 
 /* SGU gating — progen.py:182-184: out = xs * (Gp + spatial_biases[m]) and its backward (dxs, dGp, dbias; dbias nullable) */
 int progen_sgu_gate_fwd(const void* xs, long long ldx, const void* gp, long long ldg, const float* bias, void* out,

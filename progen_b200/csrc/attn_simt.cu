@@ -164,10 +164,11 @@ __global__ void __launch_bounds__(128) attn_bwd_dkv_kernel(const TO* __restrict_
   float dk[DH], dv[DH];
 #pragma unroll
   for (int d = 0; d < DH; ++d) { dk[d] = 0.f; dv[d] = 0.f; }
-  const int nwin = dm.n / dm.w;
-  // query offsets r relative to this key: r in [0, w - 1 - i] (same window) and, if a next window exists,
-  // r in [w - i, 2w - 1 - i]
-  const int nq = (dm.w - i) + ((win + 1 < nwin) ? dm.w : 0);
+  const int nwin = (dm.n + dm.w - 1) / dm.w;          // the last window may be partial (a cut backward)
+  // query offsets r relative to this key: the own window's queries from the key on, below min(window end, n), then, if
+  // a next window exists, its queries below n.  At whole windows: r in [0, w - 1 - i] and [w - i, 2w - 1 - i].
+  const int own_end = min((win + 1) * dm.w, dm.n);
+  const int nq = (own_end - pos) + ((win + 1 < nwin) ? min((win + 2) * dm.w, dm.n) - own_end : 0);
   for (int r = lane; r < nq; r += 32) {
     const long long tq = t + r;
     float q[DH], dO[DH];
@@ -232,11 +233,20 @@ int launch_bwd(const void* qkv, const void* out, const void* dout, const float* 
     return PROGEN_ERR_UNSUPPORTED;                                                        \
   } while (0)
 
+namespace {
+// the one launcher of both backward entry points (they differ in their host check only)
+int bwd(const void* qkv, const void* out, const void* dout, const float* lse, void* dqkv, float* delta, int dtype, int B,
+        int seq_len, int window, int heads, int dim_head, void* stream) {
+  AttnDims dm{(long long)B * seq_len, seq_len, window, heads, dim_head, 3LL * heads * dim_head};
+  ATTN_DISPATCH(launch_bwd, qkv, out, dout, lse, dqkv, delta, dm, (cudaStream_t)stream);
+}
+}  // namespace
+
 extern "C" {
 
 // The forward takes any seq_len: the last window may be partial.  A query at pos reads keys (win - 1) * w .. pos only, so
-// a forward cut short of the model's sequence length computes the first seq_len rows of the full one, bitwise.  The
-// backward keeps whole windows (a key's gradient reads the whole next window).
+// a forward cut short of the model's sequence length computes the first seq_len rows of the full one, bitwise.
+// progen_local_attn_bwd_simt keeps whole windows; progen_local_attn_bwd_cut_simt takes any seq_len (see the header).
 int progen_local_attn_fwd_simt(const void* qkv, void* out, float* lse, int dtype, int B, int seq_len, int window,
                                int heads, int dim_head, void* stream) {
   PG_CHECK_ARG(B > 0 && seq_len > 0 && window > 0 && heads > 0);
@@ -248,8 +258,14 @@ int progen_local_attn_bwd_simt(const void* qkv, const void* out, const void* dou
                                float* delta, int dtype, int B, int seq_len, int window, int heads, int dim_head,
                                void* stream) {
   PG_CHECK_ARG(B > 0 && seq_len > 0 && window > 0 && seq_len % window == 0 && heads > 0);
-  AttnDims dm{(long long)B * seq_len, seq_len, window, heads, dim_head, 3LL * heads * dim_head};
-  ATTN_DISPATCH(launch_bwd, qkv, out, dout, lse, dqkv, delta, dm, (cudaStream_t)stream);
+  return bwd(qkv, out, dout, lse, dqkv, delta, dtype, B, seq_len, window, heads, dim_head, stream);
+}
+
+int progen_local_attn_bwd_cut_simt(const void* qkv, const void* out, const void* dout, const float* lse, void* dqkv,
+                                   float* delta, int dtype, int B, int seq_len, int window, int heads, int dim_head,
+                                   void* stream) {
+  PG_CHECK_ARG(B > 0 && seq_len > 0 && window > 0 && heads > 0);
+  return bwd(qkv, out, dout, lse, dqkv, delta, dtype, B, seq_len, window, heads, dim_head, stream);
 }
 
 }  // extern "C"

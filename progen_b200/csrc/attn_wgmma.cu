@@ -308,8 +308,8 @@ __global__ void __launch_bounds__(128) attn_bwd_dq_wgmma_kernel(const __grid_con
 }
 
 // ================================================================================================ dK, dV
-// One CTA per 64-key tile; streams the 64-query tiles that can see it (own window from the diagonal on, then the whole
-// next window).  Works on transposed scores: S^T = K Q^T so that keys are the accumulator rows.
+// One CTA per 64-key tile; streams the 64-query tiles that can see it (own window from the diagonal on, then the next
+// window; both end at seq_len).  Works on transposed scores: S^T = K Q^T so that keys are the accumulator rows.
 __global__ void __launch_bounds__(128) attn_bwd_dkv_wgmma_kernel(const __grid_constant__ CUtensorMap tm_qkv,
                                                                  const __grid_constant__ CUtensorMap tm_do,
                                                                  const float* __restrict__ lse, const float* __restrict__ delta,
@@ -323,9 +323,12 @@ __global__ void __launch_bounds__(128) attn_bwd_dkv_wgmma_kernel(const __grid_co
   const int I = dm.h * DH;
   const long long ld = 3LL * I;
   const int row0 = b * dm.n;
-  const int nwin = dm.n / dm.w;
-  const int nown = (dm.w - j0) / TILE;                // query tiles of the own window at or after the diagonal
-  const int nnext = (win + 1 < nwin) ? dm.w / TILE : 0;
+  const int nwin = (dm.n + dm.w - 1) / dm.w;          // the last window may be partial (a cut backward)
+  // query tiles of the own window at or after the diagonal, below min(window end, n); then those of the next window,
+  // below n.  At whole windows: (w - j0) / 64 and w / 64.
+  const int own_end = min((win + 1) * dm.w, dm.n);
+  const int nown = (own_end - k0) / TILE;
+  const int nnext = (win + 1 < nwin) ? (min((win + 2) * dm.w, dm.n) - own_end) / TILE : 0;
   const int ntiles = nown + nnext;
   auto q_pos = [&](int qt) { return qt < nown ? win * dm.w + j0 + qt * TILE : (win + 1) * dm.w + (qt - nown) * TILE; };
   auto issue = [&](int qt, int st) {                  // Q and dO tiles of query tile qt -> stage st
@@ -427,13 +430,35 @@ template <typename K> int prepare(K kern) {
   return PROGEN_OK;
 }
 
-// full_windows: seq_len must be whole windows (the backward kernels stream the whole next window of every key tile).
-// The forward only needs whole 64-row tiles: a query tile of a partial last window reads the previous window and its own
-// keys up to the diagonal, the same key tiles it reads at full length, so no key at or beyond seq_len is touched.
+// full_windows: seq_len must be whole windows (progen_local_attn_bwd_tc keeps that contract).  The forward and the cut
+// backward only need whole 64-row tiles: a query tile of a partial last window reads the previous window and its own
+// keys up to the diagonal, the same key tiles it reads at full length, and a key tile streams the query tiles below
+// seq_len only, so no row at or beyond seq_len is touched.
 int check_dims(const void* qkv, int B, int seq_len, int window, int heads, int dim_head, bool full_windows) {
   PG_CHECK_ARG(qkv != nullptr && B > 0 && heads > 0 && dim_head == DH && window % TILE == 0 && seq_len > 0 &&
                seq_len % (full_windows ? window : TILE) == 0);
   PG_CHECK_ARG((long long)B * seq_len < (1ll << 31));
+  return PROGEN_OK;
+}
+
+// the one launcher of both backward entry points (they differ in their host check only)
+int bwd_tc(const void* qkv, const void* out, const void* dout, const float* lse, void* dqkv, float* delta,
+           const float* rot_sin, const float* rot_cos, int B, int seq_len, int window, int heads, cudaStream_t s) {
+  int rc;
+  const int I = heads * DH;
+  const uint64_t T = (uint64_t)B * seq_len;
+  CUtensorMap tq, tdo;
+  if ((rc = pg_tensor_map_2d_bf16(qkv, 3ull * I, T, 3ull * I, DH, TILE, &tq))) return rc;
+  if ((rc = pg_tensor_map_2d_bf16(dout, (uint64_t)I, T, (uint64_t)I, DH, TILE, &tdo))) return rc;
+  if ((rc = prepare(attn_bwd_dq_wgmma_kernel))) return rc;
+  if ((rc = prepare(attn_bwd_dkv_wgmma_kernel))) return rc;
+  const Dims dm{seq_len, window, heads, rot_sin, rot_cos};
+  const dim3 grid(seq_len / TILE, heads, B);
+  // the dQ kernel also produces delta for the dK/dV kernel that follows it on the same stream
+  attn_bwd_dq_wgmma_kernel<<<grid, 128, SMEM_BYTES, s>>>(tq, tdo, (const bf16*)out, (const bf16*)dout, lse, delta, (bf16*)dqkv, dm);
+  PG_LAUNCH_CHECK();
+  attn_bwd_dkv_wgmma_kernel<<<grid, 128, SMEM_BYTES, s>>>(tq, tdo, lse, delta, (bf16*)dqkv, dm);
+  PG_LAUNCH_CHECK();
   return PROGEN_OK;
 }
 
@@ -464,24 +489,16 @@ int progen_local_attn_fwd_tc(const void* qkv, void* out, float* lse, int B, int 
 int progen_local_attn_bwd_tc(const void* qkv, const void* out, const void* dout, const float* lse, void* dqkv, float* delta,
                              const float* rot_sin, const float* rot_cos, int B, int seq_len, int window, int heads, int dim_head,
                              void* stream) {
-  int rc = check_dims(qkv, B, seq_len, window, heads, dim_head, true);
-  if (rc) return rc;
-  const int I = heads * DH;
-  const uint64_t T = (uint64_t)B * seq_len;
-  CUtensorMap tq, tdo;
-  if ((rc = pg_tensor_map_2d_bf16(qkv, 3ull * I, T, 3ull * I, DH, TILE, &tq))) return rc;
-  if ((rc = pg_tensor_map_2d_bf16(dout, (uint64_t)I, T, (uint64_t)I, DH, TILE, &tdo))) return rc;
-  if ((rc = prepare(attn_bwd_dq_wgmma_kernel))) return rc;
-  if ((rc = prepare(attn_bwd_dkv_wgmma_kernel))) return rc;
-  const Dims dm{seq_len, window, heads, rot_sin, rot_cos};
-  const dim3 grid(seq_len / TILE, heads, B);
-  cudaStream_t s = (cudaStream_t)stream;
-  // the dQ kernel also produces delta for the dK/dV kernel that follows it on the same stream
-  attn_bwd_dq_wgmma_kernel<<<grid, 128, SMEM_BYTES, s>>>(tq, tdo, (const bf16*)out, (const bf16*)dout, lse, delta, (bf16*)dqkv, dm);
-  PG_LAUNCH_CHECK();
-  attn_bwd_dkv_wgmma_kernel<<<grid, 128, SMEM_BYTES, s>>>(tq, tdo, lse, delta, (bf16*)dqkv, dm);
-  PG_LAUNCH_CHECK();
-  return PROGEN_OK;
+  const int rc = check_dims(qkv, B, seq_len, window, heads, dim_head, true);
+  return rc ? rc : bwd_tc(qkv, out, dout, lse, dqkv, delta, rot_sin, rot_cos, B, seq_len, window, heads, (cudaStream_t)stream);
+}
+
+// the same with a partial last window: seq_len % 64 == 0 (the forward's rule)
+int progen_local_attn_bwd_cut_tc(const void* qkv, const void* out, const void* dout, const float* lse, void* dqkv,
+                                 float* delta, const float* rot_sin, const float* rot_cos, int B, int seq_len, int window,
+                                 int heads, int dim_head, void* stream) {
+  const int rc = check_dims(qkv, B, seq_len, window, heads, dim_head, false);
+  return rc ? rc : bwd_tc(qkv, out, dout, lse, dqkv, delta, rot_sin, rot_cos, B, seq_len, window, heads, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -45,6 +45,23 @@ def iterator_from_sequences(seqs, seq_len, batch_size, skip=0, loop=False):
             return
 
 
+def group_by_length(batches):
+    """Length-grouped micro-batches: the rows of `batches` (the micro-batches of one effective batch, (b_i, n+1) integer
+    rows each) sorted by counted length (`engine.counted_length`; stable, shortest first) and split again into
+    micro-batches of the original sizes.  Every optimizer update sees the same sequences; each micro-step then runs at
+    a cut length close to its rows' own (DESIGN.md §3.10).  Pure host work."""
+    from .engine import counted_length
+    if not batches:
+        return []
+    rows = np.concatenate([np.asarray(b) for b in batches])
+    order = np.argsort(counted_length(rows[:, 1:]), kind='stable')
+    out, r0 = [], 0
+    for b in batches:
+        out.append(rows[order[r0:r0 + len(b)]])
+        r0 += len(b)
+    return out
+
+
 def synthetic_iterator(seq_len, batch_size, seed=42, vocab=256):
     """uniform-random [0, vocab) rows of seq_len + 1 tokens (BASELINE.json north_star), endless"""
     rng = np.random.default_rng(seed)

@@ -45,6 +45,23 @@ def cut_length(labels):
     return min(n, -(-need // CUT_ALIGN) * CUT_ALIGN)
 
 
+def check_length(labels, length, what):
+    """the row length of a forward or training step over the rows with labels [N, n] (host): `length` None means their
+    cut_length; otherwise it must be n or a multiple of CUT_ALIGN below n that covers every counted position of the
+    rows.  ProgenError otherwise, before any device work."""
+    labels = np.asarray(labels)
+    n = labels.shape[1]
+    if length is None:
+        return cut_length(labels)
+    if isinstance(length, (bool, np.bool_)) or not isinstance(length, (int, np.integer)) or \
+            not (length == n or (0 < length < n and length % CUT_ALIGN == 0)):
+        raise L.ProgenError(f'{what}: length must be seq_len ({n}) or a multiple of {CUT_ALIGN} below it, got {length!r}')
+    if len(labels) and int(counted_length(labels).max()) > length:
+        raise L.ProgenError(f'{what}: length {length} cuts off counted positions (cut_length of these rows: '
+                            f'{cut_length(labels)})')
+    return int(length)
+
+
 def layer_kinds(depth, global_mlp_depth, ff_glu):
     """reference progen.py:210-212"""
     out = []
@@ -159,28 +176,32 @@ def _deinterleave(a):
 class Acts:
     """One activation set: the buffers one forward pass runs on (B sequences of n positions, T = B * n token rows).
     `X` lists the residual stream at every LayerNorm input and `lay` one scratch dict per layer.  The training set keeps
-    all of them (the backward pass reads them); the inference set (`inplace`) repeats one residual buffer, updated in
-    place, and one layer's scratch, and stores no GLU / GELU pre-activation (`u` is None)."""
+    all of them (the backward pass reads them) and its backward temporaries by name in `grad`; the inference set
+    (`inplace`) repeats one residual buffer, updated in place, and one layer's scratch, and stores no GLU / GELU
+    pre-activation (`u` is None)."""
 
-    def __init__(self, B, n, tok, labels, X, lay, meanf, rstdf, yf, logits, inplace=False, rows=None, res=None):
+    def __init__(self, B, n, tok, labels, X, lay, meanf, rstdf, yf, logits, inplace=False, rows=None, res=None, grad=None):
         self.B, self.n, self.T = B, n, B * n
         self.tok, self.labels, self.X, self.lay = tok, labels, X, lay
         self.meanf, self.rstdf, self.yf, self.logits = meanf, rstdf, yf, logits
         self.inplace = inplace
         self.rows = rows        # inference: [B, n+1] int32 staging of the input rows (one H2D copy per chunk)
         self.res = res          # inference: flat fp32 per-chunk results (see Engine.score)
+        self.grad = grad        # training: {name: [T, ...] backward temporary}, shared by all layers
 
     def view(self, B, n):
-        """the first B sequences of this set, cut to their first n positions (same memory): a ragged last chunk or a
-        cut forward runs on the cached buffers.  `rows` is the contiguous (B, n+1) prefix of the staging buffer."""
+        """the first B sequences of this set, cut to their first n positions (same memory): a ragged last chunk, a cut
+        forward or a cut training step runs on the cached buffers.  `rows` is the contiguous (B, n+1) prefix of the
+        staging buffer."""
         if (B, n) == (self.B, self.n):
             return self
         T = B * n
         cut = lambda t: None if t is None else t[:T]
         rows = None if self.rows is None else self.rows.view(-1)[:B * (n + 1)].view(B, n + 1)
+        grad = None if self.grad is None else {k: cut(v) for k, v in self.grad.items()}
         return Acts(B, n, cut(self.tok), cut(self.labels), [cut(x) for x in self.X],
                     [{k: cut(v) for k, v in s.items()} for s in self.lay], cut(self.meanf), cut(self.rstdf), cut(self.yf),
-                    cut(self.logits), self.inplace, rows, self.res)
+                    cut(self.logits), self.inplace, rows, self.res, grad)
 
 
 class Engine:
@@ -343,7 +364,12 @@ class Engine:
         half = hid // 2
         if 'sgu' in self.kinds:
             self.dpj, self.dsg, self.dgp, self.dgn = A(T, half), A(T, half), A(T, half), A(T, half)
-        self.acts = Acts(B, self.n, self.tok, self.labels, self.X, self.lay, self.meanf, self.rstdf, self.yf, self.logits)
+        grad = dict(dres=self.dres, dres_lp=self.dres_lp, dy=self.dy, dqkv=self.dqkv, datt=self.datt, delta=self.delta,
+                    du=self.du, dh_=self.dh_, dlogits=self.dlogits, ce_w=self.ce_w, logp=self.logp)
+        if 'sgu' in self.kinds:
+            grad.update(dpj=self.dpj, dsg=self.dsg, dgp=self.dgp, dgn=self.dgn)
+        self.acts = Acts(B, self.n, self.tok, self.labels, self.X, self.lay, self.meanf, self.rstdf, self.yf, self.logits,
+                         grad=grad)
 
     def inference_acts(self, B):
         """Activation set of a forward pass that keeps no training state, for up to B sequences: one fp32 residual buffer
@@ -378,26 +404,27 @@ class Engine:
     def _mm(self, **kw):
         L.gemm(backend=self.backend, in_dtype=self.act_dt, **kw)
 
-    def lora_fwd(self, x, K, module, N):
-        """adapters: u = x A of projection `module` (input x [T, K], N outputs) -> the tail (u, s B) of its GEMM"""
+    def lora_fwd(self, x, K, module, N, acts):
+        """adapters: u = x A of projection `module` (input x [T, K], N outputs; T from the training set or its view
+        `acts`) -> the tail (u, s B) of its GEMM"""
         lo = self.lora
         if lo is None:
             return {}
-        u, seg = lo.u[module], lo.layout.seg
-        self.fwd_gemm(x, K, seg(lo.lp, module, 'lora_a'), lo.r, u)
+        u, seg = lo.u[module][:acts.T], lo.layout.seg
+        self.fwd_gemm(x, K, seg(lo.lp, module, 'lora_a'), lo.r, u, acts=acts)
         return dict(A2=u, lda2=lo.r, B2=seg(lo.lp, module, 'lora_b'), ldb2=N, K2=lo.r)
 
-    def lora_bwd(self, x, K, module, dy, N):
+    def lora_bwd(self, x, K, module, dy, N, acts):
         """adapters: from the projection's output gradient dy [T, N], g' = s g = dy (s B)^T, dB += u^T dy (scaled by s
         after the backward pass), dA += x^T g' -> the tail (g', A^T) of its input-gradient GEMM"""
         lo = self.lora
         if lo is None:
             return {}
         seg = lo.layout.seg
-        g, A = lo.g, seg(lo.lp, module, 'lora_a')
-        self.dgrad_gemm(dy, N, seg(lo.lp, module, 'lora_b'), lo.r, g)
-        self.wgrad_gemm(lo.u[module], lo.r, dy, N, seg(lo.grads, module, 'lora_b'))
-        self.wgrad_gemm(x, K, g, lo.r, seg(lo.grads, module, 'lora_a'))
+        g, A = lo.g[:acts.T], seg(lo.lp, module, 'lora_a')
+        self.dgrad_gemm(dy, N, seg(lo.lp, module, 'lora_b'), lo.r, g, acts=acts)
+        self.wgrad_gemm(lo.u[module][:acts.T], lo.r, dy, N, seg(lo.grads, module, 'lora_b'), acts=acts)
+        self.wgrad_gemm(x, K, g, lo.r, seg(lo.grads, module, 'lora_a'), acts=acts)
         return dict(A2=g, lda2=lo.r, B2=A, ldb2=lo.r, K2=lo.r)
 
     def fwd_gemm(self, x, K, w, N, out, epi=L.EPI_STORE, out_dtype=None, acts=None, **kw):
@@ -406,26 +433,27 @@ class Engine:
         self._mm(M=(acts or self.acts).T, N=N, K=K, A=x, lda=K, B=w, ldb=N, b_mn=True, out=out, ldo=kw.pop('ldo', N), epi=epi,
                  out_dtype=self.act_dt if out_dtype is None else out_dtype, **kw)
 
-    def dgrad_gemm(self, dy, N_out, w, K_in, out, epi=L.EPI_STORE, **kw):
+    def dgrad_gemm(self, dy, N_out, w, K_in, out, epi=L.EPI_STORE, acts=None, **kw):
         """out[T,K_in] = dy[T,N_out] @ w[K_in,N_out]^T  (w rows are the output features: K-major B operand)"""
-        self._mm(M=self.T, N=K_in, K=N_out, A=dy, lda=N_out, B=w, ldb=N_out, out=out, ldo=kw.pop('ldo', K_in), epi=epi,
+        self._mm(M=(acts or self.acts).T, N=K_in, K=N_out, A=dy, lda=N_out, B=w, ldb=N_out, out=out, ldo=kw.pop('ldo', K_in), epi=epi,
                  out_dtype=self.act_dt, **kw)
 
-    def wgrad_gemm(self, x, K_in, dy, N_out, dw):
+    def wgrad_gemm(self, x, K_in, dy, N_out, dw, acts=None):
         """dw[K_in,N_out] += x[T,K_in]^T @ dy[T,N_out]  (both operands MN-major, the token dimension is K)"""
-        split = self.wgrad_split(K_in, N_out) if self.backend == L.BACKEND_TC else 1
-        self._mm(M=K_in, N=N_out, K=self.T, A=x, lda=K_in, a_mn=True, B=dy, ldb=N_out, b_mn=True, out=dw, ldo=N_out,
+        split = self.wgrad_split(K_in, N_out, acts) if self.backend == L.BACKEND_TC else 1
+        self._mm(M=K_in, N=N_out, K=(acts or self.acts).T, A=x, lda=K_in, a_mn=True, B=dy, ldb=N_out, b_mn=True, out=dw, ldo=N_out,
                  epi=L.EPI_ACCUM, out_dtype=L.F32, split_k=split, atomic=split > 1)
 
-    def wgrad_split(self, K_in, N_out):
+    def wgrad_split(self, K_in, N_out, acts=None):
         """K split of a weight-gradient GEMM (one CTA per 128 x 128 output tile and K slice): the split in 1..8 whose CTAs
         fill the largest fraction of their waves over the SMs, the smallest such split on ties"""
         tiles = ((K_in + 127) // 128) * ((N_out + 127) // 128)
         fill = lambda s: tiles * s / (-(-tiles * s // self.num_sms) * self.num_sms)
-        return max(range(1, min(8, max(1, self.T // 64)) + 1), key=lambda s: (round(fill(s), 6), -s))
+        return max(range(1, min(8, max(1, (acts or self.acts).T // 64)) + 1), key=lambda s: (round(fill(s), 6), -s))
 
-    def colsum(self, t, N, out, ld=None):
-        L.check(self.lib.progen_colsum(t.data_ptr(), N if ld is None else ld, L.dt(t), out.data_ptr(), self.T, N, L.stream()), 'colsum')
+    def colsum(self, t, N, out, ld=None, acts=None):
+        L.check(self.lib.progen_colsum(t.data_ptr(), N if ld is None else ld, L.dt(t), out.data_ptr(), (acts or self.acts).T, N,
+                                       L.stream()), 'colsum')
 
     def ln_fwd(self, x, ldx, scale, y, ldy, mean, rstd, dcols, shift, acts=None):
         a = acts or self.acts
@@ -466,10 +494,10 @@ class Engine:
         lib, st = self.lib, L.stream()
         cfg, d, I, hid, T, n = self.cfg, self.d, self.I, self.hid, acts.T, acts.n
         shift = cfg['shift_tokens']
-        lo = self.lora if acts is self.acts else None       # adapters run on the training set only
+        lo = None if acts.inplace else self.lora            # adapters run on the training set (or its cut view) only
         if lo is not None:
-            lo.activations(T)
-        tail = self.lora_fwd if lo is not None else (lambda *a: {})
+            lo.activations(self.acts.T)
+        tail = (lambda *a: self.lora_fwd(*a, acts=acts)) if lo is not None else (lambda *a: {})
         L.check(lib.progen_embed_fwd(acts.tok.data_ptr(), self.Pf(P + 'embed', 'embeddings').data_ptr(), acts.X[0].data_ptr(),
                                      T, d, self.V, st), 'embed_fwd')
         for i, kind in enumerate(self.kinds):
@@ -538,15 +566,21 @@ class Engine:
         L.check(self.lib.progen_local_attn_fwd_simt(qkv.data_ptr(), out.data_ptr(), lse.data_ptr(), self.act_dt, B, n,
                                                     self.w, self.h, self.dh, L.stream()), 'local_attn_fwd')
 
-    def attn_bwd(self, qkv, out, dout, lse, dqkv):
+    def attn_bwd(self, qkv, out, dout, lse, dqkv, acts=None):
+        """attention backward on the training set or its cut view `acts`; a cut that ends inside a window runs the
+        `_cut_` entry point, every whole-window step the whole-window one"""
+        a = acts or self.acts
+        B, n, delta = a.B, a.n, a.grad['delta']
+        lib = self.lib
         if self.attn_tc:
-            L.check(self.lib.progen_local_attn_bwd_tc(qkv.data_ptr(), out.data_ptr(), dout.data_ptr(), lse.data_ptr(), dqkv.data_ptr(),
-                                                      self.delta.data_ptr(), self.rot_sin.data_ptr(), self.rot_cos.data_ptr(),
-                                                      self.B, self.n, self.w, self.h, self.dh, L.stream()), 'local_attn_bwd')
+            fn = lib.progen_local_attn_bwd_tc if n % self.w == 0 else lib.progen_local_attn_bwd_cut_tc
+            L.check(fn(qkv.data_ptr(), out.data_ptr(), dout.data_ptr(), lse.data_ptr(), dqkv.data_ptr(), delta.data_ptr(),
+                       self.rot_sin.data_ptr(), self.rot_cos.data_ptr(), B, n, self.w, self.h, self.dh, L.stream()),
+                    'local_attn_bwd')
             return     # rotary backward is fused into the kernel's epilogue
-        L.check(self.lib.progen_local_attn_bwd_simt(qkv.data_ptr(), out.data_ptr(), dout.data_ptr(), lse.data_ptr(), dqkv.data_ptr(),
-                                                    self.delta.data_ptr(), self.act_dt, self.B, self.n, self.w, self.h, self.dh,
-                                                    L.stream()), 'local_attn_bwd')
+        fn = lib.progen_local_attn_bwd_simt if n % self.w == 0 else lib.progen_local_attn_bwd_cut_simt
+        L.check(fn(qkv.data_ptr(), out.data_ptr(), dout.data_ptr(), lse.data_ptr(), dqkv.data_ptr(), delta.data_ptr(), self.act_dt,
+                   B, n, self.w, self.h, self.dh, L.stream()), 'local_attn_bwd')
 
     # ------------------------------------------------------------------------------------------ scoring (inference)
     def _chunks(self, rows, batch_size, n):
@@ -580,13 +614,7 @@ class Engine:
         if batch_size < 1:
             raise L.ProgenError(f'score: batch_size must be >= 1, got {batch_size}')
         N, n, d = rows.shape[0], self.n, self.d
-        if length is not None:
-            if not isinstance(length, (int, np.integer)) or not (length == n or (0 < length < n and length % CUT_ALIGN == 0)):
-                raise L.ProgenError(f'score: length must be seq_len ({n}) or a multiple of {CUT_ALIGN} below it, got {length!r}')
-            if N and int(counted_length(rows[:, 1:].numpy()).max()) > length:
-                raise L.ProgenError(f'score: length {length} cuts off counted positions (cut_length of these rows: '
-                                    f'{cut_length(rows[:, 1:].numpy())})')
-        cut = n if length is None else int(length)
+        cut = n if length is None else check_length(rows[:, 1:].numpy(), length, 'score')
         out = dict(log_likelihood=np.zeros(N, np.float32), num_tokens=np.zeros(N, np.int64))
         if tokens:
             out['token_logp'] = np.zeros((N, n), np.float32)
@@ -619,22 +647,38 @@ class Engine:
     def loss_and_grad(self, data, global_batch=None, zero_grads=True):
         """data: (B, n+1) integer rows -> (device scalar loss, grads accumulated into self.grads).
         Mirrors utils.py:61-76: ids = data[:, :-1], labels = data[:, 1:], mean over rows of the masked CE.
-        `global_batch` (DDP): scale by 1/global_batch so that a SUM all-reduce yields the global-mean gradient."""
-        B = self.load_batch(data)
-        self.train_step((), global_batch or B, zero_grads)
+        `global_batch` (DDP): scale by 1/global_batch so that a SUM all-reduce yields the global-mean gradient.
+        The step runs at the rows' row_length (DESIGN.md §3.10)."""
+        n = self.row_length(data)
+        B = self.load_batch(data, n)
+        self.train_step((), global_batch or B, zero_grads, length=n)
         return self.loss
 
-    def load_batch(self, data):
-        """host (or device) rows (B, n+1) -> self.tok / self.labels; returns B"""
+    def row_length(self, data, length=None, what='training step'):
+        """the row length a training step on rows `data` (B, n+1) runs at: check_length of host rows (None: their
+        cut_length); rows on the device run at seq_len (their cut length would need a host sync)"""
+        if isinstance(data, torch.Tensor) and data.is_cuda:
+            if length not in (None, self.n):
+                raise L.ProgenError(f'{what}: rows on the device run at seq_len ({self.n}), got length {length!r}')
+            return self.n
+        rows = np.asarray(data)
+        if rows.ndim != 2 or rows.shape[1] != self.n + 1:
+            raise L.ProgenError(f'{what}: rows must be (B, seq_len + 1 = {self.n + 1}), got {rows.shape}')
+        return check_length(rows[:, 1:], length, what)
+
+    def load_batch(self, data, length=None):
+        """host (or device) rows (B, n+1) -> self.tok / self.labels, cut to their first `length` positions (default
+        seq_len) in the layout of the training set's (B, length) view; returns B"""
         data = torch.as_tensor(np.asarray(data).astype(np.int32) if not isinstance(data, torch.Tensor) else data)
         B = data.shape[0]
         self.ensure_batch(B)
-        dd = data.to(device=self.dev, dtype=torch.int32, non_blocking=True)
-        self.tok.copy_(dd[:, :-1].reshape(-1))
-        self.labels.copy_(dd[:, 1:].reshape(-1))
+        n = self.n if length is None else length
+        dd = data[:, :n + 1].to(device=self.dev, dtype=torch.int32, non_blocking=True)
+        self.tok[:B * n].view(B, n).copy_(dd[:, :-1])
+        self.labels[:B * n].view(B, n).copy_(dd[:, 1:])
         return B
 
-    def train_step(self, objective, global_rows, zero_grads=True, backward=True):
+    def train_step(self, objective, global_rows, zero_grads=True, backward=True, length=None):
         """forward + loss head + backward of one training objective on rows resident in self.tok / self.labels.
         `objective` (also the tail of Trainer's graph key) selects the loss head:
           ()                    the language-model loss: the masked cross entropy, mean over rows (utils.py:45-59);
@@ -648,8 +692,13 @@ class Engine:
                                 adapters with a head (lora.Adapters with head_outputs): the base stays frozen.
         The loss is scaled by 1/global_rows (the preference loss: 1/global pairs), so that a SUM all-reduce of the
         per-rank gradients is the global mean.  With adapters (self.lora) no base gradient is computed.
-        `backward=False`: the forward and the loss only (a validation loss), no gradient."""
+        `backward=False`: the forward and the loss only (a validation loss), no gradient.
+        `length` (default seq_len): run on the first `length` positions of every row only, on the (B, length) view of
+        the training set (DESIGN.md §3.10); it must cover every counted position of the rows (check_length).  Nothing
+        is allocated per length."""
         lib, st, lo, d = self.lib, L.stream(), self.lora, self.d
+        a = self.acts.view(self.B, self.n if length is None else int(length))
+        g = a.grad
         kind = objective[0] if objective else None
         pairs = self.B // 2
         if kind == 'preference' and 2 * pairs != self.B:
@@ -660,25 +709,25 @@ class Engine:
             # the backward pass ends by scaling the whole B gradient by s (Adapters.scale_b_grads): an accumulated one
             # would be scaled twice
             raise L.ProgenError('adapters: gradients cannot accumulate across steps (zero_grads=False)')
-        self._forward_device(logits=kind != 'property')
+        self._forward_device(a, logits=kind != 'property')
         if kind is None:
             self.loss.zero_()
         if zero_grads and backward:
             self.train_grads().zero_()
         if kind is None:
-            L.check(lib.progen_ce_fwd_bwd(self.logits.data_ptr(), L.F32, self.labels.data_ptr(), self.ce_w.data_ptr(),
-                                          self.loss.data_ptr(), self.dlogits.data_ptr() if backward else 0, self.act_dt,
-                                          self.B, self.n, self.V, 1.0 / global_rows, st), 'ce_fwd_bwd')
+            L.check(lib.progen_ce_fwd_bwd(a.logits.data_ptr(), L.F32, a.labels.data_ptr(), g['ce_w'].data_ptr(),
+                                          self.loss.data_ptr(), g['dlogits'].data_ptr() if backward else 0, self.act_dt,
+                                          a.B, a.n, self.V, 1.0 / global_rows, st), 'ce_fwd_bwd')
         elif kind == 'preference':
-            L.check(lib.progen_preference_head(self.logits.data_ptr(), L.F32, self.labels.data_ptr(), self.ref.data_ptr(),
-                                               self.logp.data_ptr(), self.seq_ll.data_ptr(), self.seq_count.data_ptr(),
-                                               self.ce_w.data_ptr(), self.stats.data_ptr(), self.loss.data_ptr(),
-                                               self.ce_scratch.data_ptr(), self.dlogits.data_ptr(), self.act_dt, pairs,
-                                               self.n, self.V, objective[1], 1.0 / global_rows, st), 'preference_head')
+            L.check(lib.progen_preference_head(a.logits.data_ptr(), L.F32, a.labels.data_ptr(), self.ref.data_ptr(),
+                                               g['logp'].data_ptr(), self.seq_ll.data_ptr(), self.seq_count.data_ptr(),
+                                               g['ce_w'].data_ptr(), self.stats.data_ptr(), self.loss.data_ptr(),
+                                               self.ce_scratch.data_ptr(), g['dlogits'].data_ptr(), self.act_dt, pairs,
+                                               a.n, self.V, objective[1], 1.0 / global_rows, st), 'preference_head')
         else:
-            B, C, reg = self.B, lo.head_outputs, objective[1] == L.TASK_REGRESSION
-            L.check(lib.progen_masked_mean_pool(self.yf.data_ptr(), d, self.act_dt, self.labels.data_ptr(),
-                                                self.emb.data_ptr(), B, self.n, d, st), 'masked_mean_pool')
+            B, C, reg = a.B, lo.head_outputs, objective[1] == L.TASK_REGRESSION
+            L.check(lib.progen_masked_mean_pool(a.yf.data_ptr(), d, self.act_dt, a.labels.data_ptr(),
+                                                self.emb.data_ptr(), B, a.n, d, st), 'masked_mean_pool')
             L.check(lib.progen_property_head(self.emb.data_ptr(), lo.head(lo.params, 'w').data_ptr(),
                                              lo.head(lo.params, 'b').data_ptr(), B, d, C, objective[1],
                                              self.ptarget.data_ptr() if reg else 0, 0 if reg else self.pclass.data_ptr(),
@@ -688,24 +737,24 @@ class Engine:
         if not backward:
             return
         if kind == 'property':
-            L.check(lib.progen_masked_mean_pool_bwd(self.demb.data_ptr(), self.labels.data_ptr(), self.dy.data_ptr(), d,
-                                                    self.act_dt, self.B, self.n, d, st), 'masked_mean_pool_bwd')
+            L.check(lib.progen_masked_mean_pool_bwd(self.demb.data_ptr(), a.labels.data_ptr(), g['dy'].data_ptr(), d,
+                                                    self.act_dt, a.B, a.n, d, st), 'masked_mean_pool_bwd')
         else:
             hw = P + 'linear'
             if lo is None:
-                self.colsum(self.dlogits, self.V, self.G(hw, 'b'))
-                self.wgrad_gemm(self.yf, d, self.dlogits, self.V, self.G(hw, 'w'))
-            self.dgrad_gemm(self.dlogits, self.V, self.W(hw, 'w'), d, self.dy)
-        self._backward_body()
+                self.colsum(g['dlogits'], self.V, self.G(hw, 'b'), acts=a)
+                self.wgrad_gemm(a.yf, d, g['dlogits'], self.V, self.G(hw, 'w'), acts=a)
+            self.dgrad_gemm(g['dlogits'], self.V, self.W(hw, 'w'), d, g['dy'], acts=a)
+        self._backward_body(a)
 
     def train_grads(self):
         """the flat gradient buffer a training step writes: the adapters' with adapters (the base is frozen)"""
         return self.base_grads() if self.lora is None else self.lora.grads
 
-    def load_preference(self, rows, ref):
+    def load_preference(self, rows, ref, length=None):
         """rows (2P, n+1): the chosen rows, then their rejected rows; ref [2P] float32: the reference log-likelihoods in
-        the same order -> self.tok / self.labels / self.ref; returns P"""
-        B = self.load_batch(rows)
+        the same order -> self.tok / self.labels (cut to `length` as in load_batch) / self.ref; returns P"""
+        B = self.load_batch(rows, length)
         self.ref.copy_(torch.as_tensor(np.asarray(ref, np.float32)), non_blocking=True)
         return B // 2
 
@@ -715,19 +764,21 @@ class Engine:
         return dict(policy_chosen=st[:, 0].copy(), policy_rejected=st[:, 1].copy(), margin=st[:, 2].copy(),
                     loss=st[:, 3].copy())
 
-    def ln_bwd_res(self, dy, x, scale, mean, rstd, dscale, shift, next_bias_grad=None):
-        """LN(+shift) backward into the residual-gradient stream; `next_bias_grad` (+= column sums of the updated dres) is
-        the bias gradient of the block that is differentiated next (its output bias sees exactly this dres)."""
+    def ln_bwd_res(self, a, dy, x, scale, mean, rstd, dscale, shift, next_bias_grad=None):
+        """LN(+shift) backward into the residual-gradient stream of the training set or its cut view `a`;
+        `next_bias_grad` (+= column sums of the updated dres) is the bias gradient of the block that is differentiated
+        next (its output bias sees exactly this dres)."""
+        g = a.grad
         L.check(self.lib.progen_ln_shift_bwd(dy.data_ptr(), self.d, self.act_dt, x.data_ptr(), self.d, L.F32, scale.data_ptr(),
-                                             mean.data_ptr(), rstd.data_ptr(), self.dres.data_ptr(),
-                                             self.dres_lp.data_ptr() if self.mp else 0, self.d, L.ptr(dscale),
-                                             L.ptr(next_bias_grad), self.T, self.d, self.n, int(shift), 1, L.stream()), 'ln_bwd')
+                                             mean.data_ptr(), rstd.data_ptr(), g['dres'].data_ptr(),
+                                             g['dres_lp'].data_ptr() if self.mp else 0, self.d, L.ptr(dscale),
+                                             L.ptr(next_bias_grad), a.T, self.d, a.n, int(shift), 1, L.stream()), 'ln_bwd')
 
     # ------------------------------------------------------------------------------------------ property head
-    def load_property(self, rows, task, targets):
+    def load_property(self, rows, task, targets, length=None):
         """rows (B, n+1) and checked targets (regression: float32 [B, C]; classification: int32 [B]) -> self.tok /
-        self.labels / self.ptarget or self.pclass; returns B"""
-        B = self.load_batch(rows)
+        self.labels (cut to `length` as in load_batch) / self.ptarget or self.pclass; returns B"""
+        B = self.load_batch(rows, length)
         t = torch.as_tensor(targets)
         if task == L.TASK_REGRESSION:
             self.ptarget[:t.numel()].copy_(t.reshape(-1), non_blocking=True)
@@ -770,94 +821,99 @@ class Engine:
             out_p[r0:r0 + B] = host[B * d:].reshape(B, C)
         return out_p, out_e
 
-    def _backward_body(self):
-        """the backward pass below the loss head (train_step), from self.dy = d loss / d (final LayerNorm output).
+    def _backward_body(self, v):
+        """the backward pass below the loss head (train_step) on the training set or its cut view `v` (B, n and T from
+        it), from v.grad['dy'] = d loss / d (final LayerNorm output).
         With adapters (self.lora) the base is frozen: no base weight, bias, LayerNorm-scale, SGU or embedding
         gradient is computed, and every adapted projection's input gradient carries its adapter's tail (lora_bwd)."""
         lib, st = self.lib, L.stream()
-        cfg, d, I, hid, T, n = self.cfg, self.d, self.I, self.hid, self.T, self.n
+        cfg, d, I, hid, T, n = self.cfg, self.d, self.I, self.hid, v.T, v.n
         shift = cfg['shift_tokens']
         lo = self.lora
         frozen = lo is not None
         G = (lambda module, name: None) if frozen else self.G
-        tail = self.lora_bwd if frozen else (lambda *a: {})
+        tail = (lambda *a: self.lora_bwd(*a, acts=v)) if frozen else (lambda *a: {})
+        mm = dict(acts=v)
+        g_ = v.grad
+        dres_lp, dy, dqkv, datt = g_['dres_lp'], g_['dy'], g_['dqkv'], g_['datt']
         hl = P + 'layer_norm'
-        self.dres.zero_()
+        g_['dres'].zero_()
         nl = len(self.kinds)
-        self.ln_bwd_res(self.dy, self.X[-1], self.Pf(hl, 'scale'), self.meanf, self.rstdf, G(hl, 'scale'), False,
+        self.ln_bwd_res(v, dy, v.X[-1], self.Pf(hl, 'scale'), v.meanf, v.rstdf, G(hl, 'scale'), False,
                         next_bias_grad=G(P + f'ff{nl - 1}/~/linear_1', 'b'))
         for i in reversed(range(len(self.kinds))):
-            kind, s = self.kinds[i], self.lay[i]
+            kind, s = self.kinds[i], v.lay[i]
             a, f = P + f'attn{i}/~/', P + f'ff{i}/~/'
-            x0, x1 = self.X[2 * i], self.X[2 * i + 1]
-            dres_lp = self.dres_lp
+            x0, x1 = v.X[2 * i], v.X[2 * i + 1]
             # ---- FeedForward backward (d(proj_out bias) = colsum(dres) was produced by the previous LN backward)
             if kind == 'sgu':
                 half = hid // 2
                 g = f + 'sgu'
+                dpj, dsg, dgp, dgn = g_['dpj'], g_['dsg'], g_['dgp'], g_['dgn']
                 if not frozen:
-                    self.wgrad_gemm(s['pj'], half, dres_lp, d, self.G(f + 'linear_1', 'w'))
-                self.dgrad_gemm(dres_lp, d, self.W(f + 'linear_1', 'w'), half, self.dpj, **tail(s['pj'], half, f + 'linear_1', dres_lp, d))
+                    self.wgrad_gemm(s['pj'], half, dres_lp, d, self.G(f + 'linear_1', 'w'), **mm)
+                self.dgrad_gemm(dres_lp, d, self.W(f + 'linear_1', 'w'), half, dpj, **mm, **tail(s['pj'], half, f + 'linear_1', dres_lp, d))
                 if not frozen:
-                    self.colsum(self.dpj, half, self.G(g + '/~/linear', 'b'))
-                    self.wgrad_gemm(s['sg'], half, self.dpj, half, self.G(g + '/~/linear', 'w'))
-                self.dgrad_gemm(self.dpj, half, self.W(g + '/~/linear', 'w'), half, self.dsg)
-                da = self.dh_                                            # gradient wrt gelu output a = [xs | gate], [T, hid]
-                L.check(lib.progen_sgu_gate_bwd(self.dsg.data_ptr(), half, s['hact'].data_ptr(), hid, s['gp'].data_ptr(), half,
-                                                self.Pf(g, 'spatial_biases').data_ptr(), da.data_ptr(), hid, self.dgp.data_ptr(),
+                    self.colsum(dpj, half, self.G(g + '/~/linear', 'b'), **mm)
+                    self.wgrad_gemm(s['sg'], half, dpj, half, self.G(g + '/~/linear', 'w'), **mm)
+                self.dgrad_gemm(dpj, half, self.W(g + '/~/linear', 'w'), half, dsg, **mm)
+                da = g_['dh_']                                           # gradient wrt gelu output a = [xs | gate], [T, hid]
+                L.check(lib.progen_sgu_gate_bwd(dsg.data_ptr(), half, s['hact'].data_ptr(), hid, s['gp'].data_ptr(), half,
+                                                self.Pf(g, 'spatial_biases').data_ptr(), da.data_ptr(), hid, dgp.data_ptr(),
                                                 half, L.ptr(G(g, 'spatial_biases')), self.act_dt, T, half, n, st),
                         'sgu_gate_bwd')
+                # the spatial matrices keep their leading dimension self.n; a cut step uses their top-left n x n block
                 if not frozen:
                     # d spatial_weights = tril(sum_b dGp_b @ gn_b^T)
-                    self._mm(M=n, N=n, K=half, A=self.dgp, lda=half, B=s['gn'], ldb=half, out=self.G(g, 'spatial_weights'), ldo=n,
-                             epi=L.EPI_ACCUM, out_dtype=L.F32, batch=self.B, a_batch_rows=n, b_batch_rows=n, batch_reduce=True,
-                             atomic=True, tril=True, tril_rows=n)
+                    self._mm(M=n, N=n, K=half, A=dgp, lda=half, B=s['gn'], ldb=half, out=self.G(g, 'spatial_weights'),
+                             ldo=self.n, epi=L.EPI_ACCUM, out_dtype=L.F32, batch=v.B, a_batch_rows=n, b_batch_rows=n,
+                             batch_reduce=True, atomic=True, tril=True, tril_rows=n)
                 # d gn_b = tril(W)^T @ dGp_b
-                self._mm(M=n, N=half, K=n, A=self.wm[i], lda=n, a_mn=True, B=self.dgp, ldb=half, b_mn=True, out=self.dgn,
-                         ldo=half, out_dtype=self.act_dt, batch=self.B, b_batch_rows=n, d_batch_rows=n, causal=2)
+                self._mm(M=n, N=half, K=n, A=self.wm[i], lda=self.n, a_mn=True, B=dgp, ldb=half, b_mn=True, out=dgn,
+                         ldo=half, out_dtype=self.act_dt, batch=v.B, b_batch_rows=n, d_batch_rows=n, causal=2)
                 gate = s['hact'][:, half:]
-                L.check(lib.progen_ln_shift_bwd(self.dgn.data_ptr(), half, self.act_dt, gate.data_ptr(), hid, self.act_dt,
+                L.check(lib.progen_ln_shift_bwd(dgn.data_ptr(), half, self.act_dt, gate.data_ptr(), hid, self.act_dt,
                                                 self.Pf(g + '/~/layer_norm', 'scale').data_ptr(), s['mean3'].data_ptr(),
                                                 s['rstd3'].data_ptr(), 0, da[:, half:].data_ptr(), hid,
                                                 L.ptr(G(g + '/~/layer_norm', 'scale')), 0, T, half, n, 0, 0, st), 'ln_bwd_sgu')
                 L.check(lib.progen_gelu_bwd(da.data_ptr(), s['u'].data_ptr(), self.act_dt, T * hid, st), 'gelu_bwd')
                 du, n_in = da, hid
                 if not frozen:
-                    self.colsum(du, n_in, self.G(f + 'linear', 'b'))
+                    self.colsum(du, n_in, self.G(f + 'linear', 'b'), **mm)
             elif kind == 'glu':
                 # the epilogue also adds the column sums of du into the proj_in bias gradient (interleaved like du)
                 if not frozen:
-                    self.wgrad_gemm(s['hact'], hid, dres_lp, d, self.G(f + 'linear_1', 'w'))
-                self.dgrad_gemm(dres_lp, d, self.W(f + 'linear_1', 'w'), hid, self.du, epi=L.EPI_GLU_BWD, ldo=2 * hid,
-                                aux=s['u'], ldaux=2 * hid, colsum=G(f + 'linear', 'b'),
+                    self.wgrad_gemm(s['hact'], hid, dres_lp, d, self.G(f + 'linear_1', 'w'), **mm)
+                self.dgrad_gemm(dres_lp, d, self.W(f + 'linear_1', 'w'), hid, g_['du'], epi=L.EPI_GLU_BWD, ldo=2 * hid,
+                                aux=s['u'], ldaux=2 * hid, colsum=G(f + 'linear', 'b'), **mm,
                                 **tail(s['hact'], hid, f + 'linear_1', dres_lp, d))
-                du, n_in = self.du, 2 * hid
+                du, n_in = g_['du'], 2 * hid
             else:
                 if not frozen:
-                    self.wgrad_gemm(s['hact'], hid, dres_lp, d, self.G(f + 'linear_1', 'w'))
-                self.dgrad_gemm(dres_lp, d, self.W(f + 'linear_1', 'w'), hid, self.dh_, epi=L.EPI_GELU_BWD, aux=s['u'], ldaux=hid,
-                                colsum=G(f + 'linear', 'b'), **tail(s['hact'], hid, f + 'linear_1', dres_lp, d))
-                du, n_in = self.dh_, hid
+                    self.wgrad_gemm(s['hact'], hid, dres_lp, d, self.G(f + 'linear_1', 'w'), **mm)
+                self.dgrad_gemm(dres_lp, d, self.W(f + 'linear_1', 'w'), hid, g_['dh_'], epi=L.EPI_GELU_BWD, aux=s['u'], ldaux=hid,
+                                colsum=G(f + 'linear', 'b'), **mm, **tail(s['hact'], hid, f + 'linear_1', dres_lp, d))
+                du, n_in = g_['dh_'], hid
             if not frozen:
-                self.wgrad_gemm(s['y2'], d, du, n_in, self.G(f + 'linear', 'w'))
-            self.dgrad_gemm(du, n_in, self.W(f + 'linear', 'w'), d, self.dy, **tail(s['y2'], d, f + 'linear', du, n_in))
-            self.ln_bwd_res(self.dy, x1, self.Pf(f + 'layer_norm', 'scale'), s['mean2'], s['rstd2'], G(f + 'layer_norm', 'scale'), shift,
+                self.wgrad_gemm(s['y2'], d, du, n_in, self.G(f + 'linear', 'w'), **mm)
+            self.dgrad_gemm(du, n_in, self.W(f + 'linear', 'w'), d, dy, **mm, **tail(s['y2'], d, f + 'linear', du, n_in))
+            self.ln_bwd_res(v, dy, x1, self.Pf(f + 'layer_norm', 'scale'), s['mean2'], s['rstd2'], G(f + 'layer_norm', 'scale'), shift,
                             next_bias_grad=G(a + 'linear_1', 'b'))
             # ---- LocalAttention backward
             if not frozen:
-                self.wgrad_gemm(s['att'], I, dres_lp, d, self.G(a + 'linear_1', 'w'))
-            self.dgrad_gemm(dres_lp, d, self.W(a + 'linear_1', 'w'), I, self.datt, **tail(s['att'], I, a + 'linear_1', dres_lp, d))
-            self.attn_bwd(s['qkv'], s['att'], self.datt, s['lse'], self.dqkv)
+                self.wgrad_gemm(s['att'], I, dres_lp, d, self.G(a + 'linear_1', 'w'), **mm)
+            self.dgrad_gemm(dres_lp, d, self.W(a + 'linear_1', 'w'), I, datt, **mm, **tail(s['att'], I, a + 'linear_1', dres_lp, d))
+            self.attn_bwd(s['qkv'], s['att'], datt, s['lse'], dqkv, **mm)
             if not self.attn_tc:
-                L.check(lib.progen_rotary_bwd(self.dqkv.data_ptr(), 3 * I, self.act_dt, self.rot_sin.data_ptr(),
+                L.check(lib.progen_rotary_bwd(dqkv.data_ptr(), 3 * I, self.act_dt, self.rot_sin.data_ptr(),
                                               self.rot_cos.data_ptr(), T, 3 * I, n, self.dh, st), 'rotary_bwd')
             if not frozen:
-                self.wgrad_gemm(s['y1'], d, self.dqkv, 3 * I, self.G(a + 'linear', 'w'))
-            self.dgrad_gemm(self.dqkv, 3 * I, self.W(a + 'linear', 'w'), d, self.dy, **tail(s['y1'], d, a + 'linear', self.dqkv, 3 * I))
-            self.ln_bwd_res(self.dy, x0, self.Pf(a + 'layer_norm', 'scale'), s['mean1'], s['rstd1'], G(a + 'layer_norm', 'scale'), shift,
+                self.wgrad_gemm(s['y1'], d, dqkv, 3 * I, self.G(a + 'linear', 'w'), **mm)
+            self.dgrad_gemm(dqkv, 3 * I, self.W(a + 'linear', 'w'), d, dy, **mm, **tail(s['y1'], d, a + 'linear', dqkv, 3 * I))
+            self.ln_bwd_res(v, dy, x0, self.Pf(a + 'layer_norm', 'scale'), s['mean1'], s['rstd1'], G(a + 'layer_norm', 'scale'), shift,
                             next_bias_grad=G(P + f'ff{i - 1}/~/linear_1', 'b') if i > 0 else None)
         if frozen:
             lo.scale_b_grads()
             return
-        L.check(lib.progen_embed_bwd(self.tok.data_ptr(), self.dres.data_ptr(), self.G(P + 'embed', 'embeddings').data_ptr(),
+        L.check(lib.progen_embed_bwd(v.tok.data_ptr(), g_['dres'].data_ptr(), self.G(P + 'embed', 'embeddings').data_ptr(),
                                      T, d, self.V, st), 'embed_bwd')

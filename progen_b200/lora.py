@@ -173,7 +173,8 @@ class Adapters:
                     'adapter grad s')
 
     def activations(self, T):
-        """u [T, r] per adapted projection (kept for the backward pass) and one g [T, r] scratch; a new row count
+        """u [T, r] per adapted projection (kept for the backward pass) and one g [T, r] scratch, T the training set's
+        B * seq_len rows; a cut step uses their first B * length rows (Engine.lora_fwd / lora_bwd).  A new row count
         re-allocates them, which invalidates captured graphs like Engine.ensure_batch does"""
         if self.T != T:
             A = lambda: torch.empty(T, self.r, device=self.eng.dev, dtype=self.eng.act)

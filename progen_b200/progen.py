@@ -349,8 +349,9 @@ class ProGen:
         rows, ref, beta, _ = check_pairs(chosen, rejected, ref_chosen, ref_rejected, beta, None, self.config['seq_len'])
         self._ensure_loaded(params)
         eng = self.engine
-        P = eng.load_preference(rows, ref)
-        eng.train_step(('preference', beta), P)
+        n = eng.row_length(rows)                        # one cut length over all 2P rows (DESIGN.md §3.10)
+        P = eng.load_preference(rows, ref, n)
+        eng.train_step(('preference', beta), P, length=n)
         return float(eng.loss.item()), eng.export_grads(), eng.preference_stats(P)
 
     def score(self, params, data, *, batch_size=64, return_tokens=False, return_embeddings=False):
@@ -589,8 +590,9 @@ class ProGen:
         self._ensure_loaded(params)
         lo = self._attach_adapters(adapters, lora_alpha, head)
         eng = self.engine
-        B = eng.load_property(r, code, y)
-        eng.train_step(('property', code), B)
+        n = eng.row_length(r)
+        B = eng.load_property(r, code, y, n)
+        eng.train_step(('property', code), B, length=n)
         grads, hgrads = lo.split(lo.layout.unpack(lo.grads))
         return float(eng.loss.item()), grads, hgrads, eng.property_stats(B)['prediction']
 

@@ -57,12 +57,29 @@ class Trainer:
         self.ws = torch.empty(L.load().progen_optim_workspace_floats(), device=self.eng.dev)
         self.gnorm_sq = torch.zeros(1, device=self.eng.dev)
         self.rank, self.world = PAR.world() if data_parallel else (0, 1)
-        self._graph, self._graph_key, self._graph_epoch = None, None, 0
-        # cuda_graph=True: after two eager steps of one batch shape the step is captured and replayed from then on
-        self._auto_graph, self._eager_key = bool(cuda_graph), None
+        # captured steps by (key, row length): the key is (rows, global_rows) + objective; all of them hold for one
+        # batch size and one alloc_epoch.  _graph / _graph_key / _graph_length: the most recently installed one.
+        self._graphs, self._graph_epoch = {}, 0
+        self._installed, self._graph_key, self._graph_length = None, None, None
+        # cuda_graph=True: the second eager step of one (key, row length) is captured and replayed from then on
+        self._auto_graph, self._eager_runs = bool(cuda_graph), {}
         self.skip_allreduce = False                       # bench.py: "step without the exchange" for comm_exposed_ms
         if optim_state is not None:
             self.load_optim_state(optim_state)
+
+    @property
+    def _graph(self):
+        """the most recently installed captured step, or None"""
+        return self._installed
+
+    @_graph.setter
+    def _graph(self, g):
+        """`_graph = None` drops every captured step (before the communicator they reference goes away, or to step
+        eagerly)"""
+        if g is not None:
+            raise L.ProgenError('install a captured step with capture_graph')
+        self._graphs, self._eager_runs = {}, {}
+        self._installed, self._graph_key, self._graph_length = None, None, None
 
     @property
     def G(self):
@@ -70,24 +87,36 @@ class Trainer:
         return self.eng.base_grads() if self.lora is None else self.lora.grads
 
     # ---- one micro-step of train.py:186-190
-    def step(self, data, sync_loss=False, global_batch=None):
+    def step(self, data, sync_loss=False, global_batch=None, length=None):
         """data: this rank's rows, (b, n+1) integers; `global_batch` = rows of the UNSHARDED batch (utils.py:83-91: the
         masked mean divides by the real row count, so ragged shards — 5 rows over 2 ranks = 3 + 2, or ranks with no rows
         at all — must all scale by 1/5).  Without it the shards are assumed equal.  Returns the device scalar loss
-        (global mean when sync_loss)."""
+        (global mean when sync_loss).
+        `length`: the row length the step runs at (DESIGN.md §3.10).  None: the rows' `engine.cut_length` in a single
+        process, seq_len under data parallelism (every rank must run one length: pass the cut_length of the global
+        batch); rows on the device run at seq_len.  Otherwise seq_len or a multiple of 128 below it that covers every
+        counted position of the rows (ProgenError before any device work)."""
         rows = data.shape[0]
         gb = int(global_batch) if global_batch is not None else rows * self.world
-        return self._step(rows, gb, (), lambda: self.eng.load_batch(data), sync_loss)
+        n = self._length(data, length, 'step')
+        return self._step(rows, gb, (), lambda: self.eng.load_batch(data, n), sync_loss, n)
 
     def step_resident(self, global_batch=None, sync_loss=False):
-        """same, on tokens/labels already copied into engine.tok / engine.labels (bench: inputs resident in HBM)"""
-        return self._step(self.eng.B, global_batch or self.eng.B * self.world, (), None, sync_loss)
+        """same, on tokens/labels already copied into engine.tok / engine.labels (bench: inputs resident in HBM), at
+        seq_len"""
+        return self._step(self.eng.B, global_batch or self.eng.B * self.world, (), None, sync_loss, self.eng.n)
 
-    def _step(self, rows, global_rows, objective, load, sync_loss):
-        """One micro-step of `objective` (Engine.train_step) on `rows` rows, then the optimizer update.  `load()` makes
-        the rows resident (None: they are); its H2D copies stay outside the graph.  A captured graph whose key is
-        (rows, global_rows) + objective replays; otherwise the step runs eagerly, and with cuda_graph=True the second
-        eager step in a row of one key is captured for the next one to replay."""
+    def _length(self, rows, length, what):
+        """the row length of a step on `rows` (see `step`)"""
+        if length is None and self.world > 1:
+            length = self.eng.n
+        return self.eng.row_length(rows, length, what)
+
+    def _step(self, rows, global_rows, objective, load, sync_loss, length):
+        """One micro-step of `objective` (Engine.train_step) on `rows` rows at row length `length`, then the optimizer
+        update.  `load()` makes the rows resident (None: they are); its H2D copies stay outside the graph.  A captured
+        graph of (key, length), key = (rows, global_rows) + objective, replays; otherwise the step runs eagerly, and
+        with cuda_graph=True the second eager step of one (key, length) is captured for the next one to replay."""
         eng = self.eng
         eng.lora = self.lora
         if rows == 0:
@@ -99,21 +128,20 @@ class Trainer:
         self._drop_graph_unless(rows)
         if load is not None:
             load()
-        if self._graph is not None and self._graph_key == key:
-            return self._replay(sync_loss)
-        eng.train_step(objective, global_rows)
+        g = self._graphs.get((key, length))
+        if g is not None:
+            return self._replay(sync_loss, g)
+        eng.train_step(objective, global_rows, length=length)
         loss = self._eager_update(sync_loss)
         if self._auto_graph:
-            # _eager_key starts as None, so _eager_run is set here before it is read
-            self._eager_run = self._eager_run + 1 if key == self._eager_key else 1
-            self._eager_key = key
-            if self._eager_run >= 2:
-                self.capture_graph(rows, global_rows, objective=objective)   # capture does not execute: eng.loss
-                self._eager_run = 0                                         # still holds this step's value
+            runs = self._eager_runs[(key, length)] = self._eager_runs.get((key, length), 0) + 1
+            if runs >= 2:
+                # capture does not execute: eng.loss still holds this step's value
+                self.capture_graph(rows, global_rows, objective=objective, length=length)
         return loss
 
     # ---- CUDA graph of the whole step: forward, loss, backward, (gradient all-reduce), norm, AdamW, masked copies
-    def capture_graph(self, batch_rows, global_batch=None, install=True, objective=()):
+    def capture_graph(self, batch_rows, global_batch=None, install=True, objective=(), length=None):
         """Capture one training step for batches of `batch_rows` rows into a CUDA graph; later `step` / `step_resident`
         calls with that shape replay it.  The step-dependent optimizer scalars live on the device
         (`progen_adamw_step`), so the graph is identical for every step.  Under data parallelism the NCCL all-reduce
@@ -121,23 +149,29 @@ class Trainer:
         after at least one eager step of the same shape (kernel attributes, tensor maps, buffers and the NCCL communicator
         must exist before capture).  `install=False` returns the graph without making it the one `step` replays.
         `objective` (Engine.train_step) selects the loss: ('preference', beta) captures the step `preference_step`
-        replays, with batch_rows = 2 * pairs and global_batch = the global pair count."""
+        replays, with batch_rows = 2 * pairs and global_batch = the global pair count.  `length` (default seq_len): the
+        row length of the captured step; one graph is kept per (key, length), and a step replays the one of its own."""
         gb = global_batch or batch_rows * self.world
+        length = self.eng.n if length is None else int(length)
         eng = self.eng
         eng.lora = self.lora
         eng.ensure_batch(batch_rows)
+        self._drop_graph_unless(batch_rows)
         torch.cuda.synchronize()
         g = torch.cuda.CUDAGraph()
         with torch.cuda.graph(g):
-            eng.train_step(objective, gb)
+            eng.train_step(objective, gb, length=length)
             self._allreduce_grads()
             self._update()
         if install:
-            self._graph, self._graph_key, self._graph_epoch = g, (batch_rows, gb) + objective, eng.alloc_epoch
+            key = (batch_rows, gb) + objective
+            self._graphs[(key, length)] = g
+            self._installed, self._graph_key, self._graph_length, self._graph_epoch = g, key, length, eng.alloc_epoch
         return g
 
     # ---- preference (DPO) fine-tuning
-    def preference_step(self, chosen, rejected, ref_chosen, ref_rejected, beta=0.1, sync_loss=False, global_pairs=None):
+    def preference_step(self, chosen, rejected, ref_chosen, ref_rejected, beta=0.1, sync_loss=False, global_pairs=None,
+                        length=None):
         """One micro-step of preference (DPO) fine-tuning on this rank's pairs: the loss and gradient of
         `ProGen.preference_loss_and_grad`, then the same clip / AdamW / apply_every update as `step`.  chosen / rejected:
         (P, n+1) integer rows; ref_chosen / ref_rejected [P]: their log-likelihoods under the frozen reference (`score`).
@@ -145,24 +179,26 @@ class Trainer:
         P_global (default: equal shards, P * world); a rank without pairs contributes zeros but joins the all-reduce.
         With cuda_graph=True the step is captured after two eager steps of one (P, global_pairs, beta) and replayed from
         then on.  Returns the device scalar loss (global mean when sync_loss); `preference_stats()` has the per-pair
-        statistics."""
+        statistics.  `length` as in `step`, over the chosen and rejected rows together."""
         from .preference import check_pairs
         gp = global_pairs
         if gp is None and self.world > 1:
             gp = len(chosen) * self.world
         rows, ref, beta, gp = check_pairs(chosen, rejected, ref_chosen, ref_rejected, beta, gp, self.eng.n,
                                           what='preference_step', allow_empty=True)
+        n = self._length(rows, length, 'preference_step')             # one length over all 2P rows
         P = rows.shape[0] // 2
         self._pref_pairs = P
-        return self._step(2 * P, gp, ('preference', beta), lambda: self.eng.load_preference(rows, ref), sync_loss)
+        return self._step(2 * P, gp, ('preference', beta), lambda: self.eng.load_preference(rows, ref, n), sync_loss, n)
 
     # ---- property fine-tuning (a head on the pooled embedding, adapters on the frozen base)
-    def property_step(self, rows, targets, sync_loss=False):
+    def property_step(self, rows, targets, sync_loss=False, length=None):
         """One micro-step of property fine-tuning: the loss and gradients of `ProGen.property_loss_and_grad` over the
         adapters and the head, then one clip / AdamW / apply_every update of both (weight decay on every trained
         parameter).  rows: (B, n+1) integer rows; targets: regression float [B, C], classification class indices [B].
         With cuda_graph=True the step is captured after two eager steps of one batch size and replayed from then on.
-        Single process only.  Returns the device scalar loss; `property_stats()` has the predictions and per-row losses."""
+        Single process only.  Returns the device scalar loss; `property_stats()` has the predictions and per-row losses.
+        `length` as in `step`."""
         from .property import check_rows, check_targets
         if self.task is None:
             raise L.ProgenError('property_step: this trainer has no property head (model.trainer(..., head=, task=))')
@@ -175,8 +211,9 @@ class Trainer:
         if B < 1:
             raise L.ProgenError('property_step: needs at least one row')
         y = check_targets(targets, task, self.lora.head_outputs, B, 'property_step')
+        n = self._length(r, length, 'property_step')
         self._prop_rows = B
-        return self._step(B, B, ('property', self.task), lambda: self.eng.load_property(r, self.task, y), sync_loss)
+        return self._step(B, B, ('property', self.task), lambda: self.eng.load_property(r, self.task, y, n), sync_loss, n)
 
     def property_stats(self):
         """the last `property_step`'s predictions [B, C] (regression values, or class logits) and per-row losses [B] as
@@ -232,22 +269,24 @@ class Trainer:
         """a different batch size re-allocates the engine's activation buffers: the captured pointers would dangle"""
         if self._graph is not None and (batch_rows != self._graph_key[0] or
                                         self.eng.alloc_epoch != self._graph_epoch):
-            self._graph, self._graph_key = None, None      # (model.apply / sampling with another batch size re-allocates too)
+            self._graph = None                             # (model.apply / sampling with another batch size re-allocates too)
 
-    def _replay(self, sync_loss=False):
-        self._graph.replay()
+    def _replay(self, sync_loss=False, graph=None):
+        """replay `graph` (default: the most recently installed one)"""
+        (graph or self._installed).replay()
         self.count += 1
         if sync_loss and self.world > 1:
             PAR.allreduce_scalar_(self.eng.loss)           # logged loss only; the next replay zeroes it again
         return self.eng.loss
 
-    def evaluate(self, data):
-        """validation loss (train.py:207-211): forward + loss only"""
+    def evaluate(self, data, length=None):
+        """validation loss (train.py:207-211): forward + loss only; `length` as in `step`"""
         eng = self.eng
+        n = self._length(data, length, 'evaluate')
         eng.lora = self.lora
-        B = eng.load_batch(data)
+        B = eng.load_batch(data, n)
         self._drop_graph_unless(B)
-        eng.train_step((), B, backward=False)
+        eng.train_step((), B, backward=False, length=n)
         return eng.loss
 
     # ---- checkpoint interchange (haiku-shaped trees, train.py:196-202)

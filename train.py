@@ -1,6 +1,10 @@
 """train.py — drop-in for the reference CLI (lucidrains/progen train.py:36-57: same flags and defaults), running the
 H100 engine.  Additions: --synthetic (uniform-random tokens, the BASELINE workload), --num_steps, --text_file (one
-sequence per line, instead of TFRecords whose reader needs tensorflow).  Launch with torchrun for --data_parallel.
+sequence per line, instead of TFRecords whose reader needs tensorflow), --group_by_length (sort the rows of each
+effective batch by counted length before splitting it into micro-batches).  Launch with torchrun for --data_parallel.
+
+Every micro-step runs at its rows' cut length (`engine.cut_length`: the longest counted length rounded up to 128);
+under data parallelism every rank runs the cut length of the global micro-batch.
 
 Fine-tuning: --init_checkpoint DIR starts from the newest checkpoint there (its params and model_config).  With
 --lora_rank R (and --lora_alpha, default R) only low-rank adapters train on the frozen base; the checkpoints written
@@ -23,6 +27,8 @@ from progen_b200 import ProGen
 from progen_b200 import parallel as PAR
 from progen_b200.checkpoint import count_params, get_checkpoint_fns, last_checkpoint_file, load_checkpoint_file
 from progen_b200.data import decode_tokens, iterator_from_sequences, iterator_from_tfrecords_folder, synthetic_iterator
+from progen_b200.data import group_by_length as length_grouped
+from progen_b200.engine import counted_length, cut_length
 from progen_b200.utils import sample, confirm, exists
 
 
@@ -55,10 +61,12 @@ from progen_b200.utils import sample, confirm, exists
 @click.option('--init_checkpoint', default=None, help='fine-tune: start from the newest checkpoint in this directory')
 @click.option('--lora_rank', default=None, type=int, help='train low-rank adapters of this rank on the frozen --init_checkpoint')
 @click.option('--lora_alpha', default=None, type=float, help='adapter scale alpha (s = alpha / rank; default: the rank)')
+@click.option('--group_by_length', default=False, is_flag=True,
+              help='sort the rows of each effective batch by length into its micro-batches (each runs at its cut length)')
 def main(seed, batch_size, grad_accum_every, learning_rate, weight_decay, data_parallel, max_grad_norm, validate_every,
          sample_every, checkpoint_every, checkpoint_path, checkpoint_keep_n, config_path, model_name, prime_length, seq_len,
          mixed_precision, data_path, wandb_off, wandb_project_name, new, synthetic, text_file, num_steps, cuda_graph,
-         init_checkpoint, lora_rank, lora_alpha):
+         init_checkpoint, lora_rank, lora_alpha, group_by_length):
     if data_parallel and 'RANK' in os.environ:
         import torch.distributed as dist
         torch.cuda.set_device(int(os.environ.get('LOCAL_RANK', '0')))
@@ -166,18 +174,26 @@ def main(seed, batch_size, grad_accum_every, learning_rate, weight_decay, data_p
 
     effective_batch_size = batch_size * grad_accum_every
     run_id = None
-    t0, tokens = time.time(), 0
+    t0, tokens, counted = time.time(), 0, 0
     for i, seq_index in enumerate(range(start_seq_index, total_train_seqs, effective_batch_size)):
         if num_steps is not None and i >= num_steps:
             break
+        group = []
         for _ in range(grad_accum_every):
             try:
-                data = next(train_dataset)
+                group.append(next(train_dataset))
             except StopIteration:
-                return
+                break
+        # (Adam and the clipping see the micro-steps of a grouped effective batch in another order: hence opt-in)
+        for data in length_grouped(group) if group_by_length else group:
             local = PAR.shard_batch(data) if world > 1 else data
-            loss = trainer.step(local, sync_loss=True, global_batch=data.shape[0])
+            # every rank holds the global micro-batch: the ranks agree on its cut length without communicating
+            length = cut_length(data[:, 1:]) if world > 1 else None
+            loss = trainer.step(local, sync_loss=True, global_batch=data.shape[0], length=length)
             tokens += data.shape[0] * seq_len
+            counted += int(counted_length(data[:, 1:]).sum())
+        if len(group) < grad_accum_every:
+            return
         if rank == 0:
             print(f'loss: {loss.item()}')
         if i % checkpoint_every == 0 and rank == 0:
@@ -204,7 +220,9 @@ def main(seed, batch_size, grad_accum_every, learning_rate, weight_decay, data_p
                 trainer.eng.load_params(params)            # the engine's base again (apply loaded the merged weights)
             print(prime_str, '\n', '*' * 40, '\n', decode_tokens(sampled[prime_length:]))
     if rank == 0:
-        print(f'tokens/sec (host clock, incl. logging syncs): {tokens / max(1e-9, time.time() - t0):.0f}')
+        elapsed = max(1e-9, time.time() - t0)
+        print(f'tokens/sec (host clock, incl. logging syncs): {tokens / elapsed:.0f}')
+        print(f'counted tokens/sec (the positions the loss counts, same clock): {counted / elapsed:.0f}')
     if world > 1:
         import torch.distributed as dist
         trainer._graph = None                      # a captured step references the communicator: drop it before NCCL goes away
