@@ -149,6 +149,24 @@ int progen_property_head(const float* emb, const float* w, const float* bias, in
                          const int* cls, float inv_batch, float* pred, float* row_loss, float* loss, float* dpred, float* dw,
                          float* db, float* demb, void* stream);
 
+/* residue (per-position) head (DESIGN.md §3.11): pred [B*L, C] (fp32) = h [B*L, d] W [d, C] + bias, h the final LayerNorm
+ * output in dtype (stride ldh), L any row length of a cut view; a position's prediction does not depend on the other rows.
+ * Targets in the same [B*L] layout: y [B*L, C] float (regression; a position is unlabelled when its values are NaN) or
+ * cls [B*L] int (classification; -1 = unlabelled).  Training (y or cls non-null, B <= 4096): *count = N, the labelled
+ * positions; pos_loss [B*L] (0 where unlabelled); *loss = sum over labelled positions of pos_loss / N, in double, rows in
+ * order; dpred [B*L, C] = d loss / d pred (0 where unlabelled); dy [B*L, d] in dtype (stride ldy) = dpred W^T, +0.0 on
+ * unlabelled rows, every row written.  Regression pos_loss = sum_c (p - y)^2 / C, classification lse(p) - p[y].  Every
+ * sum runs in a fixed order: the outputs are the same bits in every launch.  With y and cls null only pred is written. */
+int progen_residue_head(const void* h, long long ldh, int dtype, const float* w, const float* bias, int B, int L, int d, int C,
+                        int task, const float* y, const int* cls, float* pred, float* pos_loss, int* count, float* loss,
+                        float* dpred, void* dy, long long ldy, void* stream);
+/* weight gradient of the residue head: dw [d, C] = sum h^T dpred and db [C] = sum dpred over the labelled positions
+ * (unlabelled ones are skipped), written, not accumulated.  Each row's positions are summed in ascending order into
+ * workspace [B, (d + 1) C] floats, then the rows in row order: the order does not depend on L, so a cut view and the
+ * full-length view of the same rows give the same bits. */
+int progen_residue_head_wgrad(const void* h, long long ldh, int dtype, const float* dpred, const float* y, const int* cls,
+                              int B, int L, int d, int C, float* workspace, float* dw, float* db, void* stream);
+
 /* backward of apply_rotary_pos_emb (progen.py:36-41) on the [T, ncols] q|k|v gradient, in place */
 int progen_rotary_bwd(void* dqkv, long long ld, int dtype, const float* sin_t, const float* cos_t, long long T, int ncols,
                       int seq_len, int dim_head, void* stream);

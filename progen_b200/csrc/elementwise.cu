@@ -670,6 +670,202 @@ __global__ void property_head_params_kernel(const float* __restrict__ emb, const
   dw[i] = s;
 }
 
+// ------------------------------------------------------------------------------------------ residue (per-position) head
+// The property head applied at every position of a [B*L, d] view of the final LayerNorm output (DESIGN.md §3.11).  A position
+// is labelled when its target is: class index >= 0 (classification), a non-NaN first value (regression; the host refuses a
+// partly-NaN position).  Every sum below runs in a fixed order that depends on neither the other rows nor the row length L.
+constexpr int RES_MAX_ROWS = 4096;    // rows of one training launch: per-row partials of the count and the loss in shared memory
+
+__device__ __forceinline__ bool residue_labelled(const float* y, const int* cls, long long pos, int C) {
+  return cls != nullptr ? cls[pos] >= 0 : !isnan(y[pos * C]);
+}
+
+// *count = number of labelled positions: row b's count by one thread, then the row counts in row order by thread 0.
+__global__ void residue_count_kernel(const float* __restrict__ y, const int* __restrict__ cls, int B, int L, int C,
+                                     int* __restrict__ count) {
+  __shared__ int rc[RES_MAX_ROWS];
+  for (int b = threadIdx.x; b < B; b += blockDim.x) {
+    int s = 0;
+    for (int t = 0; t < L; ++t) s += residue_labelled(y, cls, (long long)b * L + t, C) ? 1 : 0;
+    rc[b] = s;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    int s = 0;
+    for (int b = 0; b < B; ++b) s += rc[b];
+    *count = s;
+  }
+}
+
+// One warp per position, 8 positions per 256-thread block, grid-stride.  Lane l owns the columns k = 4l + 128j: it sums
+// h[k] W[k, c] over its columns in ascending k, then an xor butterfly adds the 32 lane partials (every lane ends with the
+// same bits), then + bias[c].  Training: every lane computes the position's loss and d p from those bits (regression
+// loss = sum_c (p - y)^2 / C, d p = 2 (p - y) / C / N; classification loss = lse(p) - p[y], d p = (softmax(p) -
+// onehot(y)) / N, N = *count), and dy[k] = sum_c dp_c W[k, c] in c order for its own columns.  An unlabelled position
+// gets loss 0, d p 0 and dy +0.0, so every row of dy is written.  CT: the compile-time bound of C (registers).
+template <typename TH, int CT>
+__global__ void residue_head_kernel(const TH* __restrict__ h, long long ldh, const float* __restrict__ w,
+                                    const float* __restrict__ bias, long long rows, int d, int C, int task,
+                                    const float* __restrict__ y, const int* __restrict__ cls, const int* __restrict__ count,
+                                    float* __restrict__ pred, float* __restrict__ pos_loss, float* __restrict__ dpred,
+                                    TH* __restrict__ dy, long long ldy) {
+  const int lane = threadIdx.x & 31;
+  const bool train = y != nullptr || cls != nullptr;
+  const float inv_n = train ? 1.f / (float)max(*count, 1) : 0.f;
+  for (long long pos = (long long)blockIdx.x * ROWS_PER_BLOCK + (threadIdx.x >> 5); pos < rows;
+       pos += (long long)gridDim.x * ROWS_PER_BLOCK) {
+    const TH* hr = h + pos * ldh;
+    float acc[CT];
+#pragma unroll
+    for (int c = 0; c < CT; ++c) acc[c] = 0.f;
+    for (int k = lane * 4; k < d; k += 128) {
+      float v[4];
+      load4<TH>(hr + k, v);
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const float* wk = w + (long long)(k + i) * C;
+#pragma unroll
+        for (int c = 0; c < CT; ++c)
+          if (c < C) acc[c] = fmaf(v[i], wk[c], acc[c]);
+      }
+    }
+#pragma unroll
+    for (int c = 0; c < CT; ++c) {
+      if (c < C) {
+#pragma unroll
+        for (int off = 16; off > 0; off >>= 1) acc[c] += __shfl_xor_sync(0xffffffffu, acc[c], off);
+        acc[c] += bias[c];
+        if ((c & 31) == lane) pred[pos * C + c] = acc[c];
+      }
+    }
+    if (!train) continue;
+    const bool lab = residue_labelled(y, cls, pos, C);
+    float l = 0.f;
+    if (lab && task == PROGEN_TASK_REGRESSION) {
+      const float* yp = y + pos * C;
+#pragma unroll
+      for (int c = 0; c < CT; ++c) {
+        if (c < C) {
+          const float r = acc[c] - yp[c];
+          l += r * r;
+          acc[c] = 2.f * r / (float)C * inv_n;
+        }
+      }
+      l /= (float)C;
+    } else if (lab) {
+      const int yc = min(max(cls[pos], 0), C - 1);
+      float mx = -INFINITY, py = 0.f;
+#pragma unroll
+      for (int c = 0; c < CT; ++c) {
+        if (c < C) {
+          mx = fmaxf(mx, acc[c]);
+          if (c == yc) py = acc[c];
+        }
+      }
+      float se = 0.f;
+#pragma unroll
+      for (int c = 0; c < CT; ++c)
+        if (c < C) se += expf(acc[c] - mx);
+      l = mx + logf(se) - py;
+      const float inv = 1.f / se;
+#pragma unroll
+      for (int c = 0; c < CT; ++c)
+        if (c < C) acc[c] = (expf(acc[c] - mx) * inv - (c == yc ? 1.f : 0.f)) * inv_n;
+    }
+    if (lane == 0) pos_loss[pos] = l;
+#pragma unroll
+    for (int c = 0; c < CT; ++c)
+      if (c < C && (c & 31) == lane) dpred[pos * C + c] = lab ? acc[c] : 0.f;
+    TH* dr = dy + pos * ldy;
+    for (int k = lane * 4; k < d; k += 128) {
+      float s[4] = {0.f, 0.f, 0.f, 0.f};
+      if (lab) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const float* wk = w + (long long)(k + i) * C;
+#pragma unroll
+          for (int c = 0; c < CT; ++c)
+            if (c < C) s[i] = fmaf(acc[c], wk[c], s[i]);
+        }
+      }
+      store4(dr + k, s);
+    }
+  }
+}
+
+// *loss = sum over labelled positions of pos_loss / N: row b's sum (positions ascending, in double) by one thread, then
+// the row sums in row order by thread 0.
+__global__ void residue_loss_kernel(const float* __restrict__ pos_loss, const float* __restrict__ y,
+                                    const int* __restrict__ cls, const int* __restrict__ count, int B, int L, int C,
+                                    float* __restrict__ loss) {
+  __shared__ double rs[RES_MAX_ROWS];
+  for (int b = threadIdx.x; b < B; b += blockDim.x) {
+    double s = 0.0;
+    for (int t = 0; t < L; ++t) {
+      const long long pos = (long long)b * L + t;
+      if (residue_labelled(y, cls, pos, C)) s += (double)pos_loss[pos];
+    }
+    rs[b] = s;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double s = 0.0;
+    for (int b = 0; b < B; ++b) s += rs[b];
+    *loss = (float)(s / (double)max(*count, 1));
+  }
+}
+
+// Stage 1 of the head's weight gradient: one thread per (row b, i = k C + c), i < (d + 1) C, k == d standing for the bias:
+// ws[b, i] = sum over the labelled positions t of row b, ascending, of h[b, t, k] dp[b, t, c] (the bias: dp[b, t, c]).
+// Unlabelled positions are skipped.  Loads run four positions ahead of the sequential sum.
+template <typename TH>
+__global__ void residue_wgrad_rows_kernel(const TH* __restrict__ h, long long ldh, const float* __restrict__ dpred,
+                                          const float* __restrict__ y, const int* __restrict__ cls, int L, int d, int C,
+                                          float* __restrict__ ws) {
+  const long long dc1 = (long long)(d + 1) * C;
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= dc1) return;
+  const int b = blockIdx.y;
+  const int k = (int)(i / C), c = (int)(i % C);
+  const bool is_bias = k == d;
+  const long long p0 = (long long)b * L;
+  float s = 0.f;
+  int t = 0;
+  for (; t + 4 <= L; t += 4) {
+    bool lab[4];
+    float hv[4], dv[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const long long pos = p0 + t + j;
+      lab[j] = residue_labelled(y, cls, pos, C);
+      hv[j] = is_bias ? 1.f : to_f32(h[pos * ldh + k]);
+      dv[j] = dpred[pos * C + c];
+    }
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+      if (lab[j]) s = is_bias ? s + dv[j] : fmaf(hv[j], dv[j], s);
+  }
+  for (; t < L; ++t) {
+    const long long pos = p0 + t;
+    if (!residue_labelled(y, cls, pos, C)) continue;
+    const float dv = dpred[pos * C + c];
+    s = is_bias ? s + dv : fmaf(to_f32(h[pos * ldh + k]), dv, s);
+  }
+  ws[(long long)b * dc1 + i] = s;
+}
+
+// Stage 2: dW[k, c] (and db[c]) = sum_b ws[b, i] in row order.  Written, not accumulated.
+__global__ void residue_wgrad_reduce_kernel(const float* __restrict__ ws, int B, int d, int C, float* __restrict__ dw,
+                                            float* __restrict__ db) {
+  const long long dc = (long long)d * C, dc1 = dc + C;
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= dc1) return;
+  float s = 0.f;
+  for (int b = 0; b < B; ++b) s += ws[(long long)b * dc1 + i];
+  if (i < dc) dw[i] = s;
+  else db[i - dc] = s;
+}
+
 // ------------------------------------------------------------------------------------------ rotary backward
 // forward (GEMM epilogue): o0 = x0 c - x1 s, o1 = x1 c + x0 s  =>  dx0 = d0 c + d1 s, dx1 = d1 c - d0 s.  In place.
 template <typename TO>
@@ -1033,6 +1229,66 @@ int progen_property_head(const float* emb, const float* w, const float* bias, in
   const long long dc = (long long)d * C;
   property_head_params_kernel<<<(unsigned)((dc + 255) / 256 + 1), 256, 0, s>>>(emb, dpred, row_loss, B, d, C, inv_batch, dw,
                                                                                db, loss);
+  PG_LAUNCH_CHECK();
+  return PROGEN_OK;
+}
+
+int progen_residue_head(const void* h, long long ldh, int dtype, const float* w, const float* bias, int B, int L, int d, int C,
+                        int task, const float* y, const int* cls, float* pred, float* pos_loss, int* count, float* loss,
+                        float* dpred, void* dy, long long ldy, void* stream) {
+  if (C < 1 || C > PROGEN_PROPERTY_MAX_OUTPUTS) {
+    progen_set_error("residue_head: %d outputs, the head supports 1..%d (PROGEN_PROPERTY_MAX_OUTPUTS)", C,
+                     PROGEN_PROPERTY_MAX_OUTPUTS);
+    return PROGEN_ERR_ARG;
+  }
+  PG_CHECK_ARG(B > 0 && L > 0 && d > 0 && d % 4 == 0 && ldh >= d && ldh % 4 == 0 && h && w && bias && pred);
+  PG_CHECK_ARG(dtype == PG_F32 || dtype == PG_BF16);
+  PG_CHECK_ARG(task == PROGEN_TASK_REGRESSION || task == PROGEN_TASK_CLASSIFICATION);
+  if (task == PROGEN_TASK_CLASSIFICATION && C < 2) {
+    progen_set_error("residue_head: classification needs at least 2 classes, got %d", C);
+    return PROGEN_ERR_ARG;
+  }
+  const bool train = y != nullptr || cls != nullptr;
+  if (train) {
+    PG_CHECK_ARG((task == PROGEN_TASK_REGRESSION ? y != nullptr && cls == nullptr : cls != nullptr && y == nullptr));
+    PG_CHECK_ARG(pos_loss && count && loss && dpred && dy && ldy >= d && ldy % 4 == 0 && B <= RES_MAX_ROWS);
+  }
+  cudaStream_t s = (cudaStream_t)stream;
+  const long long rows = (long long)B * L;
+  if (train) {
+    residue_count_kernel<<<1, 1024, 0, s>>>(y, cls, B, L, C, count);
+    PG_LAUNCH_CHECK();
+  }
+  const long long blocks = (rows + ROWS_PER_BLOCK - 1) / ROWS_PER_BLOCK, cap = (long long)pg_num_sms() * 16;
+  const int grid = (int)(blocks < cap ? blocks : cap);
+#define RES_HEAD(TH, CT) residue_head_kernel<TH, CT><<<grid, 256, 0, s>>>((const TH*)h, ldh, w, bias, rows, d, C, task, y, cls, \
+                                                                          count, pred, pos_loss, dpred, (TH*)dy, ldy)
+#define RES_HEAD_C(TH) do { if (C <= 4) RES_HEAD(TH, 4); else if (C <= 8) RES_HEAD(TH, 8); else RES_HEAD(TH, 64); } while (0)
+  if (dtype == PG_F32) RES_HEAD_C(float);
+  else RES_HEAD_C(bf16);
+#undef RES_HEAD_C
+#undef RES_HEAD
+  PG_LAUNCH_CHECK();
+  if (!train) return PROGEN_OK;
+  residue_loss_kernel<<<1, 1024, 0, s>>>(pos_loss, y, cls, count, B, L, C, loss);
+  PG_LAUNCH_CHECK();
+  return PROGEN_OK;
+}
+
+int progen_residue_head_wgrad(const void* h, long long ldh, int dtype, const float* dpred, const float* y, const int* cls,
+                              int B, int L, int d, int C, float* workspace, float* dw, float* db, void* stream) {
+  PG_CHECK_ARG(B > 0 && B <= 65535 && L > 0 && d > 0 && C >= 1 && C <= PROGEN_PROPERTY_MAX_OUTPUTS && ldh >= d);
+  PG_CHECK_ARG(h && dpred && workspace && dw && db && ((y != nullptr) != (cls != nullptr)));
+  PG_CHECK_ARG(dtype == PG_F32 || dtype == PG_BF16);
+  cudaStream_t s = (cudaStream_t)stream;
+  const long long dc1 = (long long)(d + 1) * C;
+  const dim3 grid((unsigned)((dc1 + 255) / 256), (unsigned)B);
+  if (dtype == PG_F32)
+    residue_wgrad_rows_kernel<float><<<grid, 256, 0, s>>>((const float*)h, ldh, dpred, y, cls, L, d, C, workspace);
+  else
+    residue_wgrad_rows_kernel<bf16><<<grid, 256, 0, s>>>((const bf16*)h, ldh, dpred, y, cls, L, d, C, workspace);
+  PG_LAUNCH_CHECK();
+  residue_wgrad_reduce_kernel<<<(unsigned)((dc1 + 255) / 256), 256, 0, s>>>(workspace, B, d, C, dw, db);
   PG_LAUNCH_CHECK();
   return PROGEN_OK;
 }

@@ -352,6 +352,8 @@ class Engine:
         self.emb, self.demb = F(B, d), F(B, d)
         self.pred, self.dpred, self.ptarget, self.prow_loss = F(B * C), F(B * C), F(B * C), F(B)
         self.pclass = torch.empty(B, device=dev, dtype=torch.int32)
+        # residue head (train_step): its B * n position buffers are sized for the head's outputs (ensure_residue)
+        self.res_C, self.res = 0, None
         # backward temporaries (shared by all layers)
         self.dres = F(T, d)
         self.dres_lp = A(T, d) if self.mp else self.dres
@@ -689,7 +691,10 @@ class Engine:
           ('property', task)    the property head on the pooled embedding (DESIGN.md §3.9), task L.TASK_REGRESSION or
                                 L.TASK_CLASSIFICATION, targets in self.ptarget / self.pclass (load_property); the
                                 forward stops after the final LayerNorm.  Needs
-                                adapters with a head (lora.Adapters with head_outputs): the base stays frozen.
+                                adapters with a head (lora.Adapters with head_outputs): the base stays frozen;
+          ('residue', task)     the same head at every position (DESIGN.md §3.11), mean over the labelled positions,
+                                targets in self.res (load_residue); like 'property' otherwise.  The loss is the mean
+                                over the micro-batch's own labelled positions: global_rows does not scale it.
         The loss is scaled by 1/global_rows (the preference loss: 1/global pairs), so that a SUM all-reduce of the
         per-rank gradients is the global mean.  With adapters (self.lora) no base gradient is computed.
         `backward=False`: the forward and the loss only (a validation loss), no gradient.
@@ -703,13 +708,15 @@ class Engine:
         pairs = self.B // 2
         if kind == 'preference' and 2 * pairs != self.B:
             raise L.ProgenError(f'preference step: {pairs} pairs need {2 * pairs} resident rows, have {self.B}')
-        if kind == 'property' and (lo is None or not lo.head_outputs):
-            raise L.ProgenError('property step: needs adapters with a property head (the base stays frozen)')
+        if kind in ('property', 'residue') and (lo is None or not lo.head_outputs):
+            raise L.ProgenError(f'{kind} step: needs adapters with a property head (the base stays frozen)')
+        if kind == 'residue' and self.res_C != lo.head_outputs:
+            raise L.ProgenError(f'residue step: no targets of a {lo.head_outputs}-output head are loaded (load_residue)')
         if not zero_grads and lo is not None:
             # the backward pass ends by scaling the whole B gradient by s (Adapters.scale_b_grads): an accumulated one
             # would be scaled twice
             raise L.ProgenError('adapters: gradients cannot accumulate across steps (zero_grads=False)')
-        self._forward_device(a, logits=kind != 'property')
+        self._forward_device(a, logits=kind not in ('property', 'residue'))
         if kind is None:
             self.loss.zero_()
         if zero_grads and backward:
@@ -724,6 +731,18 @@ class Engine:
                                                g['ce_w'].data_ptr(), self.stats.data_ptr(), self.loss.data_ptr(),
                                                self.ce_scratch.data_ptr(), g['dlogits'].data_ptr(), self.act_dt, pairs,
                                                a.n, self.V, objective[1], 1.0 / global_rows, st), 'preference_head')
+        elif kind == 'residue':
+            r, C = self.res, lo.head_outputs
+            y, cls = (r['y'].data_ptr(), 0) if objective[1] == L.TASK_REGRESSION else (0, r['cls'].data_ptr())
+            L.check(lib.progen_residue_head(a.yf.data_ptr(), d, self.act_dt, lo.head(lo.params, 'w').data_ptr(),
+                                            lo.head(lo.params, 'b').data_ptr(), a.B, a.n, d, C, objective[1], y, cls,
+                                            r['pred'].data_ptr(), r['loss'].data_ptr(), r['count'].data_ptr(),
+                                            self.loss.data_ptr(), r['dpred'].data_ptr(), g['dy'].data_ptr(), d, st),
+                    'residue_head')
+            if backward:
+                L.check(lib.progen_residue_head_wgrad(a.yf.data_ptr(), d, self.act_dt, r['dpred'].data_ptr(), y, cls, a.B,
+                                                      a.n, d, C, r['ws'].data_ptr(), lo.head(lo.grads, 'w').data_ptr(),
+                                                      lo.head(lo.grads, 'b').data_ptr(), st), 'residue_head_wgrad')
         else:
             B, C, reg = a.B, lo.head_outputs, objective[1] == L.TASK_REGRESSION
             L.check(lib.progen_masked_mean_pool(a.yf.data_ptr(), d, self.act_dt, a.labels.data_ptr(),
@@ -736,10 +755,11 @@ class Engine:
                                              lo.head(lo.grads, 'b').data_ptr(), self.demb.data_ptr(), st), 'property_head')
         if not backward:
             return
+        # the residue head has written d loss / d (final LayerNorm output) into g['dy'] itself
         if kind == 'property':
             L.check(lib.progen_masked_mean_pool_bwd(self.demb.data_ptr(), a.labels.data_ptr(), g['dy'].data_ptr(), d,
                                                     self.act_dt, a.B, a.n, d, st), 'masked_mean_pool_bwd')
-        else:
+        elif kind != 'residue':
             hw = P + 'linear'
             if lo is None:
                 self.colsum(g['dlogits'], self.V, self.G(hw, 'b'), acts=a)
@@ -820,6 +840,77 @@ class Engine:
             out_e[r0:r0 + B] = host[:B * d].reshape(B, d)
             out_p[r0:r0 + B] = host[B * d:].reshape(B, C)
         return out_p, out_e
+
+    # ------------------------------------------------------------------------------------------ residue head
+    def ensure_residue(self, C):
+        """the residue head's buffers for the training set's B * n positions and a C-output head: targets y [B*n, C]
+        (regression) and cls [B*n] (classification), pred and dpred [B*n, C], per-position loss [B*n], the count N and the
+        wgrad workspace [B, (d + 1) C].  A cut step uses their (B, L) prefix, so nothing is allocated per length.  Kept
+        until the batch size changes (ensure_batch) or a head with another C needs them; only that last re-allocation
+        moves pointers a captured step holds, and it advances alloc_epoch as ensure_batch does."""
+        if self.res_C == C:
+            return self.res
+        if self.res is not None:
+            self.alloc_epoch += 1
+        T, dev = self.T, self.dev
+        F = lambda *shape: torch.empty(*shape, device=dev, dtype=torch.float32)
+        self.res = dict(y=F(T * C), cls=torch.empty(T, device=dev, dtype=torch.int32), pred=F(T * C), dpred=F(T * C),
+                        loss=F(T), count=torch.zeros(1, device=dev, dtype=torch.int32), ws=F(self.B * (self.d + 1) * C))
+        self.res_C = C
+        return self.res
+
+    def load_residue(self, rows, task, targets, length=None):
+        """rows (B, n+1) and checked per-position targets (property.check_residue_targets: regression float32 [B, n, C]
+        with NaN where unlabelled, classification int32 [B, n] with -1) -> self.tok / self.labels and the residue
+        targets, cut to their first `length` positions (default seq_len) in the layout of the (B, length) view; returns B.
+        The engine's adapters (self.lora) carry the head."""
+        B = self.load_batch(rows, length)
+        n = self.n if length is None else length
+        t = torch.as_tensor(np.ascontiguousarray(np.asarray(targets)[:, :n]))
+        C = self.lora.head_outputs
+        r = self.ensure_residue(C)
+        if task == L.TASK_REGRESSION:
+            r['y'][:B * n * C].view(B, n, C).copy_(t, non_blocking=True)
+        else:
+            r['cls'][:B * n].view(B, n).copy_(t, non_blocking=True)
+        self.res_view = (B, n)
+        return B
+
+    def residue_stats(self, rows):
+        """the last residue step's predictions [rows, seq_len, C] (regression values, or class logits) and per-position
+        losses [rows, seq_len] (0 where unlabelled) as numpy float32; zero at positions beyond the step's row length"""
+        C = self.res_C
+        pred, loss = np.zeros((rows, self.n, C), np.float32), np.zeros((rows, self.n), np.float32)
+        if rows and C:
+            B, n = self.res_view
+            pred[:, :n] = self.res['pred'][:B * n * C].view(B, n, C)[:rows].cpu().numpy()
+            loss[:, :n] = self.res['loss'][:B * n].view(B, n)[:rows].cpu().numpy()
+        return dict(prediction=pred, loss=loss)
+
+    def predict_residues(self, data, w, b, length, batch_size=64):
+        """data: (N, n+1) integer rows; w [d, C], b [C] float32 head parameters -> prediction [N, n, C] numpy float32 at
+        every position (zero beyond `length`).  Runs the inference forward over the rows' first `length` positions
+        (property.residue_length: it covers every position that holds a residue), without the logits GEMM, then
+        progen_residue_head without targets, batch_size rows at a time, one D2H copy per chunk.  A position's prediction
+        depends on its own row's ids only."""
+        rows = torch.as_tensor(np.asarray(data).astype(np.int32))
+        N, d = rows.shape[0], self.d
+        C = int(np.asarray(w).shape[1])
+        out = np.zeros((N, self.n, C), np.float32)
+        if N == 0:
+            return out
+        hw = torch.tensor(np.asarray(w, np.float32), device=self.dev)
+        hb = torch.tensor(np.asarray(b, np.float32), device=self.dev)
+        res = torch.empty(min(batch_size, N) * length * C, device=self.dev, dtype=torch.float32)
+        lib, st = self.lib, L.stream()
+        for r0, acts in self._chunks(rows, batch_size, length):
+            B = acts.B
+            self._forward_device(acts, logits=False)
+            L.check(lib.progen_residue_head(acts.yf.data_ptr(), d, self.act_dt, hw.data_ptr(), hb.data_ptr(), B, acts.n, d,
+                                            C, L.TASK_REGRESSION, 0, 0, res.data_ptr(), 0, 0, 0, 0, 0, d, st),
+                    'residue_head')
+            out[r0:r0 + B, :length] = res[:B * length * C].cpu().numpy().reshape(B, length, C)
+        return out
 
     def _backward_body(self, v):
         """the backward pass below the loss head (train_step) on the training set or its cut view `v` (B, n and T from

@@ -62,6 +62,8 @@ PROTOTYPES = {
     'progen_masked_mean_pool': [_P, _LL, _I, _P, _P, _I, _I, _I, _P],
     'progen_masked_mean_pool_bwd': [_P, _P, _P, _LL, _I, _I, _I, _I, _P],
     'progen_property_head': [_P, _P, _P, _I, _I, _I, _I, _P, _P, _F, _P, _P, _P, _P, _P, _P, _P, _P],
+    'progen_residue_head': [_P, _LL, _I, _P, _P, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _LL, _P],
+    'progen_residue_head_wgrad': [_P, _LL, _I, _P, _P, _P, _I, _I, _I, _I, _P, _P, _P, _P],
     'progen_rotary_bwd': [_P, _LL, _I, _P, _P, _LL, _I, _I, _I, _P],
     'progen_local_attn_fwd_simt': [_P, _P, _P, _I, _I, _I, _I, _I, _I, _P],
     'progen_local_attn_bwd_simt': [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P],

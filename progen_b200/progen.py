@@ -558,7 +558,7 @@ class ProGen:
         """Device-resident training state over `params` (train.py's loop).  With `adapters` only the adapters train
         (the base stays bitwise unchanged); lora_alpha as in `loss_and_grad`.  With a property `head` (`init_head`) and
         its `task` ('regression' | 'classification') the adapters and the head train together through
-        `Trainer.property_step`."""
+        `Trainer.property_step` (per-sequence labels) or `Trainer.residue_step` (per-residue labels)."""
         from .trainer import Trainer
         return Trainer(self, params, adapters=adapters, lora_alpha=lora_alpha, head=head, task=task, **optim_kwargs)
 
@@ -611,3 +611,52 @@ class ProGen:
         self._ensure_loaded(params)
         pred, emb = self.engine.predict(r, head[HEAD]['w'], head[HEAD]['b'], batch_size=batch_size)
         return dict(prediction=pred, embedding=emb)
+
+    # ---- per-residue fine-tuning (DESIGN.md §3.11)
+    def residue_loss_and_grad(self, params, rows, targets, *, adapters, head, task, lora_alpha=None):
+        """Loss and gradients of per-residue fine-tuning: the property head (`init_head`) applied at every position to
+        the adapted model's final LayerNorm output h[b, t], p[b, t] = h[b, t] W + b.  rows: (B, n+1) integer rows of the
+        `collate` contract; the input at position t >= 1 is residue t - 1, so targets are indexed by position:
+        regression float [B, n, C] (or [B, n] when C == 1; NaN in every output marks an unlabelled position), loss =
+        sum over labelled (b, t) of sum_c (p - y)^2 / (C N); classification class indices [B, n] (-1: unlabelled), loss
+        = the mean cross entropy over the N labelled positions.  Position 0 (BOS) and pad inputs hold no residue and
+        must stay unlabelled.  ProGen is causal: h[b, t] has seen residues 0..t-1 only, so labels that depend on
+        downstream context are harder for it than for a bidirectional model.  The base is frozen.  Inputs are checked
+        before any device work (ProgenError names the first offending (row, position)).
+        Returns (python float loss, adapter gradients, head gradients, predictions [B, n, C] numpy float32: the
+        regression values or the class logits at every position, zero beyond the step's row length)."""
+        from .lora import check_adapters, check_rank_alpha
+        from .property import check_head, check_residue_targets, check_rows, check_task, residue_length
+        code = check_task(task)
+        C = check_head(self.config, head, task)
+        check_rank_alpha(check_adapters(self.config, adapters), lora_alpha)
+        r = check_rows(rows, self.config['seq_len'], 'residue_loss_and_grad')
+        if r.shape[0] < 1:
+            raise L.ProgenError('residue_loss_and_grad: needs at least one row')
+        y, labelled = check_residue_targets(r, targets, task, C, 'residue_loss_and_grad')
+        n = residue_length(r, labelled, None, 'residue_loss_and_grad')
+        self._ensure_loaded(params)
+        lo = self._attach_adapters(adapters, lora_alpha, head)
+        eng = self.engine
+        B = eng.load_residue(r, code, y, n)
+        eng.train_step(('residue', code), B, length=n)
+        grads, hgrads = lo.split(lo.layout.unpack(lo.grads))
+        return float(eng.loss.item()), grads, hgrads, eng.residue_stats(B)['prediction']
+
+    def predict_residues(self, params, head, data, *, batch_size=64):
+        """Per-residue predictions: the head at every position of the inference forward (pass merged parameters for a
+        fine-tuned model, as for `predict`).  data: (N, n+1) integer rows of the `collate` contract.  The forward is cut
+        to the rows' counted length rounded up to 128.  Returns a dict: prediction [N, n, C] float32 (regression values,
+        or class logits; 0 where no residue is) and mask [N, n] bool, the positions that hold residues (position t holds
+        residue t - 1).  A position's prediction depends on its own row only: results do not depend on batch_size."""
+        from .lora import HEAD
+        from .property import check_head, check_rows, residue_length, residue_positions
+        check_head(self.config, head)
+        batch_size = _batch_size(batch_size, 'predict_residues')
+        r = check_rows(data, self.config['seq_len'], 'predict_residues')
+        mask = residue_positions(r)
+        length = residue_length(r, mask, None, 'predict_residues')
+        self._ensure_loaded(params)
+        pred = self.engine.predict_residues(r, head[HEAD]['w'], head[HEAD]['b'], length, batch_size=batch_size)
+        pred[~mask] = 0.0
+        return dict(prediction=pred, mask=mask)

@@ -95,6 +95,146 @@ def check_targets(targets, task, C, B, what):
     return t.astype(np.int32)
 
 
+# ------------------------------------------------------------------------------------------------ per-residue labels
+def residue_positions(rows):
+    """rows (B, n+1) of the `collate` contract -> bool [B, n]: the positions that hold a residue.  The input id at
+    position t >= 1 is residue t - 1; position 0 (BOS) and pad inputs hold none."""
+    m = np.asarray(rows)[:, :-1] != 0
+    m[:, 0] = False
+    return m
+
+
+def check_residue_targets(rows, targets, task, C, what):
+    """Per-residue targets of checked rows (B, n+1) -> (targets, labelled [B, n] bool) in the layout the engine reads:
+    regression float32 [B, n, C] with NaN at unlabelled positions, classification int32 [B, n] with -1 there.
+    Regression targets are float [B, n, C] (or [B, n] when C == 1): a position is unlabelled when all of its values are
+    NaN; one with only some of them NaN, or with a value that is not finite in float32, is refused.  Classification
+    targets are integers [B, n] in [0, C), -1 meaning unlabelled.  A label at position 0 (BOS) or on a pad input is
+    refused, and so is a batch without a labelled position.  ProgenError names the first offending (row, position)."""
+    code = check_task(task)
+    B, n = rows.shape[0], rows.shape[1] - 1
+    first = lambda bad: tuple(int(i) for i in np.argwhere(bad)[0])
+    if code == L.TASK_REGRESSION:
+        try:
+            y = np.asarray(targets, np.float64)
+        except (TypeError, ValueError):
+            raise L.ProgenError(f'{what}: targets must be numbers, shape ({B}, {n}, {C})') from None
+        if C == 1 and y.shape == (B, n):
+            y = y[..., None]
+        if y.shape != (B, n, C):
+            raise L.ProgenError(f'{what}: targets must have shape ({B}, {n}, {C}) (rows, positions, head outputs), '
+                                f'got {y.shape}')
+        nan = np.isnan(y)
+        labelled = ~nan.all(-1)
+        part = nan.any(-1) & labelled
+        if part.any():
+            raise L.ProgenError(f'{what}: (row, position) {first(part)} has only some of its {C} values NaN; mark an '
+                                f'unlabelled position with NaN in every output')
+        with np.errstate(over='ignore', invalid='ignore'):
+            y32 = y.astype(np.float32)
+        bad = labelled & ~np.isfinite(y32).all(-1)
+        if bad.any():
+            raise L.ProgenError(f'{what}: (row, position) {first(bad)} has a value that is not finite in float32')
+        out = np.where(labelled[..., None], y32, np.float32(np.nan)).astype(np.float32)
+    else:
+        t = np.asarray(targets)
+        if t.shape != (B, n):
+            raise L.ProgenError(f'{what}: targets must have shape ({B}, {n}) (one class index per position), got {t.shape}')
+        if t.dtype.kind not in 'iu':
+            raise L.ProgenError(f'{what}: classification targets must be integer class indices, got dtype {t.dtype}')
+        bad = (t < -1) | (t >= C)
+        if bad.any():
+            raise L.ProgenError(f'{what}: (row, position) {first(bad)} has class {int(t[first(bad)])}; classes are in '
+                                f'[0, {C}) (the head has {C} classes), -1 marks an unlabelled position')
+        labelled = t >= 0
+        out = np.where(labelled, t, -1).astype(np.int32)
+    stray = labelled & ~residue_positions(rows)
+    if stray.any():
+        b, p = first(stray)
+        raise L.ProgenError(f'{what}: (row, position) {(b, p)} is labelled but holds no residue '
+                            f'({"position 0 is BOS" if p == 0 else "its input is pad"}); position t labels residue t - 1')
+    if not labelled.any():
+        raise L.ProgenError(f'{what}: no labelled position in the batch')
+    return out, labelled
+
+
+def residue_length(rows, labelled, length, what):
+    """the row length of a residue step or forward over rows (B, n+1) whose labelled (or predicted) positions are
+    `labelled` [B, n]: engine.check_length of the rows (None: their cut_length), which must also cover every labelled
+    position; None grows the cut to cover them (only rows with a pad inside a sequence need that)"""
+    from .engine import CUT_ALIGN, check_length
+    n = rows.shape[1] - 1
+    cut = check_length(rows[:, 1:], length, what)
+    cols = np.flatnonzero(np.asarray(labelled).any(0))
+    need = int(cols[-1]) + 1 if cols.size else 1
+    if need <= cut:
+        return cut
+    if length is not None:
+        raise L.ProgenError(f'{what}: length {length} cuts off labelled position {need - 1}')
+    return min(n, -(-need // CUT_ALIGN) * CUT_ALIGN)
+
+
+def read_residue_labelled(lines, task):
+    """Per-residue labels of a text file, one `sequence<TAB>labels` line per sequence (blank lines skipped):
+    classification labels are one class character per residue, `.` for an unlabelled residue; regression labels are
+    comma-separated numbers, one per residue, `nan` for an unlabelled one.  The label count must equal the sequence's
+    length.  Returns (sequences, labels): labels a list of strings (classification) or of float64 arrays (regression).
+    A bad line raises ProgenError naming it (1-based)."""
+    code = check_task(task)
+    seqs, labels = [], []
+    for i, line in enumerate(lines, start=1):
+        line = line.rstrip('\r\n')
+        if not line.strip():
+            continue
+        parts = line.split('\t')
+        seq = parts[0].strip()
+        if not seq:
+            raise L.ProgenError(f'line {i}: empty sequence')
+        if len(parts) != 2:
+            raise L.ProgenError(f'line {i}: expected `sequence<TAB>labels`, got {len(parts) - 1} tabs')
+        lab = parts[1].strip()
+        if code == L.TASK_CLASSIFICATION:
+            got = lab
+        else:
+            try:
+                got = np.array([float(v) for v in lab.split(',')], np.float64)
+            except ValueError:
+                raise L.ProgenError(f'line {i}: per-residue values must be comma-separated numbers (nan: unlabelled)') \
+                    from None
+            if np.isinf(got).any():
+                raise L.ProgenError(f'line {i}: values must be finite or nan (unlabelled)')
+        if len(got) != len(seq):
+            raise L.ProgenError(f'line {i}: {len(got)} labels for a sequence of {len(seq)} residues')
+        seqs.append(seq)
+        labels.append(got)
+    return seqs, labels
+
+
+def residue_label_array(labels, task, classes, seq_len):
+    """file labels (read_residue_labelled) -> per-position targets of their `collate` rows: classification int32
+    [N, seq_len] (class index, -1 unlabelled), regression float64 [N, seq_len] (NaN unlabelled).  Residue i sits at
+    position i + 1; residues past position seq_len - 1 have no representation and are dropped, as collate truncates.
+    ProgenError names a class character that is not one of `classes`."""
+    code = check_task(task)
+    N = len(labels)
+    if code == L.TASK_CLASSIFICATION:
+        index = {c: k for k, c in enumerate(classes)}
+        out = np.full((N, seq_len), -1, np.int32)
+        for r, lab in enumerate(labels):
+            for i, ch in enumerate(lab[:seq_len - 1]):
+                if ch == '.':
+                    continue
+                if ch not in index:
+                    raise L.ProgenError(f'sequence {r}: class {ch!r} is not one of the training classes {classes}')
+                out[r, i + 1] = index[ch]
+        return out
+    out = np.full((N, seq_len), np.nan, np.float64)
+    for r, lab in enumerate(labels):
+        v = np.asarray(lab, np.float64)[:seq_len - 1]
+        out[r, 1:1 + len(v)] = v
+    return out
+
+
 # ------------------------------------------------------------------------------------------------ fitness.py data
 def read_labelled(lines, task):
     """Labelled sequences of a text file: `sequence<TAB>value[<TAB>value...]` (regression, the same number of values on

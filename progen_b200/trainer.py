@@ -4,7 +4,8 @@ accumulator live in flat fp32 buffers; one `step(data)` is one iteration of the 
 
 With low-rank adapters (`adapters=`) the same state exists for the adapter buffer only: the base parameters are frozen
 and bitwise unchanged, and clip / AdamW / apply_every run over the adapters (weight decay on every A and B).  A property
-head (`head=`, `task=`) joins that buffer: `property_step` trains adapters and head together (DESIGN.md §3.9)."""
+head (`head=`, `task=`) joins that buffer: `property_step` trains adapters and head together on per-sequence labels
+(DESIGN.md §3.9), `residue_step` on per-residue labels (§3.11)."""
 import torch
 
 from . import lib as L
@@ -214,6 +215,36 @@ class Trainer:
         n = self._length(r, length, 'property_step')
         self._prop_rows = B
         return self._step(B, B, ('property', self.task), lambda: self.eng.load_property(r, self.task, y, n), sync_loss, n)
+
+    # ---- per-residue fine-tuning (the same head at every position, DESIGN.md §3.11)
+    def residue_step(self, rows, targets, sync_loss=False, length=None):
+        """One micro-step of per-residue fine-tuning: the loss and gradients of `ProGen.residue_loss_and_grad` over the
+        adapters and the head, then one clip / AdamW / apply_every update of both.  rows: (B, n+1) integer rows;
+        targets per position (`property.check_residue_targets`): regression float [B, n, C] (NaN: unlabelled),
+        classification class indices [B, n] (-1: unlabelled).  With cuda_graph=True the step is captured after two eager
+        steps of one (batch size, row length) and replayed from then on.  Single process only.  Returns the device scalar
+        loss; `residue_stats()` has the predictions and per-position losses.  `length` as in `step`; it must also cover
+        every labelled position."""
+        from .property import check_residue_targets, check_rows, residue_length
+        if self.task is None:
+            raise L.ProgenError('residue_step: this trainer has no property head (model.trainer(..., head=, task=))')
+        if self.world > 1:
+            raise L.ProgenError('residue_step: data-parallel residue fine-tuning is not supported; run one process '
+                                '(data_parallel=False or without torchrun)')
+        task = 'regression' if self.task == L.TASK_REGRESSION else 'classification'
+        r = check_rows(rows, self.eng.n, 'residue_step')
+        B = r.shape[0]
+        if B < 1:
+            raise L.ProgenError('residue_step: needs at least one row')
+        y, labelled = check_residue_targets(r, targets, task, self.lora.head_outputs, 'residue_step')
+        n = residue_length(r, labelled, length, 'residue_step')
+        self._res_rows = B
+        return self._step(B, B, ('residue', self.task), lambda: self.eng.load_residue(r, self.task, y, n), sync_loss, n)
+
+    def residue_stats(self):
+        """the last `residue_step`'s predictions [B, n, C] (regression values, or class logits) and per-position losses
+        [B, n] (0 where unlabelled) as numpy float32"""
+        return self.eng.residue_stats(getattr(self, '_res_rows', 0))
 
     def property_stats(self):
         """the last `property_step`'s predictions [B, C] (regression values, or class logits) and per-row losses [B] as
