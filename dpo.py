@@ -1,7 +1,8 @@
 """dpo.py — preference (DPO) fine-tuning of a checkpoint on chosen / rejected sequence pairs, on one GPU.
 
     python dpo.py --init_checkpoint ./ckpts --pairs pairs.tsv --checkpoint_path ./ckpts_dpo --beta 0.1 \\
-        --learning_rate 1e-6 --batch_pairs 8 --grad_accum_every 1 --epochs 1 --seed 0 [--mixed_precision] [--cuda_graph]
+        --learning_rate 1e-6 --batch_pairs 8 --grad_accum_every 1 --epochs 1 --seed 0 [--mixed_precision] [--cuda_graph] \\
+        [--recompute]
 
 --pairs has one pair per line, `chosen<TAB>rejected`; each side is a text sequence, tokenized like train.py --text_file
 (data.collate).  Blank lines are skipped.  The reference model is the newest checkpoint under --init_checkpoint: the
@@ -38,8 +39,10 @@ def epoch_order(num_pairs, epoch, seed):
 @click.option('--checkpoint_keep_n', default=500)
 @click.option('--mixed_precision', default=False, is_flag=True, help='bf16 tensor-core engine')
 @click.option('--cuda_graph', default=False, is_flag=True, help='capture the step into a CUDA graph and replay it')
+@click.option('--recompute', default=False, is_flag=True,
+              help='recompute activations in the backward pass: one residual checkpoint per layer (less memory, more time)')
 def main(init_checkpoint, pairs_path, checkpoint_path, beta, learning_rate, batch_pairs, grad_accum_every, epochs, seed,
-         checkpoint_keep_n, mixed_precision, cuda_graph):
+         checkpoint_keep_n, mixed_precision, cuda_graph, recompute):
     if batch_pairs < 1 or grad_accum_every < 1 or epochs < 1:
         raise click.UsageError('--batch_pairs, --grad_accum_every and --epochs must be >= 1')
     try:
@@ -54,7 +57,7 @@ def main(init_checkpoint, pairs_path, checkpoint_path, beta, learning_rate, batc
         raise click.ClickException(f'no checkpoints found at {init_checkpoint}')
     model_kwargs = init['model_config']
     seq_len = model_kwargs['seq_len']
-    model = ProGen(**{**model_kwargs, 'mixed_precision': mixed_precision})
+    model = ProGen(**{**model_kwargs, 'mixed_precision': mixed_precision}, recompute=recompute)
     c_rows, r_rows = collate(chosen, seq_len), collate(rejected, seq_len)
     # the reference's log-likelihoods, once, before the trainer loads the policy into the same engine
     ref_c = model.score(init['params'], c_rows)['log_likelihood']

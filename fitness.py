@@ -3,7 +3,7 @@ base, and predict with it, on one GPU.
 
     python fitness.py train --init_checkpoint ./ckpts --train train.tsv [--valid valid.tsv] --task regression \\
         --lora_rank 16 [--lora_alpha 16] --checkpoint_path ./ckpts_fit --learning_rate 1e-4 --batch_size 8 --epochs 3 \\
-        --seed 0 [--mixed_precision] [--cuda_graph]
+        --seed 0 [--mixed_precision] [--cuda_graph] [--recompute]
     python fitness.py train ... --level residue --train residues.tsv --task classification ...
     python fitness.py predict --checkpoint_path ./ckpts_fit --input seqs.txt --output preds.tsv
 
@@ -158,9 +158,11 @@ def cli():
 @click.option('--checkpoint_keep_n', default=500)
 @click.option('--mixed_precision', default=False, is_flag=True, help='bf16 tensor-core engine')
 @click.option('--cuda_graph', default=False, is_flag=True, help='capture the step into a CUDA graph and replay it')
+@click.option('--recompute', default=False, is_flag=True,
+              help='recompute activations in the backward pass: one residual checkpoint per layer (less memory, more time)')
 def train(init_checkpoint, train_path, valid_path, task, level, lora_rank, lora_alpha, checkpoint_path, learning_rate,
           weight_decay, max_grad_norm, batch_size, grad_accum_every, epochs, seed, checkpoint_keep_n, mixed_precision,
-          cuda_graph):
+          cuda_graph, recompute):
     if batch_size < 1 or grad_accum_every < 1 or epochs < 1:
         raise click.UsageError('--batch_size, --grad_accum_every and --epochs must be >= 1')
     _, get_last_checkpoint, save_checkpoint = get_checkpoint_fns(checkpoint_path)
@@ -190,7 +192,7 @@ def train(init_checkpoint, train_path, valid_path, task, level, lora_rank, lora_
     base = load_checkpoint_file(base_file)
     params, model_kwargs = base['params'], base['model_config']
     seq_len = model_kwargs['seq_len']
-    model = ProGen(**{**model_kwargs, 'mixed_precision': mixed_precision})
+    model = ProGen(**{**model_kwargs, 'mixed_precision': mixed_precision}, recompute=recompute)
     if last is not None:
         if count_params(params) != last['num_params']:
             raise click.ClickException(f'base checkpoint {base_file} has changed')

@@ -6,7 +6,8 @@ batched over sequences (the reference's `vmap`, utils.py:67).  PyTorch provides 
 Data layout in HBM (tokens are rows, T = B * seq_len):
   * residual stream: fp32 [T, d], one buffer per LayerNorm input (the residual epilogue of each GEMM writes the next
     one, so nothing is copied and every LN backward still has its input); the inference set (`Engine.score`) keeps one
-    buffer and updates it in place;
+    buffer and updates it in place; a training set in recompute mode keeps one per layer input and one shared
+    attention-block output (`training_set`);
   * activations: act dtype (bf16 with mixed_precision, fp32 without), row-major [T, features];
   * q|k|v: one [T, 3*heads*dim_head] buffer, rotated in the QKV GEMM epilogue;
   * parameters, gradients, Adam moments: FLAT fp32 buffers in "engine layout" (ndim > 1 leaves first, then the
@@ -69,6 +70,75 @@ def layer_kinds(depth, global_mlp_depth, ff_glu):
         use_gmlp = (depth - i) <= global_mlp_depth
         out.append('sgu' if use_gmlp else ('glu' if ff_glu else 'gelu'))
     return out
+
+
+def training_set(cfg, B, mixed_precision, recompute=False, device='meta'):
+    """The training activation set of B rows of seq_len positions (Engine.ensure_batch), as {attribute: buffer}, and
+    the bytes it allocates.  On the default 'meta' device nothing is allocated: the count is the shapes'.
+
+    Resident (recompute=False): every LayerNorm input X[k] and one scratch dict per layer, all kept for the backward
+    pass.  Recomputed (DESIGN.md §3.12): one fp32 checkpoint per layer input X[2i] (the final LayerNorm's input
+    included), one attention-block output that every X[2i+1] aliases, and one layer scratch that every layer aliases,
+    cut from one storage as wide as the widest layer kind; the backward pass re-runs each layer into it
+    (Engine.recompute_layer).  Head buffers and backward temporaries are the same in both modes."""
+    d, n, V, h = cfg['dim'], cfg['seq_len'], cfg['num_tokens'], cfg['heads']
+    I, hid = cfg['heads'] * cfg['dim_head'], cfg['dim'] * cfg['ff_mult']
+    half = hid // 2
+    kinds = layer_kinds(cfg['depth'], cfg['global_mlp_depth'], cfg['ff_glu'])
+    act = torch.bfloat16 if mixed_precision else torch.float32
+    T = B * n
+    allocated = []
+
+    def new(shape, dtype):
+        t = torch.empty(*shape, device=device, dtype=dtype)
+        allocated.append(t)
+        return t
+    A = lambda *shape: new(shape, act)
+    F = lambda *shape: new(shape, torch.float32)
+    nl = len(kinds)
+    b = dict(tok=new((T,), torch.int32), labels=new((T,), torch.int32))
+    if not recompute:
+        b['X'] = [F(T, d) for _ in range(2 * nl + 1)]            # residual stream at every LN input
+        b['lay'] = []
+        for kind in kinds:
+            s = dict(mean1=F(T), rstd1=F(T), y1=A(T, d), qkv=A(T, 3 * I), att=A(T, I), lse=F(T, h),
+                     mean2=F(T), rstd2=F(T), y2=A(T, d))
+            if kind == 'glu':
+                s.update(u=A(T, 2 * hid), hact=A(T, hid))
+            else:
+                s.update(u=A(T, hid), hact=A(T, hid))
+            if kind == 'sgu':
+                s.update(mean3=F(T), rstd3=F(T), gn=A(T, half), gp=A(T, half), sg=A(T, half), pj=A(T, half))
+            b['lay'].append(s)
+    else:
+        ck, x_att = [F(T, d) for _ in range(nl + 1)], F(T, d)
+        b['X'] = [x for c in ck[:-1] for x in (c, x_att)] + ck[-1:]
+        common = dict(mean1=F(T), rstd1=F(T), y1=A(T, d), qkv=A(T, 3 * I), att=A(T, I), lse=F(T, h),
+                      mean2=F(T), rstd2=F(T), y2=A(T, d))
+        width = dict(glu=3 * hid, gelu=2 * hid, sgu=4 * hid)      # u, hact (and gn, gp, sg, pj) in act-dtype columns
+        wide = A(T * max(width[k] for k in kinds))
+        part = lambda col, w: wide[col * T:(col + w) * T].view(T, w)      # a contiguous [T, w] block: cuts by rows
+        per_kind = dict(glu=dict(common, u=part(0, 2 * hid), hact=part(2 * hid, hid)),
+                        gelu=dict(common, u=part(0, hid), hact=part(hid, hid)))
+        if 'sgu' in kinds:
+            per_kind['sgu'] = dict(common, u=part(0, hid), hact=part(hid, hid), mean3=F(T), rstd3=F(T),
+                                   gn=part(2 * hid, half), gp=part(2 * hid + half, half), sg=part(3 * hid, half),
+                                   pj=part(3 * hid + half, half))
+        b['lay'] = [per_kind[k] for k in kinds]
+    b.update(meanf=F(T), rstdf=F(T), yf=A(T, d), logits=F(T, V), dlogits=A(T, V), ce_w=F(T))
+    # preference (DPO) head (train_step): B = 2 * pairs rows; allocated here so a captured step's pointers stay valid
+    b.update(logp=F(T), seq_ll=F(B), seq_count=F(B), ref=F(B), stats=F(max(1, B // 2), 4), ce_scratch=F(1))
+    # property head (train_step): pooled embedding and its gradient, predictions, targets, per-row losses
+    C = L.PROPERTY_MAX_OUTPUTS
+    b.update(emb=F(B, d), demb=F(B, d), pred=F(B * C), dpred=F(B * C), ptarget=F(B * C), prow_loss=F(B),
+             pclass=new((B,), torch.int32))
+    # backward temporaries (shared by all layers)
+    b.update(dres=F(T, d))
+    b.update(dres_lp=A(T, d) if mixed_precision else b['dres'], dy=A(T, d), dqkv=A(T, 3 * I), datt=A(T, I),
+             delta=F(T, h), du=A(T, 2 * hid), dh_=A(T, hid))
+    if 'sgu' in kinds:
+        b.update(dpj=A(T, half), dsg=A(T, half), dgp=A(T, half), dgn=A(T, half))
+    return b, sum(t.numel() * t.element_size() for t in allocated)
 
 
 class ParamSpec:
@@ -176,7 +246,8 @@ def _deinterleave(a):
 class Acts:
     """One activation set: the buffers one forward pass runs on (B sequences of n positions, T = B * n token rows).
     `X` lists the residual stream at every LayerNorm input and `lay` one scratch dict per layer.  The training set keeps
-    all of them (the backward pass reads them) and its backward temporaries by name in `grad`; the inference set
+    all of them (the backward pass reads them; in recompute mode the odd X and the layers alias one buffer each, see
+    `training_set`) and its backward temporaries by name in `grad`; the inference set
     (`inplace`) repeats one residual buffer, updated in place, and one layer's scratch, and stores no GLU / GELU
     pre-activation (`u` is None)."""
 
@@ -205,9 +276,12 @@ class Acts:
 
 
 class Engine:
-    def __init__(self, cfg, mixed_precision=False, device=None):
+    def __init__(self, cfg, mixed_precision=False, device=None, recompute=False):
         L.require_device()
         self.cfg = cfg
+        # recompute: the training set keeps one residual checkpoint per layer and the backward pass re-runs each layer's
+        # forward from it (DESIGN.md §3.12); a way of running, not a property of the model
+        self.recompute = bool(recompute)
         self.dev = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
         self.mp = bool(mixed_precision)
         self.act = torch.bfloat16 if self.mp else torch.float32
@@ -260,6 +334,8 @@ class Engine:
         self.B = 0
         self.alloc_epoch = 0      # counts re-allocations of the training activations: a captured step holds for one epoch
         self.acts = None          # training activation set (ensure_batch)
+        self._train_keys = ()     # the attributes ensure_batch set from training_set
+        self.train_bytes = 0      # ... and the bytes they hold
         self.infer = None         # inference activation set (inference_acts), cached by row count
         self.loss = torch.zeros(1, device=self.dev)       # exists before the first batch: a rank without rows still reports 0
         self.loaded_token = None
@@ -312,66 +388,39 @@ class Engine:
 
     # ------------------------------------------------------------------------------------------ workspaces
     def ensure_batch(self, B):
+        """the training activation set (`training_set`) for B rows, in this engine's mode (resident or recompute);
+        kept until B or the mode changes"""
         if B == self.B:
             return
         self.B = B
         self.alloc_epoch += 1                                       # activation buffers are re-allocated below: captured
                                                                     # CUDA graphs (Trainer.capture_graph) become invalid
-        T = B * self.n
-        self.T = T
-        d, I, hid = self.d, self.I, self.hid
-        dev, act = self.dev, self.act
-        A = lambda *shape: torch.empty(*shape, device=dev, dtype=act)
-        F = lambda *shape: torch.empty(*shape, device=dev, dtype=torch.float32)
-        nl = len(self.kinds)
-        self.tok = torch.empty(T, device=dev, dtype=torch.int32)
-        self.labels = torch.empty(T, device=dev, dtype=torch.int32)
-        self.X = [F(T, d) for _ in range(2 * nl + 1)]           # residual stream at every LN input
-        self.lay = []
-        for kind in self.kinds:
-            s = dict(mean1=F(T), rstd1=F(T), y1=A(T, d), qkv=A(T, 3 * I), att=A(T, I), lse=F(T, self.h),
-                     mean2=F(T), rstd2=F(T), y2=A(T, d))
-            if kind == 'glu':
-                s.update(u=A(T, 2 * hid), hact=A(T, hid))
-            else:
-                s.update(u=A(T, hid), hact=A(T, hid))
-            if kind == 'sgu':
-                half = hid // 2
-                s.update(mean3=F(T), rstd3=F(T), gn=A(T, half), gp=A(T, half), sg=A(T, half), pj=A(T, half))
-            self.lay.append(s)
-        self.meanf, self.rstdf, self.yf = F(T), F(T), A(T, d)
-        self.logits = F(T, self.V)
-        self.dlogits = A(T, self.V)
-        self.ce_w = F(T)
-        # preference (DPO) head (train_step): B = 2 * pairs rows; allocated here so a captured step's pointers
-        # stay valid
-        self.logp, self.seq_ll, self.seq_count, self.ref = F(T), F(B), F(B), F(B)
-        self.stats, self.ce_scratch = F(max(1, B // 2), 4), F(1)
-        # property head (train_step): pooled embedding and its gradient, predictions, targets, per-row losses
-        C = L.PROPERTY_MAX_OUTPUTS
-        self.emb, self.demb = F(B, d), F(B, d)
-        self.pred, self.dpred, self.ptarget, self.prow_loss = F(B * C), F(B * C), F(B * C), F(B)
-        self.pclass = torch.empty(B, device=dev, dtype=torch.int32)
+        self.T = B * self.n
+        self.acts = None
+        for k in self._train_keys:                                  # release the old set before allocating the new one
+            setattr(self, k, None)
+        bufs, self.train_bytes = training_set(self.cfg, B, self.mp, self.recompute, self.dev)
+        vars(self).update(bufs)                                     # self.X, self.lay, self.logits, self.dres, ...
+        self._train_keys = tuple(bufs)
         # residue head (train_step): its B * n position buffers are sized for the head's outputs (ensure_residue)
         self.res_C, self.res = 0, None
-        # backward temporaries (shared by all layers)
-        self.dres = F(T, d)
-        self.dres_lp = A(T, d) if self.mp else self.dres
-        self.dy = A(T, d)
-        self.dqkv = A(T, 3 * I)
-        self.datt = A(T, I)
-        self.delta = F(T, self.h)
-        self.du = A(T, 2 * hid)
-        self.dh_ = A(T, hid)
-        half = hid // 2
-        if 'sgu' in self.kinds:
-            self.dpj, self.dsg, self.dgp, self.dgn = A(T, half), A(T, half), A(T, half), A(T, half)
         grad = dict(dres=self.dres, dres_lp=self.dres_lp, dy=self.dy, dqkv=self.dqkv, datt=self.datt, delta=self.delta,
                     du=self.du, dh_=self.dh_, dlogits=self.dlogits, ce_w=self.ce_w, logp=self.logp)
         if 'sgu' in self.kinds:
             grad.update(dpj=self.dpj, dsg=self.dsg, dgp=self.dgp, dgn=self.dgn)
         self.acts = Acts(B, self.n, self.tok, self.labels, self.X, self.lay, self.meanf, self.rstdf, self.yf, self.logits,
                          grad=grad)
+
+    def set_recompute(self, on):
+        """switch the training set between resident and recomputed activations; a change re-allocates an existing set
+        at once (advancing alloc_epoch, so captured steps are dropped before their next replay)"""
+        on = bool(on)
+        if on == self.recompute:
+            return
+        self.recompute = on
+        if self.B:
+            B, self.B = self.B, 0
+            self.ensure_batch(B)
 
     def inference_acts(self, B):
         """Activation set of a forward pass that keeps no training state, for up to B sequences: one fp32 residual buffer
@@ -493,61 +542,12 @@ class Engine:
         op is causal, so a forward on a view cut to the first n positions computes exactly those positions of the full
         one (DESIGN.md §3.6)."""
         acts = self.acts if acts is None else acts
-        lib, st = self.lib, L.stream()
-        cfg, d, I, hid, T, n = self.cfg, self.d, self.I, self.hid, acts.T, acts.n
-        shift = cfg['shift_tokens']
-        lo = None if acts.inplace else self.lora            # adapters run on the training set (or its cut view) only
-        if lo is not None:
-            lo.activations(self.acts.T)
-        tail = (lambda *a: self.lora_fwd(*a, acts=acts)) if lo is not None else (lambda *a: {})
-        L.check(lib.progen_embed_fwd(acts.tok.data_ptr(), self.Pf(P + 'embed', 'embeddings').data_ptr(), acts.X[0].data_ptr(),
-                                     T, d, self.V, st), 'embed_fwd')
-        for i, kind in enumerate(self.kinds):
-            s = acts.lay[i]
-            a, f = P + f'attn{i}/~/', P + f'ff{i}/~/'
-            # in place (inference): x0 = x1 = x2 is one buffer, and the residual epilogue without aux reads its output
-            x0, x1, x2 = acts.X[2 * i], acts.X[2 * i + 1], acts.X[2 * i + 2]
-            # ---- LocalAttention (progen.py:73-103)
-            self.ln_fwd(x0, d, self.Pf(a + 'layer_norm', 'scale'), s['y1'], d, s['mean1'], s['rstd1'], d, shift, acts=acts)
-            self.fwd_gemm(s['y1'], d, self.W(a + 'linear', 'w'), 3 * I, s['qkv'], epi=L.EPI_ROTARY, rot_sin=self.rot_sin,
-                          rot_cos=self.rot_cos, seq_len=n, dim_head=self.dh, acts=acts, **tail(s['y1'], d, a + 'linear', 3 * I))
-            if sink is not None:
-                sink(i, 'qkv', s['qkv'])
-                sink(i, 'y1', s['y1'])
-            self.attn_fwd(s['qkv'], s['att'], s['lse'], acts=acts)
-            self.fwd_gemm(s['att'], I, self.W(a + 'linear_1', 'w'), d, x1, epi=L.EPI_RESIDUAL, bias=self.Pf(a + 'linear_1', 'b'),
-                          aux=None if acts.inplace else x0, ldaux=d, acts=acts, **tail(s['att'], I, a + 'linear_1', d))
-            # ---- FeedForward (progen.py:131-149); s['u'] is None in the inference set: no pre-activation store
-            self.ln_fwd(x1, d, self.Pf(f + 'layer_norm', 'scale'), s['y2'], d, s['mean2'], s['rstd2'], d, shift, acts=acts)
-            if sink is not None:
-                sink(i, 'y2', s['y2'])
-            if kind == 'glu':
-                self.fwd_gemm(s['y2'], d, self.W(f + 'linear', 'w'), 2 * hid, s['hact'], epi=L.EPI_GLU, ldo=hid, out2=s['u'],
-                              ldo2=2 * hid, bias=self.Pf(f + 'linear', 'b'), acts=acts, **tail(s['y2'], d, f + 'linear', 2 * hid))
-                last, last_k = s['hact'], hid
-            else:
-                self.fwd_gemm(s['y2'], d, self.W(f + 'linear', 'w'), hid, s['hact'], epi=L.EPI_GELU, out2=s['u'], ldo2=hid,
-                              bias=self.Pf(f + 'linear', 'b'), acts=acts, **tail(s['y2'], d, f + 'linear', hid))
-                last, last_k = s['hact'], hid
-            if kind == 'sgu':
-                half = hid // 2
-                g = f + 'sgu'
-                gate = s['hact'][:, half:]
-                self.ln_fwd(gate, hid, self.Pf(g + '/~/layer_norm', 'scale'), s['gn'], half, s['mean3'], s['rstd3'], half, False,
-                            acts=acts)
-                # gate_b = tril(W) @ gn_b for every sequence b; masked K tiles are skipped (causal=1)
-                self._mm(M=n, N=half, K=n, A=self.wm[i], lda=self.n, B=s['gn'], ldb=half, b_mn=True, out=s['gp'], ldo=half,
-                         out_dtype=self.act_dt, batch=acts.B, b_batch_rows=n, d_batch_rows=n, causal=1)
-                if sink is not None:
-                    sink(i, 'gn', s['gn'])
-                L.check(lib.progen_sgu_gate_fwd(s['hact'].data_ptr(), hid, s['gp'].data_ptr(), half,
-                                                self.Pf(g, 'spatial_biases').data_ptr(), s['sg'].data_ptr(), half, self.act_dt,
-                                                T, half, n, st), 'sgu_gate_fwd')
-                self.fwd_gemm(s['sg'], half, self.W(g + '/~/linear', 'w'), half, s['pj'], bias=self.Pf(g + '/~/linear', 'b'),
-                              acts=acts)
-                last, last_k = s['pj'], half
-            self.fwd_gemm(last, last_k, self.W(f + 'linear_1', 'w'), d, x2, epi=L.EPI_RESIDUAL, bias=self.Pf(f + 'linear_1', 'b'),
-                          aux=None if acts.inplace else x1, ldaux=d, acts=acts, **tail(last, last_k, f + 'linear_1', d))
+        d, T = self.d, acts.T
+        tail = self._lora_tail(acts)
+        L.check(self.lib.progen_embed_fwd(acts.tok.data_ptr(), self.Pf(P + 'embed', 'embeddings').data_ptr(),
+                                          acts.X[0].data_ptr(), T, d, self.V, L.stream()), 'embed_fwd')
+        for i in range(len(self.kinds)):
+            self._layer_forward(i, acts, tail, sink)
         if sink is not None:
             return
         # ---- to_logits (progen.py:219-222)
@@ -557,6 +557,77 @@ class Engine:
             return
         self.fwd_gemm(acts.yf, d, self.W(P + 'linear', 'w'), self.V, acts.logits, bias=self.Pf(P + 'linear', 'b'), out_dtype=L.F32,
                       acts=acts)
+
+    def _lora_tail(self, acts):
+        """the forward's adapter tails on activation set `acts` (lora_fwd): adapters run on the training set (or its cut
+        view) only"""
+        lo = None if acts.inplace else self.lora
+        if lo is None:
+            return lambda *a: {}
+        lo.activations(self.acts.T)
+        return lambda *a: self.lora_fwd(*a, acts=acts)
+
+    def _layer_forward(self, i, acts, tail, sink=None, through='all'):
+        """layer i of the forward on activation set `acts`, from its input acts.X[2i]: with through='all' up to its
+        output acts.X[2i+2]; with through='ff_in' (recompute_layer) it stops before the feed-forward output GEMM, the
+        one launch that writes the next layer's input.  `tail` gives each projection's adapter tail (_lora_tail)."""
+        lib, st, kind, s = self.lib, L.stream(), self.kinds[i], acts.lay[i]
+        cfg, d, I, hid, T, n = self.cfg, self.d, self.I, self.hid, acts.T, acts.n
+        shift = cfg['shift_tokens']
+        a, f = P + f'attn{i}/~/', P + f'ff{i}/~/'
+        # in place (inference): x0 = x1 = x2 is one buffer, and the residual epilogue without aux reads its output
+        x0, x1, x2 = acts.X[2 * i], acts.X[2 * i + 1], acts.X[2 * i + 2]
+        # ---- LocalAttention (progen.py:73-103)
+        self.ln_fwd(x0, d, self.Pf(a + 'layer_norm', 'scale'), s['y1'], d, s['mean1'], s['rstd1'], d, shift, acts=acts)
+        self.fwd_gemm(s['y1'], d, self.W(a + 'linear', 'w'), 3 * I, s['qkv'], epi=L.EPI_ROTARY, rot_sin=self.rot_sin,
+                      rot_cos=self.rot_cos, seq_len=n, dim_head=self.dh, acts=acts, **tail(s['y1'], d, a + 'linear', 3 * I))
+        if sink is not None:
+            sink(i, 'qkv', s['qkv'])
+            sink(i, 'y1', s['y1'])
+        self.attn_fwd(s['qkv'], s['att'], s['lse'], acts=acts)
+        self.fwd_gemm(s['att'], I, self.W(a + 'linear_1', 'w'), d, x1, epi=L.EPI_RESIDUAL, bias=self.Pf(a + 'linear_1', 'b'),
+                      aux=None if acts.inplace else x0, ldaux=d, acts=acts, **tail(s['att'], I, a + 'linear_1', d))
+        # ---- FeedForward (progen.py:131-149); s['u'] is None in the inference set: no pre-activation store
+        self.ln_fwd(x1, d, self.Pf(f + 'layer_norm', 'scale'), s['y2'], d, s['mean2'], s['rstd2'], d, shift, acts=acts)
+        if sink is not None:
+            sink(i, 'y2', s['y2'])
+        if kind == 'glu':
+            self.fwd_gemm(s['y2'], d, self.W(f + 'linear', 'w'), 2 * hid, s['hact'], epi=L.EPI_GLU, ldo=hid, out2=s['u'],
+                          ldo2=2 * hid, bias=self.Pf(f + 'linear', 'b'), acts=acts, **tail(s['y2'], d, f + 'linear', 2 * hid))
+            last, last_k = s['hact'], hid
+        else:
+            self.fwd_gemm(s['y2'], d, self.W(f + 'linear', 'w'), hid, s['hact'], epi=L.EPI_GELU, out2=s['u'], ldo2=hid,
+                          bias=self.Pf(f + 'linear', 'b'), acts=acts, **tail(s['y2'], d, f + 'linear', hid))
+            last, last_k = s['hact'], hid
+        if kind == 'sgu':
+            half = hid // 2
+            g = f + 'sgu'
+            gate = s['hact'][:, half:]
+            self.ln_fwd(gate, hid, self.Pf(g + '/~/layer_norm', 'scale'), s['gn'], half, s['mean3'], s['rstd3'], half, False,
+                        acts=acts)
+            # gate_b = tril(W) @ gn_b for every sequence b; masked K tiles are skipped (causal=1)
+            self._mm(M=n, N=half, K=n, A=self.wm[i], lda=self.n, B=s['gn'], ldb=half, b_mn=True, out=s['gp'], ldo=half,
+                     out_dtype=self.act_dt, batch=acts.B, b_batch_rows=n, d_batch_rows=n, causal=1)
+            if sink is not None:
+                sink(i, 'gn', s['gn'])
+            L.check(lib.progen_sgu_gate_fwd(s['hact'].data_ptr(), hid, s['gp'].data_ptr(), half,
+                                            self.Pf(g, 'spatial_biases').data_ptr(), s['sg'].data_ptr(), half, self.act_dt,
+                                            T, half, n, st), 'sgu_gate_fwd')
+            self.fwd_gemm(s['sg'], half, self.W(g + '/~/linear', 'w'), half, s['pj'], bias=self.Pf(g + '/~/linear', 'b'),
+                          acts=acts)
+            last, last_k = s['pj'], half
+        if through == 'ff_in':
+            return
+        self.fwd_gemm(last, last_k, self.W(f + 'linear_1', 'w'), d, x2, epi=L.EPI_RESIDUAL, bias=self.Pf(f + 'linear_1', 'b'),
+                      aux=None if acts.inplace else x1, ldaux=d, acts=acts, **tail(last, last_k, f + 'linear_1', d))
+
+    def recompute_layer(self, i, acts=None):
+        """re-run layer i's forward on the training set (or its cut view `acts`) from its checkpoint X[2i], up to the
+        feed-forward output GEMM: its scratch and X[2i+1] (shared by every layer in recompute mode) and its adapters' u
+        then hold what the forward wrote, bitwise (the same launches on the same inputs; DESIGN.md §3.12).  The
+        feed-forward output adapter's u is kept per layer and is not re-run."""
+        acts = self.acts if acts is None else acts
+        self._layer_forward(i, acts, self._lora_tail(acts), through='ff_in')
 
     def attn_fwd(self, qkv, out, lse, acts=None):
         a = acts or self.acts
@@ -916,7 +987,8 @@ class Engine:
         """the backward pass below the loss head (train_step) on the training set or its cut view `v` (B, n and T from
         it), from v.grad['dy'] = d loss / d (final LayerNorm output).
         With adapters (self.lora) the base is frozen: no base weight, bias, LayerNorm-scale, SGU or embedding
-        gradient is computed, and every adapted projection's input gradient carries its adapter's tail (lora_bwd)."""
+        gradient is computed, and every adapted projection's input gradient carries its adapter's tail (lora_bwd).
+        In recompute mode every layer but the last is re-run (recompute_layer) before its backward."""
         lib, st = self.lib, L.stream()
         cfg, d, I, hid, T, n = self.cfg, self.d, self.I, self.hid, v.T, v.n
         shift = cfg['shift_tokens']
@@ -933,6 +1005,10 @@ class Engine:
         self.ln_bwd_res(v, dy, v.X[-1], self.Pf(hl, 'scale'), v.meanf, v.rstdf, G(hl, 'scale'), False,
                         next_bias_grad=G(P + f'ff{nl - 1}/~/linear_1', 'b'))
         for i in reversed(range(len(self.kinds))):
+            if self.recompute and i < nl - 1:
+                # the shared layer scratch still holds the last layer's forward; every other layer is re-run from its
+                # checkpoint into it (its backward reads no buffer the re-run writes besides those)
+                self.recompute_layer(i, v)
             kind, s = self.kinds[i], v.lay[i]
             a, f = P + f'attn{i}/~/', P + f'ff{i}/~/'
             x0, x1 = v.X[2 * i], v.X[2 * i + 1]

@@ -230,13 +230,16 @@ def launch_tables(tables, row_table, rows):
 class ProGen:
     def __init__(self, *, num_tokens, dim, seq_len, depth, window_size=256, global_mlp_depth=2, heads=8, dim_head=64,
                  ff_mult=4, ff_glu=True, attn_dim=None, clamp_gate=True, shift_tokens=True, mixed_precision=False,
-                 mixed_precision_policy=None):
+                 mixed_precision_policy=None, recompute=False):
         # attn_dim / clamp_gate are accepted and ignored, exactly like the reference (progen.py:201-202)
+        # recompute (DESIGN.md §3.12): training steps keep one residual checkpoint per layer and re-run each layer's
+        # forward in the backward pass; a way of running, so it is not part of `config` (nor of checkpoints)
         self.config = dict(num_tokens=num_tokens, dim=dim, seq_len=seq_len, depth=depth, window_size=window_size,
                            global_mlp_depth=global_mlp_depth, heads=heads, dim_head=dim_head, ff_mult=ff_mult,
                            ff_glu=ff_glu, attn_dim=attn_dim, clamp_gate=clamp_gate, shift_tokens=shift_tokens)
         assert seq_len % window_size == 0, 'sequence length must be divisible by the window size'   # progen.py:80
         self.mixed_precision = bool(mixed_precision)
+        self._recompute = bool(recompute)
         self._engine = None
         self._loaded = None
         self._gen_decoder = self._gen_params = None
@@ -245,8 +248,20 @@ class ProGen:
     @property
     def engine(self):
         if self._engine is None:
-            self._engine = Engine(self.config, self.mixed_precision)
+            self._engine = Engine(self.config, self.mixed_precision, recompute=self._recompute)
         return self._engine
+
+    @property
+    def recompute(self):
+        """whether training steps recompute activations (DESIGN.md §3.12); setting it re-allocates the engine's training
+        activations"""
+        return self._recompute
+
+    @recompute.setter
+    def recompute(self, on):
+        self._recompute = bool(on)
+        if self._engine is not None:
+            self._engine.set_recompute(on)
 
     def param_shapes(self):
         return build_param_specs(self.config).shapes()

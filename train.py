@@ -1,7 +1,9 @@
 """train.py — drop-in for the reference CLI (lucidrains/progen train.py:36-57: same flags and defaults), running the
 H100 engine.  Additions: --synthetic (uniform-random tokens, the BASELINE workload), --num_steps, --text_file (one
 sequence per line, instead of TFRecords whose reader needs tensorflow), --group_by_length (sort the rows of each
-effective batch by counted length before splitting it into micro-batches).  Launch with torchrun for --data_parallel.
+effective batch by counted length before splitting it into micro-batches), --recompute (keep one residual checkpoint
+per layer and re-run each layer's forward in the backward pass, DESIGN.md §3.12; a resumed run may switch it).
+Launch with torchrun for --data_parallel.
 
 Every micro-step runs at its rows' cut length (`engine.cut_length`: the longest counted length rounded up to 128);
 under data parallelism every rank runs the cut length of the global micro-batch.
@@ -63,10 +65,12 @@ from progen_b200.utils import sample, confirm, exists
 @click.option('--lora_alpha', default=None, type=float, help='adapter scale alpha (s = alpha / rank; default: the rank)')
 @click.option('--group_by_length', default=False, is_flag=True,
               help='sort the rows of each effective batch by length into its micro-batches (each runs at its cut length)')
+@click.option('--recompute', default=False, is_flag=True,
+              help='recompute activations in the backward pass: one residual checkpoint per layer (less memory, more time)')
 def main(seed, batch_size, grad_accum_every, learning_rate, weight_decay, data_parallel, max_grad_norm, validate_every,
          sample_every, checkpoint_every, checkpoint_path, checkpoint_keep_n, config_path, model_name, prime_length, seq_len,
          mixed_precision, data_path, wandb_off, wandb_project_name, new, synthetic, text_file, num_steps, cuda_graph,
-         init_checkpoint, lora_rank, lora_alpha, group_by_length):
+         init_checkpoint, lora_rank, lora_alpha, group_by_length, recompute):
     if data_parallel and 'RANK' in os.environ:
         import torch.distributed as dist
         torch.cuda.set_device(int(os.environ.get('LOCAL_RANK', '0')))
@@ -124,7 +128,7 @@ def main(seed, batch_size, grad_accum_every, learning_rate, weight_decay, data_p
         assert cfg_file.exists(), f'path to your model config {str(cfg_file)} does not exist'
         model_kwargs = toml.loads(cfg_file.read_text())
 
-    model = ProGen(**{**model_kwargs, 'mixed_precision': mixed_precision})
+    model = ProGen(**{**model_kwargs, 'mixed_precision': mixed_precision}, recompute=recompute)
     adapters, lora_cfg = None, None
     if lora and exists(last_checkpoint):
         params = base['params']
