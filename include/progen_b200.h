@@ -126,6 +126,20 @@ int progen_token_logprob(const void* logits, int dtype, const int* labels, float
 int progen_preference_head(const void* logits, int dtype, const int* labels, const float* ref_ll, float* logp, float* seq_ll,
                            float* seq_count, float* weights, float* stats, float* loss, float* ce_scratch, void* dlogits,
                            int dlogits_dtype, int pairs, int n, int V, float beta, float inv_pairs, void* stream);
+/* distillation head (DESIGN.md §3.13): student logits s [B*n, V] in dtype, teacher logits z fp32 with row b, position t at
+ * teacher + (b * teacher_row_stride + t) * V (teacher_row_stride >= n: the teacher may run at a longer row length), labels
+ * [B*n] with the loss mask m_t of progen_ce_fwd_bwd (Q8) and c_b = sum_t m_t.  Per position, lq = log_softmax(s / tau),
+ * lp = log_softmax(z / tau), KL_t = sum_v exp(lp_v) (lp_v - lq_v) (terms whose exp(lp_v) underflows to 0 add 0) and
+ * CE_t = -log_softmax(s)[label_t] (label clamped to [0, V)).  stats [B, 2] = (KL_b, CE_b) = sum_t m_t (KL_t, CE_t) / c_b;
+ * *loss = inv_batch * sum_b [(1 - alpha) tau^2 KL_b + alpha CE_b] in double, rows in order (written, not accumulated);
+ * dlogits [B*n, V] in dlogits_dtype = inv_batch m_t / c_b [(1 - alpha) tau (softmax(s / tau) - softmax(z / tau)) +
+ * alpha (softmax(s) - onehot(label_t))], every row written (+0.0 where m_t = 0; those positions do not read the teacher).
+ * weights [B*n] and scratch [2*B*n] are fp32 workspaces.  No float atomics reach stats, loss or dlogits: they are the same
+ * bits in every launch.  Refused: null pointers, V % 4 != 0, teacher_row_stride < n, tau not finite and > 0, alpha
+ * outside [0, 1], inv_batch not finite and > 0, dtypes outside the progen_ce_fwd_bwd combinations. */
+int progen_distill_head(const void* logits, int dtype, const float* teacher, long long teacher_row_stride, const int* labels,
+                        float* weights, float* scratch, float* stats, float* loss, void* dlogits, int dlogits_dtype, int B,
+                        int n, int V, float tau, float alpha, float inv_batch, void* stream);
 /* out[b, :] = sum_t mask_t x[b, t, :] / sum_t mask_t (fp32, fixed order) over rows of x [B*n, d] (stride ldx), with the
  * same mask as above: for a sequence of L residues, input positions 0..L (BOS and every residue). */
 int progen_masked_mean_pool(const void* x, long long ldx, int dtype, const int* labels, float* out, int B, int n, int d,

@@ -513,6 +513,110 @@ __global__ void preference_weights_kernel(const int* __restrict__ labels, const 
   }
 }
 
+// ------------------------------------------------------------------------------------------ distillation head
+// One warp per position t (row b = t / n, position p = t - b n), w_t = inv_batch m_t / c_b from ce_weights_kernel.
+// kl[t] = KL_t and ce[t] = CE_t (0 where m_t = 0) and the position's logit gradient, with c_kl = (1 - alpha) tau:
+//   dlogits_t = w_t [c_kl (softmax(s / tau) - softmax(z / tau)) + alpha (softmax(s) - onehot(label_t))].
+// A masked position writes a zero gradient row and does not read the teacher row.  Every sum runs in a fixed order.
+template <typename TL, typename TD>
+__global__ void distill_pos_kernel(const TL* __restrict__ logits, const float* __restrict__ teacher, long long stride,
+                                   const int* __restrict__ labels, const float* __restrict__ w, float* __restrict__ kl,
+                                   float* __restrict__ ce, TD* __restrict__ dlogits, long long T, int n, int V,
+                                   float inv_tau, float c_kl, float alpha) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (long long t = blockIdx.x * (long long)ROWS_PER_BLOCK + warp; t < T; t += (long long)gridDim.x * ROWS_PER_BLOCK) {
+    TD* dr = dlogits + t * V;
+    const float wt = w[t];
+    if (wt == 0.f) {
+      const float zero[4] = {0.f, 0.f, 0.f, 0.f};
+      for (int c = lane * 4; c < V; c += 128) store4(dr + c, zero);
+      if (lane == 0) { kl[t] = 0.f; ce[t] = 0.f; }
+      continue;
+    }
+    const TL* lr = logits + t * V;
+    const long long b = t / n;
+    const float* zr = teacher + (b * stride + (t - b * n)) * V;
+    float ms, se1;
+    warp_row_max_sumexp<TL>(lr, V, lane, ms, se1);
+    float mz = -INFINITY;
+    for (int c = lane * 4; c < V; c += 128) {
+      float z[4];
+      load4<float>(zr + c, z);
+      mz = fmaxf(mz, fmaxf(fmaxf(z[0], z[1]), fmaxf(z[2], z[3])));
+    }
+    mz = warp_max(mz);
+    float ses = 0.f, sez = 0.f;
+    for (int c = lane * 4; c < V; c += 128) {
+      float s[4], z[4];
+      load4<TL>(lr + c, s);
+      load4<float>(zr + c, z);
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        ses += expf((s[i] - ms) * inv_tau);
+        sez += expf((z[i] - mz) * inv_tau);
+      }
+    }
+    ses = warp_sum(ses);
+    sez = warp_sum(sez);
+    const float lses = logf(ses), lsez = logf(sez), inv1 = 1.f / se1;
+    const int lab = clamp_label(labels[t], V);
+    float k = 0.f;
+    for (int c = lane * 4; c < V; c += 128) {
+      float s[4], z[4], o[4];
+      load4<TL>(lr + c, s);
+      load4<float>(zr + c, z);
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const float lq = (s[i] - ms) * inv_tau - lses, lp = (z[i] - mz) * inv_tau - lsez;
+        const float q = expf(lq), p = expf(lp);
+        if (p > 0.f) k += p * (lp - lq);
+        o[i] = wt * (c_kl * (q - p) + alpha * (expf(s[i] - ms) * inv1 - ((c + i) == lab ? 1.f : 0.f)));
+      }
+      store4(dr + c, o);
+    }
+    k = warp_sum(k);
+    if (lane == 0) {
+      kl[t] = k;
+      ce[t] = (ms + logf(se1)) - to_f32(lr[lab]);
+    }
+  }
+}
+
+constexpr int DISTILL_THREADS = 256;
+
+// One block per row b: stats[b] = (sum_t kl[t], sum_t ce[t]) / c_b, each thread summing positions threadIdx.x + k *
+// DISTILL_THREADS ascending in double, then the thread partials in thread order.  Positions past a cut view hold zeros
+// in the full-length view, so a cut and the full view give the same bits.
+__global__ void distill_row_kernel(const int* __restrict__ labels, const float* __restrict__ kl, const float* __restrict__ ce,
+                                   float* __restrict__ stats, int n) {
+  const int b = blockIdx.x;
+  int first, count;
+  seq_loss_mask(labels + (long long)b * n, n, first, count);
+  double a = 0.0, c = 0.0;
+  for (int i = threadIdx.x; i < n; i += DISTILL_THREADS) {
+    a += (double)kl[(long long)b * n + i];
+    c += (double)ce[(long long)b * n + i];
+  }
+  __shared__ double ra[DISTILL_THREADS], rc[DISTILL_THREADS];
+  ra[threadIdx.x] = a;
+  rc[threadIdx.x] = c;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double sa = 0.0, sc = 0.0;
+    for (int k = 0; k < DISTILL_THREADS; ++k) { sa += ra[k]; sc += rc[k]; }
+    stats[2LL * b] = (float)(sa / (double)count);
+    stats[2LL * b + 1] = (float)(sc / (double)count);
+  }
+}
+
+// *loss = inv_batch * sum_b [(1 - alpha) tau^2 KL_b + alpha CE_b], one thread, rows in order, in double
+__global__ void distill_loss_kernel(const float* __restrict__ stats, int B, double c_kl2, double alpha, double inv_batch,
+                                    float* __restrict__ loss) {
+  double s = 0.0;
+  for (int b = 0; b < B; ++b) s += c_kl2 * (double)stats[2LL * b] + alpha * (double)stats[2LL * b + 1];
+  *loss = (float)(s * inv_batch);
+}
+
 // out[b, :] = sum_t mask_t x[b, t, :] / sum_t mask_t.  Grid (ceil(d / 128), B), 256 threads: lane owns 4 columns, warp w sums
 // rows t = w, w + 8, ... in order, then the 8 warp partials are added in order: fixed order, fp32 accumulation.
 template <typename TX>
@@ -1174,6 +1278,40 @@ int progen_preference_head(const void* logits, int dtype, const int* labels, con
   else if (f32_bf16) CE_CASE(float, bf16);
   else CE_CASE(bf16, bf16);
 #undef CE_CASE
+  PG_LAUNCH_CHECK();
+  return PROGEN_OK;
+}
+
+int progen_distill_head(const void* logits, int dtype, const float* teacher, long long teacher_row_stride, const int* labels,
+                        float* weights, float* scratch, float* stats, float* loss, void* dlogits, int dlogits_dtype, int B,
+                        int n, int V, float tau, float alpha, float inv_batch, void* stream) {
+  PG_CHECK_ARG(logits && teacher && labels && weights && scratch && stats && loss && dlogits);
+  PG_CHECK_ARG(B > 0 && n > 0 && V > 0 && V % 4 == 0 && teacher_row_stride >= n);
+  PG_CHECK_ARG(std::isfinite(tau) && tau > 0.f && std::isfinite(1.f / tau) && alpha >= 0.f && alpha <= 1.f);
+  PG_CHECK_ARG(std::isfinite(inv_batch) && inv_batch > 0.f);
+  const bool f32_f32 = dtype == PG_F32 && dlogits_dtype == PG_F32, f32_bf16 = dtype == PG_F32 && dlogits_dtype == PG_BF16,
+             bf16_bf16 = dtype == PG_BF16 && dlogits_dtype == PG_BF16;
+  if (!(f32_f32 || f32_bf16 || bf16_bf16)) {
+    progen_set_error("distill_head: unsupported dtypes %d / %d", dtype, dlogits_dtype);
+    return PROGEN_ERR_UNSUPPORTED;
+  }
+  cudaStream_t s = (cudaStream_t)stream;
+  const long long T = (long long)B * n;
+  ce_weights_kernel<<<B, 256, 0, s>>>(labels, weights, n, inv_batch);
+  PG_LAUNCH_CHECK();
+  const int grid = row_grid(T);
+  const float c_kl = (1.f - alpha) * tau;
+#define DISTILL_CASE(TL, TD) distill_pos_kernel<TL, TD><<<grid, 256, 0, s>>>((const TL*)logits, teacher, teacher_row_stride, \
+      labels, weights, scratch, scratch + T, (TD*)dlogits, T, n, V, 1.f / tau, c_kl, alpha)
+  if (f32_f32) DISTILL_CASE(float, float);
+  else if (f32_bf16) DISTILL_CASE(float, bf16);
+  else DISTILL_CASE(bf16, bf16);
+#undef DISTILL_CASE
+  PG_LAUNCH_CHECK();
+  distill_row_kernel<<<B, DISTILL_THREADS, 0, s>>>(labels, scratch, scratch + T, stats, n);
+  PG_LAUNCH_CHECK();
+  distill_loss_kernel<<<1, 1, 0, s>>>(stats, B, (1.0 - (double)alpha) * (double)tau * (double)tau, (double)alpha,
+                                      (double)inv_batch, loss);
   PG_LAUNCH_CHECK();
   return PROGEN_OK;
 }

@@ -340,6 +340,8 @@ class Engine:
         self.loss = torch.zeros(1, device=self.dev)       # exists before the first batch: a rank without rows still reports 0
         self.loaded_token = None
         self.lora = None                  # lora.Adapters: the training set runs the adapted model with a frozen base
+        self.teacher = None               # distillation (attach_teacher): a second Engine whose logits are the target
+        self.dist = None                  # ... and the distillation head's buffers (ensure_distill)
         self.lib = L.load()
         self.num_sms = torch.cuda.get_device_properties(self.dev).multi_processor_count
 
@@ -404,6 +406,7 @@ class Engine:
         self._train_keys = tuple(bufs)
         # residue head (train_step): its B * n position buffers are sized for the head's outputs (ensure_residue)
         self.res_C, self.res = 0, None
+        self.dist = None                                            # distillation head buffers (ensure_distill)
         grad = dict(dres=self.dres, dres_lp=self.dres_lp, dy=self.dy, dqkv=self.dqkv, datt=self.datt, delta=self.delta,
                     du=self.du, dh_=self.dh_, dlogits=self.dlogits, ce_w=self.ce_w, logp=self.logp)
         if 'sgu' in self.kinds:
@@ -766,6 +769,10 @@ class Engine:
           ('residue', task)     the same head at every position (DESIGN.md §3.11), mean over the labelled positions,
                                 targets in self.res (load_residue); like 'property' otherwise.  The loss is the mean
                                 over the micro-batch's own labelled positions: global_rows does not scale it.
+          ('distill', tau, alpha)  distillation from the attached teacher (DESIGN.md §3.13): the teacher's forward on
+                                the rows load_distill staged in its inference set, at teacher_length(length), then the
+                                student's forward, progen_distill_head ((1 - alpha) tau^2 KL + alpha CE per row, mean over
+                                rows; per-row (KL, CE) in self.dist['stats']) and the LM backward from dlogits.
         The loss is scaled by 1/global_rows (the preference loss: 1/global pairs), so that a SUM all-reduce of the
         per-rank gradients is the global mean.  With adapters (self.lora) no base gradient is computed.
         `backward=False`: the forward and the loss only (a validation loss), no gradient.
@@ -787,6 +794,9 @@ class Engine:
             # the backward pass ends by scaling the whole B gradient by s (Adapters.scale_b_grads): an accumulated one
             # would be scaled twice
             raise L.ProgenError('adapters: gradients cannot accumulate across steps (zero_grads=False)')
+        if kind == 'distill':
+            ta = self._teacher_view(a.B, a.n)
+            self.teacher._forward_device(ta)
         self._forward_device(a, logits=kind not in ('property', 'residue'))
         if kind is None:
             self.loss.zero_()
@@ -814,6 +824,12 @@ class Engine:
                 L.check(lib.progen_residue_head_wgrad(a.yf.data_ptr(), d, self.act_dt, r['dpred'].data_ptr(), y, cls, a.B,
                                                       a.n, d, C, r['ws'].data_ptr(), lo.head(lo.grads, 'w').data_ptr(),
                                                       lo.head(lo.grads, 'b').data_ptr(), st), 'residue_head_wgrad')
+        elif kind == 'distill':
+            dist = self.dist
+            L.check(lib.progen_distill_head(a.logits.data_ptr(), L.F32, ta.logits.data_ptr(), ta.n, a.labels.data_ptr(),
+                                            g['ce_w'].data_ptr(), dist['scratch'].data_ptr(), dist['stats'].data_ptr(),
+                                            self.loss.data_ptr(), g['dlogits'].data_ptr(), self.act_dt, a.B, a.n, self.V,
+                                            objective[1], objective[2], 1.0 / global_rows, st), 'distill_head')
         else:
             B, C, reg = a.B, lo.head_outputs, objective[1] == L.TASK_REGRESSION
             L.check(lib.progen_masked_mean_pool(a.yf.data_ptr(), d, self.act_dt, a.labels.data_ptr(),
@@ -854,6 +870,62 @@ class Engine:
         st = self.stats[:pairs].cpu().numpy() if pairs else np.zeros((0, 4), np.float32)
         return dict(policy_chosen=st[:, 0].copy(), policy_rejected=st[:, 1].copy(), margin=st[:, 2].copy(),
                     loss=st[:, 3].copy())
+
+    # ------------------------------------------------------------------------------------------ distillation
+    def attach_teacher(self, teacher):
+        """make Engine `teacher` (checked by distill.check_teacher) the target of 'distill' steps.  A teacher keeps only
+        its parameters, their compute copies and its inference set: its base gradient and any training set are released
+        (a later training step of its own allocates them again)."""
+        self.teacher = teacher
+        teacher.lora = None
+        teacher.grads = None
+        if teacher.B:
+            teacher.alloc_epoch += 1
+            teacher.B, teacher.acts, teacher.dist, teacher.res_C, teacher.res = 0, None, None, 0, None
+            for k in teacher._train_keys:
+                setattr(teacher, k, None)
+            teacher._train_keys, teacher.train_bytes = (), 0
+
+    def _teacher_view(self, B, length):
+        """the (B, teacher_length(length)) view of the teacher's inference set that load_distill filled"""
+        from .distill import teacher_length
+        t = self.teacher
+        if t is None or t.infer is None or t.infer.B < B:
+            raise L.ProgenError('distill step: no teacher rows are loaded (attach_teacher, then load_distill)')
+        return t.infer.view(B, teacher_length(length, t.n))
+
+    def ensure_distill(self):
+        """the distillation head's buffers for the training set's B rows: the per-position (KL, CE) scratch [2 B n] and
+        the per-row stats [B, 2]; a cut step uses their prefix.  Kept until the batch size changes (ensure_batch)."""
+        if self.dist is None:
+            F = lambda *shape: torch.zeros(*shape, device=self.dev, dtype=torch.float32)
+            self.dist = dict(scratch=F(2 * self.T), stats=F(self.B, 2))
+        return self.dist
+
+    def load_distill(self, data, length=None):
+        """rows (B, n+1) -> the student's self.tok / self.labels as load_batch, and the same rows, zero-padded to the
+        teacher's seq_len + 1, into the (B, teacher_length(length)) view of the teacher's inference set (allocated for B
+        rows when it holds fewer); returns B"""
+        from .distill import teacher_length
+        B = self.load_batch(data, length)
+        self.ensure_distill()
+        t = self.teacher
+        Lt = teacher_length(self.n if length is None else length, t.n)
+        ta = t.inference_acts(B).view(B, Lt)
+        rows = torch.as_tensor(np.asarray(data).astype(np.int32) if not isinstance(data, torch.Tensor) else data)
+        k = min(Lt, rows.shape[1])
+        tok = ta.tok.view(B, Lt)
+        if k < Lt:
+            tok.zero_()
+        tok[:, :k].copy_(rows[:, :k].to(device=self.dev, dtype=torch.int32), non_blocking=True)
+        return B
+
+    def distill_stats(self, rows):
+        """the last distillation step's per-row (KL, CE) as numpy float32 [rows] arrays"""
+        if not rows or self.dist is None:
+            return dict(kl=np.zeros(0, np.float32), ce=np.zeros(0, np.float32))
+        st = self.dist['stats'][:rows].cpu().numpy()
+        return dict(kl=st[:, 0].copy(), ce=st[:, 1].copy())
 
     def ln_bwd_res(self, a, dy, x, scale, mean, rstd, dscale, shift, next_bias_grad=None):
         """LN(+shift) backward into the residual-gradient stream of the training set or its cut view `a`;

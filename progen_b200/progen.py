@@ -369,6 +369,32 @@ class ProGen:
         eng.train_step(('preference', beta), P, length=n)
         return float(eng.loss.item()), eng.export_grads(), eng.preference_stats(P)
 
+    def distill_loss_and_grad(self, params, data, *, teacher, teacher_params, temperature=2.0, alpha=0.5, adapters=None,
+                              lora_alpha=None):
+        """Loss and gradients of distilling `teacher` (another ProGen with the same vocabulary and a seq_len at least
+        this model's, run on `teacher_params`) into this model (DESIGN.md §3.13).  data: (B, n+1) integer rows of the
+        `collate` contract.  Per counted position t (the loss mask of `loss_and_grad`), with s this model's logits and z
+        the teacher's: KL_t = KL(softmax(z / tau) || softmax(s / tau)) and CE_t = -log_softmax(s)[label_t]; per row, KL_b
+        and CE_b their means over the counted positions; loss = mean_b [(1 - alpha) tau^2 KL_b + alpha CE_b], tau =
+        `temperature` (finite, > 0), alpha in [0, 1].  alpha = 1 is the `loss_and_grad` loss.  The teacher's forward runs
+        in the same step, on its inference set; it keeps no gradient or training state.  With `adapters` (lora_alpha as
+        in `loss_and_grad`) the student's base is frozen.  Inputs are checked before any device work (ProgenError).
+        Returns (python float loss, gradients (the adapters' with adapters), stats), stats a dict of float32 [B] arrays
+        kl and ce (each row's KL_b and CE_b)."""
+        from .distill import check_objective, check_teacher
+        check_teacher(self, teacher, 'distill_loss_and_grad')
+        tau, alpha = check_objective(temperature, alpha, 'distill_loss_and_grad')
+        self._ensure_loaded(params)
+        lo = None if adapters is None else self._attach_adapters(adapters, lora_alpha)
+        teacher._ensure_loaded(teacher_params)
+        eng = self.engine
+        eng.attach_teacher(teacher.engine)
+        n = eng.row_length(data, what='distill_loss_and_grad')
+        B = eng.load_distill(data, n)
+        eng.train_step(('distill', tau, alpha), B, length=n)
+        grads = eng.export_grads() if lo is None else lo.layout.unpack(lo.grads)
+        return float(eng.loss.item()), grads, eng.distill_stats(B)
+
     def score(self, params, data, *, batch_size=64, return_tokens=False, return_embeddings=False):
         """Log-likelihood of sequences under the model, without keeping any training state.
         data: (B, n+1) integer rows, the contract of `loss_and_grad` and `data.collate`: ids = data[:, :-1] are fed to the
@@ -569,13 +595,17 @@ class ProGen:
             self._gen_decoder, self._gen_params = dec, params
         return dec
 
-    def trainer(self, params, *, adapters=None, lora_alpha=None, head=None, task=None, **optim_kwargs):
+    def trainer(self, params, *, adapters=None, lora_alpha=None, head=None, task=None, teacher=None, teacher_params=None,
+                **optim_kwargs):
         """Device-resident training state over `params` (train.py's loop).  With `adapters` only the adapters train
         (the base stays bitwise unchanged); lora_alpha as in `loss_and_grad`.  With a property `head` (`init_head`) and
         its `task` ('regression' | 'classification') the adapters and the head train together through
-        `Trainer.property_step` (per-sequence labels) or `Trainer.residue_step` (per-residue labels)."""
+        `Trainer.property_step` (per-sequence labels) or `Trainer.residue_step` (per-residue labels).  With a `teacher`
+        (another ProGen, as in `distill_loss_and_grad`) and its `teacher_params`, `Trainer.distill_step` distils it into
+        this model."""
         from .trainer import Trainer
-        return Trainer(self, params, adapters=adapters, lora_alpha=lora_alpha, head=head, task=task, **optim_kwargs)
+        return Trainer(self, params, adapters=adapters, lora_alpha=lora_alpha, head=head, task=task, teacher=teacher,
+                       teacher_params=teacher_params, **optim_kwargs)
 
     # ---- property fine-tuning (DESIGN.md §3.9)
     def init_head(self, rng, num_outputs):

@@ -6,6 +6,8 @@ With low-rank adapters (`adapters=`) the same state exists for the adapter buffe
 and bitwise unchanged, and clip / AdamW / apply_every run over the adapters (weight decay on every A and B).  A property
 head (`head=`, `task=`) joins that buffer: `property_step` trains adapters and head together on per-sequence labels
 (DESIGN.md §3.9), `residue_step` on per-residue labels (§3.11)."""
+import weakref
+
 import torch
 
 from . import lib as L
@@ -17,8 +19,13 @@ class Trainer:
 
     def __init__(self, model, params, learning_rate=2e-4, weight_decay=1e-3, max_grad_norm=0.5, grad_accum_every=4,
                  b1=0.9, b2=0.999, eps=1e-8, optim_state=None, data_parallel=True, cuda_graph=False, adapters=None,
-                 lora_alpha=None, head=None, task=None):
+                 lora_alpha=None, head=None, task=None, teacher=None, teacher_params=None):
         self.model = model
+        if teacher is not None or teacher_params is not None:
+            from .distill import check_teacher
+            check_teacher(model, teacher, 'trainer')
+            if teacher_params is None:
+                raise L.ProgenError('trainer: a teacher needs teacher_params')
         self.task = None
         if head is not None or task is not None:
             from .property import check_head, check_task
@@ -32,6 +39,11 @@ class Trainer:
         self.eng = model.engine
         self.eng.load_params(params)
         model._loaded = None
+        # distillation (distill_step): the teacher's engine keeps its parameters and inference set only
+        self.teacher = teacher
+        if teacher is not None:
+            teacher._ensure_loaded(teacher_params)
+            self.eng.attach_teacher(teacher.engine)
         self.lora = None
         if adapters is not None:
             from .lora import Adapters, check_adapters, check_rank_alpha
@@ -62,6 +74,9 @@ class Trainer:
         # batch size and one alloc_epoch.  _graph / _graph_key / _graph_length: the most recently installed one.
         self._graphs, self._graph_epoch = {}, 0
         self._installed, self._graph_key, self._graph_length = None, None, None
+        # the teacher's inference set at the last capture (a weak reference): a distill step's graph reads it, and
+        # inference_acts re-allocates it without advancing alloc_epoch
+        self._graph_teacher = None
         # cuda_graph=True: the second eager step of one (key, row length) is captured and replayed from then on
         self._auto_graph, self._eager_runs = bool(cuda_graph), {}
         self.skip_allreduce = False                       # bench.py: "step without the exchange" for comm_exposed_ms
@@ -168,6 +183,8 @@ class Trainer:
             key = (batch_rows, gb) + objective
             self._graphs[(key, length)] = g
             self._installed, self._graph_key, self._graph_length, self._graph_epoch = g, key, length, eng.alloc_epoch
+            t = eng.teacher
+            self._graph_teacher = None if t is None or t.infer is None else weakref.ref(t.infer)
         return g
 
     # ---- preference (DPO) fine-tuning
@@ -241,6 +258,45 @@ class Trainer:
         self._res_rows = B
         return self._step(B, B, ('residue', self.task), lambda: self.eng.load_residue(r, self.task, y, n), sync_loss, n)
 
+    # ---- distillation (a teacher's per-position distribution as the target, DESIGN.md §3.13)
+    def distill_step(self, rows, temperature, alpha, sync_loss=False, global_batch=None, length=None):
+        """One micro-step of distillation from the trainer's teacher (model.trainer(..., teacher=, teacher_params=)): the
+        loss and gradient of `ProGen.distill_loss_and_grad`, then the same clip / AdamW / apply_every update as `step`.
+        rows: this rank's (b, n+1) integer rows; global_batch, sync_loss and `length` as in `step` (the teacher runs at
+        `distill.teacher_length(length)`).  Data parallel: every rank holds its own teacher; a rank without rows joins the
+        all-reduce.  With cuda_graph=True the step, the teacher's forward included, is captured after two eager steps of
+        one (rows, global_batch, temperature, alpha, length) and replayed from then on.  Returns the device scalar loss;
+        `distill_stats()` has the per-row statistics."""
+        from .distill import check_objective
+        if self.teacher is None:
+            raise L.ProgenError('distill_step: this trainer has no teacher (model.trainer(..., teacher=, teacher_params=))')
+        tau, alpha = check_objective(temperature, alpha, 'distill_step')
+        b = rows.shape[0]
+        gb = int(global_batch) if global_batch is not None else b * self.world
+        n = self._length(rows, length, 'distill_step')
+        self._distill_rows = b
+        return self._step(b, gb, ('distill', tau, alpha), lambda: self.eng.load_distill(rows, n), sync_loss, n)
+
+    def distill_stats(self):
+        """this rank's per-row statistics of its last `distill_step` as numpy float32 [b] arrays: kl (KL_b) and ce (CE_b)"""
+        return self.eng.distill_stats(getattr(self, '_distill_rows', 0))
+
+    def evaluate_distill(self, data, temperature, alpha, length=None):
+        """validation of distillation: the distillation loss of rows `data` (forward and head only); `distill_stats()`
+        then has their per-row KL and CE"""
+        from .distill import check_objective
+        if self.teacher is None:
+            raise L.ProgenError('evaluate_distill: this trainer has no teacher')
+        tau, alpha = check_objective(temperature, alpha, 'evaluate_distill')
+        eng = self.eng
+        n = self._length(data, length, 'evaluate_distill')
+        eng.lora = self.lora
+        B = eng.load_distill(data, n)
+        self._drop_graph_unless(B)
+        self._distill_rows = B
+        eng.train_step(('distill', tau, alpha), B, backward=False, length=n)
+        return eng.loss
+
     def residue_stats(self):
         """the last `residue_step`'s predictions [B, n, C] (regression values, or class logits) and per-position losses
         [B, n] (0 where unlabelled) as numpy float32"""
@@ -299,8 +355,14 @@ class Trainer:
     def _drop_graph_unless(self, batch_rows):
         """a different batch size re-allocates the engine's activation buffers: the captured pointers would dangle"""
         if self._graph is not None and (batch_rows != self._graph_key[0] or
-                                        self.eng.alloc_epoch != self._graph_epoch):
+                                        self.eng.alloc_epoch != self._graph_epoch or self._teacher_moved()):
             self._graph = None                             # (model.apply / sampling with another batch size re-allocates too)
+
+    def _teacher_moved(self):
+        """the teacher's inference set is not the one the captured steps were recorded on (a larger `score` call on the
+        teacher re-allocated it)"""
+        ref = self._graph_teacher
+        return ref is not None and ref() is not getattr(self.eng.teacher, 'infer', None)
 
     def _replay(self, sync_loss=False, graph=None):
         """replay `graph` (default: the most recently installed one)"""

@@ -14,6 +14,14 @@ are adapter packages that name the base checkpoint file instead of storing its p
 run keeps its mode and adapter settings: --lora_rank / --lora_alpha / --init_checkpoint that disagree with the
 checkpoint in --checkpoint_path are refused.
 
+Distillation: --teacher_checkpoint DIR trains the student (a config from --config_path / --model_name, or
+--init_checkpoint, optionally with --lora_rank) on (1 - alpha) tau^2 KL(teacher || student) + alpha CE at temperature tau
+(--distill_temperature, default 2.0) and mix alpha (--distill_alpha, default 0.5), DESIGN.md §3.13.  The teacher is the
+newest package in DIR (an adapter package is merged), runs with its own config in --mixed_precision mode, and keeps no
+training state.  Validation reports the student's CE and the KL.  Packages record distill = {teacher_checkpoint (the
+teacher's file), temperature, alpha}; a resumed run refuses flags that disagree with them.  The student's packages stay
+plain packages that sample.py, generate.py, score.py and variants.py load.
+
 The loop is the reference's (train.py:184-222): for each effective batch, grad_accum_every micro-steps of
 loss+grads -> optim.update -> apply_updates; checkpoint / validate / sample on the same cadence."""
 import os
@@ -28,6 +36,9 @@ import torch
 from progen_b200 import ProGen
 from progen_b200 import parallel as PAR
 from progen_b200.checkpoint import count_params, get_checkpoint_fns, last_checkpoint_file, load_checkpoint_file
+from progen_b200.checkpoint import package_params
+from progen_b200.distill import check_objective, check_teacher
+from progen_b200.lib import ProgenError
 from progen_b200.data import decode_tokens, iterator_from_sequences, iterator_from_tfrecords_folder, synthetic_iterator
 from progen_b200.data import group_by_length as length_grouped
 from progen_b200.engine import counted_length, cut_length
@@ -67,10 +78,16 @@ from progen_b200.utils import sample, confirm, exists
               help='sort the rows of each effective batch by length into its micro-batches (each runs at its cut length)')
 @click.option('--recompute', default=False, is_flag=True,
               help='recompute activations in the backward pass: one residual checkpoint per layer (less memory, more time)')
+@click.option('--teacher_checkpoint', default=None,
+              help='distil: train on the logits of the newest package in this directory (the teacher)')
+@click.option('--distill_temperature', default=None, type=float, help='distillation temperature tau (default 2.0)')
+@click.option('--distill_alpha', default=None, type=float,
+              help='weight of the label cross entropy in the distillation loss, in [0, 1] (default 0.5)')
 def main(seed, batch_size, grad_accum_every, learning_rate, weight_decay, data_parallel, max_grad_norm, validate_every,
          sample_every, checkpoint_every, checkpoint_path, checkpoint_keep_n, config_path, model_name, prime_length, seq_len,
          mixed_precision, data_path, wandb_off, wandb_project_name, new, synthetic, text_file, num_steps, cuda_graph,
-         init_checkpoint, lora_rank, lora_alpha, group_by_length, recompute):
+         init_checkpoint, lora_rank, lora_alpha, group_by_length, recompute, teacher_checkpoint, distill_temperature,
+         distill_alpha):
     if data_parallel and 'RANK' in os.environ:
         import torch.distributed as dist
         torch.cuda.set_device(int(os.environ.get('LOCAL_RANK', '0')))
@@ -118,6 +135,7 @@ def main(seed, batch_size, grad_accum_every, learning_rate, weight_decay, data_p
         base_file = last_checkpoint_file(init_checkpoint)
         assert base_file is not None, f'no checkpoint found in --init_checkpoint {init_checkpoint}'
         lora = lora_rank is not None
+    distill = resolve_distill(last_checkpoint, checkpoint_path, teacher_checkpoint, distill_temperature, distill_alpha)
     base = load_checkpoint_file(base_file) if base_file is not None else None
     if exists(last_checkpoint):
         model_kwargs = last_checkpoint['model_config']          # resume: config comes from the checkpoint (train.py:99-100)
@@ -129,6 +147,12 @@ def main(seed, batch_size, grad_accum_every, learning_rate, weight_decay, data_p
         model_kwargs = toml.loads(cfg_file.read_text())
 
     model = ProGen(**{**model_kwargs, 'mixed_precision': mixed_precision}, recompute=recompute)
+    teacher = teacher_params = None
+    if distill is not None:
+        teacher_pkg = load_checkpoint_file(distill['teacher_checkpoint'])
+        teacher = ProGen(**{**teacher_pkg['model_config'], 'mixed_precision': mixed_precision})
+        check_teacher(model, teacher, '--teacher_checkpoint')
+        teacher_params = package_params(teacher_pkg)
     adapters, lora_cfg = None, None
     if lora and exists(last_checkpoint):
         params = base['params']
@@ -146,11 +170,14 @@ def main(seed, batch_size, grad_accum_every, learning_rate, weight_decay, data_p
         params, optim_state, start_seq_index = model.init(seed), None, 0
     trainer = model.trainer(params, learning_rate=learning_rate, weight_decay=weight_decay, max_grad_norm=max_grad_norm,
                             grad_accum_every=grad_accum_every, optim_state=optim_state, data_parallel=data_parallel,
-                            cuda_graph=cuda_graph, adapters=adapters, lora_alpha=None if lora_cfg is None else lora_cfg['alpha'])
+                            cuda_graph=cuda_graph, adapters=adapters, lora_alpha=None if lora_cfg is None else lora_cfg['alpha'],
+                            teacher=teacher, teacher_params=teacher_params)
     seq_len = model_kwargs['seq_len']                           # the --seq_len flag is dead in the reference too (train.py:137)
     num_params = model.engine.num_params
     if rank == 0 and lora:
         print(f"adapters: rank {lora_cfg['rank']}, alpha {lora_cfg['alpha']}, {trainer.lora.num_params} parameters on base {base_file}")
+    if rank == 0 and distill is not None:
+        print(f"distilling {distill['teacher_checkpoint']} at temperature {distill['temperature']}, alpha {distill['alpha']}")
 
     if synthetic:
         total_train_seqs = 10 ** 9
@@ -193,7 +220,11 @@ def main(seed, batch_size, grad_accum_every, learning_rate, weight_decay, data_p
             local = PAR.shard_batch(data) if world > 1 else data
             # every rank holds the global micro-batch: the ranks agree on its cut length without communicating
             length = cut_length(data[:, 1:]) if world > 1 else None
-            loss = trainer.step(local, sync_loss=True, global_batch=data.shape[0], length=length)
+            if distill is None:
+                loss = trainer.step(local, sync_loss=True, global_batch=data.shape[0], length=length)
+            else:
+                loss = trainer.distill_step(local, distill['temperature'], distill['alpha'], sync_loss=True,
+                                            global_batch=data.shape[0], length=length)
             tokens += data.shape[0] * seq_len
             counted += int(counted_length(data[:, 1:]).sum())
         if len(group) < grad_accum_every:
@@ -207,13 +238,22 @@ def main(seed, batch_size, grad_accum_every, learning_rate, weight_decay, data_p
                 package.update(adapters=trainer.adapters(), lora=lora_cfg, base_checkpoint=base_file, num_params=num_params)
             else:
                 package['params'] = trainer.params()
+            if distill is not None:
+                package['distill'] = dict(distill)
             save_checkpoint(package, checkpoint_keep_n)
             print(f"checkpoint to start at sequence index of {package['next_seq_index']}")
         if i % validate_every == 0:
             valid_data = next(valid_dataset)
-            vloss = trainer.evaluate(valid_data)
-            if rank == 0:
-                print(f'valid_loss: {vloss.item()}')
+            if distill is None:
+                vloss = trainer.evaluate(valid_data)
+                if rank == 0:
+                    print(f'valid_loss: {vloss.item()}')
+            else:
+                trainer.evaluate_distill(valid_data, distill['temperature'], distill['alpha'])
+                st = trainer.distill_stats()
+                if rank == 0:
+                    print(f"valid_loss: {float(st['ce'].mean())}")      # the student's CE, comparable with an LM run
+                    print(f"valid_kl: {float(st['kl'].mean())}")
         if i % sample_every == 0 and rank == 0:
             valid_data = next(valid_dataset)[0]
             prime = valid_data[:prime_length]
@@ -233,6 +273,40 @@ def main(seed, batch_size, grad_accum_every, learning_rate, weight_decay, data_p
         torch.cuda.synchronize()
         dist.barrier()
         dist.destroy_process_group()
+
+
+def resolve_distill(last_checkpoint, checkpoint_path, teacher_checkpoint, temperature, alpha):
+    """the run's distillation settings {teacher_checkpoint (file), temperature, alpha}, or None for an LM run: from the
+    flags on a new run, from the package on a resumed one (flags that disagree with it are refused)"""
+    got = last_checkpoint.get('distill') if exists(last_checkpoint) else None
+    if exists(last_checkpoint) and got is None:
+        if teacher_checkpoint is not None or temperature is not None or alpha is not None:
+            raise click.UsageError(f'--teacher_checkpoint / --distill_temperature / --distill_alpha: {checkpoint_path} '
+                                   f'holds a checkpoint of a run without a teacher; distil into another --checkpoint_path')
+        return None
+    if got is not None:
+        if teacher_checkpoint is not None and last_checkpoint_file(teacher_checkpoint) != got['teacher_checkpoint']:
+            raise click.UsageError(f"--teacher_checkpoint {teacher_checkpoint}: its newest package is not "
+                                   f"{got['teacher_checkpoint']}, the teacher of the run in {checkpoint_path}")
+        if temperature is not None and float(temperature) != float(got['temperature']):
+            raise click.UsageError(f"--distill_temperature {temperature}: the run in {checkpoint_path} distils at "
+                                   f"temperature {got['temperature']}")
+        if alpha is not None and float(alpha) != float(got['alpha']):
+            raise click.UsageError(f"--distill_alpha {alpha}: the run in {checkpoint_path} distils with alpha {got['alpha']}")
+        return dict(got)
+    if teacher_checkpoint is None:
+        if temperature is not None or alpha is not None:
+            raise click.UsageError('--distill_temperature / --distill_alpha need --teacher_checkpoint')
+        return None
+    teacher_file = last_checkpoint_file(teacher_checkpoint)
+    if teacher_file is None:
+        raise click.UsageError(f'--teacher_checkpoint {teacher_checkpoint}: no checkpoint found there')
+    try:
+        tau, a = check_objective(2.0 if temperature is None else temperature, 0.5 if alpha is None else alpha,
+                                 '--distill_temperature / --distill_alpha')
+    except ProgenError as e:
+        raise click.UsageError(str(e)) from None
+    return dict(teacher_checkpoint=teacher_file, temperature=tau, alpha=a)
 
 
 if __name__ == '__main__':
