@@ -140,6 +140,21 @@ int progen_preference_head(const void* logits, int dtype, const int* labels, con
 int progen_distill_head(const void* logits, int dtype, const float* teacher, long long teacher_row_stride, const int* labels,
                         float* weights, float* scratch, float* stats, float* loss, void* dlogits, int dlogits_dtype, int B,
                         int n, int V, float tau, float alpha, float inv_batch, void* stream);
+/* policy-gradient head (DESIGN.md §3.14): policy logits s [B*n, V] in dtype, reference logits z fp32 with row b, position
+ * t at ref + (b * ref_row_stride + t) * V (ref_row_stride >= n), labels [B*n], span [B, 2] int32 (lo_b, hi_b) clamped to
+ * [0, n] on the device, advantage [B] fp32.  Per position t of S_b = {lo_b <= t < hi_b}, N_b = |S_b|: pi = softmax(s_t),
+ * rho = softmax(z_t), logp_t = log pi[label_t] (label clamped to [0, V)), KL_t = sum_v pi_v (log pi_v - log rho_v) (terms
+ * whose pi_v underflows to 0 add 0).  L_b = (1 / N_b) sum_{S_b} (-A_b logp_t + beta KL_t); *loss = inv_rows sum_b L_b in
+ * double, rows in order (written, not accumulated); stats [B, 3] = (sum_{S_b} logp_t / N_b, sum_{S_b} KL_t / N_b, N_b);
+ * dlogits [B*n, V] in dlogits_dtype = inv_rows / N_b [A_b (pi - onehot(label_t)) + beta pi (log pi - log rho - KL_t)]
+ * on S_b and +0.0 elsewhere, every row written.  z may be null iff beta == 0; with beta == 0 it is never read, and
+ * outside the spans it is never read either.  scratch [2*B*n] is an fp32 workspace.  No float atomics reach stats, loss
+ * or dlogits: they are the same bits in every launch, and row b's do not depend on the other rows.  Refused: null
+ * pointers, V % 4 != 0, ref_row_stride < n, beta not finite or < 0, beta > 0 with a null z, inv_rows not finite and > 0,
+ * dtypes outside the progen_ce_fwd_bwd combinations. */
+int progen_policy_head(const void* logits, int dtype, const float* ref, long long ref_row_stride, const int* labels,
+                       const int* span, const float* advantage, float* scratch, float* stats, float* loss, void* dlogits,
+                       int dlogits_dtype, int B, int n, int V, float beta, float inv_rows, void* stream);
 /* out[b, :] = sum_t mask_t x[b, t, :] / sum_t mask_t (fp32, fixed order) over rows of x [B*n, d] (stride ldx), with the
  * same mask as above: for a sequence of L residues, input positions 0..L (BOS and every residue). */
 int progen_masked_mean_pool(const void* x, long long ldx, int dtype, const int* labels, float* out, int B, int n, int d,
@@ -363,6 +378,16 @@ typedef struct progen_decode_run_t {
 
 int progen_decode_run(const progen_decode_run_t* run, void* stream);
 
+/* decoder weight refresh (DESIGN.md §3.14): one leaf of a BatchDecoder written in place from device fp32 state.  w is
+ * the engine's leaf [in, out] (a vector leaf: in = 1), a [in, rank] and b [rank, out] its adapter (rank 0: none; a and b
+ * may then be null).  With c(o) = o, or with interleave = 1 the engine's GLU column order (value_j at 2j, gate_j at
+ * 2j + 1, j < out / 2) mapped to haiku's (value | gate): dst [out, in] in dst_dtype (fp32, or bf16 round-to-nearest) =
+ * cast(w[i, c(o)] + scale * sum_r a[i, r] b[r, c(o)]), r in increasing order with every product and sum rounded on its
+ * own (no FMA): a float32 host replay gives the same bits.  in = 1 is a plain (de-interleaving) copy dst[o] = w[c(o)].
+ * Refused: null w or dst, in or out < 1, rank outside [0, 64], rank > 0 with a null a or b, in = 1 or a non-finite
+ * scale, interleave with an odd out, dst_dtype not fp32 or bf16. */
+int progen_decode_load_weight(const float* w, const float* a, const float* b, int rank, float scale, int in, int out,
+                              int interleave, void* dst, int dst_dtype, void* stream);
 /* Prefill of the decoder's caches from an inference forward (generation with `prefill='forward'`): a strided row gather
  * with conversion to fp32,
  *   dst[b * dst_b_stride + g * dst_g_stride + r * dst_row_stride + c]

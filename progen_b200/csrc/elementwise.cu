@@ -617,6 +617,118 @@ __global__ void distill_loss_kernel(const float* __restrict__ stats, int B, doub
   *loss = (float)(s * inv_batch);
 }
 
+// ------------------------------------------------------------------------------------------ policy-gradient head
+// The span of row b clamped to [0, n]: positions lo <= p < hi count, N_b = hi - lo (0 when the span is empty).
+__device__ __forceinline__ void policy_span(const int* __restrict__ span, long long b, int n, int& lo, int& hi) {
+  lo = min(max(span[2 * b], 0), n);
+  hi = min(max(span[2 * b + 1], lo), n);
+}
+
+// One warp per position t (row b = t / n, position p = t - b n).  Outside the span the gradient row is +0.0 and
+// logp[t] = kl[t] = 0; the reference row is read only inside it, and only when REF (beta > 0).  Inside, with
+// lpi = log_softmax(s_t), lrho = log_softmax(z_t), pi = softmax(s_t) computed as ce_fwd_bwd_kernel does (so beta = 0,
+// A = 1 gives its gradient bits) and KL_t = sum_v pi_v (lpi_v - lrho_v) (0 where pi_v = 0):
+//   dlogits_t = inv_rows / N_b [A_b (pi - onehot(label_t)) + beta pi (lpi - lrho - KL_t)].
+// The reference's log-softmax runs through the same code as the policy's, so z = s gives lrho = lpi bitwise.
+template <typename TL, typename TD, bool REF>
+__global__ void policy_pos_kernel(const TL* __restrict__ logits, const float* __restrict__ ref, long long stride,
+                                  const int* __restrict__ labels, const int* __restrict__ span,
+                                  const float* __restrict__ adv, float* __restrict__ logp, float* __restrict__ kl,
+                                  TD* __restrict__ dlogits, long long T, int n, int V, float beta, float inv_rows) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (long long t = blockIdx.x * (long long)ROWS_PER_BLOCK + warp; t < T; t += (long long)gridDim.x * ROWS_PER_BLOCK) {
+    TD* dr = dlogits + t * V;
+    const long long b = t / n;
+    const int p = (int)(t - b * n);
+    int lo, hi;
+    policy_span(span, b, n, lo, hi);
+    if (p < lo || p >= hi) {
+      const float zero[4] = {0.f, 0.f, 0.f, 0.f};
+      for (int c = lane * 4; c < V; c += 128) store4(dr + c, zero);
+      if (lane == 0) { logp[t] = 0.f; kl[t] = 0.f; }
+      continue;
+    }
+    const float w = inv_rows / (float)(hi - lo), A = adv[b];
+    const TL* lr = logits + t * V;
+    float ms, ses;
+    warp_row_max_sumexp<TL>(lr, V, lane, ms, ses);
+    const float lses = logf(ses), inv = 1.f / ses;
+    const int lab = clamp_label(labels[t], V);
+    const float* zr = REF ? ref + (b * stride + p) * V : nullptr;
+    float mz = 0.f, lsez = 0.f, k = 0.f;
+    if (REF) {
+      float sez;
+      warp_row_max_sumexp<float>(zr, V, lane, mz, sez);
+      lsez = logf(sez);
+      for (int c = lane * 4; c < V; c += 128) {
+        float s[4], z[4];
+        load4<TL>(lr + c, s);
+        load4<float>(zr + c, z);
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const float pi = expf(s[i] - ms) * inv;
+          if (pi > 0.f) k += pi * (((s[i] - ms) - lses) - ((z[i] - mz) - lsez));
+        }
+      }
+      k = warp_sum(k);
+    }
+    for (int c = lane * 4; c < V; c += 128) {
+      float s[4], z[4] = {0.f, 0.f, 0.f, 0.f}, o[4];
+      load4<TL>(lr + c, s);
+      if (REF) load4<float>(zr + c, z);
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const float pi = expf(s[i] - ms) * inv;
+        float g = A * (pi - ((c + i) == lab ? 1.f : 0.f));
+        if (REF) g += beta * (pi * ((((s[i] - ms) - lses) - ((z[i] - mz) - lsez)) - k));
+        o[i] = w * g;
+      }
+      store4(dr + c, o);
+    }
+    if (lane == 0) {
+      logp[t] = (to_f32(lr[lab]) - ms) - lses;
+      kl[t] = k;
+    }
+  }
+}
+
+constexpr int POLICY_THREADS = 256;
+
+// One block per row b: stats[b] = (sum logp / N_b, sum KL / N_b, N_b) over the row's span, thread i summing positions
+// lo + i + k * POLICY_THREADS ascending in double, then the thread partials in thread order.  The order depends on the
+// span alone, so a cut view and the full view, or the row alone and in a batch, give the same bits.
+__global__ void policy_row_kernel(const int* __restrict__ span, const float* __restrict__ logp,
+                                  const float* __restrict__ kl, float* __restrict__ stats, int n) {
+  const int b = blockIdx.x;
+  int lo, hi;
+  policy_span(span, b, n, lo, hi);
+  double a = 0.0, c = 0.0;
+  for (int i = lo + threadIdx.x; i < hi; i += POLICY_THREADS) {
+    a += (double)logp[(long long)b * n + i];
+    c += (double)kl[(long long)b * n + i];
+  }
+  __shared__ double ra[POLICY_THREADS], rc[POLICY_THREADS];
+  ra[threadIdx.x] = a;
+  rc[threadIdx.x] = c;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double sa = 0.0, sc = 0.0;
+    for (int k = 0; k < POLICY_THREADS; ++k) { sa += ra[k]; sc += rc[k]; }
+    const int N = hi - lo;
+    stats[3LL * b] = N ? (float)(sa / (double)N) : 0.f;
+    stats[3LL * b + 1] = N ? (float)(sc / (double)N) : 0.f;
+    stats[3LL * b + 2] = (float)N;
+  }
+}
+
+// *loss = inv_rows * sum_b (-A_b logp_b + beta KL_b), one thread, rows in order, in double
+__global__ void policy_loss_kernel(const float* __restrict__ stats, const float* __restrict__ adv, int B, double beta,
+                                   double inv_rows, float* __restrict__ loss) {
+  double s = 0.0;
+  for (int b = 0; b < B; ++b) s += -(double)adv[b] * (double)stats[3LL * b] + beta * (double)stats[3LL * b + 1];
+  *loss = (float)(s * inv_rows);
+}
+
 // out[b, :] = sum_t mask_t x[b, t, :] / sum_t mask_t.  Grid (ceil(d / 128), B), 256 threads: lane owns 4 columns, warp w sums
 // rows t = w, w + 8, ... in order, then the 8 warp partials are added in order: fixed order, fp32 accumulation.
 template <typename TX>
@@ -1094,6 +1206,63 @@ __global__ void tril_cast_kernel(const float* __restrict__ w, TO* __restrict__ o
   }
 }
 
+// ------------------------------------------------------------------------------------------ decoder weight refresh
+// The engine keeps a GLU feed-forward input's columns interleaved (v0, g0, v1, g1, ...); the decoder keeps haiku's
+// (value | gate).  Column o of the decoder's leaf is column glu_col(o) of the engine's.
+__device__ __forceinline__ long long glu_col(long long o, long long out, int interleave) {
+  if (!interleave) return o;
+  const long long H = out >> 1;
+  return o < H ? 2 * o : 2 * (o - H) + 1;
+}
+
+constexpr int LW_TILE = 32, LW_MAX_RANK = 64;
+
+// dst[o, i] = cast(W[i, c(o)] + s * sum_r A[i, r] B[r, c(o)]) over one 32 x 32 tile of (i, o) per 256-thread block: W, A
+// and B tiles staged in shared memory, the transposed tile written along i.  r runs in increasing order and every
+// product and sum is rounded on its own (no FMA), so a float32 host replay gives the same bits; rank 0 is a copy.
+template <typename TD>
+__global__ void load_weight_kernel(const float* __restrict__ W, const float* __restrict__ A, const float* __restrict__ Bm,
+                                   int rank, float scale, int in, int out, int interleave, TD* __restrict__ dst) {
+  __shared__ float ws[LW_TILE][LW_TILE + 1];
+  __shared__ float as[LW_TILE][LW_MAX_RANK + 1];
+  __shared__ float bs[LW_MAX_RANK][LW_TILE];
+  const int tx = threadIdx.x, ty = threadIdx.y, tid = ty * LW_TILE + tx;
+  const int i0 = blockIdx.x * LW_TILE, o0 = blockIdx.y * LW_TILE;
+  for (int ii = ty; ii < LW_TILE; ii += 8) {
+    const int i = i0 + ii, o = o0 + tx;
+    ws[ii][tx] = (i < in && o < out) ? W[(long long)i * out + glu_col(o, out, interleave)] : 0.f;
+  }
+  for (int k = tid; k < LW_TILE * rank; k += 256) {
+    const int ii = k / rank, r = k - ii * rank, i = i0 + ii;
+    as[ii][r] = i < in ? A[(long long)i * rank + r] : 0.f;
+  }
+  for (int k = tid; k < rank * LW_TILE; k += 256) {
+    const int r = k / LW_TILE, oo = k - r * LW_TILE, o = o0 + oo;
+    bs[r][oo] = o < out ? Bm[(long long)r * out + glu_col(o, out, interleave)] : 0.f;
+  }
+  __syncthreads();
+  const int i = i0 + tx;
+  if (i >= in) return;
+  for (int oo = ty; oo < LW_TILE; oo += 8) {
+    const int o = o0 + oo;
+    if (o >= out) break;
+    float v = ws[tx][oo];
+    if (rank) {
+      float acc = 0.f;
+      for (int r = 0; r < rank; ++r) acc = __fadd_rn(acc, __fmul_rn(as[tx][r], bs[r][oo]));
+      v = __fadd_rn(v, __fmul_rn(scale, acc));
+    }
+    dst[(long long)o * in + i] = from_f32<TD>(v);
+  }
+}
+
+// a vector leaf (in = 1): dst[o] = cast(W[c(o)])
+template <typename TD>
+__global__ void load_vector_kernel(const float* __restrict__ W, long long out, int interleave, TD* __restrict__ dst) {
+  for (long long o = blockIdx.x * (long long)blockDim.x + threadIdx.x; o < out; o += (long long)gridDim.x * blockDim.x)
+    dst[o] = from_f32<TD>(W[glu_col(o, out, interleave)]);
+}
+
 // decoder-cache prefill: dst[b, g, r, c] = fp32(src[(row_map[b] * src_seq_rows + row0 + r) * ld + col0 + g * cols + c]).
 // One thread moves 16 source bytes (4 fp32 or 8 bf16) to 16 or 32 destination bytes; consecutive threads take consecutive
 // column vectors of a row, so both sides coalesce.  The source (one forward row per distinct prompt) is read once per
@@ -1316,6 +1485,37 @@ int progen_distill_head(const void* logits, int dtype, const float* teacher, lon
   return PROGEN_OK;
 }
 
+int progen_policy_head(const void* logits, int dtype, const float* ref, long long ref_row_stride, const int* labels,
+                       const int* span, const float* advantage, float* scratch, float* stats, float* loss, void* dlogits,
+                       int dlogits_dtype, int B, int n, int V, float beta, float inv_rows, void* stream) {
+  PG_CHECK_ARG(logits && labels && span && advantage && scratch && stats && loss && dlogits);
+  PG_CHECK_ARG(B > 0 && n > 0 && V > 0 && V % 4 == 0 && ref_row_stride >= n);
+  PG_CHECK_ARG(std::isfinite(beta) && beta >= 0.f && (beta == 0.f || ref));
+  PG_CHECK_ARG(std::isfinite(inv_rows) && inv_rows > 0.f);
+  const bool f32_f32 = dtype == PG_F32 && dlogits_dtype == PG_F32, f32_bf16 = dtype == PG_F32 && dlogits_dtype == PG_BF16,
+             bf16_bf16 = dtype == PG_BF16 && dlogits_dtype == PG_BF16;
+  if (!(f32_f32 || f32_bf16 || bf16_bf16)) {
+    progen_set_error("policy_head: unsupported dtypes %d / %d", dtype, dlogits_dtype);
+    return PROGEN_ERR_UNSUPPORTED;
+  }
+  cudaStream_t s = (cudaStream_t)stream;
+  const long long T = (long long)B * n;
+  const int grid = row_grid(T);
+#define POLICY_CASE(TL, TD, R) policy_pos_kernel<TL, TD, R><<<grid, 256, 0, s>>>((const TL*)logits, ref, ref_row_stride, \
+      labels, span, advantage, scratch, scratch + T, (TD*)dlogits, T, n, V, beta, inv_rows)
+  const bool r = beta > 0.f;
+  if (f32_f32) { if (r) POLICY_CASE(float, float, true); else POLICY_CASE(float, float, false); }
+  else if (f32_bf16) { if (r) POLICY_CASE(float, bf16, true); else POLICY_CASE(float, bf16, false); }
+  else { if (r) POLICY_CASE(bf16, bf16, true); else POLICY_CASE(bf16, bf16, false); }
+#undef POLICY_CASE
+  PG_LAUNCH_CHECK();
+  policy_row_kernel<<<B, POLICY_THREADS, 0, s>>>(span, scratch, scratch + T, stats, n);
+  PG_LAUNCH_CHECK();
+  policy_loss_kernel<<<1, 1, 0, s>>>(stats, advantage, B, (double)beta, (double)inv_rows, loss);
+  PG_LAUNCH_CHECK();
+  return PROGEN_OK;
+}
+
 int progen_masked_mean_pool(const void* x, long long ldx, int dtype, const int* labels, float* out, int B, int n, int d,
                             void* stream) {
   PG_CHECK_ARG(B > 0 && n > 0 && d > 0 && d % 4 == 0 && ldx >= d && ldx % 4 == 0 && x && labels && out);
@@ -1500,6 +1700,30 @@ int progen_tril_cast(const float* w, void* out, int out_dtype, int n, void* stre
   const int grid = ew_grid((long long)n * (n / 4), 256);
   if (out_dtype == PG_F32) tril_cast_kernel<float><<<grid, 256, 0, s>>>(w, (float*)out, n);
   else tril_cast_kernel<bf16><<<grid, 256, 0, s>>>(w, (bf16*)out, n);
+  PG_LAUNCH_CHECK();
+  return PROGEN_OK;
+}
+
+int progen_decode_load_weight(const float* w, const float* a, const float* b, int rank, float scale, int in, int out,
+                              int interleave, void* dst, int dst_dtype, void* stream) {
+  PG_CHECK_ARG(w && dst && in > 0 && out > 0 && rank >= 0 && rank <= LW_MAX_RANK && (interleave == 0 || interleave == 1));
+  PG_CHECK_ARG(rank == 0 || (a && b && in > 1 && std::isfinite(scale)));
+  PG_CHECK_ARG(!interleave || out % 2 == 0);
+  if (dst_dtype != PG_F32 && dst_dtype != PG_BF16) {
+    progen_set_error("decode_load_weight: unsupported dtype %d", dst_dtype);
+    return PROGEN_ERR_UNSUPPORTED;
+  }
+  cudaStream_t s = (cudaStream_t)stream;
+  if (in == 1) {
+    const int grid = ew_grid(out, 256);
+    if (dst_dtype == PG_F32) load_vector_kernel<float><<<grid, 256, 0, s>>>(w, out, interleave, (float*)dst);
+    else load_vector_kernel<bf16><<<grid, 256, 0, s>>>(w, out, interleave, (bf16*)dst);
+  } else {
+    const dim3 grid((in + LW_TILE - 1) / LW_TILE, (out + LW_TILE - 1) / LW_TILE), block(LW_TILE, 8);
+    if (dst_dtype == PG_F32)
+      load_weight_kernel<float><<<grid, block, 0, s>>>(w, a, b, rank, scale, in, out, interleave, (float*)dst);
+    else load_weight_kernel<bf16><<<grid, block, 0, s>>>(w, a, b, rank, scale, in, out, interleave, (bf16*)dst);
+  }
   PG_LAUNCH_CHECK();
   return PROGEN_OK;
 }

@@ -148,6 +148,13 @@ class BatchDecoder:
         f32 = lambda a: self._hold(torch.tensor(np.ascontiguousarray(np.asarray(a, np.float32)), device=self.dev))
         wt = lambda a: self._hold(torch.tensor(np.ascontiguousarray(np.asarray(a, np.float32).T), device=self.dev).to(weights_dtype).contiguous())
         zeros = lambda *s, dtype=torch.float32: self._hold(torch.zeros(*s, device=self.dev, dtype=dtype))
+        # (module, name) -> (the decoder's buffer of that parameter, whether it holds the transpose): load_weights
+        self.leaves = {}
+
+        def leaf(module, name, transposed, a=None):
+            ptr = (wt if transposed else f32)(params[module][name] if a is None else a)
+            self.leaves[(module, name)] = (self.keep[-1], transposed)
+            return ptr
         kinds = layer_kinds(cfg['depth'], cfg['global_mlp_depth'], cfg['ff_glu'])
         layers = (DecodeLayer * len(kinds))()
         self.state = []
@@ -157,22 +164,22 @@ class BatchDecoder:
             Lr = layers[i]
             self.caches.append({})
             Lr.kind = {'glu': 0, 'gelu': 1, 'sgu': 2}[kind]
-            Lr.ln1_scale = f32(params[a + 'layer_norm']['scale'])
-            Lr.wqkv_t = wt(params[a + 'linear']['w'])
-            Lr.wo_t = wt(params[a + 'linear_1']['w'])
-            Lr.bo = f32(params[a + 'linear_1']['b'])
-            Lr.ln2_scale = f32(params[f + 'layer_norm']['scale'])
-            Lr.win_t = wt(params[f + 'linear']['w'])
-            Lr.bin = f32(params[f + 'linear']['b'])
-            Lr.wout_t = wt(params[f + 'linear_1']['w'])
-            Lr.bout = f32(params[f + 'linear_1']['b'])
+            Lr.ln1_scale = leaf(a + 'layer_norm', 'scale', False)
+            Lr.wqkv_t = leaf(a + 'linear', 'w', True)
+            Lr.wo_t = leaf(a + 'linear_1', 'w', True)
+            Lr.bo = leaf(a + 'linear_1', 'b', False)
+            Lr.ln2_scale = leaf(f + 'layer_norm', 'scale', False)
+            Lr.win_t = leaf(f + 'linear', 'w', True)
+            Lr.bin = leaf(f + 'linear', 'b', False)
+            Lr.wout_t = leaf(f + 'linear_1', 'w', True)
+            Lr.bout = leaf(f + 'linear_1', 'b', False)
             if kind == 'sgu':
                 g = f + 'sgu'
-                Lr.sgu_ln_scale = f32(params[g + '/~/layer_norm']['scale'])
-                Lr.sgu_w = f32(params[g]['spatial_weights'])
-                Lr.sgu_b = f32(np.asarray(params[g]['spatial_biases']).reshape(-1))
-                Lr.sgu_proj_t = wt(params[g + '/~/linear']['w'])
-                Lr.sgu_proj_b = f32(params[g + '/~/linear']['b'])
+                Lr.sgu_ln_scale = leaf(g + '/~/layer_norm', 'scale', False)
+                Lr.sgu_w = leaf(g, 'spatial_weights', False)
+                Lr.sgu_b = leaf(g, 'spatial_biases', False, np.asarray(params[g]['spatial_biases']).reshape(-1))
+                Lr.sgu_proj_t = leaf(g + '/~/linear', 'w', True)
+                Lr.sgu_proj_b = leaf(g + '/~/linear', 'b', False)
                 Lr.gn_hist = self._state(zeros(B, n, hid // 2), 'gn_hist')
             Lr.kcache = self._state(zeros(B, n, I), 'kcache')           # [B, heads, n, dim_head]
             Lr.vcache = self._state(zeros(B, n, I), 'vcache')
@@ -187,10 +194,10 @@ class BatchDecoder:
         m.wdtype = L.BF16 if weights_dtype == torch.bfloat16 else L.F32
         m.shift_tokens = int(cfg['shift_tokens'])
         m.B = B
-        m.embed = f32(params[P + 'embed']['embeddings'])
-        m.lnf_scale = f32(params[P + 'layer_norm']['scale'])
-        m.whead_t = wt(params[P + 'linear']['w'])
-        m.bhead = f32(params[P + 'linear']['b'])
+        m.embed = leaf(P + 'embed', 'embeddings', False)
+        m.lnf_scale = leaf(P + 'layer_norm', 'scale', False)
+        m.whead_t = leaf(P + 'linear', 'w', True)
+        m.bhead = leaf(P + 'linear', 'b', False)
         inv_freq = 1.0 / (10000 ** (np.arange(0, cfg['dim_head'], 2, dtype=np.float64) / cfg['dim_head']))
         ang = np.arange(n, dtype=np.float64)[:, None] * inv_freq[None, :]
         m.rot_sin, m.rot_cos = f32(np.sin(ang)), f32(np.cos(ang))
@@ -211,6 +218,31 @@ class BatchDecoder:
         self.grid_bar = torch.zeros(1, device=self.dev, dtype=torch.int32)
         m.grid_bar = self.grid_bar.data_ptr()
         m.repetition_penalty = 1.0                        # constraints off
+
+    def load_weights(self, engine, lora=None):
+        """Rewrite the decoder's weights in place from an Engine of the same config (progen_decode_load_weight): every
+        parameter from its fp32 master copy, or with `lora` (lora.Adapters on that engine, whose base is frozen) only
+        the adapted projections, as W + s A B.  Allocates nothing: the caches and the device layer table keep their
+        pointers.  The weights then equal those of a decoder built from `engine.export_params()` (with lora: from the
+        float32, no-FMA W + s A B of the float32 leaves)."""
+        from .lora import adapter_modules
+        lib, st = self.lib, L.stream()
+        lay = engine.layout
+        adapted = None if lora is None else {m for m, _, _, _ in adapter_modules(self.cfg)}
+        for (module, name), (t, transposed) in self.leaves.items():
+            if adapted is not None and not (name == 'w' and module in adapted):
+                continue
+            spec = lay.by_key[(module, name)]
+            fan_in, fan_out = spec.shape if transposed else (1, spec.size)
+            a = b = 0
+            rank, scale = 0, 1.0
+            if adapted is not None:
+                la = lora.layout
+                a, b = la.seg(lora.params, module, 'lora_a').data_ptr(), la.seg(lora.params, module, 'lora_b').data_ptr()
+                rank, scale = lora.r, lora.scale
+            L.check(lib.progen_decode_load_weight(lay.seg(engine.params, module, name).data_ptr(), a, b, rank, scale,
+                                                  fan_in, fan_out, int(spec.interleave), t.data_ptr(), L.dt(t), st),
+                    f'decode_load_weight {module}/{name}')
 
     def _hold(self, t):
         self.keep.append(t)

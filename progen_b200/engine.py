@@ -342,6 +342,7 @@ class Engine:
         self.lora = None                  # lora.Adapters: the training set runs the adapted model with a frozen base
         self.teacher = None               # distillation (attach_teacher): a second Engine whose logits are the target
         self.dist = None                  # ... and the distillation head's buffers (ensure_distill)
+        self.pol = None                   # policy-gradient head buffers (load_policy); its reference is self.teacher
         self.lib = L.load()
         self.num_sms = torch.cuda.get_device_properties(self.dev).multi_processor_count
 
@@ -407,6 +408,7 @@ class Engine:
         # residue head (train_step): its B * n position buffers are sized for the head's outputs (ensure_residue)
         self.res_C, self.res = 0, None
         self.dist = None                                            # distillation head buffers (ensure_distill)
+        self.pol = None                                             # policy-gradient head buffers (load_policy)
         grad = dict(dres=self.dres, dres_lp=self.dres_lp, dy=self.dy, dqkv=self.dqkv, datt=self.datt, delta=self.delta,
                     du=self.du, dh_=self.dh_, dlogits=self.dlogits, ce_w=self.ce_w, logp=self.logp)
         if 'sgu' in self.kinds:
@@ -773,6 +775,10 @@ class Engine:
                                 the rows load_distill staged in its inference set, at teacher_length(length), then the
                                 student's forward, progen_distill_head ((1 - alpha) tau^2 KL + alpha CE per row, mean over
                                 rows; per-row (KL, CE) in self.dist['stats']) and the LM backward from dlogits.
+          ('policy', beta)      the policy-gradient loss (DESIGN.md §3.14) on the spans and advantages load_policy staged:
+                                with beta > 0 the attached reference's (self.teacher) forward first, as for 'distill',
+                                then the policy's forward, progen_policy_head (per row the span mean of -A logp + beta KL,
+                                per-row (logp, KL, N) in self.pol['stats']) and the LM backward from dlogits.
         The loss is scaled by 1/global_rows (the preference loss: 1/global pairs), so that a SUM all-reduce of the
         per-rank gradients is the global mean.  With adapters (self.lora) no base gradient is computed.
         `backward=False`: the forward and the loss only (a validation loss), no gradient.
@@ -794,7 +800,9 @@ class Engine:
             # the backward pass ends by scaling the whole B gradient by s (Adapters.scale_b_grads): an accumulated one
             # would be scaled twice
             raise L.ProgenError('adapters: gradients cannot accumulate across steps (zero_grads=False)')
-        if kind == 'distill':
+        if kind == 'policy' and self.pol is None:
+            raise L.ProgenError('policy step: no spans and advantages are loaded (load_policy)')
+        if kind == 'distill' or (kind == 'policy' and objective[1] > 0):
             ta = self._teacher_view(a.B, a.n)
             self.teacher._forward_device(ta)
         self._forward_device(a, logits=kind not in ('property', 'residue'))
@@ -830,6 +838,13 @@ class Engine:
                                             g['ce_w'].data_ptr(), dist['scratch'].data_ptr(), dist['stats'].data_ptr(),
                                             self.loss.data_ptr(), g['dlogits'].data_ptr(), self.act_dt, a.B, a.n, self.V,
                                             objective[1], objective[2], 1.0 / global_rows, st), 'distill_head')
+        elif kind == 'policy':
+            pol, beta = self.pol, objective[1]
+            L.check(lib.progen_policy_head(a.logits.data_ptr(), L.F32, ta.logits.data_ptr() if beta > 0 else 0,
+                                           ta.n if beta > 0 else a.n, a.labels.data_ptr(), pol['span'].data_ptr(),
+                                           pol['adv'].data_ptr(), pol['scratch'].data_ptr(), pol['stats'].data_ptr(),
+                                           self.loss.data_ptr(), g['dlogits'].data_ptr(), self.act_dt, a.B, a.n, self.V,
+                                           beta, 1.0 / global_rows, st), 'policy_head')
         else:
             B, C, reg = a.B, lo.head_outputs, objective[1] == L.TASK_REGRESSION
             L.check(lib.progen_masked_mean_pool(a.yf.data_ptr(), d, self.act_dt, a.labels.data_ptr(),
@@ -881,7 +896,7 @@ class Engine:
         teacher.grads = None
         if teacher.B:
             teacher.alloc_epoch += 1
-            teacher.B, teacher.acts, teacher.dist, teacher.res_C, teacher.res = 0, None, None, 0, None
+            teacher.B, teacher.acts, teacher.dist, teacher.pol, teacher.res_C, teacher.res = 0, None, None, None, 0, None
             for k in teacher._train_keys:
                 setattr(teacher, k, None)
             teacher._train_keys, teacher.train_bytes = (), 0
@@ -891,7 +906,8 @@ class Engine:
         from .distill import teacher_length
         t = self.teacher
         if t is None or t.infer is None or t.infer.B < B:
-            raise L.ProgenError('distill step: no teacher rows are loaded (attach_teacher, then load_distill)')
+            raise L.ProgenError('no teacher or reference rows are loaded (attach_teacher, then load_distill or '
+                                'load_policy)')
         return t.infer.view(B, teacher_length(length, t.n))
 
     def ensure_distill(self):
@@ -906,9 +922,15 @@ class Engine:
         """rows (B, n+1) -> the student's self.tok / self.labels as load_batch, and the same rows, zero-padded to the
         teacher's seq_len + 1, into the (B, teacher_length(length)) view of the teacher's inference set (allocated for B
         rows when it holds fewer); returns B"""
-        from .distill import teacher_length
         B = self.load_batch(data, length)
         self.ensure_distill()
+        self._stage_teacher(data, B, length)
+        return B
+
+    def _stage_teacher(self, data, B, length):
+        """rows `data`, zero-padded to the attached teacher's seq_len + 1, into the (B, teacher_length(length)) view of
+        its inference set (allocated for B rows when it holds fewer)"""
+        from .distill import teacher_length
         t = self.teacher
         Lt = teacher_length(self.n if length is None else length, t.n)
         ta = t.inference_acts(B).view(B, Lt)
@@ -918,7 +940,6 @@ class Engine:
         if k < Lt:
             tok.zero_()
         tok[:, :k].copy_(rows[:, :k].to(device=self.dev, dtype=torch.int32), non_blocking=True)
-        return B
 
     def distill_stats(self, rows):
         """the last distillation step's per-row (KL, CE) as numpy float32 [rows] arrays"""
@@ -926,6 +947,32 @@ class Engine:
             return dict(kl=np.zeros(0, np.float32), ce=np.zeros(0, np.float32))
         st = self.dist['stats'][:rows].cpu().numpy()
         return dict(kl=st[:, 0].copy(), ce=st[:, 1].copy())
+
+    # ------------------------------------------------------------------------------------------ policy gradient
+    def load_policy(self, rows, span, advantage, length=None, reference=False):
+        """rows (B, n+1) -> self.tok / self.labels as load_batch; span (B, 2) int32 and advantage [B] float32 (checked by
+        policy.check_policy_batch) into the head's device buffers, allocated with the training set for its B rows; with
+        `reference` (a step with beta > 0) the same rows into the attached reference's inference set, as load_distill
+        does for a teacher.  Returns B."""
+        B = self.load_batch(rows, length)
+        if self.pol is None:
+            F = lambda *shape: torch.zeros(*shape, device=self.dev, dtype=torch.float32)
+            self.pol = dict(span=torch.zeros(self.B, 2, device=self.dev, dtype=torch.int32), adv=F(self.B),
+                            scratch=F(2 * self.T), stats=F(self.B, 3))
+        self.pol['span'][:B].copy_(torch.as_tensor(np.asarray(span, np.int32)), non_blocking=True)
+        self.pol['adv'][:B].copy_(torch.as_tensor(np.asarray(advantage, np.float32)), non_blocking=True)
+        if reference:
+            self._stage_teacher(rows, B, length)
+        return B
+
+    def policy_stats(self, rows):
+        """the last policy-gradient step's per-row statistics over each row's span as numpy [rows] arrays: logp (mean
+        log-probability of the labels, float32), kl (mean exact KL to the reference, float32; 0 with beta = 0) and count
+        (the span's positions, int64)"""
+        if not rows or self.pol is None:
+            return dict(logp=np.zeros(0, np.float32), kl=np.zeros(0, np.float32), count=np.zeros(0, np.int64))
+        st = self.pol['stats'][:rows].cpu().numpy()
+        return dict(logp=st[:, 0].copy(), kl=st[:, 1].copy(), count=st[:, 2].astype(np.int64))
 
     def ln_bwd_res(self, a, dy, x, scale, mean, rstd, dscale, shift, next_bias_grad=None):
         """LN(+shift) backward into the residual-gradient stream of the training set or its cut view `a`;

@@ -60,6 +60,8 @@ PROTOTYPES = {
     'progen_token_logprob': [_P, _I, _P, _P, _P, _P, _I, _I, _I, _P],
     'progen_preference_head': [_P, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _F, _F, _P],
     'progen_distill_head': [_P, _I, _P, _LL, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _F, _F, _F, _P],
+    'progen_policy_head': [_P, _I, _P, _LL, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _F, _F, _P],
+    'progen_decode_load_weight': [_P, _P, _P, _I, _F, _I, _I, _I, _P, _I, _P],
     'progen_masked_mean_pool': [_P, _LL, _I, _P, _P, _I, _I, _I, _P],
     'progen_masked_mean_pool_bwd': [_P, _P, _P, _LL, _I, _I, _I, _I, _P],
     'progen_property_head': [_P, _P, _P, _I, _I, _I, _I, _P, _P, _F, _P, _P, _P, _P, _P, _P, _P, _P],

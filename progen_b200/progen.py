@@ -395,6 +395,47 @@ class ProGen:
         grads = eng.export_grads() if lo is None else lo.layout.unpack(lo.grads)
         return float(eng.loss.item()), grads, eng.distill_stats(B)
 
+    def policy_loss_and_grad(self, params, samples_or_rows, advantages, *, reference=None, reference_params=None,
+                             beta=0.04, span=None, adapters=None, lora_alpha=None):
+        """Loss and gradients of one group-relative policy-gradient step (GRPO / RLOO style) with an exact KL to a frozen
+        reference (DESIGN.md §3.14).  samples_or_rows: `generate`'s dict (rows and spans by `policy.samples_to_rows`), or
+        (B, n+1) integer rows of the `collate` contract with `span` (B, 2) giving each row's label positions lo <= t < hi.
+        advantages [B]: one float per row (e.g. `policy.group_advantages` of rewards).  Per position t of row b's span,
+        with pi = softmax of this model's logits and rho the reference's: logp_t = log pi[label_t] and KL_t = KL(pi || rho)
+        exactly (a sum over the vocabulary); L_b = mean over the span of (-A_b logp_t + beta KL_t); loss = mean_b L_b.
+        With beta > 0 `reference` (another ProGen, checked as a distillation teacher; with adapters normally a model on
+        the base params) runs its forward on `reference_params` in the same step; with beta = 0 it is not needed.  With
+        `adapters` (lora_alpha as in `loss_and_grad`) the base is frozen.  Inputs are checked before any device work
+        (ProgenError naming the row).  Returns (python float loss, gradients (the adapters' with adapters), stats), stats
+        a dict of [B] arrays: logp and kl (each row's span means, float32) and count (its span length, int64)."""
+        from .distill import check_teacher
+        from .policy import check_policy_batch, samples_to_rows
+        what = 'policy_loss_and_grad'
+        if isinstance(samples_or_rows, dict):
+            if span is not None:
+                raise L.ProgenError(f'{what}: samples carry their spans; pass span= only with rows')
+            rows, span = samples_to_rows(samples_or_rows)
+        else:
+            rows = samples_or_rows
+            if span is None:
+                raise L.ProgenError(f'{what}: rows need span= (the label positions each row is trained on)')
+        rows, span, adv, beta, B = check_policy_batch(rows, span, advantages, beta, None, self.config['seq_len'], what)
+        if beta > 0:
+            check_teacher(self, reference, what)
+            if reference_params is None:
+                raise L.ProgenError(f'{what}: a reference needs reference_params')
+        self._ensure_loaded(params)
+        lo = None if adapters is None else self._attach_adapters(adapters, lora_alpha)
+        eng = self.engine
+        if beta > 0:
+            reference._ensure_loaded(reference_params)
+            eng.attach_teacher(reference.engine)
+        n = eng.row_length(rows, what=what)
+        eng.load_policy(rows, span, adv, n, reference=beta > 0)
+        eng.train_step(('policy', beta), B, length=n)
+        grads = eng.export_grads() if lo is None else lo.layout.unpack(lo.grads)
+        return float(eng.loss.item()), grads, eng.policy_stats(B)
+
     def score(self, params, data, *, batch_size=64, return_tokens=False, return_embeddings=False):
         """Log-likelihood of sequences under the model, without keeping any training state.
         data: (B, n+1) integer rows, the contract of `loss_and_grad` and `data.collate`: ids = data[:, :-1] are fed to the
@@ -539,6 +580,18 @@ class ProGen:
           token_logp [N, seq_len] float32: log p(tokens[t] | tokens[:t]) under the unfiltered model (temperature 1) at
             generated t, 0 elsewhere — the quantity `score` reports;
           prompt_index [N] int64."""
+        return self._generate(lambda batch: self._generate_decoder(params, batch), params, prompts,
+                              num_samples=num_samples, temperature=temperature, top_k=top_k, top_p=top_p,
+                              max_length=max_length, seed=seed, batch_size=batch_size, logit_bias=logit_bias,
+                              min_new_tokens=min_new_tokens, repetition_penalty=repetition_penalty,
+                              repetition_window=repetition_window, prefill=prefill, position_bias=position_bias,
+                              fixed=fixed)
+
+    def _generate(self, decoder, params, prompts, *, num_samples=1, temperature=1.0, top_k=None, top_p=None,
+                  max_length=None, seed=0, batch_size=64, logit_bias=None, min_new_tokens=0, repetition_penalty=1.0,
+                  repetition_window=0, prefill='decode', position_bias=None, fixed=None):
+        """`generate` on the BatchDecoder `decoder(rows per launch)` returns (`Trainer.generate`: the trainer's own);
+        `params` are what forward prefill runs on"""
         from .data import encode_tokens
         from .decode import Sampling, integer, prompt_ids
         cfg = self.config
@@ -562,7 +615,7 @@ class ProGen:
         N = len(ids) * num_samples
         rows = [ids[r // num_samples] for r in range(N)]
         row_table = prompt_table[np.arange(N) // num_samples]
-        dec = self._generate_decoder(params, min(batch_size, N))
+        dec = decoder(min(batch_size, N))
         if prefill == 'forward':
             self._ensure_loaded(params)
         out = dict(tokens=np.zeros((N, n), np.int64), start=np.zeros(N, np.int64), end=np.zeros(N, np.int64),
@@ -596,16 +649,19 @@ class ProGen:
         return dec
 
     def trainer(self, params, *, adapters=None, lora_alpha=None, head=None, task=None, teacher=None, teacher_params=None,
-                **optim_kwargs):
+                reference=None, reference_params=None, **optim_kwargs):
         """Device-resident training state over `params` (train.py's loop).  With `adapters` only the adapters train
         (the base stays bitwise unchanged); lora_alpha as in `loss_and_grad`.  With a property `head` (`init_head`) and
         its `task` ('regression' | 'classification') the adapters and the head train together through
         `Trainer.property_step` (per-sequence labels) or `Trainer.residue_step` (per-residue labels).  With a `teacher`
         (another ProGen, as in `distill_loss_and_grad`) and its `teacher_params`, `Trainer.distill_step` distils it into
-        this model."""
+        this model.  With a `reference` (another ProGen, as in `policy_loss_and_grad`) and its `reference_params`,
+        `Trainer.policy_step` takes policy-gradient steps with a KL to it; `Trainer.generate` samples from the weights
+        being trained."""
         from .trainer import Trainer
         return Trainer(self, params, adapters=adapters, lora_alpha=lora_alpha, head=head, task=task, teacher=teacher,
-                       teacher_params=teacher_params, **optim_kwargs)
+                       teacher_params=teacher_params, reference=reference, reference_params=reference_params,
+                       **optim_kwargs)
 
     # ---- property fine-tuning (DESIGN.md §3.9)
     def init_head(self, rng, num_outputs):

@@ -5,7 +5,8 @@ accumulator live in flat fp32 buffers; one `step(data)` is one iteration of the 
 With low-rank adapters (`adapters=`) the same state exists for the adapter buffer only: the base parameters are frozen
 and bitwise unchanged, and clip / AdamW / apply_every run over the adapters (weight decay on every A and B).  A property
 head (`head=`, `task=`) joins that buffer: `property_step` trains adapters and head together on per-sequence labels
-(DESIGN.md §3.9), `residue_step` on per-residue labels (§3.11)."""
+(DESIGN.md §3.9), `residue_step` on per-residue labels (§3.11).  With a frozen `reference=` model `policy_step` takes
+policy-gradient steps on the model's own samples (§3.14), which `generate` draws from the weights being trained."""
 import weakref
 
 import torch
@@ -19,13 +20,17 @@ class Trainer:
 
     def __init__(self, model, params, learning_rate=2e-4, weight_decay=1e-3, max_grad_norm=0.5, grad_accum_every=4,
                  b1=0.9, b2=0.999, eps=1e-8, optim_state=None, data_parallel=True, cuda_graph=False, adapters=None,
-                 lora_alpha=None, head=None, task=None, teacher=None, teacher_params=None):
+                 lora_alpha=None, head=None, task=None, teacher=None, teacher_params=None, reference=None,
+                 reference_params=None):
         self.model = model
-        if teacher is not None or teacher_params is not None:
-            from .distill import check_teacher
-            check_teacher(model, teacher, 'trainer')
-            if teacher_params is None:
-                raise L.ProgenError('trainer: a teacher needs teacher_params')
+        if (teacher is not None or teacher_params is not None) and (reference is not None or reference_params is not None):
+            raise L.ProgenError('trainer: pass a teacher (distill_step) or a reference (policy_step), not both')
+        for other, other_params, name in ((teacher, teacher_params, 'teacher'), (reference, reference_params, 'reference')):
+            if other is not None or other_params is not None:
+                from .distill import check_teacher
+                check_teacher(model, other, 'trainer')
+                if other_params is None:
+                    raise L.ProgenError(f'trainer: a {name} needs {name}_params')
         self.task = None
         if head is not None or task is not None:
             from .property import check_head, check_task
@@ -39,11 +44,14 @@ class Trainer:
         self.eng = model.engine
         self.eng.load_params(params)
         model._loaded = None
-        # distillation (distill_step): the teacher's engine keeps its parameters and inference set only
-        self.teacher = teacher
-        if teacher is not None:
-            teacher._ensure_loaded(teacher_params)
-            self.eng.attach_teacher(teacher.engine)
+        # distillation (distill_step) or the policy step's reference: that engine keeps its parameters and inference
+        # set only, in the engine's teacher slot
+        self.teacher, self.reference = teacher, reference
+        for other, other_params in ((teacher, teacher_params), (reference, reference_params)):
+            if other is not None:
+                other._ensure_loaded(other_params)
+                self.eng.attach_teacher(other.engine)
+        self._decoder, self._decoder_count = None, None   # generate: one decoder, refreshed after every step
         self.lora = None
         if adapters is not None:
             from .lora import Adapters, check_adapters, check_rank_alpha
@@ -296,6 +304,58 @@ class Trainer:
         self._distill_rows = B
         eng.train_step(('distill', tau, alpha), B, backward=False, length=n)
         return eng.loss
+
+    # ---- policy gradient on the model's own samples (DESIGN.md §3.14)
+    def policy_step(self, rows, span, advantages, beta, sync_loss=False, global_rows=None, length=None):
+        """One micro-step of policy-gradient fine-tuning: the loss and gradient of `ProGen.policy_loss_and_grad` on this
+        rank's rows (b, n+1), their spans (b, 2) and advantages [b] (`policy.samples_to_rows`, `group_advantages`), with
+        the KL to the trainer's reference (model.trainer(..., reference=, reference_params=); needed when beta > 0),
+        then the same clip / AdamW / apply_every update as `step`.  global_rows (default b * world) scales the loss, so
+        that the all-reduced gradient is the global mean; a rank without rows contributes zeros and joins the
+        all-reduce.  sync_loss and `length` as in `step`.  With cuda_graph=True the step, the reference's forward
+        included, is captured after two eager steps of one (rows, global_rows, beta, length) and replayed from then on.
+        Returns the device scalar loss; `policy_stats()` has the per-row statistics."""
+        from .policy import check_policy_batch
+        b = len(rows)
+        gr = global_rows if global_rows is not None else (b * self.world if b else None)
+        rows, span, adv, beta, gr = check_policy_batch(rows, span, advantages, beta, gr, self.eng.n, 'policy_step',
+                                                       allow_empty=True)
+        if beta > 0 and self.reference is None:
+            raise L.ProgenError('policy_step: beta > 0 needs a reference (model.trainer(..., reference=, '
+                                'reference_params=))')
+        n = self._length(rows, length, 'policy_step')
+        self._policy_rows = b
+        return self._step(b, gr, ('policy', beta), lambda: self.eng.load_policy(rows, span, adv, n, reference=beta > 0),
+                          sync_loss, n)
+
+    def policy_stats(self):
+        """this rank's per-row statistics of its last `policy_step` as numpy [b] arrays: logp and kl (span means,
+        float32) and count (span lengths, int64)"""
+        return self.eng.policy_stats(getattr(self, '_policy_rows', 0))
+
+    def generate(self, prompts, **kw):
+        """`ProGen.generate` (same arguments and return dict) from the weights this trainer is updating: with adapters the
+        model `adapters()` describes on the frozen base, otherwise `params()`.  One decoder per trainer, rebuilt only when
+        a call needs more rows per launch than it holds; its weights are rewritten on the device
+        (BatchDecoder.load_weights) when the trainer has stepped since the last call, with no host copy of any weight.
+        prefill='forward' is refused: the engine's inference forward does not apply adapters."""
+        if kw.get('prefill', 'decode') != 'decode':
+            raise L.ProgenError("Trainer.generate: only prefill='decode' runs on the trained weights")
+        return self.model._generate(self._generate_decoder, None, prompts, **kw)
+
+    def _generate_decoder(self, batch):
+        """the trainer's BatchDecoder for `batch` rows per launch, holding the current weights"""
+        from .decode import BatchDecoder
+        dec = self._decoder
+        if dec is None or dec.B < batch:
+            self._decoder = None
+            dec = BatchDecoder(self.model.config, self.params(), batch=batch,
+                               weights_dtype=torch.bfloat16 if self.model.mixed_precision else torch.float32)
+            self._decoder, self._decoder_count = dec, None
+        if self._decoder_count != self.count:
+            dec.load_weights(self.eng, self.lora)
+            self._decoder_count = self.count
+        return dec
 
     def residue_stats(self):
         """the last `residue_step`'s predictions [B, n, C] (regression values, or class logits) and per-position losses
