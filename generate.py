@@ -3,7 +3,8 @@
     python generate.py --checkpoint_path ./ckpts --prompt "[Tax=Mammalia] #" [--prompt ... | --prompts_file f.txt]
         --num_samples 100 --temperature 1.0 [--top_k K] [--top_p 0.95] --seed 0 --batch_size 64 [--max_length L]
         [--alphabet ACDEFGHIKLMNPQRSTVWY] [--min_new_tokens N] [--repetition_penalty 1.2 --repetition_window 16]
-        [--fix 12=H,57=D,102=S] [--position_bias bias.npy] [--mixed_precision] [--prefill forward] --output samples.fasta
+        [--fix 12=H,57=D,102=S] [--position_bias bias.npy] [--require 'C-x(2,4)-C-x(3)-[LIVMFYWC]-x(8)-H-x(3,5)-H']
+        [--avoid 'N-{P}-[ST]-{P}' ...] [--mixed_precision] [--prefill forward] --output samples.fasta
 
 Runs ProGen.generate: each prompt is laid out like training data (BOS, prompt), every sequence stops at its own EOS,
 temperature / top-k / nucleus (top-p) filtering happen in the persistent decode kernel.  --alphabet restricts every
@@ -11,7 +12,10 @@ draw to those residues and EOS, --min_new_tokens forbids EOS for the first N gen
 penalises the residues present in the last --repetition_window positions (0: the whole sequence); these act on the
 logits in the kernel and leave the reported log-likelihood that of the unconstrained model.  --fix K=R,... makes
 generated residue K (1-based) of every sequence R, and no sequence ends before its last fixed residue; --position_bias
-adds row j of a float32 [T, V] .npy array to the logits of generated token j + 1 (-inf bans an id there).  A
+adds row j of a float32 [T, V] .npy array to the logits of generated token j + 1 (-inf bans an id there).
+--require PATTERN makes every sequence contain one PROSITE pattern and --avoid PATTERN (repeatable, up to 8) keeps
+each out of it, in the kernel's sampler; each record's header then ends with motif=1 when the sequence satisfies them
+(0: other constraints left no way to, and the sequence ended early).  A
 contradiction between these constraints (a fixed residue outside --alphabet, say) stops with the library's error
 message before anything runs.  --prefill forward fills
 the decoder's caches for the prompt with one forward pass per distinct prompt instead of one decode step per prompt
@@ -19,6 +23,7 @@ position (faster for long prompts; bf16 models then differ from the default by r
 drop-in, one sequence, top_k=25 with the reference's quirks), the result of a row depends only on the seed and the row.
 The FASTA has one record per row (row = prompt index * num_samples + sample index):
     >{row} prompt={i} sample={j} log_likelihood={sum of log p of the generated tokens, EOS included} length={...} eos={0|1}
+        [motif={0|1} with --require / --avoid]
     <generated residues, without the EOS; characters outside printable ASCII are written as '?'>"""
 import time
 
@@ -93,13 +98,15 @@ def load_position_bias(path):
 @click.option('--repetition_window', default=0, help='positions the repetition penalty looks back (0 = the whole sequence)')
 @click.option('--fix', default=None, help='fixed residues by 1-based generated offset, e.g. 12=H,57=D,102=S')
 @click.option('--position_bias', default=None, help='.npy float32 [T, V]: row j is added to the logits of generated token j+1')
+@click.option('--require', multiple=True, help='PROSITE pattern every sequence must contain (at most one)')
+@click.option('--avoid', multiple=True, help='PROSITE pattern no sequence may contain (repeatable, up to 8)')
 @click.option('--mixed_precision', default=False, is_flag=True, help='bf16 weights in the decode kernel')
 @click.option('--prefill', default='decode', type=click.Choice(['decode', 'forward']),
               help='prompt positions: one decode step each, or one forward pass per distinct prompt')
 @click.option('--output', default='samples.fasta')
 def main(checkpoint_path, prompts, prompts_file, num_samples, temperature, top_k, top_p, seed, batch_size, max_length,
-         alphabet, min_new_tokens, repetition_penalty, repetition_window, fix, position_bias, mixed_precision, prefill,
-         output):
+         alphabet, min_new_tokens, repetition_penalty, repetition_window, fix, position_bias, require, avoid,
+         mixed_precision, prefill, output):
     _, get_last_checkpoint, _ = get_checkpoint_fns(checkpoint_path)
     last_checkpoint = get_last_checkpoint()
     if last_checkpoint is None:
@@ -111,6 +118,8 @@ def main(checkpoint_path, prompts, prompts_file, num_samples, temperature, top_k
     try:
         fixed = None if fix is None else parse_fix(fix)
         pbias = None if position_bias is None else load_position_bias(position_bias)
+        if len(require) > 1:
+            raise ProgenError(f'--require: at most one pattern, got {len(require)}')
     except ProgenError as e:
         exit(f'ProgenError: {e}')
     prompts = list(prompts)
@@ -124,9 +133,12 @@ def main(checkpoint_path, prompts, prompts_file, num_samples, temperature, top_k
     kw = dict(num_samples=num_samples, temperature=temperature, top_k=top_k, top_p=top_p, max_length=max_length, seed=seed,
               batch_size=batch_size, logit_bias=bias, min_new_tokens=min_new_tokens, repetition_penalty=repetition_penalty,
               repetition_window=repetition_window, prefill=prefill)
-    if fixed is None and pbias is None:
+    motifs = bool(require or avoid)
+    if fixed is None and pbias is None and not motifs:
         res = model.generate(params, prompts, **kw)
     else:
+        if motifs:
+            kw.update(require=require[0] if require else None, avoid=list(avoid) or None)
         try:                                             # contradictory constraints: the library's message, no traceback
             res = model.generate(params, prompts, position_bias=pbias, fixed=fixed, **kw)
         except ProgenError as e:
@@ -138,7 +150,8 @@ def main(checkpoint_path, prompts, prompts_file, num_samples, temperature, top_k
             s, ln, fin = int(res['start'][row]), int(res['length'][row]), bool(res['finished'][row])
             body = fasta_safe(decode_tokens(res['tokens'][row, s:s + ln - int(fin)]))
             f.write(f'>{row} prompt={row // num_samples} sample={row % num_samples} '
-                    f'log_likelihood={res["log_likelihood"][row]:.6f} length={ln} eos={int(fin)}\n{body}\n')
+                    f'log_likelihood={res["log_likelihood"][row]:.6f} length={ln} eos={int(fin)}'
+                    + (f' motif={int(res["motif_match"][row])}' if motifs else '') + f'\n{body}\n')
     gen = int(res['length'].sum())
     print(f'{N} sequences, {gen} generated tokens, {int(res["finished"].sum())} ended with EOS')
     print(f'{N / secs:.2f} sequences/s, {gen / secs:.0f} generated tokens/s (wall clock, including setup)')

@@ -348,7 +348,7 @@ typedef struct progen_decode_run_t {
   int32_t repetition_window;   /* >= 0; 0 = every position since BOS */
   int32_t min_new_tokens;      /* >= 0: the first min_new_tokens draws of a row are never EOS */
   int32_t _pad2;
-  /* Row queue (sampler 1, B >= 2; all NULL / 0 = no queue): the B sequences of the launch become slots that decode the
+  /* Row queue (sampler 1, B >= 2; the four pointers NULL and num_rows 0 = no queue): the B sequences of the launch become slots that decode the
    * Q = num_rows rows of a queue.  seq, start, end, token_logp and sample_id are then indexed by the queue row ([Q] /
    * [Q, n]); caches and scratch stay per slot.  Slot b decodes row slot_row[b] (-1: idle) at position slot_pos[b], which
    * it advances by one per step.  A row retires when it draws EOS or position max_length - 1; its slot counts it in
@@ -364,7 +364,8 @@ typedef struct progen_decode_run_t {
   int32_t* next_row;           /* device: the next unclaimed queue row */
   int32_t* done;               /* device: rows retired */
   int32_t num_rows;            /* Q */
-  int32_t max_length;          /* in [2, n]: a row's last drawn position is max_length - 1 */
+  int32_t max_length;          /* in [2, n]: a row's last drawn position is max_length - 1 (0: n; needed by a queue
+                                  and by motif constraints) */
   /* Position-specific bias (sampler 1; both pointers NULL = off): tables of per-offset logit biases.  For the draw of
    * position p + 1 of row r (the queue row when there is a queue), j = p + 1 - start[r] is the 0-based generated offset;
    * if t = position_bias_table[r] >= 0 and j < position_bias_len, a[c] += position_bias[(t * position_bias_len + j) * V
@@ -374,7 +375,40 @@ typedef struct progen_decode_run_t {
   const int32_t* position_bias_table;/* [rows]: the table of each row, -1 = none */
   int32_t position_bias_len;         /* in [1, n] when position_bias is set */
   int32_t _pad3;
+  /* Motif constraints (sampler 1; NULL = off): a DEVICE progen_motif_t (below).  Needs max_length (above) in [2, n] in
+   * static launches too: a row's last drawn position is max_length - 1 with or without a queue. */
+  const struct progen_motif_t* motif;
 } progen_decode_run_t;
+
+/* Motif constraints of sampler 1 (DESIGN.md §3.3, progen_b200/motif.py): P PROSITE patterns, each of m <= 64 positions
+ * (a class of ids, mandatory or optional), matched against a row's generated tokens t_1..t_L.  A row's state is one
+ * bitset D per pattern (bit i: positions 0..i match a suffix of the tokens so far, optional positions skipped) and a flags
+ * word (bit 0: the required pattern is met).  Reading id c >= 1, with z = !(anchors & 1) || (c is t_1):
+ *   D' = closure((((D | (z ? lead : 0)) << 1) | z) & mask[k][c]),  closure(X): X |= (X << 1) & optional until stable.
+ * A pattern matches at c when D' has bit `last`.  The required pattern (pattern 0 when required = 1) is met once it
+ * matched (anchors & 2, '>': only when it matched at the latest token); its lookahead after c is 0 when met, else
+ * need[msb(D')] (D' != 0), need[64] (D' == 0 and the start state stays active), or never.  Per draw at position p + 1 of
+ * row r, after every other adjustment above, an id becomes -inf when: c >= 1 and the required pattern's lookahead exceeds
+ * the positions left after it, max_length - p - 2; c >= 1 and it completes an avoided pattern (a '>'-anchored one only
+ * at p + 1 = max_length - 1); c = 0 while the required pattern is not met, or while the D of a '>'-anchored avoided
+ * pattern has bit `last`.  After the draw of a residue, the row's state becomes its D' and flags. */
+typedef struct progen_motif_pattern_t {
+  uint64_t optional;           /* bit i: position i is optional */
+  uint64_t lead;               /* the positions before the first mandatory one (states reached without a residue) */
+  uint64_t last;               /* the bit of the pattern's last position */
+  uint64_t anchors;            /* bit 0 '<' (at t_1), bit 1 '>' (at t_L) */
+} progen_motif_pattern_t;
+typedef struct progen_motif_t {
+  int32_t num_patterns;        /* P in [1, 9] */
+  int32_t required;            /* 1: pattern 0 is required and the others avoided; 0: every pattern is avoided */
+  int32_t need[65];            /* required pattern: fewest residues completing it from the state of bit i; [64]: from
+                                  the start.  Computed with logit_bias's bans; non-increasing in i; >= 2^30: never */
+  int32_t _pad;
+  progen_motif_pattern_t pattern[9];
+  const uint64_t* mask;        /* [P, V] device: bit i of mask[k * V + c] = id c matches position i of pattern k */
+  uint64_t* state;             /* [rows, P + 1] device, zeroed by the caller: row r's D of every pattern, then its flags
+                                  (indexed by the queue row when there is a queue) */
+} progen_motif_t;
 
 int progen_decode_run(const progen_decode_run_t* run, void* stream);
 

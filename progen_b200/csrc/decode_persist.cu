@@ -1485,9 +1485,59 @@ static __device__ __forceinline__ float philox_gumbel(unsigned long long seed, l
 // registers stay out of the GEMV phases' allocation.  sv: shared memory [2 V]; red: the block-reduction scratch.
 // Constraints (progen_b200.h): after logsumexp of the raw logits, sv is overwritten with the adjusted logits a, and the
 // filter and draw below run on a unchanged: -inf and NaN never win a comparison, so only candidates can be drawn.
-// One argument (fewer registers at the call): the logit bias, the repetition penalty, min_new_tokens and the position
-// tables (pbias [tables, plen, V], ptable [rows]: each row's table or -1; pbias null = none)
-struct SampleCons { const float* bias; float theta; int window, min_new; const float* pbias; const int32_t* ptable; int plen; };
+// One argument (fewer registers at the call): the logit bias, the repetition penalty, min_new_tokens, the position
+// tables (pbias [tables, plen, V], ptable [rows]: each row's table or -1; pbias null = none) and the motif descriptor
+// (null = none) with the launch's max_length, which its lookahead counts the positions left against
+struct SampleCons {
+  const float* bias; float theta; int window, min_new; const float* pbias; const int32_t* ptable; int plen;
+  const progen_motif_t* motif; int max_length;
+};
+
+// Motif step (progen_b200.h): may id c be drawn by a row in state st ([P] bitsets, flags), given that it is the row's
+// first generated token (`first`) and `left` positions follow it before max_length?  With nx, the row's next state after
+// c is written there (the caller's c was drawn, so every pattern runs).  At most P <= 9 patterns of 64-bit operations;
+// the closure loop runs once per optional position in a row plus one.
+static __device__ __forceinline__ uint64_t ldg64(const uint64_t* p) { return __ldg(reinterpret_cast<const unsigned long long*>(p)); }
+static __device__ __forceinline__ uint64_t ldcg64(const uint64_t* p) { return __ldcg(reinterpret_cast<const unsigned long long*>(p)); }
+static __device__ __forceinline__ bool motif_allows(const progen_motif_t* M, const uint64_t* st, int c, int V, bool first,
+                                                    int left, uint64_t* nx) {
+  const int P = __ldg(&M->num_patterns);
+  const bool req = __ldg(&M->required) != 0;
+  const uint64_t flags = ldcg64(st + P);
+  if (c == 0) {                                                                // EOS: the row ends after t_L
+    if (req && !(flags & 1ull)) return false;
+    for (int k = req ? 1 : 0; k < P; ++k) {
+      const progen_motif_pattern_t* pt = M->pattern + k;
+      if ((ldg64(&pt->anchors) & 2ull) && (ldcg64(st + k) & ldg64(&pt->last))) return false;
+    }
+    return true;
+  }
+  bool ok = true;
+  uint64_t met = 0;
+  for (int k = 0; k < P; ++k) {
+    const progen_motif_pattern_t* pt = M->pattern + k;
+    const uint64_t anch = ldg64(&pt->anchors), opt = ldg64(&pt->optional), last = ldg64(&pt->last);
+    const bool z = !(anch & 1ull) || first;                                    // the start state is active at c
+    const uint64_t D = ldcg64(st + k) | (z ? ldg64(&pt->lead) : 0ull);
+    uint64_t X = ((D << 1) | (z ? 1ull : 0ull)) & ldg64(M->mask + (long long)k * V + c);
+    for (uint64_t Y = X | ((X << 1) & opt); Y != X; Y = X | ((X << 1) & opt)) X = Y;
+    const bool hit = (X & last) != 0ull;
+    if (k == 0 && req) {
+      met = ((anch & 2ull) ? 0ull : (flags & 1ull)) | (hit ? 1ull : 0ull);
+      if (!met) {
+        // need[] never increases along the pattern: the state's fewest residues left are those of its highest bit
+        const int need = X ? __ldg(&M->need[63 - __clzll((long long)X)]) : (!(anch & 1ull) ? __ldg(&M->need[64]) : 0x7fffffff);
+        if (need > left) ok = false;
+      }
+    } else if (hit && (!(anch & 2ull) || left == 0)) {
+      ok = false;
+    }
+    if (nx) nx[k] = X;
+    else if (!ok) return false;
+  }
+  if (nx) nx[P] = met;
+  return ok;
+}
 // The queue kernels' view of the slots (SLOT): this step's row and position of every slot (shared memory), the queue's
 // device state and what a refill resets.  Without a queue (slot_row null) srow[b] = b and spos[b] = the launch's position.
 struct SlotArgs {
@@ -1510,7 +1560,7 @@ static __device__ __noinline__ void sample_std_phase(const float* logits, int32_
   const int t = threadIdx.x;
   float* qv = sv + V;                                                          // kept ids: q; removed: -1
   int* redi = reinterpret_cast<int*>(red + 32);
-  const bool cons = cs.bias != nullptr || cs.theta != 1.f || cs.min_new != 0 || cs.pbias != nullptr;  // uniform
+  const bool cons = cs.bias != nullptr || cs.theta != 1.f || cs.min_new != 0 || cs.pbias != nullptr || cs.motif != nullptr;  // uniform
   const SlotArgs S = slot_args(slot...);
   // queue: slot b retires its row (counted in `done`), then claims the next row of the queue, q = next_row++.  A claimed
   // row starts at position 0: the slot's token-shift slot 0 of every layer (the only state read at position 0 before it
@@ -1587,6 +1637,8 @@ static __device__ __noinline__ void sample_std_phase(const float* logits, int32_
           const int tb = __ldg(cs.ptable + rb), j = pos + 1 - start[rb];       // (j >= 0: a drawn position)
           if (tb >= 0 && j < cs.plen) pb = cs.pbias + ((long long)tb * cs.plen + j) * V;
         }
+        const uint64_t* mst = nullptr;                                          // the row's motif state
+        if (cs.motif) mst = cs.motif->state + (long long)rb * (cs.motif->num_patterns + 1);
         float ma = -INFINITY;
         for (int c = t; c < V; c += TPB) {
           float a = sv[c];
@@ -1594,6 +1646,8 @@ static __device__ __noinline__ void sample_std_phase(const float* logits, int32_
           if (cs.bias) a = __fadd_rn(a, __ldg(cs.bias + c));                 // (no FMA with the penalty's product)
           if (pb) a = __fadd_rn(a, __ldg(pb + c));                            // a separate rounding after the bias
           if (c == 0 && no_eos) a = -INFINITY;
+          if (mst && a > -INFINITY && !motif_allows(cs.motif, mst, c, V, pos + 1 == start[rb], cs.max_length - pos - 2, nullptr))
+            a = -INFINITY;
           sv[c] = a;
           ma = fmaxf(ma, a);
         }
@@ -1652,6 +1706,10 @@ static __device__ __noinline__ void sample_std_phase(const float* logits, int32_
         seq[row + pos + 1] = id;
         if (token_logp) token_logp[row + pos + 1] = (cons ? __ldcg(lg + id) : sv[id]) - lse;   // the raw logit
         if (id == 0) { end[rb] = pos + 1; atomicAdd(n_ended, 1); }
+        else if (cons && cs.motif) {                                           // the drawn residue's next state (read next draw, after the grid barrier)
+          uint64_t* mst = cs.motif->state + (long long)rb * (cs.motif->num_patterns + 1);
+          motif_allows(cs.motif, mst, id, V, pos + 1 == start[rb], cs.max_length - pos - 2, mst);
+        }
       }
     }
     if constexpr (SLOT) {
@@ -1857,14 +1915,14 @@ static __device__ __forceinline__ void run(const progen_decode_run_t& r) {
         sample_std_phase<true>(r.logits, r.seq, r.start, r.end, r.n_ended, r.token_logp, r.logits_all, r.embed, r.x, r.sample_id, r.n, r.V,
                                d, B, r.top_k, r.temperature, r.top_p, r.seed,
                                SampleCons{r.logit_bias, r.repetition_penalty, r.repetition_window, r.min_new_tokens, r.position_bias,
-                                          r.position_bias_table, r.position_bias_len}, pos, xs, red,
+                                          r.position_bias_table, r.position_bias_len, r.motif, r.max_length}, pos, xs, red,
                                SlotArgs{s_row, s_pos, r.slot_row, r.slot_pos, r.next_row, r.done, r.layers, r.depth, r.num_rows,
                                         r.max_length, r.shift_tokens});
       } else if constexpr (STD) {
         sample_std_phase<false>(r.logits, r.seq, r.start, r.end, r.n_ended, r.token_logp, r.logits_all, r.embed, r.x, r.sample_id, r.n, r.V,
                                 d, B, r.top_k, r.temperature, r.top_p, r.seed,
                                 SampleCons{r.logit_bias, r.repetition_penalty, r.repetition_window, r.min_new_tokens, r.position_bias,
-                                          r.position_bias_table, r.position_bias_len}, pos, xs, red);
+                                          r.position_bias_table, r.position_bias_len, r.motif, r.max_length}, pos, xs, red);
       } else {
         sample_phase(r, pos, xs, red);
       }
@@ -1947,9 +2005,10 @@ int progen_decode_run(const progen_decode_run_t* r, void* stream) {
   PG_CHECK_ARG(r->window >= 1 && r->window <= 512);                    // <= 32 key slices per (sequence, head)
   // row queue: every field or none; sampler 1 on a batched tile only; at least one row per slot
   const bool queue = r->slot_row != nullptr || r->slot_pos != nullptr || r->next_row != nullptr || r->done != nullptr ||
-                     r->num_rows != 0 || r->max_length != 0;
+                     r->num_rows != 0;
+  PG_CHECK_ARG(r->max_length == 0 || (r->max_length >= 2 && r->max_length <= r->n));
   if (queue) {
-    PG_CHECK_ARG(r->sampler == 1 && r->B >= 2 && r->num_rows >= r->B && r->max_length >= 2 && r->max_length <= r->n);
+    PG_CHECK_ARG(r->sampler == 1 && r->B >= 2 && r->num_rows >= r->B && r->max_length >= 2);
     PG_CHECK_ARG(r->slot_row != nullptr && r->slot_pos != nullptr && r->next_row != nullptr && r->done != nullptr);
     PG_CHECK_ARG(r->logits_all == nullptr || r->num_rows == r->B);
   }
@@ -1962,6 +2021,15 @@ int progen_decode_run(const progen_decode_run_t* r, void* stream) {
   // position tables: both pointers or neither, a length in [1, n], sampler 1 only
   PG_CHECK_ARG((r->position_bias == nullptr) == (r->position_bias_table == nullptr));
   if (r->position_bias) PG_CHECK_ARG(r->sampler == 1 && r->position_bias_len >= 1 && r->position_bias_len <= r->n);
+  // motif constraints: sampler 1 with a max_length; the descriptor is device memory, so its header is read back here
+  if (r->motif) {
+    PG_CHECK_ARG(r->sampler == 1 && r->max_length >= 2);
+    progen_motif_t h;
+    PG_CUDA(cudaMemcpyAsync(&h, r->motif, sizeof(h), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
+    PG_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
+    PG_CHECK_ARG(h.num_patterns >= 1 && h.num_patterns <= 9 && (h.required == 0 || h.required == 1));
+    PG_CHECK_ARG(h.mask != nullptr && h.state != nullptr);
+  }
   if (r->sampler == 1) {
     PG_CHECK_ARG(std::isfinite(r->temperature) && r->temperature >= 0.f && r->top_p > 0.f && r->top_p <= 1.f);
     PG_CHECK_ARG(r->top_k >= 0 && r->top_k <= r->V);

@@ -112,7 +112,18 @@ class DecodeRun(C.Structure):
                [(k, _P) for k in ('sample_id', 'token_logp', 'end', 'n_ended', 'steps_run', 'logit_bias')] + \
                [('repetition_penalty', C.c_float), ('repetition_window', _I), ('min_new_tokens', _I), ('_pad2', _I)] + \
                [(k, _P) for k in ('slot_row', 'slot_pos', 'next_row', 'done')] + [('num_rows', _I), ('max_length', _I)] + \
-               [(k, _P) for k in ('position_bias', 'position_bias_table')] + [('position_bias_len', _I), ('_pad3', _I)]
+               [(k, _P) for k in ('position_bias', 'position_bias_table')] + [('position_bias_len', _I), ('_pad3', _I)] + \
+               [('motif', _P)]
+
+
+class MotifPattern(C.Structure):
+    _fields_ = [(k, C.c_uint64) for k in ('optional', 'lead', 'last', 'anchors')]
+
+
+class MotifDesc(C.Structure):
+    """progen_motif_t: the device descriptor of the motif constraints (include/progen_b200.h, motif.py)"""
+    _fields_ = [('num_patterns', _I), ('required', _I), ('need', _I * 65), ('_pad', _I), ('pattern', MotifPattern * 9),
+                ('mask', _P), ('state', _P)]
 
 
 class BatchDecoder:
@@ -388,7 +399,7 @@ class BatchDecoder:
 
     def generate(self, prompts, *, temperature=1.0, top_k=None, top_p=None, seed=0, sample_ids=None, max_length=None,
                  logit_bias=None, min_new_tokens=0, repetition_penalty=1.0, repetition_window=0, position_bias=None,
-                 prefilled=0):
+                 prefilled=0, motif=None):
         """The standard sampler (sampler 1 of csrc/decode_persist.cu) for up to B prompts (integer arrays of ids in [1, V)).
         Each row is laid out as training data is, [0 (BOS), prompt..., 0...], and draws positions 1 + len(prompt) ..
         max_length - 1 until it samples EOS (id 0).  Row b uses the Philox stream sample_ids[b] (default b); the
@@ -405,6 +416,8 @@ class BatchDecoder:
         before the EOS ban, for j < Lb (-1: no table; -inf bans an id at that offset).
         prefilled = P > 0: `prefill` has filled the caches of these prompts for positions < P (P <= every prompt's
         length), so the caches are not reset and the kernel starts at position P instead of 0.
+        motif: a motif.Motif (required / avoided PROSITE patterns), applied after every other adjustment: each row's
+        state starts at zero (nothing generated) and the kernel bans the ids that break the patterns (progen_b200.h).
         Returns a dict of numpy arrays: ids [R, n] int64, token_logp [R, n] float32 (log p(ids[t] | ids[:t]) at drawn t,
         else 0), end [R] int32 (position of the EOS, n if none), start [R] int32; and steps_run (positions the last
         launch consumed before every row had ended, or its full length), device_s (that launch's device time) and
@@ -414,19 +427,19 @@ class BatchDecoder:
         s = Sampling.check(self.V, self.n, self.n, False, temperature=temperature, top_k=top_k, top_p=top_p, seed=seed,
                            logit_bias=logit_bias, min_new_tokens=min_new_tokens, repetition_penalty=repetition_penalty,
                            repetition_window=repetition_window)
-        return self._generate(prompts, s, sample_ids, max_length, position_bias, prefilled=prefilled)
+        return self._generate(prompts, s, sample_ids, max_length, position_bias, prefilled=prefilled, motif=motif)
 
     def generate_queue(self, prompts, *, slots=None, temperature=1.0, top_k=None, top_p=None, seed=0, sample_ids=None,
                        max_length=None, logit_bias=None, min_new_tokens=0, repetition_penalty=1.0, repetition_window=0,
-                       position_bias=None):
+                       position_bias=None, motif=None):
         """`generate` for Q = len(prompts) rows on `slots` (default min(B, Q), 2 <= slots <= min(B, Q)) sequences of ONE
         persistent launch: the rows form a queue, and a slot whose row ends (EOS, or position max_length - 1) takes the
         next row, which starts at position 0 with its prompt decoded like generated positions (csrc/decode_persist.cu,
         progen_b200.h).  A row's bits depend on its seed, sample id, prompt, the class of `slots` (2-8 or 9-64) and
         the GPU's SM count, not on its slot or the other rows, so each row equals what `generate` gives it in a launch of
         that class; the launch merely has no slot waiting for its longest row.  position_bias's table_of_row is indexed
-        by queue row ([Q]).  Returns the dict of `generate` over the Q rows; steps_run is the positions the launch ran
-        and prefill_s is 0."""
+        by queue row ([Q]), and so is the motif state.  Returns the dict of `generate` over the Q rows; steps_run is the
+        positions the launch ran and prefill_s is 0."""
         Q = len(prompts)
         slots = min(self.B, Q) if slots is None else int(slots)
         if not 2 <= slots <= min(self.B, Q):
@@ -434,9 +447,9 @@ class BatchDecoder:
         s = Sampling.check(self.V, self.n, self.n, False, temperature=temperature, top_k=top_k, top_p=top_p, seed=seed,
                            logit_bias=logit_bias, min_new_tokens=min_new_tokens, repetition_penalty=repetition_penalty,
                            repetition_window=repetition_window)
-        return self._generate(prompts, s, sample_ids, max_length, position_bias, slots=slots)
+        return self._generate(prompts, s, sample_ids, max_length, position_bias, slots=slots, motif=motif)
 
-    def _generate(self, prompts, s, sample_ids, max_length, position_bias, prefilled=0, slots=None):
+    def _generate(self, prompts, s, sample_ids, max_length, position_bias, prefilled=0, slots=None, motif=None):
         """One sampler-1 launch with the checked settings s (a Sampling).  slots None: row b runs on sequence b, after a
         launch that consumes the prompt positions from `prefilled` on; else the rows form the queue of `slots` sequences.
         It launches a copy of self.m with this call's buffers and sampler fields, so self.m keeps what `sample` runs."""
@@ -471,6 +484,10 @@ class BatchDecoder:
             tables, table_of_row = map(to_dev, position_bias)
             m.position_bias, m.position_bias_table = tables.data_ptr(), table_of_row.data_ptr()
             m.position_bias_len = tables.shape[1]
+        m.max_length = max_length
+        if motif is not None:                             # descriptor, masks and per-row state: one zeroed device block
+            desc = self._motif_descriptor(motif, R)
+            m.motif = desc.data_ptr()
         if slots is None:
             pre = (prefilled, first - prefilled)          # prefill: only advances the caches
             main = (first, max_length - 1 - first)        # positions first .. max_length - 2 (the last writes max_length - 1)
@@ -478,7 +495,7 @@ class BatchDecoder:
             slot_row = torch.arange(slots, device=dev, dtype=torch.int32)
             slot_pos = torch.zeros(slots, device=dev, dtype=torch.int32)
             m.next_row, m.done = c + 8, c + 12
-            m.slot_row, m.slot_pos, m.num_rows, m.max_length = slot_row.data_ptr(), slot_pos.data_ptr(), R, max_length
+            m.slot_row, m.slot_pos, m.num_rows = slot_row.data_ptr(), slot_pos.data_ptr(), R
             # while rows wait in the queue every slot is busy, and a row consumes at most max_length - 1 positions
             pre, main = (0, 0), (0, -(-R * (max_length - 1) // slots) + max_length - 1)
         if not prefilled:
@@ -497,6 +514,27 @@ class BatchDecoder:
         return dict(ids=seq.cpu().numpy().astype(np.int64), token_logp=token_logp.cpu().numpy(), end=end.cpu().numpy(),
                     start=starts, steps_run=int(cnt[1]), device_s=ev[1].elapsed_time(ev[2]) / 1e3,
                     prefill_s=ev[0].elapsed_time(ev[1]) / 1e3 if pre[1] > 0 else 0.0)
+
+    def _motif_descriptor(self, motif, rows):
+        """progen_motif_t for `rows` rows in one device buffer: the descriptor, the masks [P, V] and the zeroed state
+        [rows, P + 1] behind it"""
+        mask, pat, need = motif.descriptor_arrays()
+        P = len(pat)
+        if not 1 <= P <= 9 or mask.shape != (P, self.V):
+            raise L.ProgenError(f'generate: a motif needs 1 to 9 patterns over {self.V} ids')
+        head = (C.sizeof(MotifDesc) + 15) // 16 * 16
+        buf = torch.zeros(head + mask.nbytes + rows * (P + 1) * 8, dtype=torch.uint8, device=self.dev)
+        d = MotifDesc()
+        d.num_patterns, d.required = P, int(motif.required)
+        d.need[:] = need.tolist()
+        for k in range(P):
+            d.pattern[k].optional, d.pattern[k].lead, d.pattern[k].last, d.pattern[k].anchors = (int(v) for v in pat[k])
+        d.mask, d.state = buf.data_ptr() + head, buf.data_ptr() + head + mask.nbytes
+        host = np.zeros(head + mask.nbytes, np.uint8)
+        host[:C.sizeof(MotifDesc)] = np.frombuffer(bytes(d), np.uint8)
+        host[head:] = np.frombuffer(np.ascontiguousarray(mask, np.uint64).tobytes(), np.uint8)
+        buf[:head + mask.nbytes].copy_(torch.from_numpy(host))
+        return buf
 
     def _position_bias(self, position_bias, rows):
         """checks position_bias of generate / generate_queue (`rows` rows); -> (float32 tables, int32 map) or None"""

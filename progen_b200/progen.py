@@ -518,7 +518,7 @@ class ProGen:
 
     def generate(self, params, prompts, *, num_samples=1, temperature=1.0, top_k=None, top_p=None, max_length=None, seed=0,
                  batch_size=64, logit_bias=None, min_new_tokens=0, repetition_penalty=1.0, repetition_window=0,
-                 prefill='decode', position_bias=None, fixed=None):
+                 prefill='decode', position_bias=None, fixed=None, require=None, avoid=None):
         """Sample sequences with the standard sampler of the persistent decode kernel (temperature, top-k with ties kept,
         nucleus top-p, in-kernel Philox Gumbel noise; csrc/decode_persist.cu), stopping each sequence at its EOS.
         Unlike the reference sampler (utils.sample, sample.py), a prompt is laid out as training data is: BOS (0), the
@@ -557,6 +557,15 @@ class ProGen:
             position_bias.  Offsets a prompt cannot reach before max_length, residues outside the vocabulary, and any
             reachable offset left with no candidate (say a fixed residue banned by logit_bias) raise ProgenError naming
             the prompt and the offset; an offset that allows only EOS ends the row there.
+          require / avoid (after every adjustment above): None or one PROSITE pattern that a row's generated tokens
+            t_1..t_L (before EOS, or up to max_length) must contain, and None, one pattern or a list of at most 8 that
+            they must not contain; the same for every prompt, the prompt not matched (`motif.Pattern`: elements
+            separated by '-', a letter, x, [..] or {..} with an optional (n) or (n,m) repeat, '<' / '>' anchor at t_1 /
+            t_L, at most 64 positions).  A residue is drawn only if the required pattern can still be completed before
+            max_length, EOS only once it is met, and no residue or EOS that completes an avoided pattern (a '>'-anchored
+            one: at the row's end).  A row whose other constraints leave no candidate ends with EOS unmet.  Refused
+            before anything runs: a malformed pattern, a mandatory position of the required one that logit_bias bans
+            entirely, and a prompt that leaves fewer positions than its shortest match.
         Only the ids whose adjusted logit is not -inf can be drawn.  token_logp and log_likelihood do not see the
         constraints: they stay the unfiltered model's at temperature 1, comparable with `score`.  With position tables a
         row's bits depend only on (seed, row), its prompt, its table and the launch class, not on the other rows' tables
@@ -579,17 +588,19 @@ class ProGen:
           log_likelihood [N] float64: sum of token_logp over the generated positions;
           token_logp [N, seq_len] float32: log p(tokens[t] | tokens[:t]) under the unfiltered model (temperature 1) at
             generated t, 0 elsewhere — the quantity `score` reports;
-          prompt_index [N] int64."""
+          prompt_index [N] int64;
+          motif_match [N] bool (with require or avoid): the row's generated tokens contain the required pattern and
+            none of the avoided ones, replayed on the host."""
         return self._generate(lambda batch: self._generate_decoder(params, batch), params, prompts,
                               num_samples=num_samples, temperature=temperature, top_k=top_k, top_p=top_p,
                               max_length=max_length, seed=seed, batch_size=batch_size, logit_bias=logit_bias,
                               min_new_tokens=min_new_tokens, repetition_penalty=repetition_penalty,
                               repetition_window=repetition_window, prefill=prefill, position_bias=position_bias,
-                              fixed=fixed)
+                              fixed=fixed, require=require, avoid=avoid)
 
     def _generate(self, decoder, params, prompts, *, num_samples=1, temperature=1.0, top_k=None, top_p=None,
                   max_length=None, seed=0, batch_size=64, logit_bias=None, min_new_tokens=0, repetition_penalty=1.0,
-                  repetition_window=0, prefill='decode', position_bias=None, fixed=None):
+                  repetition_window=0, prefill='decode', position_bias=None, fixed=None, require=None, avoid=None):
         """`generate` on the BatchDecoder `decoder(rows per launch)` returns (`Trainer.generate`: the trainer's own);
         `params` are what forward prefill runs on"""
         from .data import encode_tokens
@@ -612,6 +623,11 @@ class ProGen:
                           for p in prompts], V, max_length)
         tables, prompt_table = position_tables([1 + len(a) for a in ids], V, n, max_length, position_bias, fixed,
                                                sampling.logit_bias, sampling.min_new_tokens)
+        motif = None
+        if require is not None or avoid is not None:
+            from .motif import Motif
+            motif = Motif(require, avoid, V, sampling.logit_bias)
+            motif.check_reach([1 + len(a) for a in ids], max_length)
         N = len(ids) * num_samples
         rows = [ids[r // num_samples] for r in range(N)]
         row_table = prompt_table[np.arange(N) // num_samples]
@@ -625,7 +641,7 @@ class ProGen:
             chunk = [rows[r] for r in sids]
             P = dec.prefill(self.engine, chunk) if prefill == 'forward' else 0
             res = dec._generate(chunk, sampling, sids, max_length, launch_tables(tables, row_table, sids), prefilled=P,
-                                slots=slots)
+                                slots=slots, motif=motif)
             for k, key in (('tokens', 'ids'), ('token_logp', 'token_logp'), ('start', 'start'), ('end', 'end')):
                 out[k][sids[:real]] = res[key][:real]
         end = out.pop('end')
@@ -633,6 +649,9 @@ class ProGen:
         out['length'] = np.where(out['finished'], end + 1, max_length) - out['start']
         out['log_likelihood'] = out['token_logp'].astype(np.float64).sum(axis=-1)
         out['prompt_index'] = np.arange(N, dtype=np.int64) // num_samples
+        if motif is not None:
+            gen = out['length'] - out['finished']
+            out['motif_match'] = motif.matches([out['tokens'][i, s:s + g] for i, (s, g) in enumerate(zip(out['start'], gen))])
         return out
 
     def _generate_decoder(self, params, batch):
